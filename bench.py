@@ -1,4 +1,4 @@
-"""Benchmark of the render hot path (NerfModel.__call__) on B200.
+"""Benchmark of the render hot path (NerfModel.__call__) on H100.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--precision P] [--workload W]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
@@ -88,7 +88,7 @@ PARITY_BOUNDS = {
 DTYPE_NAMES = {
     'fp32': 'fp32',
     'bf16': 'bf16',
-    'fp16x3': 'fp16x3 (fp32 emulated on tcgen05: 3 fp16 MMA chains, fp32 accumulate)',
+    'fp16x3': 'fp16x3 (fp32 emulated on wgmma: 3 fp16 MMA chains, fp32 accumulate)',
 }
 
 
@@ -108,6 +108,8 @@ def parse_args():
   ap.add_argument('--no-cpu-baseline', action='store_true')
   ap.add_argument('--no-parity', action='store_true')
   ap.add_argument('--cpu-seconds', type=float, default=15.0)
+  ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                  help='write what the last timed step returned as DIR/<name>.npy (float32)')
   return ap.parse_args()
 
 
@@ -605,6 +607,7 @@ def measure(precision, wl, B, args, ctx, want_parity):
       'launches': int(launches), 'clocks': clocks, 'wall': wall,
       'field_ms': (statistics.mean(m[0] for m in field_ms), statistics.mean(m[1] for m in field_ms)),
   }
+  res['out'] = out
   if want_parity and rank == 0:
     res['parity'] = parity_check(model, variables, params_cpu, rays_host, out, wl, precision)
   res['model'], res['variables'], res['rays_host'], res['warp_extra'] = model, variables, rays_host, warp_extra
@@ -620,7 +623,7 @@ def roofline(res, wl, B, peaks, precision):
   peak = peaks.get('bf16_tflops') or peaks.get('bf16_tflops_sustained')
   peak_src = 'measured (MEASURED_PEAKS.json, burst bf16 cuBLAS 8192^3)'
   if not peak:
-    peak, peak_src = 1590.0, 'fallback (B200_PROFILING.md)'
+    peak, peak_src = 989.0, 'NVIDIA H100 SXM data sheet, dense bf16 at 700 W (not a measured rate)'
   traffic = None
   try:
     with open(os.path.join(REPO, 'profiles', 'traffic.json')) as f:
@@ -631,10 +634,7 @@ def roofline(res, wl, B, peaks, precision):
       'fp32': 'fp32 mode runs on the FFMA pipe; the fraction is still quoted against the bf16 '
               'tensor peak the north-star names',
       'fp16x3': 'ALGORITHMIC FLOPs only: the three fp16 MMA chains that emulate fp32 execute 3x '
-                'this many tensor FLOPs (no credit taken); tensor-pipe busy fraction = 3 x frac. '
-                'The kernel runs at the board power limit (see clocks: sw_power_cap, ~1.75 of '
-                '1.965 GHz, ~990 W in a 60-step run: profiles/r02_ab_x3_variants.txt), so the '
-                'fraction is bounded by energy per MMA, not by the issue rate',
+                'this many tensor FLOPs (no credit taken); tensor-pipe busy fraction = 3 x frac',
       'bf16': '',
   }
   r = {
@@ -650,8 +650,7 @@ def roofline(res, wl, B, peaks, precision):
   if precision == 'fp16x3':
     r['tensor_pipe_frac_executed'] = 3 * achieved / peak
     if peaks.get('bf16_tflops_sustained'):
-      # the power-limited tensor rate of the chip (cuBLAS bf16 back to back for 4 s runs at ~1.34 GHz under
-      # the same 1000 W cap) is the bound this kernel actually meets: executed FLOPs / sustained peak
+      # executed FLOPs over the sustained (power-limited) tensor rate of the chip
       r['tensor_pipe_frac_executed_of_sustained'] = 3 * achieved / peaks['bf16_tflops_sustained']
   return r
 
@@ -869,6 +868,8 @@ def run_b200(args):
       dist.destroy_process_group()
     return
   main = measure(precision, wl, B, args, ctx, want_parity=not args.no_parity)
+  if args.dump_outputs and rank == 0:
+    dump_outputs(main['out'], args.dump_outputs)
 
   # End to end through the C ABI's host entry point: host buffers in, host
   # buffers out, H2D + D2H inside the timed region.
@@ -981,6 +982,37 @@ def run_b200(args):
     dist.destroy_process_group()
   if bad:
     sys.exit(3)
+
+
+# --dump-outputs: at most this many bytes in all; a larger array is replaced by a fixed,
+# seeded sample of its rows (same rows from run to run)
+DUMP_LIMIT_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(out, dirname):
+  """Writes the arrays the timed path returned (model.apply's output tree) as
+  DIR/<level>_<key>.npy in float32, so that two builds can be compared output for output."""
+  import numpy as np
+  import torch
+  arrays = {}
+
+  def rec(t, prefix):
+    if isinstance(t, dict):
+      for k in sorted(t):
+        rec(t[k], f'{prefix}_{k}' if prefix else k)
+    elif isinstance(t, torch.Tensor):
+      arrays[prefix] = t.detach().float().cpu().numpy()
+
+  rec(out, '')
+  total = sum(a.nbytes for a in arrays.values())
+  os.makedirs(dirname, exist_ok=True)
+  for name, a in arrays.items():
+    if total > DUMP_LIMIT_BYTES and a.ndim > 0:
+      keep = max(1, int(a.shape[0] * DUMP_LIMIT_BYTES / total))
+      rows = np.sort(np.random.default_rng(0).choice(a.shape[0], size=keep, replace=False))
+      a = a[rows]
+      np.save(os.path.join(dirname, f'{name}_rows.npy'), rows.astype(np.float64))
+    np.save(os.path.join(dirname, f'{name}.npy'), np.ascontiguousarray(a, dtype=np.float32))
 
 
 _SAVED_STDOUT = None

@@ -1,4 +1,4 @@
-/* nerfies_b200.h - C ABI of the B200-native deformable-NeRF render hot path.
+/* nerfies_b200.h - C ABI of the Hopper-native deformable-NeRF render hot path.
  *
  * The reference (google/nerfies) is pure Python/JAX and has no FFI; the seam a
  * replacement plugs into is the Python call surface listed in SURVEY.md §8(b).
@@ -20,7 +20,7 @@
  *  - the tensor-core kernels never hang or trap on an internal protocol error:
  *    a bounded mbarrier wait raises a process-wide abort flag (mapped host
  *    memory), the kernel drains, and the _host entry point / every later call
- *    returns an error ("a tcgen05 kernel aborted ..."); results of that launch
+ *    returns an error ("a tensor-core kernel aborted ..."); results of that launch
  *    are invalid;
  *  - a handle is not thread-safe: one handle per GPU per process/rank.  Its workspace
  *    is shared by its calls: consecutive calls on one stream are ordered by the
@@ -53,8 +53,8 @@ enum nfb_warp_encoder { NFB_WARP_ENC_GLO = 0, NFB_WARP_ENC_TIME = 1, NFB_WARP_EN
 /* Arithmetic of the MLP GEMMs.  Everything else is always fp32. */
 enum nfb_precision {
   NFB_PREC_FP32 = 0,     /* fp32 FFMA on CUDA cores: general (any width / activation / condition) */
-  NFB_PREC_BF16 = 1,     /* bf16 operands, fp32 accumulate, tcgen05 tensor cores: fastest, ~1e-2  */
-  NFB_PREC_FP16X3 = 2    /* fp32 emulated on tcgen05 by three fp16 MMA chains into one fp32
+  NFB_PREC_BF16 = 1,     /* bf16 operands, fp32 accumulate, wgmma tensor cores: fastest, ~1e-2  */
+  NFB_PREC_FP16X3 = 2    /* fp32 emulated on wgmma by three fp16 MMA chains into one fp32
                           * accumulator (x_hi W_hi + x_lo W_hi + x_hi W_lo, hi = fp16(v),
                           * lo = fp16(v - hi): 22 significant bits per operand): the
                           * tensor-core mode that holds the 1e-4 parity gate.  Activations
@@ -287,14 +287,12 @@ int nfb_camera_rays(const nfb_camera* cam, long long first_pixel, long long coun
 int nfb_pixels_to_rays(const nfb_camera* cam, const float* pixels, long long n,
                        float* directions, void* stream);
 
-/* Debug aid: block 0 of the tensor-core field kernel appends (tag, clock64)
- * pairs to `buffer` (device, 1 + 2*capacity int64; buffer[0] = record count,
- * zero it first).  NULL disables tracing.  Only builds compiled with -DNFB_TRACE
- * carry the tracer; others return -1 for a non-NULL buffer. */
+/* Kept for ABI compatibility: this library carries no kernel tracer; a non-NULL
+ * buffer returns -1, NULL returns 0. */
 int nfb_set_trace(nfb_handle* h, long long* buffer, int capacity);
 
 /* Test hook for the abort path described in the conventions above: while enabled,
- * the MMA issuer of the bf16 tcgen05 kernel first waits on an mbarrier that never
+ * the weight producer of the tensor-core kernel first waits on an mbarrier that never
  * completes, so the launch must time out, drain and raise the abort flag
  * (tests/test_edge_cases_gpu.py).  The process cannot run further tensor-core
  * launches afterwards.  No reference analogue. */
@@ -309,32 +307,18 @@ int nfb_debug_provoke_timeout(nfb_handle* h, int enabled);
 int nfb_check_abort(void* stream, int synchronize);
 int nfb_reset_abort(void);
 
-/* Hardware self-test of the tcgen05 building blocks (UMMA descriptors, 128-byte
- * swizzle, TMEM, bulk-copy ring): C[128,N] = bf16(A[128,K]) x bf16(W[K,N]), fp32
- * accumulate.  K <= 320, N <= 256; device pointers. */
+/* Hardware self-test of the wgmma building blocks (GMMA descriptors, 128-byte
+ * swizzle, accumulator fragment layout): C[128,N] = bf16(A[128,K]) x bf16(W[K,N]),
+ * fp32 accumulate.  K <= 320, N <= 256; device pointers. */
 int nfb_selftest_gemm(int K, int N, const float* A, const float* W, float* C,
                       void* stream);
 
-/* Micro-benchmark of the tensor pipe (mode 0: chain of tcgen05.mma M=128,N=n) or
- * of TMEM reads (mode 1: tcgen05.ld by `nwarps` warps).  out (host, 3 int64):
- * cycles, work items, issue cycles. */
-int nfb_selftest_microbench(int mode, int n, int reps, int nwarps, long long* out);
-
-/* CTA-pair (tcgen05 cta_group::2, a 2-CTA cluster) variant of nfb_selftest_gemm:
- * C (256 x N) = bf16(A (256 x K)) x bf16(W (K x N)) times `reps`, N in {64,128,256},
- * K <= 320.  out (host, 2 x int64, nullable): cycles seen by the leader CTA from
- * the first MMA issue to completion, and the number of MMAs (M=256, K=16) issued.
- * Hardware self-test / micro-benchmark for the planned 2-CTA field kernel; no
- * reference analogue. */
-int nfb_selftest_gemm2(int K, int N, const float* A, const float* W, float* C, int reps,
-                       long long* out, void* stream);
-
-/* A-operand-in-TMEM form of tcgen05.mma, as the fp16x3 field kernel uses it:
- * C (128 x N) = A (128 x K) W (K x N) as three fp16 chains (A_hi W_hi + A_lo W_hi +
- * A_hi W_lo, fp32 accumulate), both fp16 images of A written to tensor memory with
- * tcgen05.st, W from shared memory.  K <= 256, N <= 256; `reps` repeats the chains
- * (the result is divided by reps).  out (host, 2 x int64, nullable): cycles from the
- * first issue to completion, number of MMAs.  Hardware self-test; no reference analogue. */
+/* The fp16x3 form of the same: C (128 x N) = A (128 x K) W (K x N) as three fp16
+ * chains (A_hi W_hi + A_lo W_hi + A_hi W_lo, fp32 accumulate), as the fp16x3 field
+ * kernel evaluates a layer.  K <= 320, N <= 256; `reps` repeats the chains (the
+ * result is divided by reps).  out (host, 2 x int64, nullable): cycles of the MMA
+ * phase, number of MMAs per 64 x 16 output block and repetition.  Hardware
+ * self-test; no reference analogue. */
 int nfb_selftest_gemm3(int K, int N, const float* A, const float* W, float* C, int reps,
                        long long* out, void* stream);
 
@@ -342,7 +326,7 @@ int nfb_selftest_gemm3(int K, int N, const float* A, const float* W, float* C, i
 long long nfb_kernel_launches(const nfb_handle* h);
 /* Thread-local description of the last error returned on this thread. */
 const char* nfb_last_error(void);
-/* "nerfies_b200 <version> sm_100a" */
+/* "nerfies_b200 <version> sm_90a" */
 const char* nfb_version(void);
 
 #ifdef __cplusplus

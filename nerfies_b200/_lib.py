@@ -7,7 +7,7 @@ import ctypes
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# NFB_LIB_PATH: developer override used to A/B kernel build variants (tools/build_variant.py).
+# NFB_LIB_PATH: override of the library path (to compare two builds of the kernels).
 LIB_PATH = os.environ.get('NFB_LIB_PATH') or os.path.join(_HERE, 'libnerfies_b200.so')
 
 # Every symbol include/nerfies_b200.h declares (checked by tests/test_abi.py).
@@ -16,8 +16,8 @@ SYMBOLS = [
     'nfb_set_params', 'nfb_render_forward', 'nfb_render_forward_host',
     'nfb_render_samples', 'nfb_sample_pdf', 'nfb_coarse_z_vals',
     'nfb_warp_forward', 'nfb_kernel_launches', 'nfb_last_error', 'nfb_version',
-    'nfb_set_profiling', 'nfb_field_time_ms', 'nfb_selftest_gemm', 'nfb_set_trace', 'nfb_selftest_microbench',
-    'nfb_camera_rays', 'nfb_pixels_to_rays', 'nfb_selftest_gemm2', 'nfb_selftest_gemm3',
+    'nfb_set_profiling', 'nfb_field_time_ms', 'nfb_selftest_gemm', 'nfb_set_trace',
+    'nfb_camera_rays', 'nfb_pixels_to_rays', 'nfb_selftest_gemm3',
     'nfb_debug_provoke_timeout', 'nfb_set_time_alpha', 'nfb_train_value_and_grad', 'nfb_adam_step',
     'nfb_train_value_and_grad_reg', 'nfb_warp_jacobian', 'nfb_check_abort', 'nfb_reset_abort',
 ]
@@ -121,7 +121,7 @@ def load():
   if not os.path.exists(LIB_PATH):
     raise ImportError(
         f'{LIB_PATH} is missing: build it with `python -c "import '
-        '__graft_entry__ as g; g.build()"` (nvcc, sm_100a). nerfies_b200 has '
+        '__graft_entry__ as g; g.build()"` (nvcc, sm_90a). nerfies_b200 has '
         'no CPU or PyTorch fallback.')
   lib = ctypes.CDLL(LIB_PATH)
   vp, ci, cf, cu = ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_uint
@@ -179,15 +179,11 @@ def load():
   lib.nfb_selftest_gemm.restype = ci
   lib.nfb_set_trace.argtypes = [vp, vp, ci]
   lib.nfb_set_trace.restype = ci
-  lib.nfb_selftest_microbench.argtypes = [ci, ci, ci, ci, vp]
-  lib.nfb_selftest_microbench.restype = ci
   ll = ctypes.c_longlong
   lib.nfb_camera_rays.argtypes = [ctypes.POINTER(NfbCamera), ll, ll, vp, vp, vp, vp]
   lib.nfb_camera_rays.restype = ci
   lib.nfb_pixels_to_rays.argtypes = [ctypes.POINTER(NfbCamera), vp, ll, vp, vp]
   lib.nfb_pixels_to_rays.restype = ci
-  lib.nfb_selftest_gemm2.argtypes = [ci, ci, vp, vp, vp, ci, vp, vp]
-  lib.nfb_selftest_gemm2.restype = ci
   lib.nfb_selftest_gemm3.argtypes = [ci, ci, vp, vp, vp, ci, vp, vp]
   lib.nfb_selftest_gemm3.restype = ci
   lib.nfb_debug_provoke_timeout.argtypes = [vp, ci]

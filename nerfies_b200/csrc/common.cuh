@@ -1,4 +1,4 @@
-// Shared definitions for the nerfies_b200 render kernels (sm_100a only).
+// Shared definitions for the nerfies_b200 render kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

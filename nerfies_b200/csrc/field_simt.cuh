@@ -47,15 +47,13 @@ struct FieldArgs {
   int warp_only;             // stop after the warp (nfb_warp_forward)
   int fast_encode;           // bf16 mode: octave-recurrence positional encoding
   int debug;                 // NFB_DEBUG bits (timing experiments, results are garbage): 1 = hidden-layer epilogues skip
-                             // TMEM loads, math and stores; 2 / 4 (-DNFB_EPI_DEBUG builds) = skip only the activation stores / only loads + math;
+                             // accumulator reads, math and stores; 2 / 4 (-DNFB_EPI_DEBUG builds) = skip only the activation stores / only loads + math;
                              // 8 = the MMA issuer first waits on a barrier that never completes (abort-path test)
   // fp16x3 kernel: volumetric rendering fused into the rgb epilogue (samples_per_ray a multiple
   // of 128): per-ray (rgb3, depth, med_depth, acc) and, optionally, the weights.
   float* ray_out;            // (B,6) or nullptr = no fused composite
   float* ray_weights;        // (B,S) or nullptr
   int white_bg, sample_at_infinity;
-  long long* trace;          // debug: (tag, clock) records of block 0, or nullptr
-  int trace_cap;
 };
 
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {

@@ -1,111 +1,23 @@
-// Fused per-sample field evaluation on the 5th-gen tensor cores
-// (NFB_PREC_BF16): bf16 operands, fp32 accumulation in TMEM.
-//
-// One persistent CTA per SM walks over "tile pairs" of 2 x 128 consecutive
-// (ray, sample) rows.  Every Dense layer of the warp MLP and the NeRF MLP is a
-// chain of tcgen05.mma (M=128 per sub-tile, K=16 each) whose
-//   A operand = the sub-tile's activations, bf16, in shared memory in the UMMA
-//               K-major 128B-swizzle format, written in place by the epilogue;
-//   B operand = pre-swizzled bf16 weight units streamed from L2 by
-//               cp.async.bulk through a 4-stage mbarrier ring, each unit used by
-//               both sub-tiles (256 rows per weight byte fetched);
-//   D         = fp32 accumulators in TMEM (2 sub-tiles x 256 columns).
-// Warp roles (3 warpgroups, 384 threads): warps 0-7 epilogue (one thread per row:
-// tcgen05.ld -> add.f32x2 bias from the constant bank -> cvt.relu.bf16x2 ->
-// swizzled st.shared; also the SE(3) exp-map, the positional encodings and the
-// final sigmoid/softplus), warp 8 lane 0 issues the MMAs, warp 9 lane 0 the weight
-// copies, warps 10-11 only complete the control warpgroup.  setmaxnreg gives the
-// epilogue warpgroups 232 registers per thread and leaves the control group 40.
-// The N dimension of a layer is issued in two chunks so that the epilogue of
-// chunk 0 overlaps the MMAs of chunk 1 and the next layer's first K-blocks
-// overlap the epilogue of chunk 1.
-// Activations never leave the SM; per sample 16 B (r,g,b,sigma) go to HBM.
+// Fused per-sample field evaluation on the Hopper tensor cores (wgmma) for the two
+// tensor-core precisions: bf16 (NFB_PREC_BF16: bf16 operands, fp32 accumulation) and
+// fp16x3 (NFB_PREC_FP16X3: three fp16 chains per layer, see field_tc3.cuh).  Every Dense
+// layer of the warp MLP and the NeRF MLP is a chain of wgmma over 64-column K-blocks:
+//   A = the tile's activations (or the encoded-input block) in shared memory, in the
+//       GMMA K-major 128B-swizzle format, written in place by the epilogue;
+//   B = pre-swizzled weight units streamed from L2 by cp.async.bulk through an
+//       mbarrier ring, each unit used by both consumer warpgroups;
+//   D = fp32 accumulators in registers.
+// Activations never leave the SM; per sample 16 B (r,g,b,sigma) go to HBM, or with the
+// fused composite 24 B per ray.
 #pragma once
 #include "field_simt.cuh"   // FieldArgs
+#include "field_tc3.cuh"
 #include "nfb_handle.h"
 #include "tc_common.cuh"
 #include "tc_program.cuh"
 
 namespace nfb {
 namespace tc {
-
-constexpr int kStages = 4;
-constexpr int kStageBytes = 16384;              // 128 rows x 128 B
-constexpr int kTcThreads = 384;                 // 8 epilogue warps + control warpgroup (issuer, producer, 2 idle)
-constexpr int kTcThreads16 = 640;               // 16 epilogue warps + control warpgroup
-constexpr int kDefaultEpiWarps = 8;
-constexpr int kXBytes = 2 * 4 * kABlockBytes;   // 2 sub-tiles x 4 K-blocks
-constexpr int kInBytes = 2 * kABlockBytes;
-// No alignment slack: the dynamic shared-memory window of a kernel without static
-// shared memory starts 1024-byte aligned (checked at run time, trap otherwise).
-constexpr int kAlphaBytes = 256 * 2;              // alpha-head weights, bf16
-constexpr int kTcSmemBytes = kXBytes + kInBytes + kStages * kStageBytes + kAlphaBytes + 128;
-constexpr int kPairRows = 2 * kTileRows;
-// Epilogue variants (A/B builds): software-pipelined TMEM loads of 128-column chunks.
-#ifdef NFB_PIPE_E0
-constexpr bool kPipeE0 = true;
-#else
-constexpr bool kPipeE0 = false;
-#endif
-#ifdef NFB_NO_PIPE_E1
-constexpr bool kPipeE1 = false;
-#else
-constexpr bool kPipeE1 = true;
-#endif
-
-struct TcBars {
-  uint64_t full[kStages];
-  uint64_t empty[kStages];
-  uint64_t acc_ready[2];
-  uint64_t x_free;
-  uint64_t x_ready[3];     // [0] chunk-0 epilogue done; [1]/[2] first/second half of chunk 1's
-  uint64_t never;          // never completes: NFB_DEBUG bit 8 waits on it to exercise the abort path
-  uint32_t tmem_slot;
-};
-static_assert(sizeof(TcBars) <= 128, "barrier block");
-
-// Debug timeline of block 0 (-DNFB_TRACE builds, tools/trace_tc.py): four roles (0 MMA issuer, 1/2 epilogue of sub-tile
-// 0/1 (first lane), 3 weight producer) append (tag, clock64) pairs to private
-// regions of `trace` with plain stores; trace[role] receives the record count.
-#ifdef NFB_TRACE
-struct Tracer {
-  long long* base;
-  int cap, n;
-  __device__ Tracer(const FieldArgs& a, int role) : base(nullptr), cap(0), n(0) {
-    if (a.trace && blockIdx.x == 0 && role >= 0) {
-      cap = a.trace_cap / 4;
-      base = a.trace + 4 + (size_t)role * cap * 2;
-    }
-  }
-  __device__ __forceinline__ void ev(int step, int e) {
-    if (base && n < cap) {
-      base[2 * n] = ((long long)step << 8) | e;
-      base[2 * n + 1] = clock64();
-      ++n;
-    }
-  }
-  __device__ void finish(const FieldArgs& a, int role) {
-    if (base) a.trace[role] = n;
-  }
-};
-#else
-// Production builds carry no tracer: its state would live in local memory (it is
-// captured by the epilogue lambdas) and be touched on every barrier hand-off.
-struct Tracer {
-  __device__ Tracer(const FieldArgs&, int) {}
-  __device__ __forceinline__ void ev(int, int) {}
-  __device__ __forceinline__ void finish(const FieldArgs&, int) {}
-};
-#endif
-
-// Row state owned by one epilogue thread for the lifetime of a tile pair.
-struct RowState {
-  float x[3];        // current (possibly warped) sample point
-  long long m;       // global row (clamped to a valid row)
-  long long ray;
-  bool valid;
-  float alpha;       // running alpha-head dot product
-};
 
 // [x | w_k * sin/cos features | extra | 0...] -> one 64-column K-block row.
 __device__ __forceinline__ void posenc_to_block(uint8_t* block, int r, const float* x, int F,
@@ -176,70 +88,6 @@ __device__ __forceinline__ void posenc_fast_to_block(uint8_t* block, int r, cons
   for (int c = 0; c < 8; ++c)
     if (c >= c_begin && c < c_end) store_chunk(block, r, c, feat + c * 8);
 }
-
-// One 32-column piece of a hidden layer's epilogue: + bias (packed add.f32x2),
-// (alpha head dot), round to bf16 with the ReLU folded into the conversion
-// (cvt.rn.relu.bf16x2.f32; rounding is monotone and keeps zero, so
-// relu-then-round == round-then-relu).
-__device__ __forceinline__ uint64_t pack_f32x2(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-// NFB_TC_BIAS_LDG (A/B build): the step's biases through L1 (ld.global.nc from the aux buffer) instead of
-// the kernel-parameter constant bank (24 KB of biases do not fit the constant cache: indexed LDCs miss).
-#ifdef NFB_TC_BIAS_LDG
-constexpr bool kTcBiasLdg = true;
-#else
-constexpr bool kTcBiasLdg = false;
-#endif
-__device__ __forceinline__ float4 tc_ld_bias(const float4* p, int i) {
-  if (kTcBiasLdg) return __ldg(p + i);
-  return p[i];
-}
-__device__ __forceinline__ void epi_piece(const float* v, const float4* __restrict__ bq4,
-                                          bool relu, bool adot,
-                                          const __nv_bfloat16* __restrict__ alpha_w32, float& alpha,
-                                          uint32_t* out16) {
-  float t[32];
-#pragma unroll
-  for (int j = 0; j < 32; j += 4) {
-    const float4 bq = tc_ld_bias(bq4, j >> 2);                  // warp-uniform address
-#ifdef NFB_NO_F32X2
-    t[j] = v[j] + bq.x; t[j + 1] = v[j + 1] + bq.y; t[j + 2] = v[j + 2] + bq.z; t[j + 3] = v[j + 3] + bq.w;
-#else
-    uint64_t r0, r1;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r0) : "l"(pack_f32x2(v[j], v[j + 1])), "l"(pack_f32x2(bq.x, bq.y)));
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r1) : "l"(pack_f32x2(v[j + 2], v[j + 3])), "l"(pack_f32x2(bq.z, bq.w)));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(t[j]), "=f"(t[j + 1]) : "l"(r0));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(t[j + 2]), "=f"(t[j + 3]) : "l"(r1));
-#endif
-  }
-  if (adot) {
-#pragma unroll
-    for (int j = 0; j < 32; j += 8) {
-      // shared memory, broadcast: 8 bf16 weights per 128-bit load
-      const uint4 wq = *reinterpret_cast<const uint4*>(alpha_w32 + j);
-      const uint32_t w[4] = {wq.x, wq.y, wq.z, wq.w};
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float2 wf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[q]));
-        alpha = fmaf(fmaxf(t[j + 2 * q], 0.f), wf.x, alpha);
-        alpha = fmaf(fmaxf(t[j + 2 * q + 1], 0.f), wf.y, alpha);
-      }
-    }
-  }
-  if (relu) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j)
-      asm("cvt.rn.relu.bf16x2.f32 %0, %1, %2;" : "=r"(out16[j]) : "f"(t[2 * j + 1]), "f"(t[2 * j]));
-  } else {
-#pragma unroll
-    for (int j = 0; j < 16; ++j)
-      asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(out16[j]) : "f"(t[2 * j + 1]), "f"(t[2 * j]));
-  }
-}
-
 __device__ __forceinline__ void cond_to_block(uint8_t* block, int r, const float* __restrict__ cond,
                                               int n, int c_begin = 0, int c_end = 8) {
 #pragma unroll 1
@@ -254,73 +102,142 @@ __device__ __forceinline__ void cond_to_block(uint8_t* block, int r, const float
   }
 }
 
-// kH = epilogue threads per row: 1 (8 epilogue warps) or 2 (16 warps; the two
-// threads of a row are in warps w and w+4 - same TMEM lane quarter - and split
-// every chunk's columns; the per-row scalar work is done redundantly by both).
-// kPair: the CTA-pair variant (cluster of 2, tcgen05 cta_group::2).  Every CTA
-// still owns two 128-row sub-tiles, its activations, its TMEM and its epilogue
-// warps; an MMA is M = 256 across the two CTAs' sub-tiles and each CTA stages only
-// its half (chunk_n / 2 rows) of every weight unit.  Only the leader CTA (cluster
-// rank 0) issues MMAs; every commit is multicast to both CTAs' barriers.  The
-// leader's issuer also needs the follower's "weights landed" and "activations
-// ready" events: the follower's otherwise idle issuer warp walks the same unit
-// table, waits on its local barriers and forwards each event with one remote
-// mbarrier arrive (the leader's full / x_ready barriers count one extra arrival).
-// kPairMode 1 (NFB_TC_PAIR=1): as described - validated bit-identical on the GPU.
-// kPairMode 2 (NFB_TC_PAIR=2; checked bit-identical once, tools/check_pair_mode.py,
-// not yet tuned or measured on the bench workload): the "activations ready" events skip the relay hop - the epilogue
-// threads of BOTH CTAs arrive on the leader's x_ready barriers directly (remote
-// release arrive; count 2 x kEpiThreads) - and the relay warp forwards only the
-// "weights landed" events, with a relaxed remote arrive (no data passed through
-// the relaying thread), so it is never blocked behind an activation wait.
-template <int kH, int kPairMode = 0>
-__global__ void __launch_bounds__(32 * (8 * kH + 4), 1)
-field_tc_kernel(const __grid_constant__ TcProgram prog, const __grid_constant__ TcBias biasp,
-                const FieldArgs args, const uint8_t* __restrict__ wpack,
-                const float* __restrict__ aux, int num_pairs) {
-  constexpr int kEpiWarps = 8 * kH, kMmaWarp = kEpiWarps, kProdWarp = kEpiWarps + 1;
-  constexpr int kEpiThreads = 256 * kH;
-  extern __shared__ __align__(1024) uint8_t raw[];
-  uint8_t* base = raw;
+// One 128-column accumulator chunk of a hidden layer (this thread's fragment: rows
+// arow, arow + 8; columns c*128 + 8j + 2*lq + {0, 1}) -> + bias, activation, (alpha
+// head dot product in fp32) -> the activation image of the next layer, in place.
+// `inv_s` undoes the fp16x3 power-of-two weight scale (x3_weight_scale; 1 in bf16
+// mode): acc * inv_s is exact, so fma(acc, inv_s, bias) rounds like acc + bias.
+// fp16x3 split: hi = v with the fp32 mantissa truncated to fp16's 11 significant bits
+// (the conversion is then exact), lo = fp16(v - hi) (exact subtraction):
+// v - (hi + lo) <= 2^-23 |v|, the bound of a round-to-nearest split.  ReLU rides on the
+// conversions: for v < 0 both hi and v - hi are <= 0 and convert to +0.  Conversions
+// saturate: |v| > 65504 does not become inf.
+template <bool kX3>
+__device__ __forceinline__ void epi_chunk(const float* acc, int c, const float* __restrict__ bias, float inv_s,
+                                          bool relu, bool adot, const float* __restrict__ aw, float& al0,
+                                          float& al1, uint8_t* act_hi, uint8_t* act_lo, int arow, int lq) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int col = c * 128 + 8 * j + 2 * lq;
+    const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col));
+    float v[4] = {fmaf(acc[4 * j], inv_s, b.x), fmaf(acc[4 * j + 1], inv_s, b.y),
+                  fmaf(acc[4 * j + 2], inv_s, b.x), fmaf(acc[4 * j + 3], inv_s, b.y)};
+    if (adot) {
+      // bf16 mode: bf16-rounded alpha weights, fp32 activations and accumulation
+      float2 w = __ldg(reinterpret_cast<const float2*>(aw + col));
+      if constexpr (!kX3) w = __bfloat1622float2(__floats2bfloat162_rn(w.x, w.y));
+      al0 = fmaf(relu ? fmaxf(v[0], 0.f) : v[0], w.x, al0);
+      al0 = fmaf(relu ? fmaxf(v[1], 0.f) : v[1], w.y, al0);
+      al1 = fmaf(relu ? fmaxf(v[2], 0.f) : v[2], w.x, al1);
+      al1 = fmaf(relu ? fmaxf(v[3], 0.f) : v[3], w.y, al1);
+    }
+    const uint32_t blk = (uint32_t)(2 * c + (j >> 3)) * kABlockBytes + 4 * lq;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t off = blk + swz_off(arow + 8 * h, j & 7);
+      const float a = v[2 * h], bb = v[2 * h + 1];
+      uint32_t hi, lo;
+      if constexpr (kX3) {
+        const float ta = __uint_as_float(__float_as_uint(a) & 0xFFFFE000u);
+        const float tb = __uint_as_float(__float_as_uint(bb) & 0xFFFFE000u);
+        const float da = a - ta, db = bb - tb;
+        if (relu) {
+          asm("cvt.rn.relu.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(tb), "f"(ta));
+          asm("cvt.rn.relu.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(db), "f"(da));
+        } else {
+          asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(tb), "f"(ta));
+          asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(db), "f"(da));
+        }
+        *reinterpret_cast<uint32_t*>(act_lo + off) = lo;
+      } else {
+        if (relu) asm("cvt.rn.relu.bf16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(bb), "f"(a));
+        else asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(bb), "f"(a));
+      }
+      *reinterpret_cast<uint32_t*>(act_hi + off) = hi;
+    }
+  }
+}
+
+// Per-ray part of the alpha head with an alpha condition: cond . w (bf16 mode: bf16-rounded weights).
+// Out of line: it runs once per row and tile, and inlined it costs the hot loop registers.
+template <bool kX3>
+__device__ __noinline__ float alpha_cond_dot(const float* __restrict__ cond, const float* __restrict__ w, int n) {
+  float a = 0.f;
+  for (int j = 0; j < n; ++j) {
+    float wj = __ldg(w + j);
+    if constexpr (!kX3) wj = __bfloat162float(__float2bfloat16_rn(wj));
+    a = fmaf(__ldg(cond + j), wj, a);
+  }
+  return a;
+}
+
+// Row state owned by the two row threads of a row for the lifetime of a tile.
+struct RowState {
+  float x[3];        // current (possibly warped) sample point
+  long long m;       // global row (clamped to a valid row)
+  long long ray;
+  bool valid;
+  float z, dist;     // fused composite: z of the sample, (z_next - z) * |d| (or the last-sample constant)
+  bool last;         // last sample of its ray
+};
+
+// Fused per-sample field evaluation on the Hopper tensor cores (wgmma), one kernel for
+// both tensor-core precisions (kX3: fp16x3, else bf16).
+//
+// Persistent, one CTA per SM, 384 threads, one 128-row tile at a time:
+//   warpgroup 0     : warp 0 streams the weight units (one cp.async.bulk per unit into a
+//                     ring of mbarrier-guarded slots: 2 x 32 KB fp16x3 [W_hi | W_lo], 4 x 16 KB
+//                     bf16); the other warps idle (setmaxnreg 40 / 232).
+//   warpgroups 1, 2 : rows 0-63 / 64-127.  Each issues its own wgmma (M = 64, N = 128 per
+//                     chunk, fp32 accumulators in registers: a 256-wide layer is 128 of them
+//                     per thread), A = its rows of the activation image in shared memory,
+//                     B = the weight slot shared by both.  A layer's epilogue writes the
+//                     next layer's activation image in place once the warpgroup's MMAs of
+//                     the layer are complete, so no second image is needed.
+// Shared memory (225 KB): activation image 4 K-blocks x (hi | lo) = 128 KB | input block
+// (the encoded points / conditions) hi | lo = 32 KB | weight ring 64 KB | alpha partials |
+// composite scratch | barriers.  (bf16 mode leaves the lo images unused.)
+// Per-row work (positional encodings, SE(3) exp-map, sigmoid / sigma activation, fused
+// volumetric rendering) is done by "row threads": two per row (hs = which half of the
+// input block's columns), thread t of warpgroup w owns row 64 (w - 1) + (t & 63).
+// Head layers (N = 16) leave their accumulators in a per-warpgroup scratch inside
+// activation block 0 (free at that point: the step after a head reads the input block only).
+constexpr int kWgThreads = 384;
+constexpr int kActLoOff = 4 * kABlockBytes;
+constexpr int kInOff = 8 * kABlockBytes;
+constexpr int kRingOff = 10 * kABlockBytes;
+constexpr int kRingBytes = 4 * kABlockBytes;
+constexpr int kAlphaOff = kRingOff + kRingBytes;      // per-row alpha-head partial (128 floats)
+constexpr int kScanOff = kAlphaOff + 512;             // fused composite: cross-warp partials (40 floats)
+constexpr int kBarOff = kScanOff + 256;
+constexpr int kWgSmemBytes = kBarOff + 256;
+static_assert(kWgSmemBytes <= 232448, "shared memory");
+
+struct WgBars {
+  uint64_t full[4];
+  uint64_t empty[4];       // 8 arrivals: every consumer warp, after its wgmma reading the slot completed
+  uint64_t never;          // never completes: the abort-path test hook waits on it
+};
+
+template <bool kX3>
+__global__ void __launch_bounds__(kWgThreads, 1)
+field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, const uint8_t* __restrict__ wpack,
+                const float* __restrict__ aux, int num_tiles) {
+  constexpr int kSlots = kX3 ? 2 : 4, kSlotBytes = kRingBytes / kSlots;
+  extern __shared__ __align__(1024) uint8_t base[];
   if ((smem_u32(base) & 1023u) != 0) {
     if (threadIdx.x == 0) printf("nfb: dynamic shared memory is not 1024-byte aligned\n");
     __trap();
   }
-  uint8_t* xbuf = base;                       // [2][4][16 KB]
-  uint8_t* inbuf = xbuf + kXBytes;            // [2][16 KB]
-  uint8_t* stages = inbuf + kInBytes;         // [kStages][16 KB]
-  __nv_bfloat16* alpha_s = reinterpret_cast<__nv_bfloat16*>(stages + kStages * kStageBytes);
-  TcBars* bars = reinterpret_cast<TcBars*>(reinterpret_cast<uint8_t*>(alpha_s) + kAlphaBytes);
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  constexpr bool kPair = kPairMode != 0;
-  constexpr bool kDirectX = kPairMode == 2;                  // epilogues arrive on the leader's x_ready directly
-  const uint32_t rank = kPair ? cluster_ctarank() : 0u;      // 0 = leader (issues the MMAs)
-  const bool leader = rank == 0;
-  if (tid == kMmaWarp * 32) {
-    const uint32_t relay = (kPair && leader) ? 1u : 0u;       // + the follower's forwarded arrival
-    for (int i = 0; i < kStages; ++i) { mbar_init(&bars->full[i], 1 + relay); mbar_init(&bars->empty[i], 1); }
-    mbar_init(&bars->acc_ready[0], 1); mbar_init(&bars->acc_ready[1], 1);
-    mbar_init(&bars->x_free, 1);
-    for (int k = 0; k < 3; ++k)
-      mbar_init(&bars->x_ready[k], (kDirectX && leader) ? 2 * kEpiThreads : kEpiThreads + relay);
+  WgBars* bars = reinterpret_cast<WgBars*>(base + kBarOff);
+  const int tid = threadIdx.x, wg = tid >> 7, warp = tid >> 5, lane = tid & 31;
+  if (tid == 0) {
+    for (int i = 0; i < kSlots; ++i) { mbar_init(&bars->full[i], 1); mbar_init(&bars->empty[i], 8); }
     mbar_init(&bars->never, 1);
     fence_barrier_init();
   }
-  if (warp == kMmaWarp) {
-    if constexpr (kPair) tmem_alloc2(&bars->tmem_slot, 512);
-    else tmem_alloc(&bars->tmem_slot, 512);
-  }
-  tc_fence_before();
-  if constexpr (kPair) cluster_sync_all();   // the peer's barriers are initialised before any remote arrival
-  else __syncthreads();
-  tc_fence_after();
-  // The follower's pair index is the leader's + 1: both CTAs run the same number of
-  // iterations (rows beyond the end are clamped and never stored).
-  const int pair_lim = num_pairs + (int)rank;
-  const uint32_t tmem_base = bars->tmem_slot;
+  __syncthreads();
   const bool do_warp = args.use_warp && prog.warp_type != 0;
-  // Steps executed per tile pair: the warp net's steps come first in the list.
   int first_step = 0;
   if (!do_warp) {
     while (first_step < prog.n_steps && prog.steps[first_step].epi != kEpiWarpHeads) ++first_step;
@@ -331,433 +248,191 @@ field_tc_kernel(const __grid_constant__ TcProgram prog, const __grid_constant__ 
     last_step = 0;
     while (prog.steps[last_step].epi != kEpiWarpHeads) ++last_step;
   }
+  // Tiles of this CTA: blockIdx.x, + gridDim.x, ...  With the fused composite a CTA takes whole
+  // rays - the S / 128 tiles of a ray back to back - so that transmittance and the partial sums
+  // are carried in registers from tile to tile.
+  const bool fuse = args.ray_out != nullptr && !args.warp_only;
+  const int tpr = fuse ? args.samples_per_ray / kTileRows : 1;          // tiles per group
+  const int groups = num_tiles / tpr;
+  const int bid = (int)blockIdx.x;
+  const int my_groups = bid < groups ? (groups - bid + (int)gridDim.x - 1) / (int)gridDim.x : 0;
+  const int n_my = my_groups * tpr;
+  auto tile_of = [&](int i) { return (bid + (i / tpr) * (int)gridDim.x) * tpr + (i % tpr); };
 
-  // Register split (setmaxnreg works per warpgroup): the control warpgroup (issuer,
-  // producer, two idle warps) keeps kCtlRegs, the epilogue warpgroups grow to
-  // kEpiRegs - enough to keep a whole 128-column chunk of TMEM loads in flight.
-#ifndef NFB_CTL_REGS
-#define NFB_CTL_REGS 40
-#define NFB_EPI_REGS 232   // 128 x 40 + 256 x 232 = 384 x 168
-#endif
-  constexpr int kCtlRegs = kH == 1 ? NFB_CTL_REGS : 40, kEpiRegs = kH == 1 ? NFB_EPI_REGS : 104;
-  // (each role branch executes its own setmaxnreg so that ptxas sees the budget of
-  // the region it dominates)
-  if (warp == kProdWarp) {
+  if (wg == 0) {
     // ===================== weight producer =====================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kCtlRegs));
-    // (the whole warp runs the loop; one elected lane issues the copies)
-    {
-      Tracer tr(args, lane == 0 ? 3 : -1);
-      uint32_t it = 0, dead = 0;                       // dead: see mbar_wait()
-      for (int pair = blockIdx.x; pair < pair_lim; pair += gridDim.x) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(40));
+    if (warp == 0) {
+      uint32_t sg = 0, ph = 0, dead = 0;
+      if (args.debug & 8) mbar_wait(&bars->never, 0, dead);   // test hook: provoke a wait time-out
+      uint8_t* ring = base + kRingOff;
+      for (int ti = 0; ti < n_my; ++ti) {
         for (int si = first_step; si <= last_step; ++si) {
           const TcStep& st = prog.steps[si];
-          const uint32_t unit_bytes = (uint32_t)st.chunk_n * kRowBytes;
-          // CTA pair: this CTA's half of every unit (rows rank*chunk_n/2 ..)
-          const uint32_t bytes = kPair ? unit_bytes / 2 : unit_bytes;
-          const uint8_t* src = wpack + st.w_off + (kPair ? rank * bytes : 0u);
-          for (int u = 0; u < st.n_chunks * st.nkb; ++u, ++it) {
-            const int sg = it % kStages;
-            const uint32_t ph = (it / kStages) & 1;
+          const uint32_t bytes = (kX3 ? 2u : 1u) * (uint32_t)st.chunk_n * kRowBytes;
+          const uint8_t* src = wpack + st.w_off;
+          const int n = st.n_chunks * st.nkb;
+          for (int u = 0; u < n; ++u) {
             mbar_wait(&bars->empty[sg], ph ^ 1, dead);
-            tr.ev(si, u);
-            if (elect_one()) {
+            if (!dead && elect_one()) {
               mbar_arrive_expect_tx(&bars->full[sg], bytes);
-              bulk_g2s(stages + sg * kStageBytes, src + (size_t)u * unit_bytes, bytes, &bars->full[sg]);
+              bulk_g2s(ring + sg * kSlotBytes, src + (size_t)u * bytes, bytes, &bars->full[sg]);
             }
             __syncwarp();
+            if (++sg == kSlots) { sg = 0; ph ^= 1; }
           }
         }
       }
-      if (lane == 0) tr.finish(args, 3);
     }
-  } else if (kPair && warp == kMmaWarp && !leader) {
-    // ===================== follower CTA: event relay =====================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kCtlRegs));
-    if (elect_one()) {
-      const int u_begin = prog.unit_begin[first_step], u_end = prog.unit_begin[last_step + 1];
-      uint32_t sg = 0, wph = 0, xr = 0, dead = 0;
-      for (int pair = blockIdx.x; pair < pair_lim; pair += gridDim.x) {
-        for (int u = u_begin; u < u_end; ++u) {
-          const uint32_t flags = prog.units[u].flags;
-          if constexpr (!kDirectX) {
-            // in the order the leader's issuer consumes them
-            if (flags & kUWaitX0) { mbar_wait(&bars->x_ready[0], xr & 1, dead); mbar_arrive_remote(&bars->x_ready[0], 0); }
-            if (flags & kUWaitX1) { mbar_wait(&bars->x_ready[1], xr & 1, dead); mbar_arrive_remote(&bars->x_ready[1], 0); }
-            if (flags & kUWaitX2) { mbar_wait(&bars->x_ready[2], xr & 1, dead); mbar_arrive_remote(&bars->x_ready[2], 0); }
-            mbar_wait(&bars->full[sg], wph, dead);
-            mbar_arrive_remote(&bars->full[sg], 0);
-          } else {
-            mbar_wait(&bars->full[sg], wph, dead);
-            mbar_arrive_remote_relaxed(&bars->full[sg], 0);
-          }
-          sg = (sg + 1) & (kStages - 1);
-          wph ^= (sg == 0 ? 1u : 0u);
-          xr += (flags & kUStepEnd) ? 1u : 0u;
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == kMmaWarp) {
-    // ===================== MMA issuer =====================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kCtlRegs));
-    // One elected lane walks the flattened, host-precomputed schedule (TcUnit).
-    // Per unit: issue_half0() (fence + the 4 MMAs of sub-tile 0), then the table
-    // fetch and next-operand arithmetic in the shadow of those MMAs, then
-    // issue_half1() (look-ahead probes of the next unit's barriers, the 4 MMAs of
-    // sub-tile 1, the stage-release commit and the optional accumulator / x_free
-    // commits).  A single thread runs alone here: every dependent instruction on
-    // this path is ~5 idle cycles of the tensor pipe, so there are no function calls
-    // and the slow path (a barrier that is not ready yet) is out of line.
-    if (elect_one()) {
-      Tracer tr(args, 0);
-      const uint64_t desc_hi = make_smem_desc(0) & 0xFFFFFFFF00000000ull;   // SBO/version/layout
-      const uint32_t lo_base = ((smem_u32(xbuf) & 0x3FFFFu) >> 4) | (1u << 16);   // + LBO field
-      const uint32_t st_lo = ((smem_u32(stages) & 0x3FFFFu) >> 4) | (1u << 16);
-      const uint32_t b_full = smem_u32(&bars->full[0]), b_empty = smem_u32(&bars->empty[0]);
-      const uint32_t b_acc0 = smem_u32(&bars->acc_ready[0]), b_acc1 = smem_u32(&bars->acc_ready[1]);
-      const uint32_t b_xfree = smem_u32(&bars->x_free);
-      const uint32_t b_x0 = smem_u32(&bars->x_ready[0]), b_x1 = smem_u32(&bars->x_ready[1]);
-      const uint32_t b_x2 = smem_u32(&bars->x_ready[2]);
-      const int u_begin = prog.unit_begin[first_step], u_end = prog.unit_begin[last_step + 1];
-      const int n_u = u_end - u_begin;
-      const uint4* utab = reinterpret_cast<const uint4*>(prog.units);   // 2 x uint4 per unit
-      uint32_t sg = 0, wph = 0, xr = 0, ready = 0, dead = 0;
-      if (args.debug & 8) mbar_wait(&bars->never, 0, dead);   // test hook: provoke a wait time-out
-      // entries are fetched TWO units ahead (constant bank, dynamic index)
-      uint4 c0 = utab[2 * u_begin], c1 = utab[2 * u_begin + 1];
-      int un = u_begin + (1 % n_u);
-      uint4 n0 = utab[2 * un], n1 = utab[2 * un + 1];
-      // operands of the unit about to issue (computed one unit ahead, in the
-      // bookkeeping window between the two issue blocks)
-      uint32_t d0 = tmem_base + c0.z;
-      uint64_t bd = desc_hi | (uint64_t)st_lo;
-      uint64_t ad0 = desc_hi | (uint64_t)(lo_base + c0.x);
-      // cta_group::2: M = 256 in the instruction descriptor (bits 24..28 hold M >> 4)
-      constexpr uint32_t kIdescPair = kPair ? (8u << 24) : 0u;
-      for (int pair = blockIdx.x; pair < pair_lim; pair += gridDim.x) {
-        for (int u = u_begin; u < u_end; ++u) {
-          const uint32_t flags = c1.x, need = c1.y;
-          if ((ready & need) != need) {                    // slow path: something is not there yet
-            if ((need & 2) && !(ready & 2)) mbar_wait_issuer(&bars->x_ready[0], xr & 1, dead);
-            if ((need & 4) && !(ready & 4)) mbar_wait_issuer(&bars->x_ready[1], xr & 1, dead);
-            if ((need & 8) && !(ready & 8)) mbar_wait_issuer(&bars->x_ready[2], xr & 1, dead);
-            if (!(ready & 1)) mbar_wait_issuer(&bars->full[sg], wph, dead);
-          }
-          if constexpr (kPair) issue_half0_pair(d0, ad0, bd, c0.w + kIdescPair, flags & kUAccum);
-          else issue_half0(d0, ad0, bd, c0.w, flags & kUAccum);
-          // ---- bookkeeping while sub-tile 0's MMAs execute ----
-          if (++un >= u_end) un -= n_u;
-          const uint4 f0 = utab[2 * un], f1 = utab[2 * un + 1];     // table entry two units ahead
-          const uint32_t nsg = (sg + 1) & (kStages - 1);
-          const uint32_t nwph = wph ^ (nsg == 0 ? 1u : 0u);
-          const uint32_t nxr = xr + ((flags & kUStepEnd) ? 1u : 0u);
-          const uint64_t ad1 = desc_hi | (uint64_t)(lo_base + c0.y);
-          const uint32_t px0 = (c1.z & 2) ? b_x0 : 0u, px1 = (c1.z & 4) ? b_x1 : 0u;
-          const uint32_t px2 = (c1.z & 8) ? b_x2 : 0u;
-          const uint32_t d1 = d0 + 256, idesc = c0.w + kIdescPair, bar_e = b_empty + sg * 8;
-          const uint64_t bd_cur = bd;
-          // next unit's first-half operands
-          d0 = tmem_base + n0.z;
-          bd = desc_hi | (uint64_t)(st_lo + nsg * (kStageBytes >> 4));
-          ad0 = desc_hi | (uint64_t)(lo_base + n0.x);
-          if constexpr (kPair) {
-            ready = issue_half1_pair(d1, ad1, bd_cur, idesc, flags & kUAccum, bar_e,
-                                     (flags & kUCommitXFree) ? b_xfree : 0u,
-                                     (flags & kUCommitAcc0) ? b_acc0 : ((flags & kUCommitAcc1) ? b_acc1 : 0u),
-                                     b_full + nsg * 8, nwph, px0, px1, px2, nxr & 1);
-          } else if (flags & (kUCommitXFree | kUCommitAcc0 | kUCommitAcc1)) {
-            ready = issue_half1<true>(d1, ad1, bd_cur, idesc, flags & kUAccum, bar_e,
-                                      (flags & kUCommitXFree) ? b_xfree : 0u,
-                                      (flags & kUCommitAcc0) ? b_acc0 : ((flags & kUCommitAcc1) ? b_acc1 : 0u),
-                                      b_full + nsg * 8, nwph, px0, px1, px2, nxr & 1);
-            if (flags & (kUCommitAcc0 | kUCommitAcc1)) tr.ev(c1.w, (flags & kUCommitAcc0) ? 1 : 2);
-          } else {
-            ready = issue_half1<false>(d1, ad1, bd_cur, idesc, flags & kUAccum, bar_e, 0u, 0u,
-                                       b_full + nsg * 8, nwph, px0, px1, px2, nxr & 1);
-          }
-          if (flags & kUWaitX0) tr.ev(c1.w, 0);
-          sg = nsg; wph = nwph; xr = nxr;
-          c0 = n0; c1 = n1; n0 = f0; n1 = f1;
-        }
-      }
-      tr.finish(args, 0);
-    }
-    __syncwarp();
-  } else if (warp >= kEpiWarps) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kCtlRegs));   // idle warps of the control group
   } else {
-    // ===================== epilogue: kH threads per row =====================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kEpiRegs));
-    const int s = warp / (4 * kH);                     // sub-tile
-    const int hs = (warp >> 2) & (kH - 1);             // which column half of a chunk (kH = 2)
-    const int qd = warp & 3;                           // TMEM lane quarter
-    const int r = qd * 32 + lane;                      // row within the sub-tile
-    const uint32_t t_lane = tmem_base + (((uint32_t)qd * 32) << 16) + s * 256;
-    uint8_t* xs = xbuf + s * 4 * kABlockBytes;
-    uint8_t* ins = inbuf + s * kABlockBytes;
-    const uint32_t xs_a0 = smem_u32(xs) + r * kRowBytes + ((r & 7) << 4);   // see sts_piece()
-    const int cb = hs * (8 / kH), ce = cb + 8 / kH;    // input-block chunks this thread writes
-    Tracer tr(args, (lane == 0 && qd == 0 && hs == 0) ? 1 + s : -1);
-    if (tid < 256) alpha_s[tid] = __float2bfloat16_rn(__ldg(aux + prog.alpha_w_off + tid));   // ordered by the first bar.sync
-    uint32_t n_acc0 = 0, n_acc1 = 0, n_free = 0, n_step = 0, dead = 0;
-    uint32_t sink = 0;                                 // keeps the math alive when a debug bit drops the stores
-#ifdef NFB_EPI_DEBUG
-    const int dbg = args.debug;                        // bits 2 and 4 only exist in -DNFB_EPI_DEBUG builds
-#else
-    const int dbg = 0;
-#endif
-    bool merge_alpha = false;                          // kH = 2: partner's alpha partial is waiting
-    RowState row;
+    // ===================== consumers: MMAs + epilogue of 64 rows =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(232));
+    const int cw = wg - 1, t = tid & 127, wq = t >> 5, lq = lane & 3;
+    const int arow = 64 * cw + 16 * wq + (lane >> 2);    // accumulator rows arow, arow + 8
+    const int r = 64 * cw + (t & 63), hs = t >> 6;       // row thread: row r, input-block half hs
+    const int cb = hs * 4, ce = cb + 4;                  // input-block chunks this thread writes
+    const int lr = t & 63;                               // row within the warpgroup
+    uint8_t* act_hi = base;
+    uint8_t* act_lo = base + kActLoOff;
+    uint8_t* inh = base + kInOff;
+    uint8_t* inl = inh + kABlockBytes;
+    float* alpha_s = reinterpret_cast<float*>(base + kAlphaOff);
+    float* scan_s = reinterpret_cast<float*>(base + kScanOff);
+    float* scr = reinterpret_cast<float*>(base + cw * 8192);        // head accumulators, 64 x 16
+    const uint32_t rows_off = (uint32_t)cw * 8192u;                 // this warpgroup's rows in a K-block
+    const uint32_t ring_a = smem_u32(base + kRingOff);
+    const uint32_t act_a = smem_u32(act_hi) + rows_off, in_a = smem_u32(inh) + rows_off;
+    const float alpha_b = __ldg(aux + prog.alpha_b_off);
     const int S = args.samples_per_ray;
-    auto epi_sync = [&]() { asm volatile("bar.sync 1, %0;" ::"n"(kEpiThreads) : "memory"); };
-    // "this thread's part of the activations is in shared memory" (the async-proxy
-    // fence precedes every call); mode 2 of the CTA pair signals the leader directly.
-    auto x_arrive = [&](uint64_t* bar) {
-      if constexpr (kDirectX) mbar_arrive_remote(bar, 0);
-      else mbar_arrive(bar);
-    };
+    uint32_t sg = 0, ph = 0, dead = 0;
+    auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory"); };
+    RowState row;
 
-    auto arrive_both = [&]() {
-      fence_proxy_async();
-      tc_fence_before();
-      x_arrive(&bars->x_ready[0]);
-      x_arrive(&bars->x_ready[1]);
-      x_arrive(&bars->x_ready[2]);
+    struct TilePref { float z, zn, org[3], dir[3]; };
+    auto tile_prefetch = [&](int tile, TilePref& pf) {
+      long long m = (long long)tile * kTileRows + r;
+      if (m >= args.num_rows) m = args.num_rows - 1;
+      const long long ray = m / S;
+      pf.z = args.z_vals ? __ldg(args.z_vals + m) : 0.f;
+      const bool last = m + 1 == (ray + 1) * S;
+      pf.zn = (fuse && !last && args.z_vals) ? __ldg(args.z_vals + m + 1) : 0.f;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        pf.dir[c] = __ldg(args.directions + ray * 3 + c);
+        pf.org[c] = __ldg(args.origins + ray * 3 + c);
+      }
     };
-    // Sample point of this thread's row for tile pair `pair`, and the first
-    // input block (model_utils.py:72-73; warping.py:325-326 / models.py:270).
-    auto begin_pair = [&](int pair) {
-      long long m = (long long)pair * kPairRows + s * kTileRows + r;
+    // Row state of tile `tile` (model_utils.py:72-73) and this thread's half of its first
+    // input block (warping.py:325-326 / models.py:270).
+    auto begin_tile = [&](int tile) {
+      TilePref pf;
+      tile_prefetch(tile, pf);
+      long long m = (long long)tile * kTileRows + r;
       row.valid = m < args.num_rows;
       if (!row.valid) m = args.num_rows - 1;
       row.m = m;
       row.ray = m / S;
-      const float z = args.z_vals ? __ldg(args.z_vals + m) : 0.f;
 #pragma unroll
-      for (int c = 0; c < 3; ++c)
-        row.x[c] = __ldg(args.origins + row.ray * 3 + c) + z * __ldg(args.directions + row.ray * 3 + c);
-      const float* cond = args.cond + row.ray * prog.cond_stride;
-      if (do_warp) {
-        if (args.fast_encode) posenc_fast_to_block(ins, r, row.x, prog.Fw, args.window, cond, prog.G, cb, ce);
-        else posenc_to_block(ins, r, row.x, prog.Fw, args.window, cond, prog.G, cb, ce);
-      } else {
-        if (args.warped && row.valid && hs == 0) {
-#pragma unroll
-          for (int c = 0; c < 3; ++c) args.warped[m * 3 + c] = row.x[c];
-        }
-        if (args.fast_encode) posenc_fast_to_block(ins, r, row.x, prog.Fp, nullptr, nullptr, 0, cb, ce);
-        else posenc_to_block(ins, r, row.x, prog.Fp, nullptr, nullptr, 0, cb, ce);
+      for (int c = 0; c < 3; ++c) row.x[c] = pf.org[c] + pf.z * pf.dir[c];
+      if (fuse) {
+        // dists of volumetric_rendering (model_utils.py:98-104)
+        row.z = pf.z;
+        row.last = m + 1 == (row.ray + 1) * S;
+        const float dnorm = sqrtf(pf.dir[0] * pf.dir[0] + pf.dir[1] * pf.dir[1] + pf.dir[2] * pf.dir[2]);
+        const float d = row.last ? (args.sample_at_infinity ? 1e10f : 1e-19f) : (pf.zn - pf.z);
+        row.dist = d * dnorm;
       }
-      row.alpha = hs == 0 ? __ldg(aux + prog.alpha_b_off) : 0.f;
+      if (!do_warp && args.warped && row.valid && hs == 0) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) args.warped[m * 3 + c] = row.x[c];
+      }
+      const float* cond = args.cond + row.ray * prog.cond_stride;
+      const float* window = do_warp ? args.window : nullptr;
+      // warp net: [posenc | GLO code]; NeRF net: [posenc | trunk condition]
+      const float* extra = do_warp ? cond : cond + prog.G;
+      const int F = do_warp ? prog.Fw : prog.Fp, n_extra = do_warp ? prog.G : prog.tc;
+      if constexpr (kX3) {
+        if (hs == 0) tc3::posenc_block_x3<0>(inh, inl, r, row.x, F, window, extra, n_extra);
+        else tc3::posenc_block_x3<1>(inh, inl, r, row.x, F, window, extra, n_extra);
+      } else {
+        if (args.fast_encode) posenc_fast_to_block(inh, r, row.x, F, window, extra, n_extra, cb, ce);
+        else posenc_to_block(inh, r, row.x, F, window, extra, n_extra, cb, ce);
+      }
     };
 
-    int pair = blockIdx.x;
-    epi_sync();                                        // alpha_s is visible to every epilogue thread
-    if (pair < pair_lim) {
-      begin_pair(pair);
-      arrive_both();
-    }
-    for (; pair < pair_lim; pair += gridDim.x) {
+    // fused composite: running state of the ray this CTA is on (replicated in every row thread)
+    float c_T = 1.f, c_cw = 0.f, a_r = 0.f, a_g = 0.f, a_b = 0.f, a_d = 0.f, a_w = 0.f, a_wnl = 0.f, a_med = 0.f;
+    if (n_my > 0) begin_tile(tile_of(0));
+    fence_proxy_async();
+    wg_sync();
+    for (int ti = 0; ti < n_my; ++ti) {
+      const int tile = tile_of(ti);
+      const bool has_next = ti + 1 < n_my;
       for (int si = first_step; si <= last_step; ++si) {
         const TcStep& st = prog.steps[si];
-        const float4* bias4 = kTcBiasLdg ? reinterpret_cast<const float4*>(aux + st.b_off)
-                                         : biasp.b4 + si * 64;   // this step's 256 biases
-        ++n_step;
-        if (kH == 2) epi_sync();
-        if (kH == 2 && merge_alpha) {
-          // the partner (columns' other half) left its alpha partial in the input block
-          if (hs == 0) row.alpha += reinterpret_cast<const float*>(ins)[r];
-          merge_alpha = false;
-          epi_sync();                                   // before anybody rewrites the input block
+        const float* bias = aux + st.b_off;
+        const float inv_s = kX3 ? 1.f / x3_weight_scale(__ldg(aux + prog.scale_off + si)) : 1.f;
+        const bool hidden = st.epi == kEpiHidden;
+        float acc0[64], acc1[64], acc16[8];
+        // ---- the layer's MMAs: one weight unit per (chunk, K-block), one unit in flight ----
+        uint32_t prev_sg = 0;
+        const int n_units = st.n_chunks * st.nkb;
+        for (int u = 0; u < n_units; ++u) {
+          const int c = u >= st.nkb ? 1 : 0, kb = u - c * st.nkb;
+          const int src = st.src[kb];
+          const uint32_t a_hi = src == kSrcIn ? in_a : act_a + (uint32_t)src * kABlockBytes;
+          const uint32_t a_lo = a_hi + (src == kSrcIn ? kABlockBytes : kActLoOff);
+          const uint32_t b_hi = ring_a + sg * kSlotBytes, b_lo = b_hi + (uint32_t)st.chunk_n * kRowBytes;
+          mbar_wait(&bars->full[sg], ph, dead);
+          wg_fence();
+          if (!hidden) wg_unit<kX3, 16>(acc16, a_hi, a_lo, b_hi, b_lo, kb);
+          else if (c == 0) wg_unit<kX3, 128>(acc0, a_hi, a_lo, b_hi, b_lo, kb);
+          else wg_unit<kX3, 128>(acc1, a_hi, a_lo, b_hi, b_lo, kb);
+          wg_commit();
+          if (u > 0) {
+            wg_wait<1>();
+            if (lane == 0) mbar_arrive(&bars->empty[prev_sg]);
+          }
+          prev_sg = sg;
+          if (++sg == kSlots) { sg = 0; ph ^= 1; }
         }
-        if (st.epi == kEpiHidden) {
-          const int cols = st.chunk_n / kH;            // columns of a chunk handled by this thread
-          const int np = cols / 32;                    // 32-column pieces: 4, 2 or 1
-          const int cbase = hs * cols;
+        wg_wait<0>();
+        wg_fence_regs<64>(acc0); wg_fence_regs<64>(acc1); wg_fence_regs<8>(acc16);
+        if (lane == 0) mbar_arrive(&bars->empty[prev_sg]);
+        wg_sync();      // every MMA of the warpgroup is complete: its activation rows may be overwritten
+
+        if (hidden) {
+          // ---- hidden layer: the output overwrites the input in place ----
           const bool relu = st.relu != 0, adot = st.alpha_dot != 0;
-          const __nv_bfloat16* aw = alpha_s;
-          // ---- chunk 0: results are held in registers until the MMAs of chunk 1
-          //      no longer read the blocks they overwrite ----
-          uint32_t packed[64];                         // (kH = 2 uses the first 32)
-          mbar_wait(&bars->acc_ready[0], n_acc0++ & 1, dead);
-          tc_fence_after();
-          tr.ev(si, 0);
-          if (dbg & 4) {
-#pragma unroll
-            for (int j = 0; j < 64 / kH; ++j) packed[j] = tid + j;
-          } else if (!(args.debug & 1)) {
-            if (kPipeE0 && kH == 1 && np == 4) {
-              // 128 columns: the loads of the second half are in flight while the
-              // first half is processed (tcgen05.wait::ld waits for everything issued).
-              float va[32], vb[32], vc[32], vd[32];
-              tmem_ld32(t_lane, va);
-              tmem_ld32(t_lane + 32, vb);
-#ifndef NFB_E0_ALL4
-              tmem_ld_wait();
-#endif
-              tmem_ld32(t_lane + 64, vc);
-              tmem_ld32(t_lane + 96, vd);
-#ifdef NFB_E0_ALL4
-              tmem_ld_wait();
-#endif
-              epi_piece(va, bias4, relu, adot, aw, row.alpha, packed);
-              epi_piece(vb, bias4 + 8, relu, adot, aw + 32, row.alpha, packed + 16);
-              tmem_ld_wait();
-              epi_piece(vc, bias4 + 16, relu, adot, aw + 64, row.alpha, packed + 32);
-              epi_piece(vd, bias4 + 24, relu, adot, aw + 96, row.alpha, packed + 48);
-            } else if (kH == 2 && np == 1) {
-              float va[32];
-              tmem_ld32(t_lane + cbase, va);
-              tmem_ld_wait();
-              epi_piece(va, bias4 + (cbase >> 2), relu, adot, aw + cbase, row.alpha, packed);
-            } else {
-#pragma unroll
-              for (int pp = 0; pp < 2 / kH; ++pp) {
-                if (2 * pp < np) {
-                  float va[32], vb[32];
-                  const int col = cbase + 2 * pp * 32;
-                  tmem_ld32(t_lane + col, va);
-                  tmem_ld32(t_lane + col + 32, vb);
-                  tmem_ld_wait();
-                  epi_piece(va, bias4 + (col >> 2), relu, adot, aw + col, row.alpha, packed + (2 * pp) * 16);
-                  epi_piece(vb, bias4 + (col >> 2) + 8, relu, adot, aw + col + 32, row.alpha, packed + (2 * pp + 1) * 16);
-                }
-              }
-            }
+          const float* aw = aux + prog.alpha_w_off;
+          float al0 = 0.f, al1 = 0.f;
+          epi_chunk<kX3>(acc0, 0, bias, inv_s, relu, adot, aw, al0, al1, act_hi, act_lo, arow, lq);
+          if (st.n_chunks == 2) epi_chunk<kX3>(acc1, 1, bias, inv_s, relu, adot, aw, al0, al1, act_hi, act_lo, arow, lq);
+          if (adot) {
+            // the four threads of a quad hold the row's columns
+            al0 += __shfl_xor_sync(0xffffffffu, al0, 1); al0 += __shfl_xor_sync(0xffffffffu, al0, 2);
+            al1 += __shfl_xor_sync(0xffffffffu, al1, 1); al1 += __shfl_xor_sync(0xffffffffu, al1, 2);
+            if (lq == 0) { alpha_s[arow] = al0; alpha_s[arow + 8] = al1; }
           }
-          tr.ev(si, 1);
-          mbar_wait(&bars->x_free, n_free++ & 1, dead);
-          tr.ev(si, 2);
-          if (kPipeE0 && kH == 1 && np == 4 && !(args.debug & 1) && !(dbg & 6)) {
-#pragma unroll
-            for (int p = 0; p < 4; ++p) sts_piece(xs_a0, 32 * p, packed + 16 * p);
-          } else
-#pragma unroll
-          for (int p = 0; p < 4 / kH; ++p) {
-            if (p < np && (dbg & 2)) {
-#pragma unroll
-              for (int q = 0; q < 16; ++q) sink ^= packed[p * 16 + q];
-            } else if (p < np && !(args.debug & 1)) {
-              const int col = cbase + 32 * p;
-              uint8_t* blk = xs + (col >> 6) * kABlockBytes;
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                uint4 o = make_uint4(packed[p * 16 + q * 4], packed[p * 16 + q * 4 + 1],
-                                     packed[p * 16 + q * 4 + 2], packed[p * 16 + q * 4 + 3]);
-                *reinterpret_cast<uint4*>(blk + swz_off(r, ((col & 63) >> 3) + q)) = o;
-              }
-            }
+          if (st.write_cond) {   // the rgb condition: the input block of the next step
+            const float* cond = args.cond + row.ray * prog.cond_stride + prog.rc_off;
+            if constexpr (kX3) tc3::cond_to_block_x3(inh, inl, r, cond, prog.rc, cb, ce);
+            else cond_to_block(inh, r, cond, prog.rc, cb, ce);
           }
-          // The input block is the first K-block of the next step (read right after
-          // x_ready[0]); every earlier reader of it (the skip layer) is complete.
-          if (st.write_cond)
-            cond_to_block(ins, r, args.cond + row.ray * prog.cond_stride + prog.G, prog.rc, cb, ce);
-          fence_proxy_async();
-          tc_fence_before();
-          x_arrive(&bars->x_ready[0]);
-          tr.ev(si, 3);
-          // ---- chunk 1: every MMA of the layer is complete, store directly ----
-          mbar_wait(&bars->acc_ready[1], n_acc1++ & 1, dead);
-          tc_fence_after();
-          tr.ev(si, 4);
-          if (kPipeE1 && kH == 1 && np == 4 && !(args.debug & 1) && !(dbg & 6)) {
-            // 256-wide layers: columns 128..191 are activation block 2, 192..255 block 3.
-            // Block 3's loads are in flight while block 2 is processed and handed over.
-            float va[32], vb[32], vc[32], vd[32];
-            uint32_t pk[16];
-            const uint32_t t1 = t_lane + 128;
-            tmem_ld32(t1, va);
-            tmem_ld32(t1 + 32, vb);
-#ifndef NFB_E1_ALL4
-            tmem_ld_wait();
-#endif
-            tmem_ld32(t1 + 64, vc);
-            tmem_ld32(t1 + 96, vd);
-#ifdef NFB_E1_ALL4
-            tmem_ld_wait();
-#endif
-            epi_piece(va, bias4 + 32, relu, adot, aw + 128, row.alpha, pk);
-            sts_piece(xs_a0, 128, pk);
-            epi_piece(vb, bias4 + 40, relu, adot, aw + 160, row.alpha, pk);
-            sts_piece(xs_a0, 160, pk);
-            fence_proxy_async();
-            tc_fence_before();
-            x_arrive(&bars->x_ready[1]);
-            tmem_ld_wait();
-            epi_piece(vc, bias4 + 48, relu, adot, aw + 192, row.alpha, pk);
-            sts_piece(xs_a0, 192, pk);
-            epi_piece(vd, bias4 + 56, relu, adot, aw + 224, row.alpha, pk);
-            sts_piece(xs_a0, 224, pk);
-          } else if (!(args.debug & 1)) {
-#pragma unroll
-            for (int pp = 0; pp < 2; ++pp) {
-              const bool two = (kH == 1) || np > 1;   // kH = 1: always pairs of pieces
-              if (pp * 2 < np || (kH == 2 && np == 1 && pp == 0)) {
-                float va[32], vb[32];
-                uint32_t pk[32];
-                const int col = st.chunk_n + cbase + 2 * pp * 32;
-                if (dbg & 4) {
-#pragma unroll
-                  for (int j = 0; j < 32; ++j) pk[j] = tid + j;
-                } else {
-                  tmem_ld32(t_lane + col, va);
-                  if (two) tmem_ld32(t_lane + col + 32, vb);
-                  tmem_ld_wait();
-                  epi_piece(va, bias4 + (col >> 2), relu, adot, aw + col, row.alpha, pk);
-                  if (two) epi_piece(vb, bias4 + (col >> 2) + 8, relu, adot, aw + col + 32, row.alpha, pk + 16);
-                }
-#pragma unroll
-                for (int h2 = 0; h2 < 2; ++h2) {
-                  if (dbg & 2) {
-#pragma unroll
-                    for (int q = 0; q < 16; ++q) sink ^= pk[h2 * 16 + q];
-                  } else if (h2 == 0 || two) {
-                    const int c2 = col + 32 * h2;
-                    uint8_t* blk = xs + (c2 >> 6) * kABlockBytes;
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                      uint4 o = make_uint4(pk[h2 * 16 + q * 4], pk[h2 * 16 + q * 4 + 1],
-                                           pk[h2 * 16 + q * 4 + 2], pk[h2 * 16 + q * 4 + 3]);
-                      *reinterpret_cast<uint4*>(blk + swz_off(r, ((c2 & 63) >> 3) + q)) = o;
-                    }
-                  }
-                }
-                // 256-wide layers: the first 64 columns of chunk 1 are a complete
-                // activation block - hand it to the issuer before doing the second.
-                if (kH == 1 && pp == 0 && np == 4) {
-                  fence_proxy_async();
-                  tc_fence_before();
-                  x_arrive(&bars->x_ready[1]);
-                }
-              }
-            }
-          }
-          if (kH == 2 && adot) {
-            // hand the alpha partial of this half to the partner thread of the row
-            // through the (currently unused) input block; merged at the next step.
-            if (hs == 1) reinterpret_cast<float*>(ins)[r] = row.alpha;
-            merge_alpha = true;
-          }
-          fence_proxy_async();
-          tc_fence_before();
-          if (!(kH == 1 && np == 4) || (args.debug & 1)) x_arrive(&bars->x_ready[1]);
-          x_arrive(&bars->x_ready[2]);
-          tr.ev(si, 5);
         } else {
-          // ---- heads: N = 16 accumulator columns, one chunk (both threads of a
-          //      row do the scalar work; they split the input-block chunks) ----
-          float v[16];
-          mbar_wait(&bars->acc_ready[0], n_acc0++ & 1, dead);
-          tc_fence_after();
-          tr.ev(si, 0);
-          tmem_ld16(t_lane, v);
-          tmem_ld_wait();
+          // ---- heads: N = 16 accumulator columns through the scratch to the row threads ----
+          const int l0 = 16 * wq + (lane >> 2);
 #pragma unroll
-          for (int j = 0; j < 12; j += 4) {
-            const float4 bq = tc_ld_bias(bias4, j >> 2);
-            v[j] += bq.x; v[j + 1] += bq.y; v[j + 2] += bq.z; v[j + 3] += bq.w;
+          for (int h = 0; h < 2; ++h) {
+            float* sr = scr + (l0 + 8 * h) * 16 + 2 * lq;
+            sr[0] = acc16[2 * h]; sr[1] = acc16[2 * h + 1];
+            sr[8] = acc16[4 + 2 * h]; sr[9] = acc16[5 + 2 * h];
           }
+          wg_sync();
+          float v[12];
+#pragma unroll
+          for (int j = 0; j < 12; ++j) v[j] = fmaf(scr[lr * 16 + j], inv_s, __ldg(bias + j));
+          wg_sync();      // the scratch has been read before anything overwrites block 0
           if (st.epi == kEpiWarpHeads) {
             float y[3];
             if (prog.warp_type == 2) {
@@ -774,40 +449,117 @@ field_tc_kernel(const __grid_constant__ TcProgram prog, const __grid_constant__ 
               for (int c = 0; c < 3; ++c) args.warped[row.m * 3 + c] = y[c];
             }
             if (args.warp_only) {
-              // next pair's first input block, then hand over
-              const int nxt = pair + gridDim.x;
-              if (nxt < pair_lim) begin_pair(nxt);
+              if (has_next) begin_tile(tile_of(ti + 1));
             } else {
-              if (args.fast_encode) posenc_fast_to_block(ins, r, row.x, prog.Fp, nullptr, nullptr, 0, cb, ce);
-              else posenc_to_block(ins, r, row.x, prog.Fp, nullptr, nullptr, 0, cb, ce);
+              // trunk condition (without one, the encoder's extra columns are compile-time empty)
+              const float* tcond = prog.tc ? args.cond + row.ray * prog.cond_stride + prog.G : nullptr;
+              if (!prog.tc) {
+                if constexpr (kX3) {
+                  if (hs == 0) tc3::posenc_block_x3<0>(inh, inl, r, row.x, prog.Fp, nullptr, nullptr, 0);
+                  else tc3::posenc_block_x3<1>(inh, inl, r, row.x, prog.Fp, nullptr, nullptr, 0);
+                } else {
+                  if (args.fast_encode) posenc_fast_to_block(inh, r, row.x, prog.Fp, nullptr, nullptr, 0, cb, ce);
+                  else posenc_to_block(inh, r, row.x, prog.Fp, nullptr, nullptr, 0, cb, ce);
+                }
+              } else if constexpr (kX3) {
+                if (hs == 0) tc3::posenc_block_x3<0>(inh, inl, r, row.x, prog.Fp, nullptr, tcond, prog.tc);
+                else tc3::posenc_block_x3<1>(inh, inl, r, row.x, prog.Fp, nullptr, tcond, prog.tc);
+              } else {
+                if (args.fast_encode) posenc_fast_to_block(inh, r, row.x, prog.Fp, nullptr, tcond, prog.tc, cb, ce);
+                else posenc_to_block(inh, r, row.x, prog.Fp, nullptr, tcond, prog.tc, cb, ce);
+              }
             }
-            arrive_both();
           } else {
-            if (row.valid && args.samples && hs == 0) {
-              float4 o;
-              o.x = sigmoidf(v[0]); o.y = sigmoidf(v[1]); o.z = sigmoidf(v[2]);
-              o.w = apply_act(row.alpha, prog.sigma_act);
-              reinterpret_cast<float4*>(args.samples)[row.m] = o;
+            float4 o;
+            o.x = sigmoidf(v[0]); o.y = sigmoidf(v[1]); o.z = sigmoidf(v[2]);
+            // alpha condition (Dense(1) on [bottleneck | alpha condition]): its per-ray part
+            const float a_cond = prog.ac ? alpha_cond_dot<kX3>(args.cond + row.ray * prog.cond_stride + prog.ac_off,
+                                                               aux + prog.alpha_w_off + kAlphaCondOff, prog.ac)
+                                         : 0.f;
+            o.w = apply_act(alpha_b + (alpha_s[r] + a_cond), prog.sigma_act);
+            if (hs == 0 && row.valid && args.samples) reinterpret_cast<float4*>(args.samples)[row.m] = o;
+            if (fuse && hs == 0) {
+              // ---- volumetric_rendering (model_utils.py:104-136) + median depth (:231-239, 262-263)
+              //      over the 128 samples of this tile; one sample per row thread of half 0 ----
+              const int qd = r >> 5;
+              auto bar128 = [&]() { asm volatile("bar.sync 3, 128;" ::: "memory"); };
+              if ((tile % tpr) == 0) { c_T = 1.f; c_cw = 0.f; a_r = a_g = a_b = a_d = a_w = a_wnl = a_med = 0.f; }
+              // alpha = 1 - exp(-sigma * dist) as -expm1(-x) (see composite_kernel)
+              const float al = -expm1f(-o.w * row.dist);
+              const float tf = 1.0f - al + 1e-10f;
+              float P = tf;                                    // inclusive product scan of tf
+#pragma unroll
+              for (int sh = 1; sh < 32; sh <<= 1) {
+                const float q = __shfl_up_sync(0xffffffffu, P, sh);
+                if (lane >= sh) P = P * q;
+              }
+              float excl = __shfl_up_sync(0xffffffffu, P, 1);
+              if (lane == 0) excl = 1.f;
+              if (lane == 31) scan_s[qd] = P;
+              bar128();
+              float Wq = 1.f, Wall = 1.f;
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                const float f = scan_s[q];
+                if (q < qd) Wq = Wq * f;
+                Wall = Wall * f;
+              }
+              const float Ti = (c_T * Wq) * excl;              // accum_prod (model_utils.py:110-113)
+              const float w = al * Ti;
+              if (args.ray_weights) args.ray_weights[row.m] = w;
+              float C = w;                                     // inclusive cumsum of the weights
+#pragma unroll
+              for (int sh = 1; sh < 32; sh <<= 1) {
+                const float q = __shfl_up_sync(0xffffffffu, C, sh);
+                if (lane >= sh) C = C + q;
+              }
+              float red[6] = {w * o.x, w * o.y, w * o.z, w * row.z, w, row.last ? 0.f : w};
+#pragma unroll
+              for (int k = 0; k < 6; ++k)
+#pragma unroll
+                for (int sh = 16; sh > 0; sh >>= 1) red[k] += __shfl_xor_sync(0xffffffffu, red[k], sh);
+              if (lane == 0) {
+#pragma unroll
+                for (int k = 0; k < 6; ++k) scan_s[8 + qd * 8 + k] = red[k];
+              }
+              bar128();
+              float pre = c_cw, tot[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                if (q < qd) pre += scan_s[8 + q * 8 + 4];
+#pragma unroll
+                for (int k = 0; k < 6; ++k) tot[k] += scan_s[8 + q * 8 + k];
+              }
+              const float cwt = pre + C;                       // cumsum over the ray up to this sample
+              float prev = __shfl_up_sync(0xffffffffu, cwt, 1);
+              if (lane == 0) prev = pre;
+              // first sample whose cumulative weight reaches 0.5 (opaque xor shifted, :231-238)
+              float med = (cwt >= 0.5f && !(prev >= 0.5f)) ? row.z : 0.f;
+#pragma unroll
+              for (int sh = 16; sh > 0; sh >>= 1) med += __shfl_xor_sync(0xffffffffu, med, sh);
+              if (lane == 0) scan_s[4 + qd] = med;
+              bar128();
+              a_med += scan_s[4] + scan_s[5] + scan_s[6] + scan_s[7];
+              a_r += tot[0]; a_g += tot[1]; a_b += tot[2]; a_d += tot[3]; a_w += tot[4]; a_wnl += tot[5];
+              c_T = c_T * Wall; c_cw += tot[4];
+              if ((tile % tpr) == tpr - 1 && r == 0) {
+                float rr = a_r, gg = a_g, bb = a_b;
+                if (args.white_bg) { const float bg = 1.f - a_w; rr = rr + bg; gg = gg + bg; bb = bb + bg; }
+                float* ro = args.ray_out + row.ray * 6;
+                ro[0] = rr; ro[1] = gg; ro[2] = bb; ro[3] = a_d; ro[4] = a_med;
+                ro[5] = args.sample_at_infinity ? a_wnl : a_w;
+              }
+              bar128();   // scan_s is read by every row thread before the next tile writes it
             }
-            const int nxt = pair + gridDim.x;
-            if (nxt < pair_lim) begin_pair(nxt);
-            arrive_both();
-            tr.ev(si, 5);
+            if (has_next) begin_tile(tile_of(ti + 1));
           }
         }
+        fence_proxy_async();   // this thread's shared-memory stores are visible to the next MMAs ...
+        wg_sync();             // ... of every warp of the warpgroup
       }
     }
-    tr.finish(args, 1 + s);
-    if (sink == 0x9e3779b9u && args.trace) args.trace[0] = sink;   // never true in practice
-    tc_fence_before();
   }
-  if constexpr (kPair) {
-    cluster_sync_all();        // nobody frees TMEM or exits while the peer still computes or signals
-    if (warp == kMmaWarp) tmem_dealloc2(tmem_base, 512);
-  } else {
-    __syncthreads();
-    if (warp == kMmaWarp) tmem_dealloc(tmem_base, 512);
-  }
+  __syncthreads();
 }
 
 // ---------------------------------------------------------------------------
@@ -815,73 +567,23 @@ field_tc_kernel(const __grid_constant__ TcProgram prog, const __grid_constant__ 
 // precision in nfb_api.cu) into TcPrograms, pack the weights, launch.
 // ---------------------------------------------------------------------------
 inline int tc_fail(const char* what) {
-  return fail("the tcgen05 paths (precision bf16 / fp16x3) do not support this model: %s; use precision fp32", what);
-}
-
-// fp16x3 (field_tc3.cuh): issue order of a step's (chunk, K-block) units.  A layer's output
-// reaches the next layer in two instalments: the columns of chunk 0 (activation blocks
-// < split) when the chunk-0 epilogue is done, the rest after the chunk-1 epilogue, which
-// starts only when the layer's last MMA has completed.  "Phase A" K-blocks (the input block
-// and blocks < split of the previous step) are therefore issued for BOTH chunks first, then
-// the "phase B" K-blocks: the MMAs that overlap the previous chunk-1 epilogue are n_chunks x
-// |A| units instead of |A|, and the chunk-0 accumulator completes two units before the end of
-// the step so that its epilogue overlaps the tail.  Returns the number of units.
-// Activation blocks >= this index are written by the SECOND instalment of a hidden step's
-// epilogue (chunk 1 of a two-chunk step; columns 64.. of a one-chunk 128-wide step).
-inline int x3_split_of(const TcStep& prev) {
-  if (prev.epi != kEpiHidden) return 99;
-  return prev.n_chunks == 2 ? prev.chunk_n / kBlockK : 1;
-}
-inline int x3_unit_order(const TcProgram& tp, int si, int* oc, int* okb) {
-  const TcStep& t = tp.steps[si];
-  const bool after_heads = si > 0 && tp.steps[si - 1].epi != kEpiHidden;
-  int split = 99;
-  if (si > 0 && !after_heads) split = x3_split_of(tp.steps[si - 1]);
-  int n = 0;
-  int lst[2][2][8], cnt[2][2] = {{0, 0}, {0, 0}};     // [phase][chunk] -> K-blocks
-  for (int phase = 0; phase < 2; ++phase)
-    for (int c = 0; c < t.n_chunks; ++c)
-      for (int kb = 0; kb < t.nkb; ++kb) {
-        const bool late = t.src[kb] < kSrcIn && t.src[kb] >= split;
-        if ((int)late == phase) lst[phase][c][cnt[phase][c]++] = kb;
-      }
-  auto put = [&](int c, int kb) { oc[n] = c; okb[n] = kb; ++n; };
-#ifndef NFB_X3_ORDER_OLD
-  if (t.n_chunks == 2 && cnt[1][0] > 0 && cnt[0][1] > 0) {
-    // Balanced order: A(c0), A(c1) but its last unit, B(c0), last of A(c1), B(c1).  The chunk-0
-    // accumulator completes |B| + 1 units before the end of the step (its epilogue - accumulator
-    // read, split, wait for the last reader of the blocks it overwrites, store - then has about one
-    // unit of slack before the next step's first MMA needs it), and the first phase-B unit still
-    // comes |A(c0)| + |A(c1)| - 1 units after the start of the step (the previous chunk-1 epilogue
-    // has that long).  With A, A, B, B both hand-offs were on the edge: ~2 units for a ~1.8 K-cycle chain.
-    for (int i = 0; i < cnt[0][0]; ++i) put(0, lst[0][0][i]);
-    for (int i = 0; i + 1 < cnt[0][1]; ++i) put(1, lst[0][1][i]);
-    for (int i = 0; i < cnt[1][0]; ++i) put(0, lst[1][0][i]);
-    put(1, lst[0][1][cnt[0][1] - 1]);
-    for (int i = 0; i < cnt[1][1]; ++i) put(1, lst[1][1][i]);
-    return n;
-  }
-#endif
-  for (int phase = 0; phase < 2; ++phase)
-    for (int c = 0; c < t.n_chunks; ++c)
-      for (int i = 0; i < cnt[phase][c]; ++i) put(c, lst[phase][c][i]);
-  return n;
+  return fail("the tensor-core paths (precision bf16 / fp16x3) do not support this model: %s; use precision fp32", what);
 }
 
 inline int build_tc_program(nfb_handle* h, int level, long long* wbytes, long long* aux_floats) {
   const FieldProgram& fp = h->prog[level];
   TcProgram& tp = h->tcprog[level];
   memset(&tp, 0, sizeof(tp));
-  // fp16x3 mode (field_tc3.cuh): same schedule, fp16 operands, every (chunk, K-block)
-  // has two weight units [W_hi | W_lo], and "sub-tile 1" of a unit is the lo image.
-  const bool x3 = h->cfg.precision == NFB_PREC_FP16X3;
-  const int wparts = x3 ? 2 : 1;
+  // fp16x3: every unit is [W_hi | W_lo]
+  const int wparts = h->cfg.precision == NFB_PREC_FP16X3 ? 2 : 1;
   tp.warp_pivot = fp.warp_pivot; tp.warp_trans = fp.warp_trans;
   tp.warp_type = fp.warp_type; tp.Fw = fp.Fw; tp.G = fp.G; tp.Fp = fp.Fp; tp.rc = fp.rc;
   tp.cond_stride = fp.cond_stride; tp.sigma_act = fp.sigma_act;
-  if (fp.tc || fp.ac) return tc_fail("trunk/alpha conditions");
-  if (fp.rc <= 0 || fp.rc > kBlockK) return tc_fail("rgb condition must have 1..64 channels");
-  if (fp.Dp > kBlockK || (fp.warp_type && fp.Dw > kBlockK)) return tc_fail("encoded inputs wider than 64");
+  // per-ray condition vector: [glo | trunk | alpha | rgb] (nfb_api.cu: build_programs)
+  tp.tc = fp.tc; tp.ac = fp.ac; tp.ac_off = fp.G + fp.tc; tp.rc_off = fp.G + fp.tc + fp.ac;
+  if (fp.rc > kBlockK) return tc_fail("rgb condition wider than 64 channels");
+  if (fp.ac > kBlockK) return tc_fail("alpha condition wider than 64 channels");
+  if (fp.Dp + fp.tc > kBlockK || (fp.warp_type && fp.Dw > kBlockK)) return tc_fail("encoded inputs wider than 64");
   if (fp.hidden_act != kRelu) return tc_fail("hidden activation other than relu");
   auto new_bias = [&](const Step& st) {
     int off = (int)*aux_floats;
@@ -893,31 +595,28 @@ inline int build_tc_program(nfb_handle* h, int level, long long* wbytes, long lo
     if (tp.n_steps >= kMaxTcSteps) return tc_fail("too many layers");
     TcStep& t = tp.steps[tp.n_steps];
     memset(&t, 0, sizeof(t));
-    if (st.k_x % kBlockK || st.k_x > 256 || st.k_in > kBlockK) return tc_fail("layer widths must be multiples of 64 (<= 256)");
+    if (st.k_x > 256 || st.k_in > kBlockK) return tc_fail("layer wider than 256 or inputs wider than 64");
     if (st.k_x && st.k_x != cur_width) return tc_fail("unexpected layer input width");
     t.nkb = 0;
-    // The input block is never rewritten between a step's producer and consumer,
-    // so it goes first: its MMAs can issue before the previous epilogue is done.
     if (st.k_in) t.src[t.nkb++] = kSrcIn;
-    for (int b = 0; b < st.k_x / kBlockK; ++b) t.src[t.nkb++] = b;
+    for (int b = 0; b < (st.k_x + kBlockK - 1) / kBlockK; ++b) t.src[t.nkb++] = b;
     t.epi = epi;
     if (epi == kEpiHidden) {
-      if (st.n != 128 && st.n != 256) return tc_fail("hidden widths must be 128 or 256");
-      t.n_chunks = 2; t.chunk_n = st.n / 2;
-      // fp16x3: a 128-wide layer is ONE chunk of N = 128 (half the commits of two N = 64 chunks and
-      // full-rate MMAs); its epilogue hands the output over in two 64-column instalments
-      if (x3 && st.n == 128) { t.n_chunks = 1; t.chunk_n = 128; }
+      // N is issued in chunks of 128 columns; a narrower layer is zero-padded (zero weight rows
+      // and biases give zero output columns, which the next layer's zero-padded K rows ignore)
+      if (st.n < 1 || st.n > 256) return tc_fail("hidden widths must be 1..256");
+      t.n_chunks = (st.n + 127) / 128; t.chunk_n = 128;
       if (st.act != kRelu && st.act != kNone) return tc_fail("hidden activation other than relu");
       t.relu = st.act == kRelu;
-      t.kb_free = -1;
-      for (int kb = 0; kb < t.nkb; ++kb)
-        if (t.src[kb] < kSrcIn && t.src[kb] < t.chunk_n / kBlockK) t.kb_free = kb;
     } else {
-      t.n_chunks = 1; t.chunk_n = 16; t.kb_free = -1;
+      // a head follows a hidden layer and is followed by a step that reads the input block only
+      // (its accumulators pass through activation block 0, see field_wg_kernel)
+      t.n_chunks = 1; t.chunk_n = 16;
       if (st.n > 12) return tc_fail("head wider than 12");
+      if (st.k_in) return tc_fail("head reading the encoded inputs");
     }
     t.b_off = new_bias(st);
-    // weight units: for chunk c, for kb: chunk_n rows x 128 B
+    // weight units: for chunk c, for kb: wparts x chunk_n rows x 128 B
     t.w_off = (uint32_t)*wbytes;
     for (int c = 0; c < t.n_chunks; ++c) {
       nfb_handle::TcPackJob job;
@@ -928,14 +627,13 @@ inline int build_tc_program(nfb_handle* h, int level, long long* wbytes, long lo
       for (int kb = 0; kb < t.nkb; ++kb)
         for (int j = 0; j < kBlockK; ++j) {
           int srck = -1;
-          if (t.src[kb] < kSrcIn) srck = t.src[kb] * kBlockK + j;
+          if (t.src[kb] < kSrcIn) srck = t.src[kb] * kBlockK + j < st.k_x ? t.src[kb] * kBlockK + j : -1;
           else if (j < st.k_in) srck = st.k_x + j;
           job.k_map[(size_t)kb * kBlockK + j] = srck;
         }
       h->tc_jobs.push_back(job);
       *wbytes += (long long)wparts * t.nkb * t.chunk_n * kRowBytes;
     }
-    tp.units_per_pair += wparts * t.n_chunks * t.nkb;
     ++tp.n_steps;
     return 0;
   };
@@ -954,17 +652,21 @@ inline int build_tc_program(nfb_handle* h, int level, long long* wbytes, long lo
   for (int i = 0; i < fp.nerf.n_steps; ++i) {
     const Step& st = fp.nerf.steps[i];
     if (st.dst == fp.alpha_slot && st.n == 1 && !seen_alpha) {
-      // alpha = Dense(1)(trunk_out): folded into the epilogue of the last trunk layer.
-      if (st.k_in) return tc_fail("alpha condition");
+      // alpha = Dense(1)(trunk_out), or with an alpha condition Dense(1)([bottleneck_out | alpha_cond])
+      // (models.py:206-207, modules.py:152-157): the dot product over the layer output is folded into
+      // the epilogue of the layer it reads, the per-ray condition part is added by the row threads.
+      if (st.k_in != fp.ac) return tc_fail("alpha head inputs");
       seen_alpha = true;
-      // The SIMT program runs bottleneck before alpha; the trunk's last layer is
-      // the hidden step before the bottleneck.
-      int trunk_last = seen_bottleneck ? last_hidden - 1 : last_hidden;
-      if (trunk_last < 0) return tc_fail("alpha head without a trunk layer");
-      tp.steps[trunk_last].alpha_dot = 1;
-      tp.alpha_w_off = (int)*aux_floats; *aux_floats += 256;
+      // The SIMT program runs bottleneck before alpha: without an alpha condition the alpha head
+      // reads the trunk's last layer, the hidden step before the bottleneck.
+      const int src_step = (seen_bottleneck && !st.k_in) ? last_hidden - 1 : last_hidden;
+      if (src_step < 0) return tc_fail("alpha head without a trunk layer");
+      tp.steps[src_step].alpha_dot = 1;
+      tp.alpha_w_off = (int)*aux_floats; *aux_floats += kAlphaCondOff + kBlockK;
       tp.alpha_b_off = (int)*aux_floats; *aux_floats += 4;
       h->tc_aux_jobs.push_back({st.w_off, st.k_x, st.npad, tp.alpha_w_off});
+      if (st.k_in)
+        h->tc_aux_jobs.push_back({st.w_off + st.k_x * st.npad, st.k_in, st.npad, tp.alpha_w_off + kAlphaCondOff});
       h->tc_aux_jobs.push_back({st.b_off, 1, 1, tp.alpha_b_off});
       continue;
     }
@@ -979,123 +681,13 @@ inline int build_tc_program(nfb_handle* h, int level, long long* wbytes, long lo
       if (st.act == kNone) tp.steps[last_hidden].write_cond = 1;
     }
   }
-  if (!seen_alpha || !seen_bottleneck) return tc_fail("model without bottleneck/alpha head");
-  tp.scale_off = (int)*aux_floats; *aux_floats += kMaxTcSteps;
-  // Flatten the issuer's schedule (see TcUnit).
-  tp.n_units = 0;
-  int prev_split = 99, prev_split2 = 99;
+  if (!seen_alpha) return tc_fail("model without alpha head");
   for (int si = 0; si < tp.n_steps; ++si) {
-    const TcStep& t = tp.steps[si];
-    tp.unit_begin[si] = tp.n_units;
-    if (x3) {
-      // ---- fp16x3: phase-ordered units (x3_unit_order) ----
-      int oc[16], okb[16];
-      const int n = x3_unit_order(tp, si, oc, okb);
-      const bool after_heads = si > 0 && tp.steps[si - 1].epi != kEpiHidden;
-      const int split = (si > 0 && !after_heads) ? x3_split_of(tp.steps[si - 1]) : 99;
-      if (tp.n_units + n > kMaxTcUnits) return tc_fail("too many weight units");
-      const int first = tp.n_units;
-      int last_of_chunk[2] = {-1, -1}, first_of_chunk[2] = {-1, -1}, first_late = -1, last_low = -1;
-      for (int i = 0; i < n; ++i) {
-        const int c = oc[i], kb = okb[i], b = t.src[kb];
-        if (first_of_chunk[c] < 0) first_of_chunk[c] = i;
-        last_of_chunk[c] = i;
-        if (b < kSrcIn && b >= split && first_late < 0) first_late = i;
-        // readers of the activation blocks this step's chunk-0 epilogue overwrites
-        if (t.n_chunks == 2 && b < kSrcIn && b < t.chunk_n / kBlockK) last_low = i;
-      }
-      for (int i = 0; i < n; ++i) {
-        TcUnit& u = tp.units[tp.n_units++];
-        memset(&u, 0, sizeof(u));
-        const int c = oc[i], kb = okb[i], b = t.src[kb];
-        // the activations are in tensor memory - bit 31 + column offset of the hi / lo image (32 columns per
-        // 64-wide K-block); the input block images are in shared memory at byte offsets 0 / 16 KB
-        if (b < kSrcIn) { u.a0_lo = 0x80000000u | (uint32_t)(256 + b * 32); u.a1_lo = 0x80000000u | (uint32_t)(384 + b * 32); }
-        else { u.a0_lo = 0u; u.a1_lo = (uint32_t)(kABlockBytes >> 4); }
-        u.dcol = (uint32_t)(c * t.chunk_n); u.idesc = make_idesc_f16(kTileRows, t.chunk_n);
-        u.step = (uint32_t)si;
-        if (i != first_of_chunk[c]) u.flags |= kUAccum;
-        if (i == last_of_chunk[c]) u.flags |= (c == 0 ? kUCommitAcc0 : kUCommitAcc1);
-        // x_ready[1] = "the previous chunk-1 epilogue has read its accumulator" (the first MMA of this step's
-        // chunk 1 overwrites it), x_ready[2] = "... has stored its outputs" (the phase-B K-blocks)
-        if (t.n_chunks == 2 && i == first_of_chunk[1]) u.flags |= kUWaitX1;
-        if (t.n_chunks == 1 && i == 0) u.flags |= kUWaitX1;
-        if (i == first_late) u.flags |= kUWaitX2;
-        // "the blocks chunk 0's epilogue overwrites are no longer read": a separate commit only when one of
-        // their readers is issued after chunk 0's last unit - otherwise acc_ready[0] already implies it
-        // (a commit covers every MMA issued before it) and the step is marked kb_free = -2: no x_free.
-        if (t.n_chunks == 2 && last_low > last_of_chunk[0] && i == last_low) u.flags |= kUCommitXFree;
-      }
-      if (t.n_chunks == 2) tp.steps[si].kb_free = last_low > last_of_chunk[0] ? 0 : -2;
-      tp.units[first].flags |= kUWaitX0;
-      TcUnit& last = tp.units[tp.n_units - 1];
-
-      if (first_late < 0) last.flags |= kUWaitX2;
-      last.flags |= kUStepEnd;
-      // issue-order position of every (chunk, K-block): the weight units are packed in that order
-      for (auto& job : h->tc_jobs)
-        if (job.level == level && job.step == si) {
-          job.unit_pos.assign((size_t)t.nkb, 0);
-          for (int i = 0; i < n; ++i)
-            if (oc[i] == job.chunk) job.unit_pos[(size_t)okb[i]] = i;
-        }
-      continue;
-    }
-    // A step that can start a tile pair (step 0, or the first NeRF step when the
-    // warp is skipped) follows a 1-chunk step or the prologue: nothing to split.
-    const bool after_heads = si > 0 && tp.steps[si - 1].epi != kEpiHidden;
-    if (si == 0 || after_heads) prev_split = prev_split2 = 99;
-    int kb_need = t.nkb, kb_need2 = t.nkb;
-    for (int kb = t.nkb - 1; kb >= 0; --kb) {
-      if (t.src[kb] < kSrcIn && t.src[kb] >= prev_split) kb_need = kb;
-      if (t.src[kb] < kSrcIn && t.src[kb] >= prev_split2) kb_need2 = kb;
-    }
-    bool have1 = false, have2 = false;
-    const int first = tp.n_units;
-    for (int c = 0; c < t.n_chunks; ++c)
-      for (int kb = 0; kb < t.nkb; ++kb) {
-        if (tp.n_units >= kMaxTcUnits) return tc_fail("too many weight units");
-        TcUnit& u = tp.units[tp.n_units++];
-        memset(&u, 0, sizeof(u));
-        const int b = t.src[kb];
-        const int a0 = (b < kSrcIn) ? b * kABlockBytes : kXBytes;
-        const int a1 = (b < kSrcIn) ? (4 + b) * kABlockBytes : kXBytes + kABlockBytes;
-        u.a0_lo = (uint32_t)(a0 >> 4); u.a1_lo = (uint32_t)(a1 >> 4);
-        u.dcol = (uint32_t)(c * t.chunk_n); u.idesc = make_idesc_bf16(kTileRows, t.chunk_n);
-        u.step = (uint32_t)si;
-        if (kb) u.flags |= kUAccum;
-        if (!have1 && (c == 1 || kb >= kb_need)) { u.flags |= kUWaitX1; have1 = true; }
-        if (!have2 && (c == 1 || kb >= kb_need2)) { u.flags |= kUWaitX2; have2 = true; }
-        if (kb == t.nkb - 1) u.flags |= (c == 0 ? kUCommitAcc0 : kUCommitAcc1);
-        if (t.n_chunks == 2) {
-          if (c == 1 && kb == t.kb_free) u.flags |= kUCommitXFree;
-          if (c == 0 && kb == t.nkb - 1 && t.kb_free < 0) u.flags |= kUCommitXFree;
-        }
-      }
-    tp.units[first].flags |= kUWaitX0;
-    TcUnit& last = tp.units[tp.n_units - 1];
-    if (!have1) last.flags |= kUWaitX1;   // consumed before the final commit re-arms the epilogue
-    if (!have2) last.flags |= kUWaitX2;
-    last.flags |= kUStepEnd;
-    prev_split = (t.n_chunks == 2) ? t.chunk_n / kBlockK : 99;
-    // x_ready[2] covers the second activation block written by chunk 1 (256-wide
-    // layers: block 3); otherwise it fires together with x_ready[1].
-    prev_split2 = (t.n_chunks == 2 && t.chunk_n == 128) ? 3 : prev_split;
+    const bool after_head = si > 0 && tp.steps[si - 1].epi != kEpiHidden;
+    if ((si == 0 || after_head) && (tp.steps[si].nkb != 1 || tp.steps[si].src[0] != kSrcIn))
+      return tc_fail("first layer of an MLP reading more than the encoded inputs");
   }
-  tp.unit_begin[tp.n_steps] = tp.n_units;
-  for (int i = 0; i < tp.n_units; ++i) {
-    TcUnit& u = tp.units[i];
-    u.need = 1u | ((u.flags & kUWaitX0) ? 2u : 0u) | ((u.flags & kUWaitX1) ? 4u : 0u) |
-             ((u.flags & kUWaitX2) ? 8u : 0u);
-    // Successor in issue order.  After the last unit of a tile pair comes the first
-    // unit of the next pair, which (in every mode) waits for x_ready[0] only.
-    const bool last_of_pair = (i == tp.n_units - 1) || (tp.steps[u.step].epi == kEpiWarpHeads && (u.flags & kUStepEnd));
-    const uint32_t nf = (i + 1 < tp.n_units) ? tp.units[i + 1].flags : (uint32_t)kUWaitX0;
-    u.probe_next = ((nf & kUWaitX0) ? 2u : 0u) | ((nf & kUWaitX1) ? 4u : 0u) | ((nf & kUWaitX2) ? 8u : 0u);
-    // fp16x3: W_lo follows W_hi inside the weight slot, chunk_n rows x 128 B further (in 16-byte units)
-    if (x3) u.probe_next |= (uint32_t)(tp.steps[u.step].chunk_n * (kRowBytes >> 4)) << 16;
-    (void)last_of_pair;
-  }
+  tp.scale_off = (int)*aux_floats; *aux_floats += kMaxTcSteps;
   return 0;
 }
 
@@ -1110,12 +702,9 @@ inline int create_tc(nfb_handle* h) {
   if (cudaMalloc(&h->d_wpack, (size_t)wbytes) != cudaSuccess) return fail("cudaMalloc wpack failed");
   if (cudaMalloc(&h->d_aux, (size_t)auxf * sizeof(float)) != cudaSuccess) return fail("cudaMalloc aux failed");
   if (cudaMemset(h->d_aux, 0, (size_t)auxf * sizeof(float)) != cudaSuccess) return fail("cudaMemset failed");
-  if (h->cfg.precision == NFB_PREC_FP16X3) return 0;     // tc3::create_x3 reserves that kernel's shared memory
-  if (cudaFuncSetAttribute(field_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmemBytes) != cudaSuccess ||
-      cudaFuncSetAttribute(field_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmemBytes) != cudaSuccess ||
-      cudaFuncSetAttribute(field_tc_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmemBytes) != cudaSuccess ||
-      cudaFuncSetAttribute(field_tc_kernel<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmemBytes) != cudaSuccess)
-    return fail("cannot reserve %d bytes of shared memory for the tcgen05 kernel", kTcSmemBytes);
+  if (cudaFuncSetAttribute(field_wg_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(field_wg_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmemBytes) != cudaSuccess)
+    return fail("cannot reserve %d bytes of shared memory for the tensor-core kernel", kWgSmemBytes);
   return 0;
 }
 
@@ -1163,20 +752,14 @@ inline int pack_tc(nfb_handle* h, cudaStream_t s) {
     const long long total = (long long)t.nkb * t.chunk_n * kBlockK;
     uint8_t* dst = h->d_wpack + t.w_off + (size_t)(x3 ? 2 : 1) * j.chunk * t.nkb * t.chunk_n * kRowBytes;
     // source columns n0.. of the fp32 (K x npad) matrix: shift the base pointer.
-    if (x3) {
-      // one launch per K-block: its unit [W_hi | W_lo] goes to its issue-order position in the step
-      const long long per = (long long)t.chunk_n * kBlockK;
-      for (int kb = 0; kb < t.nkb; ++kb) {
-        uint8_t* udst = h->d_wpack + t.w_off + (size_t)j.unit_pos[(size_t)kb] * 2 * t.chunk_n * kRowBytes;
-        pack_weight_x3_kernel<<<(unsigned)((per + 255) / 256), 256, 0, s>>>(
-            h->d_packed + j.simt_w_off + j.n0, j.ld, d_maps + map_off + (size_t)kb * kBlockK, 1, j.n - j.n0, t.chunk_n,
-            h->d_aux + h->tcprog[j.level].scale_off + j.step, udst);
-        if (kb) h->launches++;
-      }
-    } else
-    pack_weight_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(
-        h->d_packed + j.simt_w_off + j.n0, j.ld, d_maps + map_off, t.nkb, j.n - j.n0, t.chunk_n,
-        reinterpret_cast<__nv_bfloat16*>(dst));
+    if (x3)
+      pack_weight_x3_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(
+          h->d_packed + j.simt_w_off + j.n0, j.ld, d_maps + map_off, t.nkb, j.n - j.n0, t.chunk_n,
+          h->d_aux + h->tcprog[j.level].scale_off + j.step, dst);
+    else
+      pack_weight_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(
+          h->d_packed + j.simt_w_off + j.n0, j.ld, d_maps + map_off, t.nkb, j.n - j.n0, t.chunk_n,
+          reinterpret_cast<__nv_bfloat16*>(dst));
     h->launches++;
     map_off += j.k_map.size();
   }
@@ -1186,75 +769,26 @@ inline int pack_tc(nfb_handle* h, cudaStream_t s) {
     h->launches++;
   }
   e = cudaGetLastError();
-  // The biases travel as a kernel parameter: read them back once per parameter update.
-  std::vector<float> h_aux((size_t)h->aux_floats);
-  if (e == cudaSuccess)
-    e = cudaMemcpyAsync(h_aux.data(), h->d_aux, h_aux.size() * sizeof(float), cudaMemcpyDeviceToHost, s);
   if (e == cudaSuccess) e = cudaStreamSynchronize(s);
   cudaFree(d_maps);
-  if (e != cudaSuccess) return fail("tcgen05 weight packing failed: %s", cudaGetErrorString(e));
-  for (int lv = 0; lv < 2; ++lv) {
-    const TcProgram& tp = h->tcprog[lv];
-    memset(&h->tcbias[lv], 0, sizeof(TcBias));
-    for (int si = 0; si < tp.n_steps; ++si)
-      memcpy(reinterpret_cast<float*>(h->tcbias[lv].b4) + si * 256, h_aux.data() + tp.steps[si].b_off, 256 * sizeof(float));
-    if (x3) {
-      X3Consts& c = h->x3c[lv];
-      memset(&c, 0, sizeof(c));
-      memcpy(c.b4, h->tcbias[lv].b4, sizeof(c.b4));
-      memcpy(c.alpha4, h_aux.data() + tp.alpha_w_off, 256 * sizeof(float));
-      c.alpha_b = h_aux[tp.alpha_b_off];
-      for (int si = 0; si < tp.n_steps; ++si) c.inv_scale[si] = 1.f / x3_weight_scale(h_aux[tp.scale_off + si]);
-    }
-  }
+  if (e != cudaSuccess) return fail("tensor-core weight packing failed: %s", cudaGetErrorString(e));
   return 0;
 }
 
 inline int run_field_tc(nfb_handle* h, int level, const FieldArgs& a, cudaStream_t s) {
-  const long long pairs = (a.num_rows + kPairRows - 1) / kPairRows;
-  const int grid = (int)std::min<long long>(pairs, h->sm_count);
-  // NFB_TC_EPI_WARPS=8|16 selects the epilogue width (default: see kDefaultEpiWarps).
-  // Developer builds only (-DNFB_DEV_KNOBS, tools/build_variant.py): the release library reads
-  // no environment variables.  NFB_TC_PAIR=1|2 selects the CTA-pair (cta_group::2) variants.
-#ifdef NFB_DEV_KNOBS
-  static const int epi_warps = getenv("NFB_TC_EPI_WARPS") ? atoi(getenv("NFB_TC_EPI_WARPS")) : kDefaultEpiWarps;
-  const char* pair_env = getenv("NFB_TC_PAIR");
-  const int pair_mode = pair_env ? atoi(pair_env) : 0;
-#else
-  const int epi_warps = kDefaultEpiWarps, pair_mode = 0;
-#endif
-  if (pair_mode == 1 || pair_mode == 2) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(h->sm_count & ~1)); cfg.blockDim = dim3(kTcThreads);
-    cfg.dynamicSmemBytes = kTcSmemBytes; cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    // persistent kernel: no more clusters than can be co-resident (GPCs with an odd
-    // number of free SMs leave one SM without a partner)
-    static int max_clusters = -1;
-    if (max_clusters < 0) {
-      int n = 0;
-      if (cudaOccupancyMaxActiveClusters(&n, field_tc_kernel<1, 1>, &cfg) != cudaSuccess || n < 1)
-        return fail("cudaOccupancyMaxActiveClusters failed for the CTA-pair kernel: %s", cudaGetErrorString(cudaGetLastError()));
-      max_clusters = n;
-    }
-    const int grid2 = 2 * (int)std::min<long long>((pairs + 1) / 2, max_clusters);
-    cfg.gridDim = dim3((unsigned)grid2);
-    auto kern = pair_mode == 2 ? field_tc_kernel<1, 2> : field_tc_kernel<1, 1>;
-    cudaError_t le = cudaLaunchKernelEx(&cfg, kern, h->tcprog[level], h->tcbias[level], a,
-                                        (const uint8_t*)h->d_wpack, (const float*)h->d_aux, (int)pairs);
-    if (le != cudaSuccess) return fail("field_tc_kernel (CTA pair) launch failed: %s", cudaGetErrorString(le));
-    h->launches++;
-    return 0;
-  }
-  if (epi_warps == 16)
-    field_tc_kernel<2><<<grid, kTcThreads16, kTcSmemBytes, s>>>(h->tcprog[level], h->tcbias[level], a, h->d_wpack, h->d_aux, (int)pairs);
+  const long long tiles = (a.num_rows + kTileRows - 1) / kTileRows;
+  if (tiles > 0x7fffffffLL) return fail("too many rows for one launch");
+  const bool fuse = a.ray_out != nullptr && !a.warp_only;
+  if (fuse && (a.samples_per_ray % kTileRows != 0 || a.num_rows % a.samples_per_ray != 0))
+    return fail("fused composite needs samples_per_ray to be a multiple of %d", kTileRows);
+  const long long groups = fuse ? a.num_rows / a.samples_per_ray : tiles;
+  const int grid = (int)std::min<long long>(groups, h->sm_count);
+  if (h->cfg.precision == NFB_PREC_FP16X3)
+    field_wg_kernel<true><<<grid, kWgThreads, kWgSmemBytes, s>>>(h->tcprog[level], a, h->d_wpack, h->d_aux, (int)tiles);
   else
-    field_tc_kernel<1><<<grid, kTcThreads, kTcSmemBytes, s>>>(h->tcprog[level], h->tcbias[level], a, h->d_wpack, h->d_aux, (int)pairs);
+    field_wg_kernel<false><<<grid, kWgThreads, kWgSmemBytes, s>>>(h->tcprog[level], a, h->d_wpack, h->d_aux, (int)tiles);
   cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail("field_tc_kernel launch failed: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail("field_wg_kernel launch failed: %s", cudaGetErrorString(e));
   h->launches++;
   return 0;
 }

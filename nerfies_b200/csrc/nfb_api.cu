@@ -18,8 +18,6 @@
 #include "camera_kernels.cuh"
 #include "tc_common.cuh"
 #include "tc_selftest.cuh"
-#include "tc_selftest2.cuh"
-#include "tc_selftest3.cuh"
 #ifdef NFB_WITH_TC
 #include "field_tc.cuh"
 #include "field_tc3.cuh"
@@ -370,7 +368,6 @@ int run_field(nfb_handle* h, int level, long long rows, int S, const float* orig
   a.cond = h->d_cond; a.window = h->d_window; a.samples = samples; a.warped = warped;
   a.num_rows = rows; a.samples_per_ray = S; a.use_warp = use_warp; a.warp_only = warp_only;
   a.fast_encode = h->cfg.precision == NFB_PREC_BF16;
-  a.trace = h->trace; a.trace_cap = h->trace_cap;
 #ifdef NFB_DEV_KNOBS
   {
     // developer builds only: timing experiments whose results are garbage (see FieldArgs::debug)
@@ -388,10 +385,9 @@ int run_field(nfb_handle* h, int level, long long rows, int S, const float* orig
     rc = launch_check(h, "field_simt_kernel");
   } else {
 #ifdef NFB_WITH_TC
-    rc = h->cfg.precision == NFB_PREC_FP16X3 ? nfb::tc3::run_field_x3(h, level, a, s)
-                                             : nfb::tc::run_field_tc(h, level, a, s);
+    rc = nfb::tc::run_field_tc(h, level, a, s);
 #else
-    rc = fail("precision %d needs the tcgen05 path, which this build does not contain", h->cfg.precision);
+    rc = fail("precision %d needs the tensor-core path, which this build does not contain", h->cfg.precision);
 #endif
   }
   if (prof && rc == 0) {
@@ -430,7 +426,7 @@ int run_resample(nfb_handle* h, int B, const float* zc, const float* wc, const f
   return launch_check(h, "resample_kernel");
 }
 
-// The tcgen05 kernels never trap on a protocol error (see tc_common.cuh,
+// The tensor-core kernels never trap on a protocol error (see tc_common.cuh,
 // mbar_wait): they raise a flag in mapped pinned host memory instead.  One int per
 // process; every device's copy of the g_nfb_abort symbol points at it.
 int* g_abort_host = nullptr;
@@ -456,7 +452,7 @@ int ensure_abort_flag() {
 
 int abort_check() {
   if (g_abort_host && *reinterpret_cast<volatile int*>(g_abort_host))
-    return fail("a tcgen05 kernel aborted: an mbarrier wait timed out (protocol error); its results are invalid "
+    return fail("a tensor-core kernel aborted: an mbarrier wait timed out (protocol error); its results are invalid "
                 "and tensor-core launches are refused until nfb_reset_abort()");
   return 0;
 }
@@ -487,7 +483,7 @@ int check_call(nfb_handle* h, int B) {
 extern "C" {
 
 const char* nfb_last_error(void) { return g_error.c_str(); }
-const char* nfb_version(void) { return "nerfies_b200 0.1 sm_100a"; }
+const char* nfb_version(void) { return "nerfies_b200 0.1 sm_90a"; }
 long long nfb_kernel_launches(const nfb_handle* h) { return h ? h->launches : 0; }
 
 static int launch_camera(const nfb_camera* cam, const float* pixels_in, long long first, long long count,
@@ -532,10 +528,8 @@ int nfb_pixels_to_rays(const nfb_camera* cam, const float* pixels, long long n, 
 
 int nfb_set_trace(nfb_handle* h, long long* buffer, int capacity) {
   if (!h) return fail("null handle");
-#ifndef NFB_TRACE
-  if (buffer) return fail("this build carries no tracer; rebuild with -DNFB_TRACE (tools/build_variant.py)");
-#endif
-  h->trace = buffer; h->trace_cap = buffer ? capacity : 0;
+  (void)capacity;
+  if (buffer) return fail("this build carries no tracer");
   return 0;
 }
 
@@ -585,73 +579,12 @@ int nfb_reset_abort(void) {
   return 0;
 }
 
-int nfb_selftest_gemm(int K, int N, const float* A, const float* W, float* C, void* stream) {
+static int selftest_gemm(bool x3, int K, int N, const float* A, const float* W, float* C, int reps, long long* out,
+                         cudaStream_t s) {
   using namespace nfb::tc;
   if (K < 1 || K > kSelfMaxKb * kBlockK || N < 1 || N > 256) return fail("selftest: K<=320, N<=256");
+  if (reps < 1) return fail("selftest: reps must be >= 1");
   if (ensure_abort_flag() || abort_check()) return -1;
-  cudaStream_t s = (cudaStream_t)stream;
-  const int nkb = (K + kBlockK - 1) / kBlockK;
-  const int n_rows = (N + 15) / 16 * 16;
-  std::vector<int> k_map(nkb * kBlockK, -1);
-  for (int k = 0; k < K; ++k) k_map[k] = k;
-  int* d_map = nullptr;
-  __nv_bfloat16* d_w = nullptr;
-  NFB_CUDA(cudaMalloc(&d_map, k_map.size() * sizeof(int)));
-  NFB_CUDA(cudaMalloc(&d_w, (size_t)nkb * n_rows * kRowBytes));
-  NFB_CUDA(cudaMemcpyAsync(d_map, k_map.data(), k_map.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-  const long long total = (long long)nkb * n_rows * kBlockK;
-  pack_weight_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(W, N, d_map, nkb, N, n_rows, d_w);
-  NFB_CUDA(cudaFuncSetAttribute(tc_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSelfSmemBytes));
-  tc_selftest_kernel<<<1, 160, kSelfSmemBytes, s>>>(A, K, d_w, nkb, n_rows, N, C);
-  cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  cudaFree(d_map);
-  cudaFree(d_w);
-  if (e != cudaSuccess) return fail("selftest kernel failed: %s", cudaGetErrorString(e));
-  return abort_check();
-}
-
-int nfb_selftest_gemm2(int K, int N, const float* A, const float* W, float* C, int reps, long long* out,
-                       void* stream) {
-  using namespace nfb::tc;
-  if (K < 1 || K > kSelfMaxKb * kBlockK || (N != 64 && N != 128 && N != 256)) return fail("selftest2: K<=320, N in {64,128,256}");
-  if (reps < 1) return fail("selftest2: reps must be >= 1");
-  if (ensure_abort_flag() || abort_check()) return -1;
-  cudaStream_t s = (cudaStream_t)stream;
-  const int nkb = (K + kBlockK - 1) / kBlockK;
-  std::vector<int> k_map(nkb * kBlockK, -1);
-  for (int k = 0; k < K; ++k) k_map[k] = k;
-  int* d_map = nullptr;
-  __nv_bfloat16* d_w = nullptr;
-  long long* d_out = nullptr;
-  NFB_CUDA(cudaMalloc(&d_map, k_map.size() * sizeof(int)));
-  NFB_CUDA(cudaMalloc(&d_w, (size_t)nkb * N * kRowBytes));
-  NFB_CUDA(cudaMalloc(&d_out, 2 * sizeof(long long)));
-  NFB_CUDA(cudaMemsetAsync(d_out, 0, 2 * sizeof(long long), s));
-  NFB_CUDA(cudaMemcpyAsync(d_map, k_map.data(), k_map.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-  const long long total = (long long)nkb * N * kBlockK;
-  pack_weight_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(W, N, d_map, nkb, N, N, d_w);
-  NFB_CUDA(cudaFuncSetAttribute(tc_selftest2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSelf2SmemBytes));
-  tc_selftest2_kernel<<<2, 160, kSelf2SmemBytes, s>>>(A, K, d_w, nkb, N, C, reps, d_out);
-  cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  long long h_out[2] = {0, 0};
-  if (e == cudaSuccess) e = cudaMemcpy(h_out, d_out, sizeof(h_out), cudaMemcpyDeviceToHost);
-  cudaFree(d_map); cudaFree(d_w); cudaFree(d_out);
-  if (e != cudaSuccess) return fail("selftest2 kernel failed: %s", cudaGetErrorString(e));
-  if (out) { out[0] = h_out[0]; out[1] = h_out[1]; }
-  return abort_check();
-}
-
-int nfb_selftest_gemm3(int K, int N, const float* A, const float* W, float* C, int reps, long long* out,
-                       void* stream) {
-  using namespace nfb::tc;
-  if (K < 1 || K > kSelf3MaxKb * kBlockK || N < 1 || N > 256) return fail("selftest3: K<=256, N<=256");
-  if (reps < 1) return fail("selftest3: reps must be >= 1");
-  if ((long long)((K + kBlockK - 1) / kBlockK) * 2 * ((N + 15) / 16 * 16) * kRowBytes > kSelf3WBytes)
-    return fail("selftest3: the packed weights must fit %d bytes of shared memory", kSelf3WBytes);
-  if (ensure_abort_flag() || abort_check()) return -1;
-  cudaStream_t s = (cudaStream_t)stream;
   const int nkb = (K + kBlockK - 1) / kBlockK;
   const int n_rows = (N + 15) / 16 * 16;
   std::vector<int> k_map(nkb * kBlockK, -1);
@@ -661,53 +594,46 @@ int nfb_selftest_gemm3(int K, int N, const float* A, const float* W, float* C, i
   long long* d_out = nullptr;
   float* d_max = nullptr;
   NFB_CUDA(cudaMalloc(&d_map, k_map.size() * sizeof(int)));
-  NFB_CUDA(cudaMalloc(&d_w, (size_t)nkb * 2 * n_rows * kRowBytes));
+  NFB_CUDA(cudaMalloc(&d_w, (size_t)nkb * (x3 ? 2 : 1) * n_rows * kRowBytes));
   NFB_CUDA(cudaMalloc(&d_out, 2 * sizeof(long long)));
   NFB_CUDA(cudaMalloc(&d_max, sizeof(float)));
   NFB_CUDA(cudaMemsetAsync(d_out, 0, 2 * sizeof(long long), s));
   NFB_CUDA(cudaMemsetAsync(d_max, 0, sizeof(float), s));
   NFB_CUDA(cudaMemcpyAsync(d_map, k_map.data(), k_map.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-  absmax_kernel<<<32, 256, 0, s>>>(W, (long long)K * N, d_max);
   const long long total = (long long)nkb * n_rows * kBlockK;
-  pack_weight_x3_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(W, N, d_map, nkb, N, n_rows, d_max, d_w);
-  float h_max = 0.f;
-  NFB_CUDA(cudaMemcpyAsync(&h_max, d_max, sizeof(float), cudaMemcpyDeviceToHost, s));
-  NFB_CUDA(cudaStreamSynchronize(s));
-  const float inv_scale = 1.f / x3_weight_scale(h_max) / (float)reps;
-  NFB_CUDA(cudaFuncSetAttribute(tc_selftest3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSelf3SmemBytes));
-  tc_selftest3_kernel<<<1, 160, kSelf3SmemBytes, s>>>(A, K, d_w, nkb, n_rows, N, inv_scale, C, reps, d_out);
+  float scale = 1.f;
+  if (x3) {
+    absmax_kernel<<<32, 256, 0, s>>>(W, (long long)K * N, d_max);
+    pack_weight_x3_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(W, N, d_map, nkb, N, n_rows, d_max, d_w);
+    float h_max = 0.f;
+    NFB_CUDA(cudaMemcpyAsync(&h_max, d_max, sizeof(float), cudaMemcpyDeviceToHost, s));
+    NFB_CUDA(cudaStreamSynchronize(s));
+    scale = 1.f / x3_weight_scale(h_max) / (float)reps;
+    NFB_CUDA(cudaFuncSetAttribute(tc_selftest_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSelfSmemBytes));
+    tc_selftest_kernel<true><<<1, 128, kSelfSmemBytes, s>>>(A, K, d_w, nkb, n_rows, N, scale, reps, C, d_out);
+  } else {
+    pack_weight_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(W, N, d_map, nkb, N, n_rows,
+                                                                      reinterpret_cast<__nv_bfloat16*>(d_w));
+    NFB_CUDA(cudaFuncSetAttribute(tc_selftest_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSelfSmemBytes));
+    tc_selftest_kernel<false><<<1, 128, kSelfSmemBytes, s>>>(A, K, d_w, nkb, n_rows, N, scale, reps, C, d_out);
+  }
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) e = cudaStreamSynchronize(s);
   long long h_out[2] = {0, 0};
   if (e == cudaSuccess) e = cudaMemcpy(h_out, d_out, sizeof(h_out), cudaMemcpyDeviceToHost);
   cudaFree(d_map); cudaFree(d_w); cudaFree(d_out); cudaFree(d_max);
-  if (e != cudaSuccess) return fail("selftest3 kernel failed: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail("selftest kernel failed: %s", cudaGetErrorString(e));
   if (out) { out[0] = h_out[0]; out[1] = h_out[1]; }
   return abort_check();
 }
 
-int nfb_selftest_microbench(int mode, int n, int reps, int nwarps, long long* out) {
-  using namespace nfb::tc;
-  if (!out || n < 16 || n > 256 || n % 16) return fail("microbench: bad arguments");
-  if (ensure_abort_flag() || abort_check()) return -1;
-  long long* d = nullptr;
-  unsigned char* g = nullptr;
-  NFB_CUDA(cudaMalloc(&d, 4 * sizeof(long long)));
-  NFB_CUDA(cudaMemset(d, 0, 4 * sizeof(long long)));
-  NFB_CUDA(cudaMalloc(&g, 8 * 16384));
-  NFB_CUDA(cudaMemset(g, 0, 8 * 16384));
-  const int smem = ((mode & 255) >= 4 && (mode & 255) <= 6) ? 224 * 1024 : 7 * 16384;
-  NFB_CUDA(cudaFuncSetAttribute(tc_microbench_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  // mode bits 9..: grid size minus one (chip-wide contention experiments)
-  const int grid = (mode >> 9) + 1;
-  mode &= 511;
-  tc_microbench_kernel<<<grid, 320, smem>>>(mode, n, reps, nwarps, d, g, smem / 4);
-  cudaError_t e = cudaDeviceSynchronize();
-  cudaFree(g);
-  if (e == cudaSuccess) e = cudaMemcpy(out, d, 3 * sizeof(long long), cudaMemcpyDeviceToHost);
-  cudaFree(d);
-  if (e != cudaSuccess) return fail("microbench failed: %s", cudaGetErrorString(e));
-  return abort_check();
+int nfb_selftest_gemm(int K, int N, const float* A, const float* W, float* C, void* stream) {
+  return selftest_gemm(false, K, N, A, W, C, 1, nullptr, (cudaStream_t)stream);
+}
+
+int nfb_selftest_gemm3(int K, int N, const float* A, const float* W, float* C, int reps, long long* out,
+                       void* stream) {
+  return selftest_gemm(true, K, N, A, W, C, reps, out, (cudaStream_t)stream);
 }
 
 int nfb_create(const nfb_config* cfg, int max_rays, nfb_handle** out) {
@@ -726,7 +652,7 @@ int nfb_create(const nfb_config* cfg, int max_rays, nfb_handle** out) {
   if (cudaGetDevice(&h->device) != cudaSuccess) return bail(fail("cudaGetDevice failed"));
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, h->device) != cudaSuccess) return bail(fail("cudaGetDeviceProperties failed"));
-  if (prop.major != 10) return bail(fail("device is sm_%d%d; this library is built for sm_100a only", prop.major, prop.minor));
+  if (prop.major != 9) return bail(fail("device is sm_%d%d; this library is built for sm_90a only", prop.major, prop.minor));
   h->sm_count = prop.multiProcessorCount;
   if (ensure_abort_flag()) return bail(-1);
   if (build_programs(h)) return bail(-1);
@@ -756,7 +682,6 @@ int nfb_create(const nfb_config* cfg, int max_rays, nfb_handle** out) {
   cudaFuncSetAttribute(nfb::resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
 #ifdef NFB_WITH_TC
   if (c.precision != NFB_PREC_FP32 && nfb::tc::create_tc(h)) return bail(-1);
-  if (c.precision == NFB_PREC_FP16X3 && nfb::tc3::create_x3(h)) return bail(-1);
 #endif
   *out = h;
   return 0;

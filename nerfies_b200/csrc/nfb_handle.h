@@ -85,7 +85,7 @@ struct nfb_handle {
   cudaEvent_t ev[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};
   bool ev_valid[2] = {false, false};
   int cond_stride = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   nfb::Net time_net{};                // TimeEncoder MLP ('time' / 'blend' warp metadata encoders)
   float time_alpha = 0.f;             // warp_extra['time_alpha'] (nfb_set_time_alpha)
   cudaStream_t last_stream = nullptr;  // stream of the previous call (see enter_stream)
@@ -97,19 +97,13 @@ struct nfb_handle {
   float *d_dcond = nullptr, *d_tr_out = nullptr, *d_tr_w = nullptr, *d_loss = nullptr;
   float* d_ttape = nullptr; long long ttape_floats = 0;     // tangent tape (train_reg.cuh)
   int* d_sel = nullptr; long long sel_cap = 0;              // selected tape rows (median-depth samples)
-  int x3_pair_ok = -1;                // fp16x3 CTA-pair launch: -1 unknown, 0 unavailable, n = co-resident clusters
   int debug_bits = 0;                 // FieldArgs::debug bits set through the test hook (abort-path test)
-  long long* trace = nullptr;
-  int trace_cap = 0;
   // tensor-core path (precision != fp32)
   nfb::tc::TcProgram tcprog[2];
-  nfb::tc::TcBias tcbias[2];          // host copy of the per-step biases (kernel parameter)
-  nfb::tc::X3Consts x3c[2];           // fp16x3 mode: biases + alpha head (kernel parameter)
-  unsigned char* d_wpack = nullptr;   // bf16 weight units, shared-memory image
+  unsigned char* d_wpack = nullptr;   // weight units, shared-memory image (bf16, or fp16 hi | lo)
   float* d_aux = nullptr;             // fp32 biases + alpha head
   long long wpack_bytes = 0, aux_floats = 0;
-  struct TcPackJob { int level, step, chunk; int simt_w_off, ld, n, n0, k_total; std::vector<int> k_map;
-                     std::vector<int> unit_pos; };   // fp16x3: issue-order position of each K-block's unit within the step
+  struct TcPackJob { int level, step, chunk; int simt_w_off, ld, n, n0, k_total; std::vector<int> k_map; };
   std::vector<TcPackJob> tc_jobs;
   struct TcAuxJob { int src_off, count, stride, dst_off; };
   std::vector<TcAuxJob> tc_aux_jobs;

@@ -1,14 +1,14 @@
-// tcgen05 / TMEM / mbarrier / bulk-copy primitives (inline PTX, sm_100a) and
-// the shared-memory operand format used by the tensor-core field kernel.
+// mbarrier / bulk-copy / wgmma primitives (inline PTX, sm_90a) and the
+// shared-memory operand format used by the tensor-core field kernel.
 //
-// Operand format ("K-major, 128-byte swizzle", the UMMA canonical layout
+// Operand format ("K-major, 128-byte swizzle", the GMMA canonical layout
 // Swizzle<3,4,3> o ((8,m),(8,2)) of 16-byte units): an operand with R rows and
-// K columns of bf16 is cut into K-blocks of 64 columns.  One K-block is R rows
-// of 128 bytes; inside each row the eight 16-byte chunks are XOR-permuted with
+// K columns of bf16 / fp16 is cut into K-blocks of 64 columns.  One K-block is R
+// rows of 128 bytes; inside each row the eight 16-byte chunks are XOR-permuted with
 // (row & 7).  Blocks start on 1024-byte boundaries, 8-row groups are 1024 bytes
-// apart (the descriptor's stride byte offset).  One tcgen05.mma consumes K=16
-// (32 bytes of every row), so stepping K inside a block adds 32 bytes to the
-// descriptor's start address.
+// apart (the descriptor's stride byte offset).  One wgmma consumes K=16 (32 bytes
+// of every row), so stepping K inside a block adds 32 bytes to the descriptor's
+// start address.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -32,9 +32,7 @@ __device__ __host__ __forceinline__ uint32_t swz_off(int row, int chunk) {
   return (uint32_t)(row * kRowBytes + ((chunk ^ (row & 7)) << 4));
 }
 
-// Warp-uniform leader election (elect.sync).  Control flow stays uniform for the
-// whole warp, so the compiler keeps descriptors in uniform registers instead of
-// wrapping every tcgen05 instruction in a divergence "waterfall" loop.
+// Warp-uniform leader election (elect.sync): control flow stays uniform for the whole warp.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
   asm volatile(
@@ -45,7 +43,6 @@ __device__ __forceinline__ bool elect_one() {
       : "r"(0xffffffffu));
   return pred != 0;
 }
-
 // ---- mbarrier ----------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -72,85 +69,32 @@ __device__ int* g_nfb_abort = nullptr;
 // abort flag, marks itself `dead` and returns; a dead thread returns from every
 // later wait at once.  All roles of a CTA wait concurrently, so their time-outs
 // expire together and the kernel drains; the host API then reports the error.
-// Deliberately no __trap()/printf here: trap exits inside the epilogue keep ptxas
-// from allocating the registers that setmaxnreg.inc hands to those warpgroups, and
-// the spin loop is four PTX instructions (it sits on every hand-off's critical path).
-template <bool kBusyPoll>
-__device__ __forceinline__ void mbar_wait_impl(uint64_t* bar, uint32_t parity, uint32_t& dead) {
+// Deliberately no __trap()/printf here: trap exits inside the consumer warpgroups keep
+// ptxas from allocating the registers that setmaxnreg.inc hands to them.
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, uint32_t& dead) {
   if (dead) return;
   const uint32_t addr = smem_u32(bar);
   uint32_t done;
   constexpr uint32_t kWaitProbes = 1u << 22;
-  if (kBusyPoll) {
-    // test_wait never suspends the thread: lowest wake-up latency, burns issue slots.
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .u32 n;\n\t"
-        "mov.u32 n, 0;\n"
-        "NFB_W: mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "@p bra NFB_D;\n\t"
-        "add.u32 n, n, 1;\n\t"
-        "setp.ne.u32 p, n, %3;\n\t"
-        "@p bra NFB_W;\n\t"
-        "setp.eq.u32 p, n, 0;\n"
-        "NFB_D: selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(addr), "r"(parity), "r"(kWaitProbes * 16)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .u32 n;\n\t"
-        "mov.u32 n, 0;\n"
-        "NFB_W: mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "@p bra NFB_D;\n\t"
-        "add.u32 n, n, 1;\n\t"
-        "setp.ne.u32 p, n, %3;\n\t"
-        "@p bra NFB_W;\n\t"
-        "setp.eq.u32 p, n, 0;\n"
-        "NFB_D: selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(addr), "r"(parity), "r"(kWaitProbes)
-        : "memory");
-  }
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .u32 n;\n\t"
+      "mov.u32 n, 0;\n"
+      "NFB_W: mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+      "@p bra NFB_D;\n\t"
+      "add.u32 n, n, 1;\n\t"
+      "setp.ne.u32 p, n, %3;\n\t"
+      "@p bra NFB_W;\n\t"
+      "setp.eq.u32 p, n, 0;\n"
+      "NFB_D: selp.u32 %0, 1, 0, p;\n\t}"
+      : "=r"(done)
+      : "r"(addr), "r"(parity), "r"(kWaitProbes)
+      : "memory");
   if (!done) {                       // time-out: raise the abort flag, give up for good
     volatile int* ab = g_nfb_abort;
     if (ab) *ab = 1;
     dead = 1;
   }
 }
-#ifdef NFB_WAIT_TEST
-constexpr bool kEpiBusyPoll = true;
-#else
-constexpr bool kEpiBusyPoll = false;
-#endif
-#if defined(NFB_WAIT_TEST) || defined(NFB_WAIT_TEST_ISSUER)
-constexpr bool kIssuerBusyPoll = true;
-#else
-constexpr bool kIssuerBusyPoll = false;
-#endif
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, uint32_t& dead) {
-  mbar_wait_impl<kEpiBusyPoll>(bar, parity, dead);
-}
-__device__ __forceinline__ void mbar_wait_issuer(uint64_t* bar, uint32_t parity, uint32_t& dead) {
-  mbar_wait_impl<kIssuerBusyPoll>(bar, parity, dead);
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t dead = 0;
-  mbar_wait(bar, parity, dead);
-}
-
-// Non-blocking probe of a phase (true = complete).
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
-  uint32_t done;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(done)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return done != 0;
-}
-
 // ---- bulk async copy (TMA engine, 1-D) -----------------------------------------
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes,
                                          uint64_t* bar) {
@@ -160,378 +104,90 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
       "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
       : "memory");
 }
-// Same, delivered to the same shared-memory offset (and mbarrier) of every CTA in `mask`.
-__device__ __forceinline__ void bulk_g2s_multicast(void* smem_dst, const void* gmem_src, uint32_t bytes,
-                                                   uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::
-          "r"(smem_u32(smem_dst)),
-      "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "h"(mask)
-      : "memory");
-}
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// ---- TMEM ----------------------------------------------------------------------
-// Warp-collective.  Writes the allocated base address to *smem_slot.
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_slot)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// 32 consecutive accumulator columns of this thread's TMEM lane.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// 16 packed 32-bit values -> 16 consecutive TMEM columns of this thread's lane.
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// ---- UMMA descriptors ----------------------------------------------------------
-// Shared-memory matrix descriptor: K-major, SWIZZLE_128B, 8-row groups 1024 B
-// apart (cute::UMMA::SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout_type=2 [61,64)).
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
+// ---- wgmma (warpgroup MMA, sm_90a) ----------------------------------------------
+// Shared-memory matrix descriptor: K-major, SWIZZLE_128B, 8-row groups 1024 B apart
+// (GMMA descriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), layout [62,64) = 1).
+__device__ __forceinline__ uint64_t make_wg_desc(uint32_t saddr) {
   uint64_t d = (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;           // leading byte offset (unused for swizzled K-major)
-  d |= (uint64_t)(1024 >> 4) << 32; // stride byte offset
-  d |= (uint64_t)1 << 46;           // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;           // SWIZZLE_128B
+  d |= (uint64_t)1 << 16;            // leading byte offset (unused for swizzled K-major)
+  d |= (uint64_t)(1024 >> 4) << 32;  // stride byte offset
+  d |= (uint64_t)1 << 62;            // SWIZZLE_128B
   return d;
 }
-// Instruction descriptor for kind::f16, bf16 x bf16 -> f32, both K-major
-// (cute::UMMA::InstrDescriptor: c_format [4,6)=1, a_format [7,10)=1,
-// b_format [10,13)=1, n>>3 [17,23), m>>4 [24,29)).
-__device__ __host__ __forceinline__ uint32_t make_idesc_bf16(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) |
-         ((uint32_t)(m >> 4) << 24);
-}
-// Same for fp16 x fp16 -> f32 (operand format 0).
-__device__ __host__ __forceinline__ uint32_t make_idesc_f16(int m, int n) {
-  return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-// D[tmem] (+)= A[smem] * B[smem]; issued by one thread.
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrives on `bar` when every tcgen05.mma issued so far by this thread is done.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving accumulator reads across a wgmma wait.
+template <int N>
+__device__ __forceinline__ void wg_fence_regs(float* d) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// One weight unit of the fused field kernel, issued by a single thread as ONE
-// instruction block: tcgen05.fence, non-blocking probes of the barriers the NEXT
-// unit will need, 8 tcgen05.mma (4 K-slices x 2 sub-tiles), the commits - and
-// only then the probe results are read.  mbarrier probes cost 90-150 cycles and
-// the tensor queue is shallow, so a probe *between* units would idle the pipe;
-// here it is in flight while the MMAs queue.
-//   bar_* are shared-memory addresses (0 = skip); returns bit0/1/2 = the probed
-//   weight / x_ready[0] / x_ready[1] phase is complete.
-template <bool kOptionalCommits>
-__device__ __forceinline__ uint32_t issue_unit(uint32_t d0, uint32_t d1, uint64_t ad0, uint64_t ad1,
-                                               uint64_t bd, uint32_t idesc, uint32_t accumulate,
-                                               uint32_t bar_empty, uint32_t bar_xfree,
-                                               uint32_t bar_acc, uint32_t probe_w, uint32_t par_w,
-                                               uint32_t probe_x0, uint32_t probe_x1, uint32_t par_x) {
-  uint32_t out;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred pacc, pt, pw, px0, px1, pd0, pd1, pcx, pca;\n\t"
-      ".reg .b64 a01, a02, a03, a11, a12, a13, b1, b2, b3;\n\t"
-      ".reg .b32 t0, t1;\n\t"
-      "tcgen05.fence::after_thread_sync;\n\t"
-      "setp.ne.b32 pacc, %7, 0;\n\t"
-      "setp.eq.b32 pt, 0, 0;\n\t"
-      "setp.ne.b32 pd0, %13, 0;\n\t"
-      "setp.ne.b32 pd1, %14, 0;\n\t"
-      "setp.ne.b32 pcx, %9, 0;\n\t"
-      "setp.ne.b32 pca, %10, 0;\n\t"
-      "setp.eq.b32 px0, 1, 0;\n\t"
-      "setp.eq.b32 px1, 1, 0;\n\t"
-      "add.u64 a01, %3, 2;\n\t add.u64 a02, %3, 4;\n\t add.u64 a03, %3, 6;\n\t"
-      "add.u64 a11, %4, 2;\n\t add.u64 a12, %4, 4;\n\t add.u64 a13, %4, 6;\n\t"
-      "add.u64 b1, %5, 2;\n\t add.u64 b2, %5, 4;\n\t add.u64 b3, %5, 6;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%1], %3, %5, %6, pacc;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%1], a01, b1, %6, pt;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%1], a02, b2, %6, pt;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%1], a03, b3, %6, pt;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%2], %4, %5, %6, pacc;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%2], a11, b1, %6, pt;\n\t"
-      // probes as late as their ~150-cycle latency allows: two MMAs (128 cycles of
-      // queue) still follow, and the later the probe the likelier the copy has landed
-      "mbarrier.test_wait.parity.shared::cta.b64 pw, [%11], %12;\n\t"
-      "@pd0 mbarrier.test_wait.parity.shared::cta.b64 px0, [%13], %15;\n\t"
-      "@pd1 mbarrier.test_wait.parity.shared::cta.b64 px1, [%14], %15;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%2], a12, b2, %6, pt;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%2], a13, b3, %6, pt;\n\t"
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%8];\n\t"
-      // A tcgen05.commit occupies an issue slot behind the MMAs (~120 cycles measured)
-      // even when predicated off: branch around the optional ones.
-      "@pcx tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%9];\n\t"
-      "@pca tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%10];\n\t"
-      "selp.u32 %0, 1, 0, pw;\n\t"
-      "selp.u32 t0, 2, 0, px0;\n\t"
-      "selp.u32 t1, 4, 0, px1;\n\t"
-      "or.b32 %0, %0, t0;\n\t"
-      "or.b32 %0, %0, t1;\n\t"
-      "}"
-      : "=r"(out)
-      : "r"(d0), "r"(d1), "l"(ad0), "l"(ad1), "l"(bd), "r"(idesc), "r"(accumulate), "r"(bar_empty),
-        "r"(bar_xfree), "r"(bar_acc), "r"(probe_w), "r"(par_w), "r"(probe_x0), "r"(probe_x1),
-        "r"(par_x)
-      : "memory");
-  return out;
+#define NFB_WG_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), \
+                     "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+// D(64 x 16, fp32 registers) (+)= A(64 x 16, smem) * B(16 x 16, smem)^T
+template <bool kBf16>
+__device__ __forceinline__ void wg_mma_n16(float* d, uint64_t a, uint64_t b, uint32_t accumulate) {
+  if constexpr (kBf16)
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+                 : NFB_WG_D8(0) : "l"(a), "l"(b), "r"(accumulate));
+  else
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+                 : NFB_WG_D8(0) : "l"(a), "l"(b), "r"(accumulate));
 }
+#define NFB_WG_N128_REGS                                                                            \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                        \
+  "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                \
+  "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                \
+  "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+#define NFB_WG_N128_OPS                                                                              \
+  : NFB_WG_D8(0), NFB_WG_D8(8), NFB_WG_D8(16), NFB_WG_D8(24), NFB_WG_D8(32), NFB_WG_D8(40),          \
+    NFB_WG_D8(48), NFB_WG_D8(56)                                                                     \
+  : "l"(a), "l"(b), "r"(accumulate)
+// D(64 x 128, fp32 registers) (+)= A(64 x 16, smem) * B(128 x 16, smem)^T
+template <bool kBf16>
+__device__ __forceinline__ void wg_mma_n128(float* d, uint64_t a, uint64_t b, uint32_t accumulate) {
+  if constexpr (kBf16)
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " NFB_WG_N128_REGS NFB_WG_N128_OPS);
+  else
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " NFB_WG_N128_REGS NFB_WG_N128_OPS);
+}
+#undef NFB_WG_N128_REGS
+#undef NFB_WG_N128_OPS
+#undef NFB_WG_D8
 
-// First half of a unit: fence + the 4 MMAs of sub-tile 0.  The caller does its
-// loop bookkeeping between issue_half0() and issue_half1(): the thread is not
-// needed while these MMAs execute, and the tensor queue is too shallow to bridge
-// a gap *between* units.
-__device__ __forceinline__ void issue_half0(uint32_t d0, uint64_t ad0, uint64_t bd, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred pacc, pt;\n\t"
-      ".reg .b64 a1, a2, a3, b1, b2, b3;\n\t"
-      "tcgen05.fence::after_thread_sync;\n\t"
-      "setp.ne.b32 pacc, %4, 0;\n\t"
-      "setp.eq.b32 pt, 0, 0;\n\t"
-      "add.u64 a1, %1, 2;\n\t add.u64 a2, %1, 4;\n\t add.u64 a3, %1, 6;\n\t"
-      "add.u64 b1, %2, 2;\n\t add.u64 b2, %2, 4;\n\t add.u64 b3, %2, 6;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, pacc;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], a1, b1, %3, pt;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], a2, b2, %3, pt;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], a3, b3, %3, pt;\n\t"
-      "}"
-      ::"r"(d0), "l"(ad0), "l"(bd), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Second half: look-ahead probes, the 4 MMAs of sub-tile 1, commits; returns the
-// probe bits (see issue_unit).
-template <bool kOptionalCommits>
-__device__ __forceinline__ uint32_t issue_half1(uint32_t d1, uint64_t ad1, uint64_t bd, uint32_t idesc,
-                                                uint32_t accumulate, uint32_t bar_empty,
-                                                uint32_t bar_xfree, uint32_t bar_acc, uint32_t probe_w,
-                                                uint32_t par_w, uint32_t probe_x0, uint32_t probe_x1,
-                                                uint32_t probe_x2, uint32_t par_x) {
-  uint32_t out;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred pacc, pt, pw, px0, px1, px2, pd0, pd1, pd2, pcx, pca;\n\t"
-      ".reg .b64 a1, a2, a3, b1, b2, b3;\n\t"
-      ".reg .b32 t0, t1, t2;\n\t"
-      "setp.ne.b32 pacc, %5, 0;\n\t"
-      "setp.eq.b32 pt, 0, 0;\n\t"
-      "setp.ne.b32 pd0, %11, 0;\n\t"
-      "setp.ne.b32 pd1, %12, 0;\n\t"
-      "setp.ne.b32 pd2, %13, 0;\n\t"
-      "setp.ne.b32 pcx, %7, 0;\n\t"
-      "setp.ne.b32 pca, %8, 0;\n\t"
-      "setp.eq.b32 px0, 1, 0;\n\t"
-      "setp.eq.b32 px1, 1, 0;\n\t"
-      "setp.eq.b32 px2, 1, 0;\n\t"
-      "add.u64 a1, %2, 2;\n\t add.u64 a2, %2, 4;\n\t add.u64 a3, %2, 6;\n\t"
-      "add.u64 b1, %3, 2;\n\t add.u64 b2, %3, 4;\n\t add.u64 b3, %3, 6;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%1], %2, %3, %4, pacc;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%1], a1, b1, %4, pt;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 pw, [%9], %10;\n\t"
-      "@pd0 mbarrier.test_wait.parity.shared::cta.b64 px0, [%11], %14;\n\t"
-      "@pd1 mbarrier.test_wait.parity.shared::cta.b64 px1, [%12], %14;\n\t"
-      "@pd2 mbarrier.test_wait.parity.shared::cta.b64 px2, [%13], %14;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%1], a2, b2, %4, pt;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%1], a3, b3, %4, pt;\n\t"
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%6];\n\t"
-      "@pcx tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%7];\n\t"
-      "@pca tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%8];\n\t"
-      "selp.u32 %0, 1, 0, pw;\n\t"
-      "selp.u32 t0, 2, 0, px0;\n\t"
-      "selp.u32 t1, 4, 0, px1;\n\t"
-      "selp.u32 t2, 8, 0, px2;\n\t"
-      "or.b32 %0, %0, t0;\n\t"
-      "or.b32 %0, %0, t1;\n\t"
-      "or.b32 %0, %0, t2;\n\t"
-      "}"
-      : "=r"(out)
-      : "r"(d1), "l"(ad1), "l"(bd), "r"(idesc), "r"(accumulate), "r"(bar_empty), "r"(bar_xfree),
-        "r"(bar_acc), "r"(probe_w), "r"(par_w), "r"(probe_x0), "r"(probe_x1), "r"(probe_x2),
-        "r"(par_x)
-      : "memory");
-  return out;
-}
-
-// ---- CTA-pair (cta_group::2) variants of the two issue blocks -------------------
-// Same structure as issue_half0 / issue_half1; the MMAs are M = 256 across the two
-// CTAs of the cluster and every commit is multicast to the barrier at the same
-// shared-memory offset in both CTAs.
-__device__ __forceinline__ void issue_half0_pair(uint32_t d0, uint64_t ad0, uint64_t bd, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred pacc, pt;\n\t"
-      ".reg .b64 a1, a2, a3, b1, b2, b3;\n\t"
-      "tcgen05.fence::after_thread_sync;\n\t"
-      "setp.ne.b32 pacc, %4, 0;\n\t"
-      "setp.eq.b32 pt, 0, 0;\n\t"
-      "add.u64 a1, %1, 2;\n\t add.u64 a2, %1, 4;\n\t add.u64 a3, %1, 6;\n\t"
-      "add.u64 b1, %2, 2;\n\t add.u64 b2, %2, 4;\n\t add.u64 b3, %2, 6;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, pacc;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], a1, b1, %3, pt;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], a2, b2, %3, pt;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], a3, b3, %3, pt;\n\t"
-      "}"
-      ::"r"(d0), "l"(ad0), "l"(bd), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t issue_half1_pair(uint32_t d1, uint64_t ad1, uint64_t bd, uint32_t idesc,
-                                                     uint32_t accumulate, uint32_t bar_empty,
-                                                     uint32_t bar_xfree, uint32_t bar_acc, uint32_t probe_w,
-                                                     uint32_t par_w, uint32_t probe_x0, uint32_t probe_x1,
-                                                     uint32_t probe_x2, uint32_t par_x) {
-  uint32_t out;
-  const uint16_t both = 0x3;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred pacc, pt, pw, px0, px1, px2, pd0, pd1, pd2, pcx, pca;\n\t"
-      ".reg .b64 a1, a2, a3, b1, b2, b3;\n\t"
-      ".reg .b32 t0, t1, t2;\n\t"
-      "setp.ne.b32 pacc, %5, 0;\n\t"
-      "setp.eq.b32 pt, 0, 0;\n\t"
-      "setp.ne.b32 pd0, %11, 0;\n\t"
-      "setp.ne.b32 pd1, %12, 0;\n\t"
-      "setp.ne.b32 pd2, %13, 0;\n\t"
-      "setp.ne.b32 pcx, %7, 0;\n\t"
-      "setp.ne.b32 pca, %8, 0;\n\t"
-      "setp.eq.b32 px0, 1, 0;\n\t"
-      "setp.eq.b32 px1, 1, 0;\n\t"
-      "setp.eq.b32 px2, 1, 0;\n\t"
-      "add.u64 a1, %2, 2;\n\t add.u64 a2, %2, 4;\n\t add.u64 a3, %2, 6;\n\t"
-      "add.u64 b1, %3, 2;\n\t add.u64 b2, %3, 4;\n\t add.u64 b3, %3, 6;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%1], %2, %3, %4, pacc;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%1], a1, b1, %4, pt;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 pw, [%9], %10;\n\t"
-      "@pd0 mbarrier.test_wait.parity.shared::cta.b64 px0, [%11], %14;\n\t"
-      "@pd1 mbarrier.test_wait.parity.shared::cta.b64 px1, [%12], %14;\n\t"
-      "@pd2 mbarrier.test_wait.parity.shared::cta.b64 px2, [%13], %14;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%1], a2, b2, %4, pt;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%1], a3, b3, %4, pt;\n\t"
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%6], %15;\n\t"
-      "@pcx tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%7], %15;\n\t"
-      "@pca tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%8], %15;\n\t"
-      "selp.u32 %0, 1, 0, pw;\n\t"
-      "selp.u32 t0, 2, 0, px0;\n\t"
-      "selp.u32 t1, 4, 0, px1;\n\t"
-      "selp.u32 t2, 8, 0, px2;\n\t"
-      "or.b32 %0, %0, t0;\n\t"
-      "or.b32 %0, %0, t1;\n\t"
-      "or.b32 %0, %0, t2;\n\t"
-      "}"
-      : "=r"(out)
-      : "r"(d1), "l"(ad1), "l"(bd), "r"(idesc), "r"(accumulate), "r"(bar_empty), "r"(bar_xfree),
-        "r"(bar_acc), "r"(probe_w), "r"(par_w), "r"(probe_x0), "r"(probe_x1), "r"(probe_x2),
-        "r"(par_x), "h"(both)
-      : "memory");
-  return out;
-}
-
-// Cluster helpers for the CTA-pair kernels.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// Arrives on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster.
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-  uint32_t raddr;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(smem_u32(bar)), "r"(cta));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(raddr) : "memory");
-}
-// Same without release semantics: for events whose data never passed through this
-// thread (a TMA-filled weight stage observed complete on the local barrier).
-__device__ __forceinline__ void mbar_arrive_remote_relaxed(uint64_t* bar, uint32_t cta) {
-  uint32_t raddr;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(smem_u32(bar)), "r"(cta));
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(raddr) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_slot)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
+// One K-block (64 columns = 4 K-steps) of a warpgroup's 64 rows against one weight
+// unit.  bf16: x W.  fp16x3: per K step x_hi W_hi, x_hi W_lo, x_lo W_hi into the same
+// accumulator.  a_* / b_* are shared-memory byte addresses of the K-block images.
+template <bool kX3, int N>
+__device__ __forceinline__ void wg_unit(float* d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+                                        uint32_t accumulate) {
+  const uint64_t ah = make_wg_desc(a_hi), al = make_wg_desc(a_lo);
+  const uint64_t bh = make_wg_desc(b_hi), bl = make_wg_desc(b_lo);
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    const uint64_t o = (uint64_t)(2 * ks);     // +32 bytes per K step, in 16-byte units
+    const uint32_t acc = (accumulate || ks) ? 1u : 0u;
+    if constexpr (N == 16) {
+      wg_mma_n16<!kX3>(d, ah + o, bh + o, acc);
+      if constexpr (kX3) { wg_mma_n16<false>(d, ah + o, bl + o, 1u); wg_mma_n16<false>(d, al + o, bh + o, 1u); }
+    } else {
+      wg_mma_n128<!kX3>(d, ah + o, bh + o, acc);
+      if constexpr (kX3) { wg_mma_n128<false>(d, ah + o, bl + o, 1u); wg_mma_n128<false>(d, al + o, bh + o, 1u); }
+    }
+  }
 }
 
 // ---- bf16 helpers ---------------------------------------------------------------

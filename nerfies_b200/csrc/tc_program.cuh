@@ -7,77 +7,34 @@ namespace tc {
 
 constexpr int kMaxTcSteps = 24;
 constexpr int kSrcIn = 4;     // K-block source: 0..3 = activation block, 4 = input block
+constexpr int kAlphaCondOff = 256;   // alpha-condition weights, after the 256 trunk weights
 
 enum Epi { kEpiHidden = 0, kEpiWarpHeads = 1, kEpiRgbOut = 2 };
 
-// One Dense layer as a chain of tcgen05.mma over K-blocks of 64 columns.
+// One Dense layer as a chain of wgmma over K-blocks of 64 columns.  A weight unit is
+// one (N-chunk, K-block) pair; units are packed and streamed chunk-major.
 struct TcStep {
-  uint32_t w_off;      // byte offset of the first weight unit (bf16, pre-swizzled)
+  uint32_t w_off;      // byte offset of the first weight unit (pre-swizzled)
   int nkb;             // K-blocks
   int src[6];          // per K-block source
   int n_chunks;        // the N dimension is issued as 1 or 2 chunks ...
-  int chunk_n;         // ... of this many columns (multiple of 16)
+  int chunk_n;         // ... of this many columns (128, or 16 for a head)
   int b_off;           // float offset of the bias (256 floats reserved) in the aux buffer
   int epi;             // Epi
   int relu;            // hidden activation (relu) or identity (bottleneck)
   int alpha_dot;       // this epilogue also accumulates the alpha head (Dense(1))
   int write_cond;      // this epilogue also writes the rgb condition into the input block
-  int kb_free;         // chunk 1 commits "chunk-0 destination blocks are free" after this kb
-};
-
-// The MMA issuer's schedule, flattened: one entry per weight unit (8 MMAs).
-constexpr int kMaxTcUnits = 128;
-enum UnitFlags {
-  kUAccum = 1,          // first MMA accumulates (not the first K-block of the chunk)
-  kUWaitX0 = 2,         // wait x_ready[0] (first unit of a step)
-  kUWaitX1 = 4,         // wait x_ready[1] before this unit
-  kUCommitAcc0 = 8,     // commit acc_ready[0] after this unit
-  kUCommitAcc1 = 16,    // commit acc_ready[1] after this unit
-  kUCommitXFree = 32,   // commit x_free after this unit
-  kUStepEnd = 64,       // last unit of its step
-  kUWaitX2 = 128,       // wait x_ready[2] (second half of the previous chunk-1 epilogue)
-};
-// Everything the issuer needs is precomputed on the host so that the single
-// issuing thread executes as few (serially dependent) instructions as possible
-// between two issue blocks.
-struct TcUnit {
-  uint32_t a0_lo, a1_lo;   // A descriptor low words of sub-tile 0/1, relative to the activation base
-  uint32_t dcol;           // accumulator column offset (sub-tile 0; sub-tile 1 = +256)
-  uint32_t idesc;          // tcgen05 instruction descriptor (M=128, N=chunk)
-  uint32_t flags;          // UnitFlags of this unit
-  uint32_t need;           // look-ahead bits that must be set before issuing: 1 weights | 2/4/8 x_ready[0/1/2]
-  uint32_t probe_next;     // which x_ready barriers the NEXT unit (cyclically) needs: 2 | 4 | 8
-  uint32_t step;
 };
 
 struct TcProgram {
   int n_steps;
   TcStep steps[kMaxTcSteps];
-  int n_units;
-  int unit_begin[kMaxTcSteps + 1];    // first unit of every step
-  TcUnit units[kMaxTcUnits];
   int warp_type, Fw, G, Fp, rc, cond_stride, sigma_act;
+  int tc, ac;                     // trunk / alpha condition widths
+  int ac_off, rc_off;             // offsets of the alpha / rgb condition in the per-ray condition vector
   int warp_pivot, warp_trans;     // SE3Field use_pivot / use_translation
-  int alpha_w_off, alpha_b_off;   // aux float offsets
+  int alpha_w_off, alpha_b_off;   // aux float offsets (alpha weights: trunk part, then the condition part)
   int scale_off;                  // fp16x3: aux offset of the per-step max |W| (kMaxTcSteps floats)
-  uint32_t units_per_pair;        // weight units streamed per tile pair
-};
-
-// Per-step biases (256 floats each), passed as a __grid_constant__ kernel
-// parameter: the epilogue reads them from the constant bank through the uniform
-// datapath instead of through the shared-memory pipe the MMAs are fed from.
-struct alignas(16) TcBias {
-  float4 b4[kMaxTcSteps * 64];
-};
-
-// fp16x3 mode (field_tc3.cuh): per-step biases + the alpha head (Dense(1) on the
-// trunk output) in fp32, read from the kernel-parameter constant bank.
-struct alignas(16) X3Consts {
-  float4 b4[kMaxTcSteps * 64];
-  float4 alpha4[64];
-  float inv_scale[kMaxTcSteps];   // 1 / (power-of-two weight scale of the step), see x3_weight_scale()
-  float alpha_b;
-  float pad[3];
 };
 
 }  // namespace tc

@@ -11,7 +11,7 @@
 //                 dW = [X | IN]^T dZ  (reduction over the rows: split + atomicAdd)
 //   * colsum_kernel (bias gradients), encode / se3 / raw-activation kernels and their
 //     adjoints, the adjoint of volumetric_rendering, embedding scatter-add, Adam.
-// 180 GB of HBM holds the tape of a whole gpu_fullhd training batch (~31 GB); the
+// 80 GB of HBM holds the tape of a whole gpu_fullhd training batch (~31 GB); the
 // caller may still process a batch in ray chunks (gradients accumulate).
 // z_fine is a constant of the fine level (lax.stop_gradient, model_utils.py:211).
 #pragma once

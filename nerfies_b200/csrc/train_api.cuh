@@ -53,7 +53,7 @@ TapeLayout tape_layout(const nfb::FieldProgram& p, long long rows) {
 // Rows per split of a weight-gradient GEMM (reduction over the rows of the batch; the partial tiles are
 // atomicAdd-ed).  The output is tiny (<= 3 x 2 tiles of 128 x 128), so the split count sets the parallelism:
 // aim at ~4 CTAs per resident slot (2 per SM) whatever the layer's width; a fixed 2048 rows left a 128-wide
-// layer of a 131,072-row chunk with 64 CTAs for 148 SMs, 8192 rows measured 3x slower.
+// layer of a 131,072-row chunk with 64 CTAs for 132 SMs, 8192 rows measured 3x slower.
 inline long long dw_split(const nfb_handle* h, long long M, int N, long long K) {
   const long long tiles = ((M + nfb::train::kT2 - 1) / nfb::train::kT2) * ((N + nfb::train::kT2 - 1) / nfb::train::kT2);
   const long long want = std::max<long long>(1, (8LL * h->sm_count) / tiles);   // splits

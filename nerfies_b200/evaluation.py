@@ -8,7 +8,7 @@ are exchanged with ONE all_gather per chunk of the packed 24 B/ray/level result
 (the reference's lax.all_gather, eval.py:339, moves the same values as 4 arrays
 per level).  With device_count == 1 there is no collective.
 
-`render_frame` is the B200-native form of the same job (eval.py:330-353 +
+`render_frame` is the GPU-native form of the same job (eval.py:330-353 +
 datasets/core.py:50-75): every rank generates the rays of its contiguous slab of
 the frame on the GPU (camera_rays_kernel), renders it in large launches, and the
 frame is assembled with a single all_gather of 24 B/ray at the end - instead of
@@ -145,7 +145,7 @@ def render_image(state, rays_dict, model_fn, device_count, rng, chunk=8192,
 
 def render_frame(model, params, camera, warp_extra, metadata=None, max_rays=65536,
                  default_ret_key=None, timings=None):
-  """One full frame from a Camera, B200-native (eval.py:330-353 without the host
+  """One full frame from a Camera, GPU-native (eval.py:330-353 without the host
   loop): rank r renders pixels [r * n, (r + 1) * n) of the row-major frame,
   n = ceil(h * w / world); rays come from camera_rays_kernel on the device
   (datasets/core.py:50-75), the slab is rendered in launches of up to `max_rays`

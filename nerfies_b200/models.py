@@ -1,6 +1,6 @@
 """Host-side mirror of nerfies/models.py: NerfModel / construct_nerf.
 
-The arithmetic runs in libnerfies_b200.so (hand-written sm_100a CUDA) through
+The arithmetic runs in libnerfies_b200.so (hand-written sm_90a CUDA) through
 the C ABI of include/nerfies_b200.h; this module keeps the reference's call
 surface on top of it (SURVEY.md §8b):
 
@@ -307,7 +307,7 @@ class NerfModel:
 
   def handle(self, num_rays: int = 0) -> _Handle:
     if not torch.cuda.is_available():
-      raise RuntimeError('nerfies_b200 needs a CUDA device (sm_100a); there is '
+      raise RuntimeError('nerfies_b200 needs a CUDA device (sm_90a); there is '
                          'no CPU fallback')
     want = max(self.batch_size, num_rays)
     if self._handle is None or self._handle.max_rays < want:
@@ -719,7 +719,7 @@ def construct_nerf(key, config: configs.ModelConfig, batch_size: int,
                    use_warp_jacobian: bool = False, use_weights: bool = False,
                    precision: str = 'fp32', device=None):
   """Same signature and return value as models.construct_nerf
-  (models.py:378-489) plus the B200-only keywords `precision` and `device`.
+  (models.py:378-489) plus the nerfies_b200-only keywords `precision` and `device`.
 
   Note: like the reference, `use_trunk_condition` is NOT forwarded from the
   config (models.py:424-463)."""

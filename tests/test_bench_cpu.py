@@ -1,4 +1,4 @@
-"""Host logic of bench.py's CPU legs (the reference arm the driver runs beside the b200 arm)."""
+"""Host logic of bench.py's CPU legs (the reference arm measured beside the GPU arm)."""
 import os
 import sys
 

@@ -182,36 +182,6 @@ def test_protocol_error_aborts_instead_of_hanging():
       out.stdout, out.stderr[-2000:])
 
 
-def test_cta_pair_variant_is_bit_identical(monkeypatch):
-  """NFB_TC_PAIR=1: the experimental cta_group::2 field kernel (two CTAs share every
-  weight unit, one issuer feeds both SMs) computes the same per-row arithmetic, so
-  its outputs equal the default tcgen05 kernel's bit for bit - including ragged
-  sizes where the follower CTA's tile lies beyond the end.  The release library reads
-  no environment variables: this runs only against a developer build
-  (`python tools/build_variant.py dev -DNFB_DEV_KNOBS`, loaded through NFB_LIB_PATH)."""
-  from nerfies_b200 import _lib
-  if 'libnfb_dev' not in _lib.LIB_PATH:
-    pytest.skip('needs the -DNFB_DEV_KNOBS developer build (NFB_LIB_PATH=nerfies_b200/_variants/libnfb_dev.so)')
-  spec = O.OracleSpec(num_coarse_samples=128, num_fine_samples=128, near=0.02, far=0.83,
-                      num_nerf_point_freqs=8, sigma_activation='softplus', use_warp=True,
-                      use_appearance_metadata=True, num_warp_embeddings=9,
-                      num_appearance_embeddings=9)
-  p = tree_to_device(O.make_trained_like(O.init_params(spec, 1)), DEV)
-  model = model_from_spec(spec_to_dict(spec), precision='bf16', device=DEV, batch_size=700)
-  for n in (700, 1, 3):                      # 700*128 rows = 350 pairs; tiny batches: 1 pair
-    rays = _rays(n, spec, 11 + n)
-    monkeypatch.delenv('NFB_TC_PAIR', raising=False)
-    a = model.apply({'params': p}, rays, warp_extra={'alpha': 6.0}, return_points=True)
-    torch.cuda.synchronize()
-    monkeypatch.setenv('NFB_TC_PAIR', '1')
-    b = model.apply({'params': p}, rays, warp_extra={'alpha': 6.0}, return_points=True)
-    torch.cuda.synchronize()
-    for lv in ('coarse', 'fine'):
-      for k in ('rgb', 'depth', 'acc', 'warped_points'):
-        assert torch.equal(a[lv][k], b[lv][k]), (n, lv, k)
-  monkeypatch.delenv('NFB_TC_PAIR', raising=False)
-
-
 @pytest.mark.parametrize('variant', ['default', 'white_bg_no_infinity', 'fullhd_256'])
 def test_fused_composite_matches_the_staged_path(variant):
   """fp16x3: when a ray is a whole number of 128-sample tiles the field kernel finishes the

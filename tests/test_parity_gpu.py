@@ -76,8 +76,8 @@ def _check_level(name, level, got, ref, z, use_warp):
 
 
 def _golden_model(g, precision):
-  """The tcgen05 modes cover the gin-file widths (trunk 256, warp/rgb 128, relu, rgb
-  condition only); for the small fixtures they refuse loudly - skip those."""
+  """The tensor-core modes cover relu MLPs up to 256 wide with encoded inputs and
+  conditions of up to 64 columns; for other models they refuse loudly - skip those."""
   from nerfies_b200 import _lib
   model = model_from_spec(g.spec_dict, device=DEV, precision=precision)
   if precision != 'fp32':
@@ -85,7 +85,7 @@ def _golden_model(g, precision):
       model.handle(64)
     except _lib.NfbError as e:
       assert 'use precision fp32' in str(e)
-      pytest.skip(f'{g.name}: not a tcgen05 shape ({e})')
+      pytest.skip(f'{g.name}: not a tensor-core shape ({e})')
   return model
 
 
@@ -310,7 +310,7 @@ def _oracle_case(spec, num_rays, seed, alpha, precision='fp32'):
   return p, rays, model
 
 
-# Both parity-holding modes: fp32 (CUDA cores) and fp16x3 (tcgen05, three fp16 MMA
+# Both parity-holding modes: fp32 (CUDA cores) and fp16x3 (wgmma, three fp16 MMA
 # chains per layer into one fp32 accumulator) must meet the same 1e-4 per stage.
 @pytest.mark.parametrize('precision', ['fp32', 'fp16x3'])
 @pytest.mark.parametrize('dims', ['quarterhd', 'vrig', 'fullhd_small'])
@@ -575,7 +575,8 @@ def test_bf16_end_to_end_and_host_path():
 
 def test_bf16_rejects_unsupported_models():
   from nerfies_b200 import _lib
-  g = Golden('se3_small')   # 64-wide trunk: not a tensor-core shape
-  model = model_from_spec(g.spec_dict, precision='bf16', device=DEV)
+  g = Golden('se3_small')
+  # elu hidden layers: the tensor-core kernels implement relu only
+  model = model_from_spec({**g.spec_dict, 'activation': 'elu'}, precision='bf16', device=DEV)
   with pytest.raises(_lib.NfbError, match='precision fp32'):
     model.handle(16)
