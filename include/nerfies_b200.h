@@ -287,10 +287,6 @@ int nfb_camera_rays(const nfb_camera* cam, long long first_pixel, long long coun
 int nfb_pixels_to_rays(const nfb_camera* cam, const float* pixels, long long n,
                        float* directions, void* stream);
 
-/* Kept for ABI compatibility: this library carries no kernel tracer; a non-NULL
- * buffer returns -1, NULL returns 0. */
-int nfb_set_trace(nfb_handle* h, long long* buffer, int capacity);
-
 /* Test hook for the abort path described in the conventions above: while enabled,
  * the weight producer of the tensor-core kernel first waits on an mbarrier that never
  * completes, so the launch must time out, drain and raise the abort flag

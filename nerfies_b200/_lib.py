@@ -16,7 +16,7 @@ SYMBOLS = [
     'nfb_set_params', 'nfb_render_forward', 'nfb_render_forward_host',
     'nfb_render_samples', 'nfb_sample_pdf', 'nfb_coarse_z_vals',
     'nfb_warp_forward', 'nfb_kernel_launches', 'nfb_last_error', 'nfb_version',
-    'nfb_set_profiling', 'nfb_field_time_ms', 'nfb_selftest_gemm', 'nfb_set_trace',
+    'nfb_set_profiling', 'nfb_field_time_ms', 'nfb_selftest_gemm',
     'nfb_camera_rays', 'nfb_pixels_to_rays', 'nfb_selftest_gemm3',
     'nfb_debug_provoke_timeout', 'nfb_set_time_alpha', 'nfb_train_value_and_grad', 'nfb_adam_step',
     'nfb_train_value_and_grad_reg', 'nfb_warp_jacobian', 'nfb_check_abort', 'nfb_reset_abort',
@@ -177,8 +177,6 @@ def load():
   lib.nfb_field_time_ms.restype = cf
   lib.nfb_selftest_gemm.argtypes = [ci, ci, vp, vp, vp, vp]
   lib.nfb_selftest_gemm.restype = ci
-  lib.nfb_set_trace.argtypes = [vp, vp, ci]
-  lib.nfb_set_trace.restype = ci
   ll = ctypes.c_longlong
   lib.nfb_camera_rays.argtypes = [ctypes.POINTER(NfbCamera), ll, ll, vp, vp, vp, vp]
   lib.nfb_camera_rays.restype = ci

@@ -82,45 +82,65 @@ __device__ __forceinline__ float posenc_feature(const float x[3], int f) {
   return sinf(a);
 }
 
-// SE3Field.warp tail (warping.py:330-345) + rigid_body.exp_se3
-// (rigid_body.py:54-89), written exactly as the reference does (no small-angle
-// guard).  wv = [w(3), v(3)] raw head outputs, x the sample point.
-// pivot / trans (nullable): SE3Field use_pivot / use_translation (warping.py:339-352):
-// x + pivot -> rigid transform -> - pivot -> + trans.
-__device__ __forceinline__ void se3_apply(const float wv[6], const float x_in[3],
-                                          float out[3], const float* pivot = nullptr,
-                                          const float* trans = nullptr) {
-  float x[3] = {x_in[0], x_in[1], x_in[2]};
-  if (pivot) { x[0] = x[0] + pivot[0]; x[1] = x[1] + pivot[1]; x[2] = x[2] + pivot[2]; }
-  float theta = sqrtf(wv[0] * wv[0] + wv[1] * wv[1] + wv[2] * wv[2]);
-  float w0 = wv[0] / theta, w1 = wv[1] / theta, w2 = wv[2] / theta;
-  float v0 = wv[3] / theta, v1 = wv[4] / theta, v2 = wv[5] / theta;
+// ---------------------------------------------------------------------------
+// Scalar interface of the warp tail: float in the render kernels, forward-mode
+// numbers (train.cuh: Fwd) in the training kernels.  Num<S>::c makes a constant.
+// ---------------------------------------------------------------------------
+template <class S> struct Num;
+template <> struct Num<float> {
+  static __device__ __forceinline__ float c(float x) { return x; }
+};
+__device__ __forceinline__ float nsqrt(float x) { return sqrtf(x); }
+__device__ __forceinline__ float nsin(float x) { return sinf(x); }
+__device__ __forceinline__ float ncos(float x) { return cosf(x); }
+
+// SE3Field.warp tail (warping.py:330-352) + rigid_body.exp_se3 (rigid_body.py:54-97),
+// written exactly as the reference does (no small-angle guard).  in[0..5] = w, v raw
+// head outputs, in[6..] = (pivot), (translation); x = the sample point:
+// x + pivot -> rigid transform -> - pivot -> + translation.
+template <class S>
+__device__ __forceinline__ void se3_tail(const S* in, const S* x_in, bool pivot, bool trans, S* out) {
+  const S zero = Num<S>::c(0.f), one = Num<S>::c(1.f);
+  const S theta = nsqrt(in[0] * in[0] + in[1] * in[1] + in[2] * in[2]);
+  const S w[3] = {in[0] / theta, in[1] / theta, in[2] / theta};
+  const S v[3] = {in[3] / theta, in[4] / theta, in[5] / theta};
+  S x[3] = {x_in[0], x_in[1], x_in[2]};
+  const S* pv = in + 6;
+  const S* tr = in + (pivot ? 9 : 6);
+  if (pivot)
+    for (int c = 0; c < 3; ++c) x[c] = x[c] + pv[c];
   // W = skew(w); W2 = W @ W.
-  float W[3][3] = {{0.f, -w2, w1}, {w2, 0.f, -w0}, {-w1, w0, 0.f}};
-  float W2[3][3];
-#pragma unroll
+  const S W[3][3] = {{zero, zero - w[2], w[1]}, {w[2], zero, zero - w[0]}, {zero - w[1], w[0], zero}};
+  S W2[3][3];
   for (int i = 0; i < 3; ++i)
-#pragma unroll
-    for (int j = 0; j < 3; ++j)
-      W2[i][j] = W[i][0] * W[0][j] + W[i][1] * W[1][j] + W[i][2] * W[2][j];
-  float s = sinf(theta), c = cosf(theta);
-  float omc = 1.0f - c, tms = theta - s;
-  float v[3] = {v0, v1, v2};
-#pragma unroll
+    for (int j = 0; j < 3; ++j) W2[i][j] = W[i][0] * W[0][j] + W[i][1] * W[1][j] + W[i][2] * W[2][j];
+  const S s = nsin(theta), c = ncos(theta);
+  const S omc = one - c, tms = theta - s;
   for (int i = 0; i < 3; ++i) {
-    float R[3], M[3];
-#pragma unroll
+    S rx = zero, p = zero;
     for (int j = 0; j < 3; ++j) {
-      float eye = (i == j) ? 1.f : 0.f;
-      R[j] = eye + s * W[i][j] + omc * W2[i][j];
-      M[j] = theta * eye + omc * W[i][j] + tms * W2[i][j];
+      const S eye = (i == j) ? one : zero;
+      const S R = eye + s * W[i][j] + omc * W2[i][j];
+      const S M = theta * eye + omc * W[i][j] + tms * W2[i][j];
+      rx = rx + R * x[j];
+      p = p + M * v[j];
     }
-    float p = M[0] * v[0] + M[1] * v[1] + M[2] * v[2];
-    float rx = R[0] * x[0] + R[1] * x[1] + R[2] * x[2];
-    out[i] = (rx + p) / 1.0f;
+    out[i] = rx + p;
+    if (pivot) out[i] = out[i] - pv[i];
+    if (trans) out[i] = out[i] + tr[i];
   }
-  if (pivot) { out[0] = out[0] - pivot[0]; out[1] = out[1] - pivot[1]; out[2] = out[2] - pivot[2]; }
-  if (trans) { out[0] = out[0] + trans[0]; out[1] = out[1] + trans[1]; out[2] = out[2] + trans[2]; }
+}
+
+// The warp of both field types: SE(3) (warp_type 2, heads [w v (p) (t)]) or the
+// TranslationField's y = x + t (warping.py:156).
+template <class S>
+__device__ __forceinline__ void warp_tail(int warp_type, const S* head, const S* x, bool pivot, bool trans,
+                                          S* y) {
+  if (warp_type == 2) {
+    se3_tail(head, x, pivot, trans, y);
+  } else {
+    for (int c = 0; c < 3; ++c) y[c] = x[c] + head[c];
+  }
 }
 
 }  // namespace nfb

@@ -45,10 +45,8 @@ struct FieldArgs {
   int samples_per_ray;       // S
   int use_warp;              // run the warp net
   int warp_only;             // stop after the warp (nfb_warp_forward)
-  int fast_encode;           // bf16 mode: octave-recurrence positional encoding
-  int debug;                 // NFB_DEBUG bits (timing experiments, results are garbage): 1 = hidden-layer epilogues skip
-                             // accumulator reads, math and stores; 2 / 4 (-DNFB_EPI_DEBUG builds) = skip only the activation stores / only loads + math;
-                             // 8 = the MMA issuer first waits on a barrier that never completes (abort-path test)
+  int debug;                 // test hook (nfb_debug_provoke_timeout): bit 8 = the weight producer of the
+                             // tensor-core kernel first waits on a barrier that never completes
   // fp16x3 kernel: volumetric rendering fused into the rgb epilogue (samples_per_ray a multiple
   // of 128): per-ray (rgb3, depth, med_depth, acc) and, optionally, the weights.
   float* ray_out;            // (B,6) or nullptr = no fused composite
@@ -82,7 +80,7 @@ struct SimtSmem {
 // One Dense step on the CTA's 64-row tile.
 template <int NJ>
 __device__ __forceinline__ void simt_dense(const Step& st, const float* __restrict__ params,
-                                           const SimtSmem& sm, int hidden_act_override) {
+                                           const SimtSmem& sm) {
   const int tid = threadIdx.x;
   const int lane = tid & 31;
   const int g = tid >> 5;                 // row group: rows 8g..8g+7
@@ -161,14 +159,14 @@ __device__ __forceinline__ void simt_run_net(const Net& net, const float* params
   for (int s = 0; s < net.n_steps; ++s) {
     const Step& st = net.steps[s];
     switch (st.npad / 32) {
-      case 1: simt_dense<1>(st, params, sm, 0); break;
-      case 2: simt_dense<2>(st, params, sm, 0); break;
-      case 3: simt_dense<3>(st, params, sm, 0); break;
-      case 4: simt_dense<4>(st, params, sm, 0); break;
-      case 5: simt_dense<5>(st, params, sm, 0); break;
-      case 6: simt_dense<6>(st, params, sm, 0); break;
-      case 7: simt_dense<7>(st, params, sm, 0); break;
-      default: simt_dense<8>(st, params, sm, 0); break;
+      case 1: simt_dense<1>(st, params, sm); break;
+      case 2: simt_dense<2>(st, params, sm); break;
+      case 3: simt_dense<3>(st, params, sm); break;
+      case 4: simt_dense<4>(st, params, sm); break;
+      case 5: simt_dense<5>(st, params, sm); break;
+      case 6: simt_dense<6>(st, params, sm); break;
+      case 7: simt_dense<7>(st, params, sm); break;
+      default: simt_dense<8>(st, params, sm); break;
     }
   }
 }
@@ -220,17 +218,10 @@ field_simt_kernel(const __grid_constant__ FieldProgram prog, const FieldArgs arg
     __syncthreads();
     simt_run_net(prog.warp, args.params, sm);
     if (part == 0) {
-      float y[3];
-      if (prog.warp_type == 2) {
-        float wv[12];
+      float h[12], y[3];
 #pragma unroll
-        for (int q = 0; q < 12; ++q) wv[q] = sm.out[q * kRS + r];
-        se3_apply(wv, x, y, prog.warp_pivot ? wv + 6 : nullptr,
-                  prog.warp_trans ? wv + (prog.warp_pivot ? 9 : 6) : nullptr);
-      } else {
-#pragma unroll
-        for (int c = 0; c < 3; ++c) y[c] = x[c] + sm.out[c * kRS + r];  // warping.py:156
-      }
+      for (int q = 0; q < 12; ++q) h[q] = sm.out[q * kRS + r];
+      warp_tail(prog.warp_type, h, x, prog.warp_pivot, prog.warp_trans, y);
 #pragma unroll
       for (int c = 0; c < 3; ++c) sm.wp[c * kTM + r] = y[c];
       if (args.warped && valid) {

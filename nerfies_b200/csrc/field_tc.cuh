@@ -19,34 +19,6 @@
 namespace nfb {
 namespace tc {
 
-// [x | w_k * sin/cos features | extra | 0...] -> one 64-column K-block row.
-__device__ __forceinline__ void posenc_to_block(uint8_t* block, int r, const float* x, int F,
-                                             const float* __restrict__ window,
-                                             const float* __restrict__ extra, int n_extra,
-                                             int c_begin = 0, int c_end = 8) {
-  const int nf = 6 * F;
-#pragma unroll 1
-  for (int c = c_begin; c < c_end; ++c) {
-    float v[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int k = c * 8 + j;
-      float val = 0.f;
-      if (k < 3) {
-        val = x[k];
-      } else if (k < 3 + nf) {
-        const int f = k - 3;
-        val = posenc_feature(x, f);
-        if (window) val = __ldg(window + f / 6) * val;
-      } else if (k < 3 + nf + n_extra) {
-        val = __ldg(extra + (k - 3 - nf));
-      }
-      v[j] = val;
-    }
-    store_chunk(block, r, c, v);
-  }
-}
-
 // bf16 mode: the encoded features are rounded to bf16 (rel. 4e-3) before they
 // reach the tensor cores, so the octave recurrence
 //   sin 2a = 2 sin a cos a,  cos 2a = 1 - 2 sin^2 a
@@ -87,6 +59,20 @@ __device__ __forceinline__ void posenc_fast_to_block(uint8_t* block, int r, cons
 #pragma unroll
   for (int c = 0; c < 8; ++c)
     if (c >= c_begin && c < c_end) store_chunk(block, r, c, feat + c * 8);
+}
+// This thread's half `hs` (32 columns) of row r of the input block, [x | window * posenc(x) | extra | 0...],
+// in the kernel's precision: fp16 hi / lo images (kX3) or bf16.  Inlined: a call with a literal null `extra`
+// and n_extra = 0 carries no extra-column code (register pressure).
+template <bool kX3>
+__device__ __forceinline__ void encode_input(uint8_t* in_block, int r, int hs, const float* x, int F,
+                                             const float* __restrict__ window,
+                                             const float* __restrict__ extra, int n_extra) {
+  if constexpr (kX3) {
+    if (hs == 0) tc3::posenc_block_x3<0>(in_block, in_block + kABlockBytes, r, x, F, window, extra, n_extra);
+    else tc3::posenc_block_x3<1>(in_block, in_block + kABlockBytes, r, x, F, window, extra, n_extra);
+  } else {
+    posenc_fast_to_block(in_block, r, x, F, window, extra, n_extra, 4 * hs, 4 * hs + 4);
+  }
 }
 __device__ __forceinline__ void cond_to_block(uint8_t* block, int r, const float* __restrict__ cond,
                                               int n, int c_begin = 0, int c_end = 8) {
@@ -308,38 +294,30 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
     auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory"); };
     RowState row;
 
-    struct TilePref { float z, zn, org[3], dir[3]; };
-    auto tile_prefetch = [&](int tile, TilePref& pf) {
-      long long m = (long long)tile * kTileRows + r;
-      if (m >= args.num_rows) m = args.num_rows - 1;
-      const long long ray = m / S;
-      pf.z = args.z_vals ? __ldg(args.z_vals + m) : 0.f;
-      const bool last = m + 1 == (ray + 1) * S;
-      pf.zn = (fuse && !last && args.z_vals) ? __ldg(args.z_vals + m + 1) : 0.f;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        pf.dir[c] = __ldg(args.directions + ray * 3 + c);
-        pf.org[c] = __ldg(args.origins + ray * 3 + c);
-      }
-    };
     // Row state of tile `tile` (model_utils.py:72-73) and this thread's half of its first
     // input block (warping.py:325-326 / models.py:270).
     auto begin_tile = [&](int tile) {
-      TilePref pf;
-      tile_prefetch(tile, pf);
       long long m = (long long)tile * kTileRows + r;
       row.valid = m < args.num_rows;
       if (!row.valid) m = args.num_rows - 1;
       row.m = m;
       row.ray = m / S;
+      const float z = args.z_vals ? __ldg(args.z_vals + m) : 0.f;
+      float org[3], dir[3];
 #pragma unroll
-      for (int c = 0; c < 3; ++c) row.x[c] = pf.org[c] + pf.z * pf.dir[c];
+      for (int c = 0; c < 3; ++c) {
+        dir[c] = __ldg(args.directions + row.ray * 3 + c);
+        org[c] = __ldg(args.origins + row.ray * 3 + c);
+      }
+#pragma unroll
+      for (int c = 0; c < 3; ++c) row.x[c] = org[c] + z * dir[c];
       if (fuse) {
         // dists of volumetric_rendering (model_utils.py:98-104)
-        row.z = pf.z;
+        row.z = z;
         row.last = m + 1 == (row.ray + 1) * S;
-        const float dnorm = sqrtf(pf.dir[0] * pf.dir[0] + pf.dir[1] * pf.dir[1] + pf.dir[2] * pf.dir[2]);
-        const float d = row.last ? (args.sample_at_infinity ? 1e10f : 1e-19f) : (pf.zn - pf.z);
+        const float zn = (!row.last && args.z_vals) ? __ldg(args.z_vals + m + 1) : 0.f;
+        const float dnorm = sqrtf(dir[0] * dir[0] + dir[1] * dir[1] + dir[2] * dir[2]);
+        const float d = row.last ? (args.sample_at_infinity ? 1e10f : 1e-19f) : (zn - z);
         row.dist = d * dnorm;
       }
       if (!do_warp && args.warped && row.valid && hs == 0) {
@@ -347,17 +325,9 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
         for (int c = 0; c < 3; ++c) args.warped[m * 3 + c] = row.x[c];
       }
       const float* cond = args.cond + row.ray * prog.cond_stride;
-      const float* window = do_warp ? args.window : nullptr;
       // warp net: [posenc | GLO code]; NeRF net: [posenc | trunk condition]
-      const float* extra = do_warp ? cond : cond + prog.G;
-      const int F = do_warp ? prog.Fw : prog.Fp, n_extra = do_warp ? prog.G : prog.tc;
-      if constexpr (kX3) {
-        if (hs == 0) tc3::posenc_block_x3<0>(inh, inl, r, row.x, F, window, extra, n_extra);
-        else tc3::posenc_block_x3<1>(inh, inl, r, row.x, F, window, extra, n_extra);
-      } else {
-        if (args.fast_encode) posenc_fast_to_block(inh, r, row.x, F, window, extra, n_extra, cb, ce);
-        else posenc_to_block(inh, r, row.x, F, window, extra, n_extra, cb, ce);
-      }
+      encode_input<kX3>(inh, r, hs, row.x, do_warp ? prog.Fw : prog.Fp, do_warp ? args.window : nullptr,
+                        do_warp ? cond : cond + prog.G, do_warp ? prog.G : prog.tc);
     };
 
     // fused composite: running state of the ray this CTA is on (replicated in every row thread)
@@ -435,13 +405,7 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
           wg_sync();      // the scratch has been read before anything overwrites block 0
           if (st.epi == kEpiWarpHeads) {
             float y[3];
-            if (prog.warp_type == 2) {
-              se3_apply(v, row.x, y, prog.warp_pivot ? v + 6 : nullptr,
-                        prog.warp_trans ? v + (prog.warp_pivot ? 9 : 6) : nullptr);
-            } else {
-#pragma unroll
-              for (int c = 0; c < 3; ++c) y[c] = row.x[c] + v[c];
-            }
+            warp_tail(prog.warp_type, v, row.x, prog.warp_pivot, prog.warp_trans, y);
 #pragma unroll
             for (int c = 0; c < 3; ++c) row.x[c] = y[c];
             if (args.warped && row.valid && hs == 0) {
@@ -450,24 +414,11 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
             }
             if (args.warp_only) {
               if (has_next) begin_tile(tile_of(ti + 1));
-            } else {
-              // trunk condition (without one, the encoder's extra columns are compile-time empty)
-              const float* tcond = prog.tc ? args.cond + row.ray * prog.cond_stride + prog.G : nullptr;
-              if (!prog.tc) {
-                if constexpr (kX3) {
-                  if (hs == 0) tc3::posenc_block_x3<0>(inh, inl, r, row.x, prog.Fp, nullptr, nullptr, 0);
-                  else tc3::posenc_block_x3<1>(inh, inl, r, row.x, prog.Fp, nullptr, nullptr, 0);
-                } else {
-                  if (args.fast_encode) posenc_fast_to_block(inh, r, row.x, prog.Fp, nullptr, nullptr, 0, cb, ce);
-                  else posenc_to_block(inh, r, row.x, prog.Fp, nullptr, nullptr, 0, cb, ce);
-                }
-              } else if constexpr (kX3) {
-                if (hs == 0) tc3::posenc_block_x3<0>(inh, inl, r, row.x, prog.Fp, nullptr, tcond, prog.tc);
-                else tc3::posenc_block_x3<1>(inh, inl, r, row.x, prog.Fp, nullptr, tcond, prog.tc);
-              } else {
-                if (args.fast_encode) posenc_fast_to_block(inh, r, row.x, prog.Fp, nullptr, tcond, prog.tc, cb, ce);
-                else posenc_to_block(inh, r, row.x, prog.Fp, nullptr, tcond, prog.tc, cb, ce);
-              }
+            } else if (prog.tc) {   // NeRF net inputs: [posenc | trunk condition]
+              encode_input<kX3>(inh, r, hs, row.x, prog.Fp, nullptr,
+                                args.cond + row.ray * prog.cond_stride + prog.G, prog.tc);
+            } else {                // without one, the encoder's extra columns are compile-time empty
+              encode_input<kX3>(inh, r, hs, row.x, prog.Fp, nullptr, nullptr, 0);
             }
           } else {
             float4 o;

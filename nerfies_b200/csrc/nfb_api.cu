@@ -18,10 +18,7 @@
 #include "camera_kernels.cuh"
 #include "tc_common.cuh"
 #include "tc_selftest.cuh"
-#ifdef NFB_WITH_TC
 #include "field_tc.cuh"
-#include "field_tc3.cuh"
-#endif
 
 namespace {
 
@@ -277,13 +274,8 @@ int build_tables(nfb_handle* h) {
   return 0;
 }
 
-// cosine_easing_window (modules.py:274-294) in float32.
-int set_window(nfb_handle* h, float alpha, cudaStream_t stream) {
-  if (h->cfg.warp_field_type == NFB_WARP_NONE) return 0;
-  if (alpha == h->h_window_alpha) return 0;
-  const int F = h->cfg.num_warp_freqs;
-  if (F > 64) return fail("num_warp_freqs > 64");
-  float w[64];
+// cosine_easing_window (modules.py:274-294) in float32: w[0..F).
+void easing_window(float alpha, int F, float* w) {
   const float pi = 3.14159274101257324f;  // float32(np.pi)
   for (int k = 0; k < F; ++k) {
     float x = alpha - (float)k;
@@ -293,6 +285,15 @@ int set_window(nfb_handle* h, float alpha, cudaStream_t stream) {
     volatile float cv = cosf(arg);
     w[k] = 0.5f * (1.f + cv);
   }
+}
+
+int set_window(nfb_handle* h, float alpha, cudaStream_t stream) {
+  if (h->cfg.warp_field_type == NFB_WARP_NONE) return 0;
+  if (alpha == h->h_window_alpha) return 0;
+  const int F = h->cfg.num_warp_freqs;
+  if (F > 64) return fail("num_warp_freqs > 64");
+  float w[64];
+  easing_window(alpha, F, w);
   // Stream-ordered copy from pageable memory: the driver stages it before returning.
   NFB_CUDA(cudaMemcpyAsync(h->d_window, w, F * sizeof(float), cudaMemcpyHostToDevice, stream));
   h->h_window_alpha = alpha;
@@ -333,15 +334,7 @@ int run_cond(nfb_handle* h, int B, const float* viewdirs, const unsigned* warp_i
     if (enc == NFB_WARP_ENC_TIME) t.time_f = reinterpret_cast<const float*>(warp_id);
     else t.time_id = warp_id;
     const float alpha = enc == NFB_WARP_ENC_TIME ? h->time_alpha : (float)t.F;   // modules.py:318-319
-    const float pi = 3.14159274101257324f;
-    for (int k = 0; k < t.F; ++k) {                     // cosine_easing_window (modules.py:274-294)
-      float x = alpha - (float)k;
-      x = fminf(fmaxf(x, 0.f), 1.f);
-      volatile float arg = pi * x;
-      arg = arg + pi;
-      volatile float cv = cosf(arg);
-      t.window[k] = 0.5f * (1.f + cv);
-    }
+    easing_window(alpha, t.F, t.window);
     t.blend = enc == NFB_WARP_ENC_BLEND; t.time_alpha = h->time_alpha;
     t.cond = h->d_cond; t.stride = h->cond_stride; t.G = h->prog[0].G; t.num_rays = B;
     nfb::time_embed_kernel<<<(B + nfb::kTimeRays - 1) / nfb::kTimeRays, nfb::kTimeThreads, 0, s>>>(t);
@@ -367,15 +360,7 @@ int run_field(nfb_handle* h, int level, long long rows, int S, const float* orig
   a.params = h->d_packed; a.origins = origins; a.directions = directions; a.z_vals = z;
   a.cond = h->d_cond; a.window = h->d_window; a.samples = samples; a.warped = warped;
   a.num_rows = rows; a.samples_per_ray = S; a.use_warp = use_warp; a.warp_only = warp_only;
-  a.fast_encode = h->cfg.precision == NFB_PREC_BF16;
-#ifdef NFB_DEV_KNOBS
-  {
-    // developer builds only: timing experiments whose results are garbage (see FieldArgs::debug)
-    static const int dbg = getenv("NFB_DEBUG") ? atoi(getenv("NFB_DEBUG")) : 0;
-    a.debug = dbg;
-  }
-#endif
-  a.debug |= h->debug_bits;
+  a.debug = h->debug_bits;
   const bool prof = h->profiling && !warp_only;
   if (prof) NFB_CUDA(cudaEventRecord(h->ev[level][0], s));
   int rc;
@@ -384,11 +369,7 @@ int run_field(nfb_handle* h, int level, long long rows, int S, const float* orig
     nfb::field_simt_kernel<<<(unsigned)tiles, nfb::kSimtThreads, nfb::kSimtSmemBytes, s>>>(h->prog[level], a);
     rc = launch_check(h, "field_simt_kernel");
   } else {
-#ifdef NFB_WITH_TC
     rc = nfb::tc::run_field_tc(h, level, a, s);
-#else
-    rc = fail("precision %d needs the tensor-core path, which this build does not contain", h->cfg.precision);
-#endif
   }
   if (prof && rc == 0) {
     NFB_CUDA(cudaEventRecord(h->ev[level][1], s));
@@ -426,6 +407,17 @@ int run_resample(nfb_handle* h, int B, const float* zc, const float* wc, const f
   return launch_check(h, "resample_kernel");
 }
 
+// One level of nfb_render_forward: the field at the S samples of every ray, then volumetric
+// rendering into `out` (and `weights`, if not null).
+int render_level(nfb_handle* h, int level, int B, int S, const float* origins, const float* directions,
+                 const float* z, bool use_warp, float* out, float* weights, cudaStream_t s) {
+  const long long rows = (long long)B * S;
+  if (can_fuse_composite(h, S))   // field + volumetric rendering in one kernel: 24 B per ray (+ the weights) leave the SM
+    return run_field(h, level, rows, S, origins, directions, z, nullptr, nullptr, use_warp, false, s, out, weights);
+  if (run_field(h, level, rows, S, origins, directions, z, h->d_samples, nullptr, use_warp, false, s)) return -1;
+  return run_composite(h, B, S, h->d_samples, z, directions, out, weights, s);
+}
+
 // The tensor-core kernels never trap on a protocol error (see tc_common.cuh,
 // mbar_wait): they raise a flag in mapped pinned host memory instead.  One int per
 // process; every device's copy of the g_nfb_abort symbol points at it.
@@ -433,7 +425,6 @@ int* g_abort_host = nullptr;
 unsigned long long g_abort_devices = 0;   // devices whose symbol has been set
 
 int ensure_abort_flag() {
-#ifdef NFB_WITH_TC
   int dev = 0;
   NFB_CUDA(cudaGetDevice(&dev));
   if (!g_abort_host) {
@@ -446,7 +437,6 @@ int ensure_abort_flag() {
     NFB_CUDA(cudaMemcpyToSymbol(nfb::tc::g_nfb_abort, &dptr, sizeof(dptr)));
     g_abort_devices |= 1ull << dev;
   }
-#endif
   return 0;
 }
 
@@ -524,13 +514,6 @@ int nfb_pixels_to_rays(const nfb_camera* cam, const float* pixels, long long n, 
                        void* stream) {
   if (!pixels && n > 0) return fail("null argument");
   return launch_camera(cam, pixels, 0, n, nullptr, directions, nullptr, stream);
-}
-
-int nfb_set_trace(nfb_handle* h, long long* buffer, int capacity) {
-  if (!h) return fail("null handle");
-  (void)capacity;
-  if (buffer) return fail("this build carries no tracer");
-  return 0;
 }
 
 int nfb_debug_provoke_timeout(nfb_handle* h, int enabled) {
@@ -680,18 +663,14 @@ int nfb_create(const nfb_config* cfg, int max_rays, nfb_handle** out) {
     return bail(fail("cannot reserve %d bytes of shared memory", nfb::kSimtSmemBytes));
   cudaFuncSetAttribute(nfb::composite_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
   cudaFuncSetAttribute(nfb::resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
-#ifdef NFB_WITH_TC
   if (c.precision != NFB_PREC_FP32 && nfb::tc::create_tc(h)) return bail(-1);
-#endif
   *out = h;
   return 0;
 }
 
 void nfb_destroy(nfb_handle* h) {
   if (!h) return;
-#ifdef NFB_WITH_TC
   nfb::tc::destroy_tc(h);
-#endif
   float* bufs[] = {h->d_packed, h->d_warp_table, h->d_app_table, h->d_cam_table, h->d_zlin,
                    h->d_lower, h->d_upper, h->d_ulin, h->d_window, h->d_cond, h->d_zc, h->d_zf,
                    h->d_wc, h->d_samples, h->d_out_c, h->d_out_f, h->d_in};
@@ -746,9 +725,7 @@ int nfb_set_params(nfb_handle* h, const float* const* tensors, const long long* 
                                                             p.cols, p.ld, p.c_off);
     if (launch_check(h, "pack_kernel")) return -1;
   }
-#ifdef NFB_WITH_TC
   if (h->cfg.precision != NFB_PREC_FP32 && nfb::tc::pack_tc(h, s)) return -1;
-#endif
   h->params_set = true;
   return 0;
 }
@@ -815,27 +792,14 @@ int nfb_render_forward(nfb_handle* h, int B, const float* origins, const float* 
   // coarse level (models.py:332-349)
   if (nfb_coarse_z_vals(h, B, t_rand, h->d_zc, stream)) return -1;
   float* wc = w_coarse ? w_coarse : h->d_wc;
-  float* oc = out_coarse ? out_coarse : h->d_out_c;
-  if (can_fuse_composite(h, nc)) {
-    // field + volumetric rendering in one kernel: 24 B per ray (+ the coarse weights) leave the SM
-    if (run_field(h, 0, (long long)B * nc, nc, origins, directions, h->d_zc, nullptr, nullptr,
-                  use_warp, false, s, oc, wc)) return -1;
-  } else {
-    if (run_field(h, 0, (long long)B * nc, nc, origins, directions, h->d_zc, h->d_samples, nullptr,
-                  use_warp, false, s)) return -1;
-    if (run_composite(h, B, nc, h->d_samples, h->d_zc, directions, oc, wc, s)) return -1;
-  }
+  if (render_level(h, 0, B, nc, origins, directions, h->d_zc, use_warp, out_coarse ? out_coarse : h->d_out_c,
+                   wc, s)) return -1;
   if (!fine) return 0;
   // hierarchical resampling + fine level (models.py:352-370)
   float* zf = z_fine ? z_fine : h->d_zf;
   if (run_resample(h, B, h->d_zc, wc, u_rand, zf, s)) return -1;
-  float* of = out_fine ? out_fine : h->d_out_f;
-  if (can_fuse_composite(h, nfine))
-    return run_field(h, 1, (long long)B * nfine, nfine, origins, directions, zf, nullptr, nullptr,
-                     use_warp, false, s, of, w_fine);
-  if (run_field(h, 1, (long long)B * nfine, nfine, origins, directions, zf, h->d_samples, nullptr,
-                use_warp, false, s)) return -1;
-  return run_composite(h, B, nfine, h->d_samples, zf, directions, of, w_fine, s);
+  return render_level(h, 1, B, nfine, origins, directions, zf, use_warp, out_fine ? out_fine : h->d_out_f,
+                      w_fine, s);
 }
 
 int nfb_render_forward_host(nfb_handle* h, int B, const float* origins, const float* directions,

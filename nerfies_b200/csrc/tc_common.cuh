@@ -205,23 +205,6 @@ __device__ __forceinline__ void store_chunk(uint8_t* block, int row, int chunk, 
   *reinterpret_cast<uint4*>(block + swz_off(row, chunk)) = q;
 }
 
-// Stores one 32-column piece (16 packed bf16 pairs) of a row into the activation
-// blocks.  `a0` = shared address of the row's chunk 0 in block 0 with the row's
-// swizzle term folded in (base + row*128 + ((row&7)<<4)); chunk c of the row is at
-// a0 ^ (c<<4).  The xor is a volatile asm so that ptxas recomputes the address (one
-// LOP3) instead of keeping 16 loop-invariant addresses alive across the layer loop.
-__device__ __forceinline__ void sts_piece(uint32_t a0, int col, const uint32_t* pk16) {
-  const uint32_t base = a0 + (uint32_t)(col >> 6) * 16384u;
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    uint32_t addr;
-    asm volatile("xor.b32 %0, %1, %2;" : "=r"(addr) : "r"(base), "r"((uint32_t)((((col & 63) >> 3) + q) << 4)));
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(pk16[q * 4]),
-                 "r"(pk16[q * 4 + 1]), "r"(pk16[q * 4 + 2]), "r"(pk16[q * 4 + 3])
-                 : "memory");
-  }
-}
-
 // Weight packing (global memory image of the shared-memory operand): the
 // (in,out) fp32 kernel W[k][n] of a Dense layer becomes, per K-block kb, a
 // contiguous unit of `n_rows` rows x 128 bytes holding W^T (row n, column k),

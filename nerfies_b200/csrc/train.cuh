@@ -20,6 +20,72 @@
 #include "ray_kernels.cuh"
 
 namespace nfb {
+
+// ---------------------------------------------------------------------------
+// Forward-mode numbers with N tangent directions over a scalar type T (float or
+// another Fwd, for second derivatives): the scalar type of the warp tail's
+// derivatives (se3_tail, common.cuh).
+// ---------------------------------------------------------------------------
+template <int N, class T>
+struct Fwd {
+  T v;
+  T d[N];
+};
+template <int N, class T> struct Num<Fwd<N, T>> {
+  static __device__ __forceinline__ Fwd<N, T> c(float x) {
+    Fwd<N, T> r;
+    r.v = Num<T>::c(x);
+#pragma unroll
+    for (int i = 0; i < N; ++i) r.d[i] = Num<T>::c(0.f);
+    return r;
+  }
+};
+template <int N, class T> __device__ __forceinline__ Fwd<N, T> operator+(const Fwd<N, T>& a, const Fwd<N, T>& b) {
+  Fwd<N, T> r; r.v = a.v + b.v;
+#pragma unroll
+  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] + b.d[i];
+  return r;
+}
+template <int N, class T> __device__ __forceinline__ Fwd<N, T> operator-(const Fwd<N, T>& a, const Fwd<N, T>& b) {
+  Fwd<N, T> r; r.v = a.v - b.v;
+#pragma unroll
+  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] - b.d[i];
+  return r;
+}
+template <int N, class T> __device__ __forceinline__ Fwd<N, T> operator*(const Fwd<N, T>& a, const Fwd<N, T>& b) {
+  Fwd<N, T> r; r.v = a.v * b.v;
+#pragma unroll
+  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] * b.v + a.v * b.d[i];
+  return r;
+}
+template <int N, class T> __device__ __forceinline__ Fwd<N, T> operator/(const Fwd<N, T>& a, const Fwd<N, T>& b) {
+  Fwd<N, T> r; r.v = a.v / b.v;
+#pragma unroll
+  for (int i = 0; i < N; ++i) r.d[i] = (a.d[i] - r.v * b.d[i]) / b.v;
+  return r;
+}
+template <int N, class T> __device__ __forceinline__ Fwd<N, T> nsqrt(const Fwd<N, T>& a) {
+  Fwd<N, T> r; r.v = nsqrt(a.v);
+  const T k = Num<T>::c(0.5f) / r.v;
+#pragma unroll
+  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] * k;
+  return r;
+}
+template <int N, class T> __device__ __forceinline__ Fwd<N, T> nsin(const Fwd<N, T>& a) {
+  Fwd<N, T> r; r.v = nsin(a.v);
+  const T c = ncos(a.v);
+#pragma unroll
+  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] * c;
+  return r;
+}
+template <int N, class T> __device__ __forceinline__ Fwd<N, T> ncos(const Fwd<N, T>& a) {
+  Fwd<N, T> r; r.v = ncos(a.v);
+  const T s = Num<T>::c(0.f) - nsin(a.v);
+#pragma unroll
+  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] * s;
+  return r;
+}
+
 namespace train {
 
 constexpr int kTile = 64;      // C tile (kTile x kTile), 256 threads, 4 x 4 per thread
@@ -337,8 +403,8 @@ __global__ void encode_bwd_kernel(const EncodeBwdArgs a) {
 }
 
 // ---------------------------------------------------------------------------
-// Warp tail (R5) and its adjoint by forward-mode duals (9 or 15 directions: the
-// head outputs w, v, (pivot), (translation) and the point).
+// Warp tail (R5) and its adjoint by forward mode (one direction per head output:
+// w, v, (pivot), (translation)).
 // ---------------------------------------------------------------------------
 struct WarpTailArgs {
   const float* head; int ld;  // (rows, ld): [w v (p) (t)] or the translation (3)
@@ -350,111 +416,22 @@ struct WarpTailArgs {
 __global__ void warp_tail_kernel(const WarpTailArgs a) {
   const long long m = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= a.rows) return;
-  const float* h = a.head + m * a.ld;
-  float x[3] = {a.pts[m * 3], a.pts[m * 3 + 1], a.pts[m * 3 + 2]}, y[3];
-  if (a.warp_type == 2) {
-    float wv[12];
-#pragma unroll
-    for (int q = 0; q < 12; ++q) wv[q] = h[q];
-    se3_apply(wv, x, y, a.pivot ? wv + 6 : nullptr, a.trans ? wv + (a.pivot ? 9 : 6) : nullptr);
-  } else {
-#pragma unroll
-    for (int c = 0; c < 3; ++c) y[c] = x[c] + h[c];
-  }
+  const float x[3] = {a.pts[m * 3], a.pts[m * 3 + 1], a.pts[m * 3 + 2]};
+  float y[3];
+  warp_tail(a.warp_type, a.head + m * a.ld, x, a.pivot != 0, a.trans != 0, y);
 #pragma unroll
   for (int c = 0; c < 3; ++c) a.warped[m * 3 + c] = y[c];
 }
 
-// Forward-mode dual number with N tangent directions.
-template <int N>
-struct Dual {
-  float v; float d[N];
-};
-template <int N> __device__ __forceinline__ Dual<N> dconst(float v) {
-  Dual<N> r; r.v = v;
-#pragma unroll
-  for (int i = 0; i < N; ++i) r.d[i] = 0.f;
-  return r;
-}
-template <int N> __device__ __forceinline__ Dual<N> operator+(const Dual<N>& a, const Dual<N>& b) {
-  Dual<N> r; r.v = a.v + b.v;
-#pragma unroll
-  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] + b.d[i];
-  return r;
-}
-template <int N> __device__ __forceinline__ Dual<N> operator-(const Dual<N>& a, const Dual<N>& b) {
-  Dual<N> r; r.v = a.v - b.v;
-#pragma unroll
-  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] - b.d[i];
-  return r;
-}
-template <int N> __device__ __forceinline__ Dual<N> operator*(const Dual<N>& a, const Dual<N>& b) {
-  Dual<N> r; r.v = a.v * b.v;
-#pragma unroll
-  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] * b.v + a.v * b.d[i];
-  return r;
-}
-template <int N> __device__ __forceinline__ Dual<N> operator/(const Dual<N>& a, const Dual<N>& b) {
-  Dual<N> r; r.v = a.v / b.v;
-  const float inv = 1.f / b.v;
-#pragma unroll
-  for (int i = 0; i < N; ++i) r.d[i] = (a.d[i] - r.v * b.d[i]) * inv;
-  return r;
-}
-template <int N> __device__ __forceinline__ Dual<N> dsqrt(const Dual<N>& a) {
-  Dual<N> r; r.v = sqrtf(a.v);
-  const float k = 0.5f / r.v;
-#pragma unroll
-  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] * k;
-  return r;
-}
-template <int N> __device__ __forceinline__ Dual<N> dsin(const Dual<N>& a) {
-  Dual<N> r; r.v = sinf(a.v);
-  const float c = cosf(a.v);
-#pragma unroll
-  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] * c;
-  return r;
-}
-template <int N> __device__ __forceinline__ Dual<N> dcos(const Dual<N>& a) {
-  Dual<N> r; r.v = cosf(a.v);
-  const float s = -sinf(a.v);
-#pragma unroll
-  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] * s;
-  return r;
-}
-
-// SE3Field.warp tail (warping.py:330-352) on duals; in[0..5] = w, v, in[6..8] = pivot,
-// in[9..11] = translation, x = point (all seeded by the caller).
-template <int N>
-__device__ void se3_dual(const Dual<N>* in, const Dual<N>* x_in, bool pivot, bool trans, Dual<N>* out) {
-  using D = Dual<N>;
-  D theta = dsqrt(in[0] * in[0] + in[1] * in[1] + in[2] * in[2]);
-  D w[3] = {in[0] / theta, in[1] / theta, in[2] / theta};
-  D v[3] = {in[3] / theta, in[4] / theta, in[5] / theta};
-  D x[3] = {x_in[0], x_in[1], x_in[2]};
-  const D* pv = in + 6;
-  const D* tr = in + (pivot ? 9 : 6);
-  if (pivot) for (int c = 0; c < 3; ++c) x[c] = x[c] + pv[c];
-  D zero = dconst<N>(0.f), one = dconst<N>(1.f);
-  D W[3][3] = {{zero, zero - w[2], w[1]}, {w[2], zero, zero - w[0]}, {zero - w[1], w[0], zero}};
-  D W2[3][3];
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) W2[i][j] = W[i][0] * W[0][j] + W[i][1] * W[1][j] + W[i][2] * W[2][j];
-  D s = dsin(theta), c = dcos(theta);
-  D omc = one - c, tms = theta - s;
-  for (int i = 0; i < 3; ++i) {
-    D rx = zero, p = zero;
-    for (int j = 0; j < 3; ++j) {
-      D eye = (i == j) ? one : zero;
-      D R = eye + s * W[i][j] + omc * W2[i][j];
-      D M = theta * eye + omc * W[i][j] + tms * W2[i][j];
-      rx = rx + R * x[j];
-      p = p + M * v[j];
-    }
-    out[i] = rx + p;
-    if (pivot) out[i] = out[i] - pv[i];
-    if (trans) out[i] = out[i] + tr[i];
-  }
+// The SE(3) tail y at (h, x) with one tangent direction per head output:
+// y[i].d[q] = d y_i / d head_q for q < nh (zero beyond; h[q] = 0 there).
+__device__ __forceinline__ void se3_head_jacobian(const float h[12], const float x[3], int nh, bool pivot,
+                                                  bool trans, Fwd<12, float> y[3]) {
+  using S = Fwd<12, float>;
+  S in[12], xs[3];
+  for (int q = 0; q < 12; ++q) { in[q] = Num<S>::c(h[q]); if (q < nh) in[q].d[q] = 1.f; }
+  for (int c = 0; c < 3; ++c) xs[c] = Num<S>::c(x[c]);
+  se3_tail(in, xs, pivot, trans, y);
 }
 
 struct WarpTailBwdArgs {
@@ -473,18 +450,14 @@ __global__ void warp_tail_bwd_kernel(const WarpTailBwdArgs a) {
     for (int c = 0; c < 3; ++c) dh[c] += g[c];       // warped = x + t
     return;
   }
-  // d(warped)/d(head) by forward mode: one direction per head output (the points carry
-  // no parameter upstream: x = o + z d with z a constant).
-  constexpr int N = 12;
+  // The points carry no parameter upstream: x = o + z d with z a constant.
   const int nh = 6 + (a.pivot ? 3 : 0) + (a.trans ? 3 : 0);
-  Dual<N> in[12], x[3], out[3];
-  for (int q = 0; q < 12; ++q) {
-    in[q] = dconst<N>(q < nh ? a.head[m * a.ld + q] : 0.f);
-    if (q < nh) in[q].d[q] = 1.f;
-  }
-  for (int c = 0; c < 3; ++c) x[c] = dconst<N>(a.pts[m * 3 + c]);
-  se3_dual<N>(in, x, a.pivot != 0, a.trans != 0, out);
-  for (int q = 0; q < nh; ++q) dh[q] += g[0] * out[0].d[q] + g[1] * out[1].d[q] + g[2] * out[2].d[q];
+  float h[12], x[3];
+  Fwd<12, float> y[3];
+  for (int q = 0; q < 12; ++q) h[q] = q < nh ? a.head[m * a.ld + q] : 0.f;
+  for (int c = 0; c < 3; ++c) x[c] = a.pts[m * 3 + c];
+  se3_head_jacobian(h, x, nh, a.pivot != 0, a.trans != 0, y);
+  for (int q = 0; q < nh; ++q) dh[q] += g[0] * y[0].d[q] + g[1] * y[1].d[q] + g[2] * y[2].d[q];
 }
 
 // ---------------------------------------------------------------------------

@@ -20,110 +20,6 @@ namespace nfb {
 namespace train {
 
 // ---------------------------------------------------------------------------
-// Forward-mode numbers over an arbitrary scalar type (float or another Fwd).
-// ---------------------------------------------------------------------------
-template <int N, class T>
-struct Fwd {
-  T v;
-  T d[N];
-};
-template <class S> struct Num;
-template <> struct Num<float> {
-  static __device__ __forceinline__ float c(float x) { return x; }
-};
-template <int N, class T> struct Num<Fwd<N, T>> {
-  static __device__ __forceinline__ Fwd<N, T> c(float x) {
-    Fwd<N, T> r;
-    r.v = Num<T>::c(x);
-#pragma unroll
-    for (int i = 0; i < N; ++i) r.d[i] = Num<T>::c(0.f);
-    return r;
-  }
-};
-__device__ __forceinline__ float nsqrt(float x) { return sqrtf(x); }
-__device__ __forceinline__ float nsin(float x) { return sinf(x); }
-__device__ __forceinline__ float ncos(float x) { return cosf(x); }
-template <int N, class T> __device__ __forceinline__ Fwd<N, T> operator+(const Fwd<N, T>& a, const Fwd<N, T>& b) {
-  Fwd<N, T> r; r.v = a.v + b.v;
-#pragma unroll
-  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] + b.d[i];
-  return r;
-}
-template <int N, class T> __device__ __forceinline__ Fwd<N, T> operator-(const Fwd<N, T>& a, const Fwd<N, T>& b) {
-  Fwd<N, T> r; r.v = a.v - b.v;
-#pragma unroll
-  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] - b.d[i];
-  return r;
-}
-template <int N, class T> __device__ __forceinline__ Fwd<N, T> operator*(const Fwd<N, T>& a, const Fwd<N, T>& b) {
-  Fwd<N, T> r; r.v = a.v * b.v;
-#pragma unroll
-  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] * b.v + a.v * b.d[i];
-  return r;
-}
-template <int N, class T> __device__ __forceinline__ Fwd<N, T> operator/(const Fwd<N, T>& a, const Fwd<N, T>& b) {
-  Fwd<N, T> r; r.v = a.v / b.v;
-#pragma unroll
-  for (int i = 0; i < N; ++i) r.d[i] = (a.d[i] - r.v * b.d[i]) / b.v;
-  return r;
-}
-template <int N, class T> __device__ __forceinline__ Fwd<N, T> nsqrt(const Fwd<N, T>& a) {
-  Fwd<N, T> r; r.v = nsqrt(a.v);
-  const T k = Num<T>::c(0.5f) / r.v;
-#pragma unroll
-  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] * k;
-  return r;
-}
-template <int N, class T> __device__ __forceinline__ Fwd<N, T> nsin(const Fwd<N, T>& a) {
-  Fwd<N, T> r; r.v = nsin(a.v);
-  const T c = ncos(a.v);
-#pragma unroll
-  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] * c;
-  return r;
-}
-template <int N, class T> __device__ __forceinline__ Fwd<N, T> ncos(const Fwd<N, T>& a) {
-  Fwd<N, T> r; r.v = ncos(a.v);
-  const T s = Num<T>::c(0.f) - nsin(a.v);
-#pragma unroll
-  for (int i = 0; i < N; ++i) r.d[i] = a.d[i] * s;
-  return r;
-}
-
-// SE3Field.warp tail (warping.py:330-352; rigid_body.py:54-97) over any scalar type:
-// in[0..5] = w, v, in[6..] = (pivot), (translation); x = the point.
-template <class S>
-__device__ void se3_generic(const S* in, const S* x_in, bool pivot, bool trans, S* out) {
-  const S zero = Num<S>::c(0.f), one = Num<S>::c(1.f);
-  const S theta = nsqrt(in[0] * in[0] + in[1] * in[1] + in[2] * in[2]);
-  const S w[3] = {in[0] / theta, in[1] / theta, in[2] / theta};
-  const S v[3] = {in[3] / theta, in[4] / theta, in[5] / theta};
-  S x[3] = {x_in[0], x_in[1], x_in[2]};
-  const S* pv = in + 6;
-  const S* tr = in + (pivot ? 9 : 6);
-  if (pivot)
-    for (int c = 0; c < 3; ++c) x[c] = x[c] + pv[c];
-  const S W[3][3] = {{zero, zero - w[2], w[1]}, {w[2], zero, zero - w[0]}, {zero - w[1], w[0], zero}};
-  S W2[3][3];
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) W2[i][j] = W[i][0] * W[0][j] + W[i][1] * W[1][j] + W[i][2] * W[2][j];
-  const S s = nsin(theta), c = ncos(theta);
-  const S omc = one - c, tms = theta - s;
-  for (int i = 0; i < 3; ++i) {
-    S rx = zero, p = zero;
-    for (int j = 0; j < 3; ++j) {
-      const S eye = (i == j) ? one : zero;
-      const S R = eye + s * W[i][j] + omc * W2[i][j];
-      const S M = theta * eye + omc * W[i][j] + tms * W2[i][j];
-      rx = rx + R * x[j];
-      p = p + M * v[j];
-    }
-    out[i] = rx + p;
-    if (pivot) out[i] = out[i] - pv[i];
-    if (trans) out[i] = out[i] + tr[i];
-  }
-}
-
-// ---------------------------------------------------------------------------
 // utils.general_loss_with_squared_residual (utils.py:264-331) and d loss / d squared_x.
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ void general_loss(float sq, float alpha, float scale, float& loss, float& dloss) {
@@ -355,7 +251,7 @@ __device__ void se3_second_order(const float* h, const float Th[3][12], const fl
     if (q >= kQ0 && q < kQ0 + 4 && q < nh) in[q].d[q - kQ0].v = 1.f;
   }
   for (int c = 0; c < 3; ++c) { xs[c] = Num<Out>::c(x[c]); xs[c].v.d[c] = 1.f; }
-  se3_generic<Out>(in, xs, pivot, trans, out);
+  se3_tail(in, xs, pivot, trans, out);
   for (int q = kQ0; q < kQ0 + 4 && q < nh; ++q) {
     float acc = 0.f;
     for (int i = 0; i < 3; ++i)
@@ -375,8 +271,7 @@ __global__ void __launch_bounds__(64) jac_elastic_kernel(const JacArgs a) {
     for (int j = 0; j < 3; ++j) Th[j][q] = q < nh ? a.thead[(r * 3 + j) * a.ld + q] : 0.f;
   }
   for (int c = 0; c < 3; ++c) x[c] = a.pts[row * 3 + c];
-  // first derivatives of the tail w.r.t. the head outputs (needed for d_thead too)
-  float dy_dh[3][12];
+  // J = d warp / d x: forward mode over the point, the head outputs carry their tangents Th
   if (a.warp_type == 2) {
     using S = Fwd<3, float>;
     S in[12], xs[3], out[3];
@@ -385,7 +280,7 @@ __global__ void __launch_bounds__(64) jac_elastic_kernel(const JacArgs a) {
       for (int j = 0; j < 3; ++j) in[q].d[j] = Th[j][q];
     }
     for (int c = 0; c < 3; ++c) { xs[c] = Num<S>::c(x[c]); xs[c].d[c] = 1.f; }
-    se3_generic<S>(in, xs, a.pivot != 0, a.trans != 0, out);
+    se3_tail(in, xs, a.pivot != 0, a.trans != 0, out);
     for (int i = 0; i < 3; ++i)
       for (int j = 0; j < 3; ++j) J[i][j] = out[i].d[j];
   } else {
@@ -418,20 +313,12 @@ __global__ void __launch_bounds__(64) jac_elastic_kernel(const JacArgs a) {
       for (int q = 0; q < 3; ++q) a.d_thead[(r * 3 + j) * a.ld + q] = G[q][j];     // J_qj = delta + Th[j][q]
     return;
   }
-  {
-    // d y_i / d head_q at (h, x): one direction per head output
-    using S = Fwd<12, float>;
-    S in[12], xs[3], out[3];
-    for (int q = 0; q < 12; ++q) { in[q] = Num<S>::c(h[q]); if (q < nh) in[q].d[q] = 1.f; }
-    for (int c = 0; c < 3; ++c) xs[c] = Num<S>::c(x[c]);
-    se3_generic<S>(in, xs, a.pivot != 0, a.trans != 0, out);
-    for (int i = 0; i < 3; ++i)
-      for (int q = 0; q < 12; ++q) dy_dh[i][q] = out[i].d[q];
-  }
+  Fwd<12, float> y[3];
+  se3_head_jacobian(h, x, nh, a.pivot != 0, a.trans != 0, y);
   // J_ij = sum_q dy_i/dh_q Th[j][q] + dy_i/dx_j  ->  dL/dTh[j][q] = sum_i G_ij dy_i/dh_q
   for (int j = 0; j < 3; ++j)
     for (int q = 0; q < nh; ++q)
-      a.d_thead[(r * 3 + j) * a.ld + q] = G[0][j] * dy_dh[0][q] + G[1][j] * dy_dh[1][q] + G[2][j] * dy_dh[2][q];
+      a.d_thead[(r * 3 + j) * a.ld + q] = G[0][j] * y[0].d[q] + G[1][j] * y[1].d[q] + G[2][j] * y[2].d[q];
   float dh[12];
   for (int q = 0; q < 12; ++q) dh[q] = 0.f;
   se3_second_order<0>(h, Th, x, nh, a.pivot != 0, a.trans != 0, G, dh);
