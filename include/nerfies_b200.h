@@ -287,6 +287,30 @@ int nfb_camera_rays(const nfb_camera* cam, long long first_pixel, long long coun
 int nfb_pixels_to_rays(const nfb_camera* cam, const float* pixels, long long n,
                        float* directions, void* stream);
 
+/* ---- per-frame image metrics of eval.py:process_batch ------------------------
+ * Images are (num_images, height, width, channels) float32, channels interleaved (what
+ * render_frame returns for 'rgb'), channels in 1..4, height and width >= 161 (MS-SSIM's five
+ * scales must each be at least 11x11).  No handle; the caller provides the workspace.
+ *
+ * Bytes of device workspace nfb_image_metrics needs for this shape (< 0: invalid shape). */
+long long nfb_image_metrics_workspace_size(int num_images, int height, int width, int channels);
+
+/* eval.py:process_batch metrics (eval.py:58-62, 120-122, 140) for num_images (h, w, c) images:
+ *   ms_ssim (N)   = tf.image.ssim_multiscale(target, image, max_val=1) with TF's defaults (power
+ *                   factors 0.0448 0.2856 0.3001 0.2363 0.1333, 11x11 Gaussian of sigma 1.5,
+ *                   k1 0.01, k2 0.03);
+ *   mse (N)       = mean((image - target)^2);
+ *   depth_abs (N) = nanmean(|depth_target - depth|) over (h, w) per image (depth, depth_target
+ *                   (N, h, w), nullable together; NaN when every difference is NaN).
+ * Output pointers are device pointers and nullable.  workspace: device, 256-byte aligned, at least
+ * nfb_image_metrics_workspace_size bytes.  Sums are taken in a fixed order in fp64: two calls on
+ * the same input give bit-identical results. */
+int nfb_image_metrics(int num_images, int height, int width, int channels,
+                      const float* image, const float* target,
+                      const float* depth, const float* depth_target,
+                      void* workspace, long long workspace_bytes,
+                      float* ms_ssim, float* mse, float* depth_abs, void* stream);
+
 /* Test hook for the abort path described in the conventions above: while enabled,
  * the weight producer of the tensor-core kernel first waits on an mbarrier that never
  * completes, so the launch must time out, drain and raise the abort flag

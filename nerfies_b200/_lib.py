@@ -20,6 +20,7 @@ SYMBOLS = [
     'nfb_camera_rays', 'nfb_pixels_to_rays', 'nfb_selftest_gemm3',
     'nfb_debug_provoke_timeout', 'nfb_set_time_alpha', 'nfb_train_value_and_grad', 'nfb_adam_step',
     'nfb_train_value_and_grad_reg', 'nfb_warp_jacobian', 'nfb_check_abort', 'nfb_reset_abort',
+    'nfb_image_metrics_workspace_size', 'nfb_image_metrics',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -182,6 +183,10 @@ def load():
   lib.nfb_camera_rays.restype = ci
   lib.nfb_pixels_to_rays.argtypes = [ctypes.POINTER(NfbCamera), vp, ll, vp, vp]
   lib.nfb_pixels_to_rays.restype = ci
+  lib.nfb_image_metrics_workspace_size.argtypes = [ci, ci, ci, ci]
+  lib.nfb_image_metrics_workspace_size.restype = ll
+  lib.nfb_image_metrics.argtypes = [ci, ci, ci, ci, vp, vp, vp, vp, vp, ll, vp, vp, vp, vp]
+  lib.nfb_image_metrics.restype = ci
   lib.nfb_selftest_gemm3.argtypes = [ci, ci, vp, vp, vp, ci, vp, vp]
   lib.nfb_selftest_gemm3.restype = ci
   lib.nfb_debug_provoke_timeout.argtypes = [vp, ci]

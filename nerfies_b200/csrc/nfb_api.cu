@@ -16,6 +16,7 @@
 #include "field_simt.cuh"
 #include "ray_kernels.cuh"
 #include "camera_kernels.cuh"
+#include "metrics_kernels.cuh"
 #include "tc_common.cuh"
 #include "tc_selftest.cuh"
 #include "field_tc.cuh"
@@ -468,6 +469,94 @@ int check_call(nfb_handle* h, int B) {
   return 0;
 }
 
+// Workspace of nfb_image_metrics: levels 1..4 of both images, then the fp64 partials of each
+// scale's SSIM CTAs and of the level-0 downsample CTAs; every region 256-byte aligned.
+struct MetricsPlan {
+  int h[nfb::metrics::kScales], w[nfb::metrics::kScales];
+  int tiles_x[nfb::metrics::kScales], tiles_y[nfb::metrics::kScales];
+  long long level_off[nfb::metrics::kScales];   // bytes; X of level k, then Y (k >= 1)
+  long long part_off[nfb::metrics::kScales];
+  int pool_blocks;
+  long long err_off, bytes;
+};
+
+int metrics_plan(int N, int height, int width, int C, MetricsPlan* p) {
+  using namespace nfb::metrics;
+  if (N < 1 || N > 65535) return fail("num_images=%d outside [1, 65535]", N);
+  if (C < 1 || C > 4) return fail("channels=%d outside [1, 4]", C);
+  if (height < kMinSize || width < kMinSize)
+    return fail("MS-SSIM needs images of at least %dx%d (each of the %d scales must be >= %dx%d); got %dx%d",
+                kMinSize, kMinSize, kScales, kTaps, kTaps, height, width);
+  if ((height - kHalo + kTileH - 1) / kTileH > 65535) return fail("height=%d too large", height);
+  auto align = [](long long b) { return (b + 255) / 256 * 256; };
+  long long off = 0;
+  for (int k = 0; k < kScales; ++k) {
+    p->h[k] = k ? (p->h[k - 1] + 1) / 2 : height;
+    p->w[k] = k ? (p->w[k - 1] + 1) / 2 : width;
+    p->tiles_x[k] = (p->w[k] - kHalo + kTileW - 1) / kTileW;
+    p->tiles_y[k] = (p->h[k] - kHalo + kTileH - 1) / kTileH;
+    p->level_off[k] = off;
+    if (k) off += 2 * align((long long)N * p->h[k] * p->w[k] * C * sizeof(float));
+  }
+  for (int k = 0; k < kScales; ++k) {
+    p->part_off[k] = off;
+    off += align((long long)N * C * p->tiles_x[k] * p->tiles_y[k] * 2 * sizeof(double));
+  }
+  p->pool_blocks = (int)(((long long)p->h[1] * p->w[1] + kThreads - 1) / kThreads);
+  p->err_off = off;
+  off += align((long long)N * p->pool_blocks * 3 * sizeof(double));
+  p->bytes = off;
+  return 0;
+}
+
+template <int C>
+void launch_metrics(const MetricsPlan& p, int N, const float* image, const float* target,
+                    const float* depth, const float* depth_target, char* ws, float* ms_ssim,
+                    float* mse, float* depth_abs, cudaStream_t s) {
+  using namespace nfb::metrics;
+  float g[kTaps];                                      // _fspecial_gauss's kernel is the outer product of g
+  double gs = 0.0;
+  for (int t = 0; t < kTaps; ++t) gs += exp(-0.5 * (t - 5) * (t - 5) / (1.5 * 1.5));
+  for (int t = 0; t < kTaps; ++t) g[t] = (float)(exp(-0.5 * (t - 5) * (t - 5) / (1.5 * 1.5)) / gs);
+  const float* x = image;
+  const float* y = target;
+  for (int k = 0; k < kScales; ++k) {
+    if (k < kScales - 1) {                             // level k + 1 (and, from level 0, MSE / depth)
+      PoolArgs pa{};
+      pa.x = x; pa.y = y; pa.h = p.h[k]; pa.w = p.w[k];
+      pa.x_out = reinterpret_cast<float*>(ws + p.level_off[k + 1]);
+      pa.y_out = pa.x_out + (long long)N * p.h[k + 1] * p.w[k + 1] * C;
+      if (k == 0) {
+        pa.err_part = reinterpret_cast<double*>(ws + p.err_off);
+        pa.depth = depth; pa.depth_target = depth_target;
+      }
+      const long long blocks = ((long long)p.h[k + 1] * p.w[k + 1] + kThreads - 1) / kThreads;
+      downsample_kernel<C><<<dim3((unsigned)blocks, N), kThreads, 0, s>>>(pa);
+    }
+    SsimArgs sa{};
+    sa.x = x; sa.y = y; sa.h = p.h[k]; sa.w = p.w[k];
+    sa.tiles_x = p.tiles_x[k]; sa.tiles_y = p.tiles_y[k];
+    sa.part = reinterpret_cast<double*>(ws + p.part_off[k]);
+    for (int t = 0; t < kTaps; ++t) sa.g[t] = g[t];
+    ssim_level_kernel<C><<<dim3(sa.tiles_x, sa.tiles_y, N), kThreads, 0, s>>>(sa);
+    if (k < kScales - 1) {
+      x = reinterpret_cast<const float*>(ws + p.level_off[k + 1]);
+      y = x + (long long)N * p.h[k + 1] * p.w[k + 1] * C;
+    }
+  }
+  FinalArgs fa{};
+  fa.C = C; fa.pool_blocks = p.pool_blocks;
+  fa.values = (long long)p.h[0] * p.w[0] * C;
+  for (int k = 0; k < kScales; ++k) {
+    fa.tiles[k] = p.tiles_x[k] * p.tiles_y[k];
+    fa.outputs[k] = (long long)(p.h[k] - kHalo) * (p.w[k] - kHalo);
+    fa.part[k] = reinterpret_cast<const double*>(ws + p.part_off[k]);
+  }
+  fa.err_part = reinterpret_cast<const double*>(ws + p.err_off);
+  fa.ms_ssim = ms_ssim; fa.mse = mse; fa.depth_abs = depth_abs;
+  finalize_kernel<<<N, kThreads, 0, s>>>(fa);
+}
+
 }  // namespace
 
 extern "C" {
@@ -514,6 +603,39 @@ int nfb_pixels_to_rays(const nfb_camera* cam, const float* pixels, long long n, 
                        void* stream) {
   if (!pixels && n > 0) return fail("null argument");
   return launch_camera(cam, pixels, 0, n, nullptr, directions, nullptr, stream);
+}
+
+long long nfb_image_metrics_workspace_size(int num_images, int height, int width, int channels) {
+  MetricsPlan p;
+  return metrics_plan(num_images, height, width, channels, &p) ? -1 : p.bytes;
+}
+
+int nfb_image_metrics(int num_images, int height, int width, int channels, const float* image,
+                      const float* target, const float* depth, const float* depth_target, void* workspace,
+                      long long workspace_bytes, float* ms_ssim, float* mse, float* depth_abs, void* stream) {
+  MetricsPlan p;
+  if (metrics_plan(num_images, height, width, channels, &p)) return -1;
+  if (!image || !target) return fail("image and target must not be null");
+  if ((depth == nullptr) != (depth_target == nullptr)) return fail("depth and depth_target are nullable only together");
+  if (depth_abs && !depth) return fail("depth_abs needs depth and depth_target");
+  if (!workspace || workspace_bytes < p.bytes)
+    return fail("workspace of %lld bytes is smaller than the %lld bytes nfb_image_metrics_workspace_size returns",
+                workspace ? workspace_bytes : 0ll, p.bytes);
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail("workspace must be 256-byte aligned");
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
+    return fail("no CUDA device: nerfies_b200 has no CPU path");
+  char* ws = static_cast<char*>(workspace);
+  cudaStream_t s = (cudaStream_t)stream;
+  switch (channels) {
+    case 1: launch_metrics<1>(p, num_images, image, target, depth, depth_target, ws, ms_ssim, mse, depth_abs, s); break;
+    case 2: launch_metrics<2>(p, num_images, image, target, depth, depth_target, ws, ms_ssim, mse, depth_abs, s); break;
+    case 3: launch_metrics<3>(p, num_images, image, target, depth, depth_target, ws, ms_ssim, mse, depth_abs, s); break;
+    default: launch_metrics<4>(p, num_images, image, target, depth, depth_target, ws, ms_ssim, mse, depth_abs, s); break;
+  }
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("image metrics launch failed: %s", cudaGetErrorString(e));
+  return 0;
 }
 
 int nfb_debug_provoke_timeout(nfb_handle* h, int enabled) {

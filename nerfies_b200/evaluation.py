@@ -13,12 +13,21 @@ datasets/core.py:50-75): every rank generates the rays of its contiguous slab of
 the frame on the GPU (camera_rays_kernel), renders it in large launches, and the
 frame is assembled with a single all_gather of 24 B/ray at the end - instead of
 h*w/chunk host round trips with a collective each.
+
+`compute_metrics`, `compute_multiscale_ssim` and `compute_psnr` are the per-frame
+metrics of eval.py:process_batch (eval.py:58-62, 120-122, 140; utils.py:94-103),
+computed on the device by the library's metrics kernels (`nfb_image_metrics`).
 """
+import ctypes
 import math
 import time
 
 import torch
 import torch.distributed as dist
+
+from nerfies_b200 import _lib
+
+MIN_METRICS_SIZE = 161   # MS-SSIM: each of the 5 scales (161 -> 81 -> 41 -> 21 -> 11) >= 11x11
 
 _TREE_TYPES = (dict,)
 _KEYS = (('rgb', slice(0, 3)), ('depth', 3), ('med_depth', 4), ('acc', 5))
@@ -202,3 +211,102 @@ def render_frame(model, params, camera, warp_extra, metadata=None, max_rays=6553
   frame = buf[:total]
   return {k: frame[:, i].reshape((h, w) + ((3,) if k == 'rgb' else ()))
           for k, i in _KEYS}
+
+
+def _check_images(a, b, what):
+  for t in (a, b):
+    if not torch.is_tensor(t):
+      raise ValueError(f'{what} must be torch tensors on a CUDA device')
+  if a.shape != b.shape:
+    raise ValueError(f'{what}: shapes {tuple(a.shape)} and {tuple(b.shape)} differ')
+  if a.dim() not in (3, 4):
+    raise ValueError(f'{what}: expected (h, w, c) or (N, h, w, c) images, got {tuple(a.shape)}')
+  if a.dtype != torch.float32 or b.dtype != torch.float32:
+    raise ValueError(f'{what}: dtype must be float32, got {a.dtype} and {b.dtype}')
+  h, w, c = a.shape[-3:]
+  if h < MIN_METRICS_SIZE or w < MIN_METRICS_SIZE:
+    raise ValueError(f'{what}: MS-SSIM needs images of at least {MIN_METRICS_SIZE}x{MIN_METRICS_SIZE} '
+                     f'(each of its 5 scales must be >= 11x11); got {h}x{w}')
+  if not 1 <= c <= 4:
+    raise ValueError(f'{what}: {c} channels; 1 to 4 are supported')
+  if not (a.is_cuda and b.is_cuda) or a.device != b.device:
+    raise ValueError(f'{what} must live on one CUDA device: nerfies_b200 has no CPU path')
+
+
+def _image_metrics(image, target, depth=None, depth_target=None):
+  """One nfb_image_metrics call on (N, h, w, c) images; returns (ms_ssim, mse, depth_abs), (N,)."""
+  n, h, w, c = image.shape
+  dev = image.device
+  lib = _lib.load()
+  ws_bytes = lib.nfb_image_metrics_workspace_size(n, h, w, c)
+  if ws_bytes < 0:
+    raise ValueError(lib.nfb_last_error().decode())
+  image, target = image.contiguous(), target.contiguous()
+  if depth is not None:
+    depth, depth_target = depth.contiguous(), depth_target.contiguous()
+  out = torch.empty(3, n, dtype=torch.float32, device=dev)
+  ptr = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
+  with torch.cuda.device(dev):
+    workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    _lib.check(lib.nfb_image_metrics(
+        n, h, w, c, ptr(image), ptr(target), ptr(depth), ptr(depth_target), ptr(workspace), ws_bytes,
+        ptr(out[0]), ptr(out[1]), ptr(out[2]) if depth is not None else None,
+        ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+  return out[0], out[1], (out[2] if depth is not None else None)
+
+
+def compute_multiscale_ssim(image1, image2):
+  """eval.py:58-62: tf.image.ssim_multiscale(image1, image2, max_val=1.0) with TF's defaults, on
+  the GPU.  image1, image2: CUDA float32 (h, w, c) or (N, h, w, c), h, w >= 161, c in 1..4.
+  Returns a 0-d or (N,) tensor on the device (the mean over channels, like TF)."""
+  _check_images(image1, image2, 'compute_multiscale_ssim')
+  batched = image1.dim() == 4
+  a, b = (image1, image2) if batched else (image1[None], image2[None])
+  ssim = _image_metrics(a, b)[0]
+  return ssim if batched else ssim[0]
+
+
+def compute_psnr(mse):
+  """utils.py:94-103: PSNR of a mean squared error for pixel values in [0, 1]."""
+  if torch.is_tensor(mse):
+    return -10. * torch.log(mse) / math.log(10.)
+  return -10. * math.log(mse) / math.log(10.)
+
+
+def compute_metrics(rgb, rgb_target, depth_med=None, depth_target=None):
+  """The `out` dict of eval.py:process_batch (eval.py:118-140) from ONE library call:
+  {'mse', 'psnr', 'ssim'} and, with depth, 'depth_abs'.
+
+  rgb, rgb_target: CUDA float32 (h, w, c) or (N, h, w, c) (render_frame's 'rgb' and
+  batch['rgb']); depth_med (h, w) / (N, h, w) and depth_target of the same shape or with a
+  trailing 1 (datasets/core.py:610).  Values are 0-d tensors, or (N,) for a batch; per image.
+
+  depth_abs = nanmean(|depth_target[..., 0] - depth_med|) per pixel.  This deviates from the
+  reference on purpose: eval.py:140 subtracts the (h, w) depth_med from the (h, w, 1)
+  depth_target, a broadcast that raises for a non-square frame and, for a square one, averages
+  the (h, w, w) array of unrelated pairs."""
+  _check_images(rgb, rgb_target, 'compute_metrics')
+  if (depth_med is None) != (depth_target is None):
+    raise ValueError('compute_metrics: pass both depth_med and depth_target, or neither')
+  batched = rgb.dim() == 4
+  image, target = (rgb, rgb_target) if batched else (rgb[None], rgb_target[None])
+  depth = dtarget = None
+  if depth_med is not None:
+    shape = tuple(image.shape[:3])
+    for name, t in (('depth_med', depth_med), ('depth_target', depth_target)):
+      if not torch.is_tensor(t) or t.dtype != torch.float32 or t.device != rgb.device:
+        raise ValueError(f'compute_metrics: {name} must be a float32 tensor on {rgb.device}')
+    if tuple(depth_med.shape) not in (shape, shape[1:]) or (tuple(depth_med.shape) == shape[1:]) == batched:
+      raise ValueError(f'compute_metrics: depth_med shape {tuple(depth_med.shape)} does not match rgb '
+                       f'{tuple(rgb.shape)}')
+    if depth_target.shape[-1:] == (1,) and depth_target.dim() == depth_med.dim() + 1:
+      depth_target = depth_target[..., 0]
+    if depth_target.shape != depth_med.shape:
+      raise ValueError(f'compute_metrics: depth_target shape {tuple(depth_target.shape)} does not match '
+                       f'depth_med {tuple(depth_med.shape)}')
+    depth, dtarget = depth_med.reshape(shape), depth_target.reshape(shape)
+  ssim, mse, depth_abs = _image_metrics(image, target, depth, dtarget)
+  out = {'mse': mse, 'psnr': compute_psnr(mse), 'ssim': ssim}
+  if depth_abs is not None:
+    out['depth_abs'] = depth_abs
+  return out if batched else {k: v[0] for k, v in out.items()}
