@@ -90,18 +90,10 @@ int build_programs(nfb_handle* h) {
   const nfb_config& c = h->cfg;
   Builder b{h};
   const bool use_warp = c.warp_field_type != NFB_WARP_NONE;
-  const int G = use_warp ? c.num_warp_features : 0;
-  const int A = c.num_appearance_features;
-  const int tc = (c.use_appearance_metadata && c.use_trunk_condition) ? A : 0;
-  const int ac = (c.use_appearance_metadata && c.use_alpha_condition) ? A : 0;
-  int rc = 0;
-  if (c.use_viewdirs) rc += 3 + 6 * c.num_nerf_viewdir_freqs;
-  rc += ac;  // models.py:206-207: guarded by use_alpha_condition
-  if (c.use_camera_metadata) rc += c.num_camera_features;
+  const nfb::CondLayout& L = h->cond_layout = nfb::cond_layout(c);
+  const int G = L.G, A = L.A, tc = L.tc, ac = L.ac, rc = L.rc();
   const int Dp = 3 + 6 * c.num_nerf_point_freqs;
   const int Dw = 3 + 6 * c.num_warp_freqs + G;
-  h->cond_stride = G + tc + ac + rc;
-  if (h->cond_stride == 0) h->cond_stride = 1;
   if (Dp + tc + ac + rc > nfb::kMaxIn || (use_warp && Dw > nfb::kMaxIn))
     return fail("input feature block wider than %d", nfb::kMaxIn);
   auto check_width = [&](int w, const char* what) {
@@ -218,7 +210,7 @@ int build_programs(nfb_handle* h) {
     p.Fw = c.num_warp_freqs; p.G = G; p.Dw = Dw;
     p.Fp = c.num_nerf_point_freqs; p.Dp = Dp;
     p.tc = tc; p.ac = ac; p.rc = rc;
-    p.cond_stride = h->cond_stride;
+    p.cond_stride = L.stride;
     p.hidden_act = c.activation; p.sigma_act = c.sigma_activation;
     p.alpha_slot = nfb::kOut0; p.rgb_slot = nfb::kOut1;
   }
@@ -315,14 +307,11 @@ int run_cond(nfb_handle* h, int B, const float* viewdirs, const unsigned* warp_i
   a.viewdirs = viewdirs; a.warp_id = warp_id; a.app_id = app_id; a.cam_id = cam_id;
   a.warp_table = h->d_warp_table; a.app_table = h->d_app_table; a.cam_table = h->d_cam_table;
   a.n_warp = c.num_warp_embeddings; a.n_app = c.num_appearance_embeddings; a.n_cam = c.num_camera_embeddings;
-  a.G = h->prog[0].G; a.A = c.num_appearance_features; a.C = c.num_camera_features;
-  a.Fv = c.num_nerf_viewdir_freqs;
-  a.use_viewdirs = c.use_viewdirs; a.use_app = c.use_appearance_metadata; a.use_cam = c.use_camera_metadata;
-  a.use_trunk_c = c.use_trunk_condition; a.use_alpha_c = c.use_alpha_condition;
-  a.stride = h->cond_stride; a.cond = h->d_cond; a.num_rays = B;
+  a.layout = h->cond_layout; a.cond = h->d_cond; a.num_rays = B;
   a.encoded = encoded;
-  if (h->prog[0].G + h->prog[0].tc + h->prog[0].ac + h->prog[0].rc == 0) return 0;
-  const long long total = (long long)B * a.stride;
+  const nfb::CondLayout& L = h->cond_layout;
+  if (L.G + L.tc + L.ac + L.rc() == 0) return 0;
+  const long long total = (long long)B * L.stride;
   const int enc = c.warp_field_type != NFB_WARP_NONE ? c.warp_metadata_encoder : NFB_WARP_ENC_GLO;
   if (enc == NFB_WARP_ENC_TIME && !encoded) a.warp_id = nullptr;   // `warp_id` carries float timestamps
   nfb::ray_cond_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(a);
@@ -337,7 +326,7 @@ int run_cond(nfb_handle* h, int B, const float* viewdirs, const unsigned* warp_i
     const float alpha = enc == NFB_WARP_ENC_TIME ? h->time_alpha : (float)t.F;   // modules.py:318-319
     easing_window(alpha, t.F, t.window);
     t.blend = enc == NFB_WARP_ENC_BLEND; t.time_alpha = h->time_alpha;
-    t.cond = h->d_cond; t.stride = h->cond_stride; t.G = h->prog[0].G; t.num_rays = B;
+    t.cond = h->d_cond; t.stride = L.stride; t.G = L.G; t.num_rays = B;
     nfb::time_embed_kernel<<<(B + nfb::kTimeRays - 1) / nfb::kTimeRays, nfb::kTimeThreads, 0, s>>>(t);
     return launch_check(h, "time_embed_kernel");
   }
@@ -773,7 +762,7 @@ int nfb_create(const nfb_config* cfg, int max_rays, nfb_handle** out) {
       dmalloc(&h->d_warp_table, (long long)c.num_warp_embeddings * c.num_warp_features) ||
       dmalloc(&h->d_app_table, (long long)c.num_appearance_embeddings * c.num_appearance_features) ||
       dmalloc(&h->d_cam_table, (long long)c.num_camera_embeddings * c.num_camera_features) ||
-      dmalloc(&h->d_cond, B * h->cond_stride) || dmalloc(&h->d_zc, B * nc) ||
+      dmalloc(&h->d_cond, B * h->cond_layout.stride) || dmalloc(&h->d_zc, B * nc) ||
       dmalloc(&h->d_zf, B * nfine) || dmalloc(&h->d_wc, B * nc) ||
       dmalloc(&h->d_samples, B * nfine * 4) || dmalloc(&h->d_out_c, B * 6) ||
       dmalloc(&h->d_out_f, B * 6) || dmalloc(&h->d_in, B * 9))

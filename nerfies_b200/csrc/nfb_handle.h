@@ -12,6 +12,7 @@
 
 #include "../../include/nerfies_b200.h"
 #include "common.cuh"
+#include "ray_kernels.cuh"
 #include "tc_program.cuh"
 
 namespace {
@@ -84,7 +85,7 @@ struct nfb_handle {
   bool profiling = false;
   cudaEvent_t ev[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};
   bool ev_valid[2] = {false, false};
-  int cond_stride = 0;
+  nfb::CondLayout cond_layout{};      // per-ray condition vectors (d_cond, d_dcond)
   int sm_count = 132;
   nfb::Net time_net{};                // TimeEncoder MLP ('time' / 'blend' warp metadata encoders)
   float time_alpha = 0.f;             // warp_extra['time_alpha'] (nfb_set_time_alpha)

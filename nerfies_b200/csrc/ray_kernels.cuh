@@ -5,14 +5,60 @@
 #pragma once
 #include <math_constants.h>
 
+#include "../../include/nerfies_b200.h"
 #include "common.cuh"
 
 namespace nfb {
 
 // ---------------------------------------------------------------------------
-// get_condition_inputs (models.py:186-228) + GloEncoder (glo.py:41-53): one
-// vector per ray  [warp glo code (G) | trunk cond | alpha cond | rgb cond].
+// The per-ray condition vector of get_condition_inputs (models.py:186-228):
+//   [warp glo code (G) | trunk (tc) | alpha (ac) | rgb: viewdir posenc (dv), appearance (ac), camera (cc)]
+// The rgb condition repeats the appearance code iff it is the alpha condition (models.py:206-207).
 // ---------------------------------------------------------------------------
+struct CondLayout {
+  int G, tc, ac, dv, cc;          // block widths (0: absent)
+  int A, C;                       // appearance / camera table widths
+  int stride;                     // floats per ray (1 when every block is absent)
+  __host__ __device__ int rc() const { return dv + ac + cc; }
+};
+
+inline CondLayout cond_layout(const nfb_config& c) {
+  CondLayout L{};
+  L.G = c.warp_field_type != NFB_WARP_NONE ? c.num_warp_features : 0;
+  L.A = c.num_appearance_features;
+  L.C = c.num_camera_features;
+  L.tc = (c.use_appearance_metadata && c.use_trunk_condition) ? L.A : 0;
+  L.ac = (c.use_appearance_metadata && c.use_alpha_condition) ? L.A : 0;
+  L.dv = c.use_viewdirs ? 3 + 6 * c.num_nerf_viewdir_freqs : 0;
+  L.cc = c.use_camera_metadata ? L.C : 0;
+  L.stride = L.G + L.tc + L.ac + L.rc();
+  if (L.stride == 0) L.stride = 1;
+  return L;
+}
+
+enum CondSource { kCondWarp, kCondApp, kCondViewdir, kCondCam, kCondPad };
+
+// Where column q of the condition vector comes from; j = the column within that source.
+__device__ __forceinline__ CondSource cond_source(const CondLayout& L, int q, int& j) {
+  if (q < L.G) { j = q; return kCondWarp; }
+  q -= L.G;
+  if (q < L.tc) { j = q; return kCondApp; }
+  q -= L.tc;
+  if (q < L.ac) { j = q; return kCondApp; }
+  q -= L.ac;
+  if (q < L.dv) { j = q; return kCondViewdir; }
+  q -= L.dv;
+  if (q < L.ac) { j = q; return kCondApp; }
+  q -= L.ac;
+  j = q;
+  return q < L.cc ? kCondCam : kCondPad;
+}
+
+// Embedding-table row of a ray (GloEncoder, glo.py:41-53): row 0 without ids, ids past the table clamp.
+__device__ __forceinline__ size_t embed_row(const unsigned* ids, int ray, int n) {
+  return min(ids ? ids[ray] : 0u, (unsigned)(n - 1));
+}
+
 struct CondArgs {
   const float* viewdirs;          // (B,3)
   const unsigned* warp_id;        // (B) or null
@@ -22,64 +68,35 @@ struct CondArgs {
   const float* app_table;         // (n_app, A)
   const float* cam_table;         // (n_cam, C)
   int n_warp, n_app, n_cam;
-  int G, A, C, Fv;
-  int use_viewdirs, use_app, use_cam;
-  int use_trunk_c, use_alpha_c;   // models.py:202-207
-  int stride;
+  CondLayout layout;
   float* cond;                    // (B, stride)
   int num_rays;
   int encoded;                    // metadata_encoded=True: the id pointers are (B, G|A|C) float embeddings
 };
 
 __global__ void ray_cond_kernel(const CondArgs a) {
+  const CondLayout& L = a.layout;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (long long)a.num_rays * a.stride) return;
-  const int ray = (int)(idx / a.stride);
-  int q = (int)(idx - (long long)ray * a.stride);
-  float v = 0.f;
-  auto app = [&](int j) {
-    if (a.encoded && a.app_id)      // models.py:198-199
-      return reinterpret_cast<const float*>(a.app_id)[(size_t)ray * a.A + j];
-    unsigned id = a.app_id ? a.app_id[ray] : 0u;
-    id = min(id, (unsigned)(a.n_app - 1));
-    return a.app_table[(size_t)id * a.A + j];
+  if (idx >= (long long)a.num_rays * L.stride) return;
+  const int ray = (int)(idx / L.stride);
+  int j;
+  const CondSource src = cond_source(L, (int)(idx - (long long)ray * L.stride), j);
+  // warping.py:186-187, models.py:198-199, 210-211: metadata_encoded passes the embeddings themselves
+  auto embed = [&](const unsigned* ids, const float* table, int n, int width) {
+    if (a.encoded && ids) return reinterpret_cast<const float*>(ids)[(size_t)ray * width + j];
+    return table[embed_row(ids, ray, n) * width + j];
   };
-  do {
-    if (q < a.G) {
-      if (a.encoded && a.warp_id) {   // warping.py:186-187
-        v = reinterpret_cast<const float*>(a.warp_id)[(size_t)ray * a.G + q];
-        break;
-      }
-      unsigned id = a.warp_id ? a.warp_id[ray] : 0u;
-      id = min(id, (unsigned)(a.n_warp - 1));
-      v = a.warp_table[(size_t)id * a.G + q];
-      break;
-    }
-    q -= a.G;
-    const int tc = (a.use_app && a.use_trunk_c) ? a.A : 0;
-    if (q < tc) { v = app(q); break; }
-    q -= tc;
-    const int ac = (a.use_app && a.use_alpha_c) ? a.A : 0;
-    if (q < ac) { v = app(q); break; }
-    q -= ac;
-    // rgb condition: [viewdir posenc][appearance iff use_alpha_condition][camera].
-    const int dv = a.use_viewdirs ? 3 + 6 * a.Fv : 0;
-    if (q < dv) {
-      float d[3] = {a.viewdirs[ray * 3 + 0], a.viewdirs[ray * 3 + 1], a.viewdirs[ray * 3 + 2]};
-      v = (q < 3) ? d[q] : posenc_feature(d, q - 3);
-      break;
-    }
-    q -= dv;
-    if (q < ac) { v = app(q); break; }
-    q -= ac;
-    if (a.encoded && a.cam_id) {      // models.py:210-211
-      v = reinterpret_cast<const float*>(a.cam_id)[(size_t)ray * a.C + q];
-      break;
-    }
-    unsigned id = a.cam_id ? a.cam_id[ray] : 0u;
-    id = min(id, (unsigned)(a.n_cam - 1));
-    v = a.cam_table[(size_t)id * a.C + q];
-  } while (false);
+  float v = 0.f;
+  if (src == kCondWarp) {
+    v = embed(a.warp_id, a.warp_table, a.n_warp, L.G);
+  } else if (src == kCondApp) {
+    v = embed(a.app_id, a.app_table, a.n_app, L.A);
+  } else if (src == kCondCam) {
+    v = embed(a.cam_id, a.cam_table, a.n_cam, L.C);
+  } else if (src == kCondViewdir) {
+    const float d[3] = {a.viewdirs[ray * 3 + 0], a.viewdirs[ray * 3 + 1], a.viewdirs[ray * 3 + 2]};
+    v = (j < 3) ? d[j] : posenc_feature(d, j - 3);
+  }
   a.cond[idx] = v;
 }
 

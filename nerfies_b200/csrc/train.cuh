@@ -5,7 +5,7 @@
 // Unlike the fused forward kernels this path is layer-wise: the forward pass keeps a
 // TAPE in HBM (every Dense layer's output, the encoded inputs, the sample points) and
 // the backward pass walks it in reverse.  All kernels are hand-written fp32 SIMT:
-//   * sgemm_kernel: one tiled GEMM template for the three shapes of a Dense layer
+//   * sgemm128_kernel: one tiled GEMM template for the three shapes of a Dense layer
 //       forward   Y  = act([X | IN] W + b)
 //       backward  dX = dZ W^T         (dZ = dY * act'(Y), formed while loading)
 //                 dW = [X | IN]^T dZ  (reduction over the rows: split + atomicAdd)
@@ -88,9 +88,6 @@ template <int N, class T> __device__ __forceinline__ Fwd<N, T> ncos(const Fwd<N,
 
 namespace train {
 
-constexpr int kTile = 64;      // C tile (kTile x kTile), 256 threads, 4 x 4 per thread
-constexpr int kBK = 16;
-
 // activation derivative expressed through the OUTPUT y = act(z) (every registered
 // activation is invertible enough for that: configs.py:27-32).
 __device__ __forceinline__ float act_grad_from_output(float y, int act) {
@@ -107,72 +104,17 @@ __device__ __forceinline__ float act_grad_from_output(float y, int act) {
 
 // ---------------------------------------------------------------------------
 // One GEMM template.  C(m, n) (+)= sum_k A(m, k) * B(k, n) with element functors:
-// slow address arithmetic, fast inner product (shared-memory tiles, 4x4 register
-// tile).  gridDim.z splits the reduction (kSplitAtomic: results are atomicAdd-ed).
+// slow address arithmetic, fast inner product.  gridDim.z splits the reduction
+// (k_per_split; the caller's FC then atomicAdd-s).
+// The layer-wise training tier is GEMM-bound (3 x the forward FLOPs per step), so the
+// inner product is shaped for shared-memory bandwidth: a 128 x 128 C tile, an 8 x 8
+// register tile per thread (two 4 x 4 quadrant pairs, so that every shared-memory read
+// is a 16-byte vector and the A reads are warp broadcasts: 64 FMAs per 4 LDS.128),
+// k-steps of 8 and a register prefetch of the next k-step's operands under the
+// arithmetic of the current one (one __syncthreads per step).
 // ---------------------------------------------------------------------------
 struct GemmShape { long long M; int N; long long K; };
 
-template <class FA, class FB, class FC>
-__global__ void __launch_bounds__(256)
-sgemm_kernel(GemmShape sh, FA fa, FB fb, FC fc, long long k_per_split) {
-  __shared__ float As[kBK][kTile + 4];
-  __shared__ float Bs[kBK][kTile + 4];
-  const int tid = threadIdx.x;
-  const int tx = tid & 15, ty = tid >> 4;
-  const long long m0 = (long long)blockIdx.x * kTile;
-  const int n0 = blockIdx.y * kTile;
-  const long long k_begin = (long long)blockIdx.z * k_per_split;
-  const long long k_end = min(sh.K, k_begin + k_per_split);
-  float acc[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-  for (long long k0 = k_begin; k0 < k_end; k0 += kBK) {
-    // A tile: kTile rows x kBK; B tile: kBK x kTile  (4 elements per thread each)
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int idx = tid + e * 256;
-      {
-        const int mm = idx / kBK, kk = idx % kBK;       // consecutive threads walk k: row-major A coalesces
-        const long long m = m0 + mm, k = k0 + kk;
-        As[kk][mm] = (m < sh.M && k < k_end) ? fa(m, k) : 0.f;
-      }
-      {
-        const int kk = idx / kTile, nn = idx % kTile;   // consecutive threads walk n
-        const long long k = k0 + kk;
-        const int n = n0 + nn;
-        Bs[kk][nn] = (k < k_end && n < sh.N) ? fb(k, n) : 0.f;
-      }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int kk = 0; kk < kBK; ++kk) {
-      const float4 a4 = *reinterpret_cast<const float4*>(&As[kk][ty * 4]);
-      const float4 b4 = *reinterpret_cast<const float4*>(&Bs[kk][tx * 4]);
-      const float a[4] = {a4.x, a4.y, a4.z, a4.w}, b[4] = {b4.x, b4.y, b4.z, b4.w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const long long m = m0 + ty * 4 + i;
-      const int n = n0 + tx * 4 + j;
-      if (m < sh.M && n < sh.N) fc(m, n, acc[i][j]);
-    }
-}
-
-// The same GEMM with a 128 x 128 C tile, an 8 x 8 register tile per thread (two 4 x 4 quadrant pairs, so that
-// every shared-memory read is a 16-byte vector and the A reads are warp broadcasts), k-steps of 8 and a register
-// prefetch of the next k-step's operands under the arithmetic of the current one (one __syncthreads per step).
-// 64 FMAs per 4 LDS.128 instead of 16 per 2: the layer-wise training tier is GEMM-bound (3 x the forward FLOPs
-// per step), and this template runs it about twice as fast as sgemm_kernel.
 // kAKFast / kBNFast: which index of the element functor is contiguous in memory (k for a row-major A, n for a
 // row-major B) - the loader walks that index with consecutive threads.
 constexpr int kT2 = 128, kBK2 = 8, kPad2 = 4;
@@ -551,50 +493,29 @@ __global__ void composite_bwd_kernel(const CompositeBwdArgs a) {
 }
 
 // ---------------------------------------------------------------------------
-// Embedding gradients: dcond (B, stride) -> table rows (glo.py:41-53), per the layout
-// ray_cond_kernel wrote: [warp glo (G) | trunk (A) | alpha (A) | rgb: viewdirs, (A), camera].
+// Embedding gradients: dcond (B, stride) -> table rows (glo.py:41-53), the adjoint of
+// ray_cond_kernel over the same layout.
 // ---------------------------------------------------------------------------
 struct CondBwdArgs {
-  const float* dcond; int stride, num_rays;
+  const float* dcond; int num_rays;
   const unsigned* warp_id; const unsigned* app_id; const unsigned* cam_id;
   float* d_warp_table; float* d_app_table; float* d_cam_table;
-  int n_warp, n_app, n_cam, G, A, C, Fv, use_viewdirs, use_app, use_cam, use_trunk_c, use_alpha_c;
+  int n_warp, n_app, n_cam;
+  CondLayout layout;
 };
 __global__ void cond_bwd_kernel(const CondBwdArgs a) {
+  const CondLayout& L = a.layout;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (long long)a.num_rays * a.stride) return;
-  const int ray = (int)(idx / a.stride);
-  int q = (int)(idx - (long long)ray * a.stride);
+  if (idx >= (long long)a.num_rays * L.stride) return;
+  const int ray = (int)(idx / L.stride);
   const float v = a.dcond[idx];
   if (v == 0.f) return;
-  auto app = [&](int j) {
-    unsigned id = a.app_id ? a.app_id[ray] : 0u;
-    id = min(id, (unsigned)(a.n_app - 1));
-    atomicAdd(a.d_app_table + (size_t)id * a.A + j, v);
-  };
-  if (q < a.G) {
-    unsigned id = a.warp_id ? a.warp_id[ray] : 0u;
-    id = min(id, (unsigned)(a.n_warp - 1));
-    atomicAdd(a.d_warp_table + (size_t)id * a.G + q, v);
-    return;
-  }
-  q -= a.G;
-  const int tc = (a.use_app && a.use_trunk_c) ? a.A : 0;
-  if (q < tc) { app(q); return; }
-  q -= tc;
-  const int ac = (a.use_app && a.use_alpha_c) ? a.A : 0;
-  if (q < ac) { app(q); return; }
-  q -= ac;
-  const int dv = a.use_viewdirs ? 3 + 6 * a.Fv : 0;
-  if (q < dv) return;                                   // view directions carry no parameter
-  q -= dv;
-  if (q < ac) { app(q); return; }
-  q -= ac;
-  if (a.use_cam && q < a.C) {
-    unsigned id = a.cam_id ? a.cam_id[ray] : 0u;
-    id = min(id, (unsigned)(a.n_cam - 1));
-    atomicAdd(a.d_cam_table + (size_t)id * a.C + q, v);
-  }
+  int j;
+  const CondSource src = cond_source(L, (int)(idx - (long long)ray * L.stride), j);
+  if (src == kCondWarp) atomicAdd(a.d_warp_table + embed_row(a.warp_id, ray, a.n_warp) * L.G + j, v);
+  else if (src == kCondApp) atomicAdd(a.d_app_table + embed_row(a.app_id, ray, a.n_app) * L.A + j, v);
+  else if (src == kCondCam) atomicAdd(a.d_cam_table + embed_row(a.cam_id, ray, a.n_cam) * L.C + j, v);
+  // view directions carry no parameter
 }
 
 // packed (K x ld, column offset) gradient -> the caller's dense (rows x cols) tensor (+=).

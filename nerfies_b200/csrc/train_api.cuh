@@ -67,15 +67,9 @@ int launch_gemm(nfb_handle* h, long long M, int N, long long K, FA fa, FB fb, FC
                 cudaStream_t s, const char* what) {
   if (M <= 0 || N <= 0 || K <= 0) return 0;
   const long long per = k_split > 0 ? k_split : K;
-#ifdef NFB_TRAIN_SGEMM64
-  dim3 grid((unsigned)((M + nfb::train::kTile - 1) / nfb::train::kTile),
-            (unsigned)((N + nfb::train::kTile - 1) / nfb::train::kTile), (unsigned)((K + per - 1) / per));
-  nfb::train::sgemm_kernel<<<grid, 256, 0, s>>>(nfb::train::GemmShape{M, N, K}, fa, fb, fc, per);
-#else
   dim3 grid((unsigned)((M + nfb::train::kT2 - 1) / nfb::train::kT2),
             (unsigned)((N + nfb::train::kT2 - 1) / nfb::train::kT2), (unsigned)((K + per - 1) / per));
   nfb::train::sgemm128_kernel<kAKFast, kBNFast><<<grid, 256, 0, s>>>(nfb::train::GemmShape{M, N, K}, fa, fb, fc, per);
-#endif
   return launch_check(h, what);
 }
 
@@ -142,20 +136,15 @@ TTapeLayout ttape_layout(const nfb::FieldProgram& p, long long sel_rows) {
   t.total = off;
   return t;
 }
-int ensure_ttape(nfb_handle* h, long long floats, long long sel_rows) {
-  if (h->ttape_floats < floats) {
-    if (h->d_ttape) cudaFree(h->d_ttape);
-    h->d_ttape = nullptr; h->ttape_floats = 0;
-    if (cudaMalloc(&h->d_ttape, (size_t)floats * sizeof(float)) != cudaSuccess)
-      return fail("training: cannot allocate a %.2f GB tangent tape", floats * 4e-9);
-    h->ttape_floats = floats;
-  }
-  if (h->sel_cap < sel_rows) {
-    if (h->d_sel) cudaFree(h->d_sel);
-    h->d_sel = nullptr; h->sel_cap = 0;
-    if (cudaMalloc(&h->d_sel, (size_t)sel_rows * sizeof(int)) != cudaSuccess) return fail("training: cudaMalloc failed");
-    h->sel_cap = sel_rows;
-  }
+// Grows the device buffer *buf of *cap elements to at least n elements (the contents are not kept).
+template <class T>
+int grow(T** buf, long long* cap, long long n, const char* what) {
+  if (*cap >= n) return 0;
+  if (*buf) cudaFree(*buf);
+  *buf = nullptr; *cap = 0;
+  if (cudaMalloc(buf, (size_t)n * sizeof(T)) != cudaSuccess)
+    return fail("training: cannot allocate a %.2f GB %s", n * sizeof(T) * 1e-9, what);
+  *cap = n;
   return 0;
 }
 
@@ -217,7 +206,7 @@ int warp_jacobian_on_tape(nfb_handle* h, const nfb::FieldProgram& p, const TapeL
     if (p.warp.steps[i].act != nfb::kRelu && p.warp.steps[i].act != nfb::kNone)
       return fail("warp Jacobian: the warp MLP must use relu (piecewise-linear) activations");
   const TTapeLayout tt = ttape_layout(p, sel_rows);
-  if (ensure_ttape(h, tt.total, 1)) return -1;
+  if (grow(&h->d_ttape, &h->ttape_floats, tt.total, "tangent tape")) return -1;
   float* T = h->d_ttape;
   if (with_grad) NFB_CUDA(cudaMemsetAsync(T + tt.d_in_t, 0, (size_t)(tt.total - tt.d_in_t) * sizeof(float), s));
   const unsigned tblocks = (unsigned)((tt.trows + 127) / 128);
@@ -231,7 +220,7 @@ int warp_jacobian_on_tape(nfb_handle* h, const nfb::FieldProgram& p, const TapeL
   j.sel = sel; j.row_w = row_w; j.jac_out = jac_out; j.R = sel_rows;
   j.warp_type = p.warp_type; j.pivot = p.warp_pivot; j.trans = p.warp_trans;
   j.with_loss = reg != nullptr; j.loss_type = reg ? reg->type : 0;
-  j.stats = reg ? reg->stats + 2 : nullptr;
+  j.stats = reg ? reg->stats + kSlotElasticLoss : nullptr;
   if (with_grad) {
     j.d_head = A + t.d_out_w[hs]; j.d_thead = T + tt.d_out_t[hs];
     j.grad_scale = reg->elastic_weight / (float)reg->batch_rays;
@@ -245,10 +234,56 @@ int warp_jacobian_on_tape(nfb_handle* h, const nfb::FieldProgram& p, const TapeL
   return 0;
 }
 
-// forward + loss + backward of one level for `R` rays (rows = R * S) on the tape.
+// warp_field.apply on the t.rows rows of the tape: the encoded points (tape.pts, tape.in_w), the warp MLP
+// (tape.out_w) and the tail (tape.warped).  The points are o + z d of the rays' S samples, or, with
+// `points` not null, the rows of `points`; `cond` holds one condition vector per ray (per point).
+int warp_forward(nfb_handle* h, const nfb::FieldProgram& p, const TapeLayout& t, const float* origins,
+                 const float* directions, const float* z, int S, const float* points, const float* cond,
+                 cudaStream_t s) {
+  using namespace nfb::train;
+  float* A = h->d_tape;
+  const unsigned blocks = (unsigned)((t.rows + 127) / 128);
+  EncodeArgs e{};
+  e.origins = origins; e.directions = directions; e.z = z; e.pts_in = points; e.cond = cond; e.window = h->d_window;
+  e.pts_out = A + t.pts; e.in = A + t.in_w; e.F = p.Fw; e.ld = t.ld_w; e.S = S;
+  e.cond_stride = h->cond_layout.stride; e.cond_off = 0; e.n_cond = p.G; e.rows = t.rows;
+  encode_kernel<<<blocks, 128, 0, s>>>(e);
+  if (launch_check(h, "encode_kernel")) return -1;
+  if (net_forward(h, p.warp, A + t.in_w, t.ld_w, t.out_w, A, t.rows, s)) return -1;
+  const int hs = p.warp.n_steps - 1;
+  WarpTailArgs w{A + t.out_w[hs], p.warp.steps[hs].npad, A + t.pts, A + t.warped, p.warp_type, p.warp_pivot,
+                 p.warp_trans, t.rows};
+  warp_tail_kernel<<<blocks, 128, 0, s>>>(w);
+  return launch_check(h, "warp_tail_kernel");
+}
+
+// Adjoint of warp_forward: tape.dwarped -> the warp MLP's parameter gradients and, += per ray of S rows,
+// the warp GLO block of `dcond`.
+int warp_backward(nfb_handle* h, const nfb::FieldProgram& p, const TapeLayout& t, int S, float* dcond,
+                  cudaStream_t s) {
+  using namespace nfb::train;
+  float* A = h->d_tape;
+  const unsigned blocks = (unsigned)((t.rows + 127) / 128);
+  const int hs = p.warp.n_steps - 1;
+  WarpTailBwdArgs w{A + t.out_w[hs], p.warp.steps[hs].npad, A + t.pts, A + t.dwarped, A + t.d_out_w[hs],
+                    p.warp_type, p.warp_pivot, p.warp_trans, t.rows};
+  warp_tail_bwd_kernel<<<blocks, 128, 0, s>>>(w);
+  if (launch_check(h, "warp_tail_bwd_kernel")) return -1;
+  if (net_backward(h, p.warp, A + t.in_w, A + t.d_in_w, t.ld_w, t.out_w, t.d_out_w, A, t.rows, s)) return -1;
+  EncodeBwdArgs e{};
+  e.pts = A + t.pts; e.window = h->d_window; e.din = A + t.d_in_w; e.F = p.Fw; e.ld = t.ld_w; e.S = S;
+  e.cond_stride = h->cond_layout.stride; e.cond_off = 0; e.n_cond = p.G; e.dpts = nullptr; e.dcond = dcond;
+  e.rows = t.rows;
+  encode_bwd_kernel<<<blocks, 128, 0, s>>>(e);
+  return launch_check(h, "encode_bwd_kernel");
+}
+
+// forward + loss + backward of one level for `R` rays (rows = R * S) on the tape; `cond` / `dcond` are
+// the R rays' condition vectors and their gradient accumulator.
 int train_level(nfb_handle* h, int level, int R, int S, const float* z, const float* origins,
-                const float* directions, const float* target, float scale, bool use_warp,
-                float* out6, float* weights, float* loss, cudaStream_t s, const RegCfg* reg = nullptr) {
+                const float* directions, const float* target, const float* cond, float* dcond, float scale,
+                bool use_warp, float* out6, float* weights, float* loss, cudaStream_t s,
+                const RegCfg* reg = nullptr) {
   using namespace nfb::train;
   const nfb::FieldProgram& p = h->prog[level];
   const long long rows = (long long)R * S;
@@ -257,26 +292,13 @@ int train_level(nfb_handle* h, int level, int R, int S, const float* z, const fl
   const bool warp = use_warp && p.warp_type != 0;
   const unsigned blocks = (unsigned)((rows + 127) / 128);
   // ---- forward ----
-  if (warp) {
-    EncodeArgs e{};
-    e.origins = origins; e.directions = directions; e.z = z; e.cond = h->d_cond; e.window = h->d_window;
-    e.pts_out = A + t.pts; e.in = A + t.in_w; e.F = p.Fw; e.ld = t.ld_w; e.S = S;
-    e.cond_stride = h->cond_stride; e.cond_off = 0; e.n_cond = p.G; e.rows = rows;
-    encode_kernel<<<blocks, 128, 0, s>>>(e);
-    if (launch_check(h, "encode_kernel")) return -1;
-    if (net_forward(h, p.warp, A + t.in_w, t.ld_w, t.out_w, A, rows, s)) return -1;
-    const int hs = p.warp.n_steps - 1;
-    WarpTailArgs w{A + t.out_w[hs], p.warp.steps[hs].npad, A + t.pts, A + t.warped, p.warp_type, p.warp_pivot,
-                   p.warp_trans, rows};
-    warp_tail_kernel<<<blocks, 128, 0, s>>>(w);
-    if (launch_check(h, "warp_tail_kernel")) return -1;
-  }
+  if (warp && warp_forward(h, p, t, origins, directions, z, S, nullptr, cond, s)) return -1;
   {
     EncodeArgs e{};
-    e.origins = origins; e.directions = directions; e.z = z; e.cond = h->d_cond; e.window = nullptr;
+    e.origins = origins; e.directions = directions; e.z = z; e.cond = cond; e.window = nullptr;
     e.pts_in = warp ? A + t.warped : nullptr; e.pts_out = warp ? nullptr : A + t.warped;
     e.in = A + t.in_n; e.F = p.Fp; e.ld = t.ld_n; e.S = S;
-    e.cond_stride = h->cond_stride; e.cond_off = p.G; e.n_cond = p.tc + p.ac + p.rc; e.rows = rows;
+    e.cond_stride = h->cond_layout.stride; e.cond_off = p.G; e.n_cond = p.tc + p.ac + p.rc; e.rows = rows;
     encode_kernel<<<blocks, 128, 0, s>>>(e);
     if (launch_check(h, "encode_kernel")) return -1;
   }
@@ -311,7 +333,7 @@ int train_level(nfb_handle* h, int level, int R, int S, const float* z, const fl
   }
   const bool want_sel = reg && warp && ((reg->elastic && level == 0 && reg->reduce == 0) || reg->warp_reg);
   if (want_sel) {
-    if (ensure_ttape(h, 0, R)) return -1;
+    if (grow(&h->d_sel, &h->sel_cap, R, "median-depth row index")) return -1;
     depth_index_kernel<<<(unsigned)((R + 7) / 8), 256, 0, s>>>(weights, R, S, h->d_sel);
     if (launch_check(h, "depth_index_kernel")) return -1;
   }
@@ -326,33 +348,20 @@ int train_level(nfb_handle* h, int level, int R, int S, const float* z, const fl
   {
     EncodeBwdArgs e{};
     e.pts = A + t.warped; e.window = nullptr; e.din = A + t.d_in_n; e.F = p.Fp; e.ld = t.ld_n; e.S = S;
-    e.cond_stride = h->cond_stride; e.cond_off = p.G; e.n_cond = p.tc + p.ac + p.rc;
-    e.dpts = warp ? A + t.dwarped : nullptr; e.dcond = h->d_dcond; e.rows = rows;
+    e.cond_stride = h->cond_layout.stride; e.cond_off = p.G; e.n_cond = p.tc + p.ac + p.rc;
+    e.dpts = warp ? A + t.dwarped : nullptr; e.dcond = dcond; e.rows = rows;
     encode_bwd_kernel<<<blocks, 128, 0, s>>>(e);
     if (launch_check(h, "encode_bwd_kernel")) return -1;
   }
   if (warp && reg && reg->warp_reg) {
     // training.py:194-207: robust loss of |points - warped_points|^2 at the median-depth sample
-    WarpMagArgs wm{A + t.pts, A + t.warped, h->d_sel, A + t.dwarped, reg->stats + (level == 0 ? 7 : 9),
+    WarpMagArgs wm{A + t.pts, A + t.warped, h->d_sel, A + t.dwarped,
+                   reg->stats + (level == 0 ? kSlotWarpRegCoarse : kSlotWarpRegFine),
                    reg->warp_reg_alpha, reg->warp_reg_scale, reg->warp_reg_weight / (float)reg->batch_rays, R};
     warp_mag_loss_kernel<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(wm);
     if (launch_check(h, "warp_mag_loss_kernel")) return -1;
   }
-  if (warp) {
-    const int hs = p.warp.n_steps - 1;
-    WarpTailBwdArgs w{A + t.out_w[hs], p.warp.steps[hs].npad, A + t.pts, A + t.dwarped, A + t.d_out_w[hs],
-                      p.warp_type, p.warp_pivot, p.warp_trans, rows};
-    warp_tail_bwd_kernel<<<blocks, 128, 0, s>>>(w);
-    if (launch_check(h, "warp_tail_bwd_kernel")) return -1;
-    if (net_backward(h, p.warp, A + t.in_w, A + t.d_in_w, t.ld_w, t.out_w, t.d_out_w, A, rows, s)) return -1;
-    EncodeBwdArgs e{};
-    e.pts = A + t.pts; e.window = h->d_window; e.din = A + t.d_in_w; e.F = p.Fw; e.ld = t.ld_w; e.S = S;
-    e.cond_stride = h->cond_stride; e.cond_off = 0; e.n_cond = p.G; e.dpts = nullptr; e.dcond = h->d_dcond;
-    e.rows = rows;
-    encode_bwd_kernel<<<blocks, 128, 0, s>>>(e);
-    if (launch_check(h, "encode_bwd_kernel")) return -1;
-  }
-  return 0;
+  return warp ? warp_backward(h, p, t, S, dcond, s) : 0;
 }
 
 int train_prepare(nfb_handle* h, int chunk_rays) {
@@ -361,12 +370,8 @@ int train_prepare(nfb_handle* h, int chunk_rays) {
   long long need = 0;
   for (int lv = 0; lv < 2; ++lv) need = std::max(need, tape_layout(h->prog[lv], (long long)chunk_rays * smax).total);
   if (h->tape_floats < need) {
-    if (h->d_tape) cudaFree(h->d_tape);
-    h->d_tape = nullptr; h->tape_floats = 0;
-    if (cudaMalloc(&h->d_tape, (size_t)need * sizeof(float)) != cudaSuccess)
-      return fail("training: cannot allocate a %.1f GB tape for %d rays per chunk", need * 4e-9, chunk_rays);
+    if (grow(&h->d_tape, &h->tape_floats, need, "tape")) return -1;
     NFB_CUDA(cudaMemset(h->d_tape, 0, (size_t)need * sizeof(float)));
-    h->tape_floats = need;
   }
   cudaFuncSetAttribute(nfb::train::composite_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
   if (!h->d_gpacked) {
@@ -378,8 +383,9 @@ int train_prepare(nfb_handle* h, int chunk_rays) {
         dm(&h->d_gwarp, (long long)c.num_warp_embeddings * c.num_warp_features) ||
         dm(&h->d_gapp, (long long)c.num_appearance_embeddings * c.num_appearance_features) ||
         dm(&h->d_gcam, (long long)c.num_camera_embeddings * c.num_camera_features) ||
-        dm(&h->d_dcond, (long long)h->max_rays * h->cond_stride) || dm(&h->d_tr_out, (long long)h->max_rays * 12) ||
-        dm(&h->d_tr_w, (long long)h->max_rays * smax) || dm(&h->d_loss, 16))
+        dm(&h->d_dcond, (long long)h->max_rays * h->cond_layout.stride) ||
+        dm(&h->d_tr_out, (long long)h->max_rays * 12) || dm(&h->d_tr_w, (long long)h->max_rays * smax) ||
+        dm(&h->d_loss, nfb::train::kLossSlots))
       return -1;
   }
   return 0;
@@ -392,30 +398,33 @@ int train_prepare_rows(nfb_handle* h, long long rows) {
 }
 
 // warp_field.apply on `n` free points (+ optional noise) on the tape of level 0: condition
-// vectors per point, encoded inputs, warp MLP, tail.  The points land in tape.pts, the warped
-// points in tape.warped.
+// vectors per point, then warp_forward.  The points land in tape.pts, the warped points in tape.warped.
 int warp_points_forward(nfb_handle* h, int n, const float* points, const float* noise, const unsigned* warp_id,
                         cudaStream_t s) {
-  using namespace nfb::train;
   const nfb::FieldProgram& p = h->prog[0];
   const TapeLayout t = tape_layout(p, n);
   float* A = h->d_tape;
-  const unsigned blocks = (unsigned)((n + 127) / 128);
-  add_noise_kernel<<<(unsigned)(((long long)n * 3 + 255) / 256), 256, 0, s>>>(points, noise, A + t.warped, (long long)n * 3);
+  nfb::train::add_noise_kernel<<<(unsigned)(((long long)n * 3 + 255) / 256), 256, 0, s>>>(points, noise, A + t.warped,
+                                                                                        (long long)n * 3);
   if (launch_check(h, "add_noise_kernel")) return -1;
   if (run_cond(h, n, A + t.warped, warp_id, nullptr, nullptr, s)) return -1;      // the "view direction" columns are unused here
-  EncodeArgs e{};
-  e.pts_in = A + t.warped; e.pts_out = A + t.pts; e.cond = h->d_cond; e.window = h->d_window;
-  e.in = A + t.in_w; e.F = p.Fw; e.ld = t.ld_w; e.S = 1;
-  e.cond_stride = h->cond_stride; e.cond_off = 0; e.n_cond = p.G; e.rows = n;
-  encode_kernel<<<blocks, 128, 0, s>>>(e);
-  if (launch_check(h, "encode_kernel")) return -1;
-  if (net_forward(h, p.warp, A + t.in_w, t.ld_w, t.out_w, A, n, s)) return -1;
-  const int hs = p.warp.n_steps - 1;
-  WarpTailArgs w{A + t.out_w[hs], p.warp.steps[hs].npad, A + t.pts, A + t.warped, p.warp_type, p.warp_pivot,
-                 p.warp_trans, n};
-  warp_tail_kernel<<<blocks, 128, 0, s>>>(w);
-  return launch_check(h, "warp_tail_kernel");
+  return warp_forward(h, p, t, nullptr, nullptr, nullptr, 1, A + t.warped, h->d_cond, s);
+}
+
+// Embedding gradients: the condition-vector gradients dcond of B rays, scattered into the tables' gradients
+// (the adjoint of run_cond).
+int run_cond_bwd(nfb_handle* h, int B, const float* dcond, const unsigned* warp_id, const unsigned* app_id,
+                 const unsigned* cam_id, cudaStream_t s) {
+  const nfb_config& c = h->cfg;
+  nfb::train::CondBwdArgs a{};
+  a.dcond = dcond; a.num_rays = B;
+  a.warp_id = warp_id; a.app_id = app_id; a.cam_id = cam_id;
+  a.d_warp_table = h->d_gwarp; a.d_app_table = h->d_gapp; a.d_cam_table = h->d_gcam;
+  a.n_warp = c.num_warp_embeddings; a.n_app = c.num_appearance_embeddings; a.n_cam = c.num_camera_embeddings;
+  a.layout = h->cond_layout;
+  const long long total = (long long)B * a.layout.stride;
+  nfb::train::cond_bwd_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(a);
+  return launch_check(h, "cond_bwd_kernel");
 }
 
 // compute_background_loss (training.py:118-135) and its gradient, in chunks of max_rays points.
@@ -423,7 +432,6 @@ int train_background(nfb_handle* h, int P, const float* points, const unsigned* 
                      float weight, cudaStream_t s) {
   using namespace nfb::train;
   const nfb::FieldProgram& p = h->prog[0];
-  const nfb_config& c = h->cfg;
   const int chunk = std::min(P, h->max_rays);
   if (train_prepare_rows(h, chunk)) return -1;
   for (int p0 = 0; p0 < P; p0 += chunk) {
@@ -432,33 +440,14 @@ int train_background(nfb_handle* h, int P, const float* points, const unsigned* 
     float* A = h->d_tape;
     if (warp_points_forward(h, n, points + (size_t)p0 * 3, noise ? noise + (size_t)p0 * 3 : nullptr, warp_ids + p0, s)) return -1;
     NFB_CUDA(cudaMemsetAsync(A + t.grad_begin, 0, (size_t)(t.grad_end - t.grad_begin) * sizeof(float), s));
-    NFB_CUDA(cudaMemsetAsync(h->d_dcond, 0, (size_t)n * h->cond_stride * sizeof(float), s));
+    NFB_CUDA(cudaMemsetAsync(h->d_dcond, 0, (size_t)n * h->cond_layout.stride * sizeof(float), s));
     // alpha = -2, scale = 0.001: the defaults of compute_background_loss, which train_step does not override
-    WarpMagArgs wm{A + t.pts, A + t.warped, nullptr, A + t.dwarped, h->d_loss + 11, -2.0f, 0.001f, weight / (float)P, n};
+    WarpMagArgs wm{A + t.pts, A + t.warped, nullptr, A + t.dwarped, h->d_loss + kSlotBackground, -2.0f, 0.001f,
+                   weight / (float)P, n};
     warp_mag_loss_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(wm);
     if (launch_check(h, "warp_mag_loss_kernel")) return -1;
-    const int hs = p.warp.n_steps - 1;
-    const unsigned blocks = (unsigned)((n + 127) / 128);
-    WarpTailBwdArgs w{A + t.out_w[hs], p.warp.steps[hs].npad, A + t.pts, A + t.dwarped, A + t.d_out_w[hs],
-                      p.warp_type, p.warp_pivot, p.warp_trans, n};
-    warp_tail_bwd_kernel<<<blocks, 128, 0, s>>>(w);
-    if (launch_check(h, "warp_tail_bwd_kernel")) return -1;
-    if (net_backward(h, p.warp, A + t.in_w, A + t.d_in_w, t.ld_w, t.out_w, t.d_out_w, A, n, s)) return -1;
-    EncodeBwdArgs e{};
-    e.pts = A + t.pts; e.window = h->d_window; e.din = A + t.d_in_w; e.F = p.Fw; e.ld = t.ld_w; e.S = 1;
-    e.cond_stride = h->cond_stride; e.cond_off = 0; e.n_cond = p.G; e.dpts = nullptr; e.dcond = h->d_dcond; e.rows = n;
-    encode_bwd_kernel<<<blocks, 128, 0, s>>>(e);
-    if (launch_check(h, "encode_bwd_kernel")) return -1;
-    CondBwdArgs a{};
-    a.dcond = h->d_dcond; a.stride = h->cond_stride; a.num_rays = n; a.warp_id = warp_ids + p0;
-    a.d_warp_table = h->d_gwarp; a.d_app_table = h->d_gapp; a.d_cam_table = h->d_gcam;
-    a.n_warp = c.num_warp_embeddings; a.n_app = c.num_appearance_embeddings; a.n_cam = c.num_camera_embeddings;
-    a.G = p.G; a.A = c.num_appearance_features; a.C = c.num_camera_features; a.Fv = c.num_nerf_viewdir_freqs;
-    a.use_viewdirs = c.use_viewdirs; a.use_app = c.use_appearance_metadata; a.use_cam = c.use_camera_metadata;
-    a.use_trunk_c = c.use_trunk_condition; a.use_alpha_c = c.use_alpha_condition;
-    const long long total = (long long)n * a.stride;
-    cond_bwd_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(a);
-    if (launch_check(h, "cond_bwd_kernel")) return -1;
+    if (warp_backward(h, p, t, 1, h->d_dcond, s)) return -1;
+    if (run_cond_bwd(h, n, h->d_dcond, warp_ids + p0, nullptr, nullptr, s)) return -1;
   }
   return 0;
 }
@@ -497,10 +486,10 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
   NFB_CUDA(cudaMemsetAsync(h->d_gwarp, 0, (size_t)std::max(1, c.num_warp_embeddings * c.num_warp_features) * sizeof(float), s));
   NFB_CUDA(cudaMemsetAsync(h->d_gapp, 0, (size_t)std::max(1, c.num_appearance_embeddings * c.num_appearance_features) * sizeof(float), s));
   NFB_CUDA(cudaMemsetAsync(h->d_gcam, 0, (size_t)std::max(1, c.num_camera_embeddings * c.num_camera_features) * sizeof(float), s));
-  NFB_CUDA(cudaMemsetAsync(h->d_loss, 0, 16 * sizeof(float), s));
+  NFB_CUDA(cudaMemsetAsync(h->d_loss, 0, nfb::train::kLossSlots * sizeof(float), s));
   // condition vectors of the whole batch (per ray), their gradient accumulator
   if (run_cond(h, B, viewdirs ? viewdirs : directions, warp_id, app_id, cam_id, s)) return -1;
-  NFB_CUDA(cudaMemsetAsync(h->d_dcond, 0, (size_t)B * h->cond_stride * sizeof(float), s));
+  NFB_CUDA(cudaMemsetAsync(h->d_dcond, 0, (size_t)B * h->cond_layout.stride * sizeof(float), s));
   if (nfb_coarse_z_vals(h, B, t_rand, h->d_zc, stream)) return -1;
   const float scale = 1.f / ((float)B * 3.f);       // mean over the local batch (training.py:173)
   RegCfg rc_{};
@@ -518,44 +507,28 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
     rc_.batch_rays = B; rc_.stats = h->d_loss;
     rcfg = &rc_;
   }
-  const float* cond_all = h->d_cond;
-  float* dcond_all = h->d_dcond;
   for (int r0 = 0; r0 < B; r0 += chunk_rays) {
     const int R = std::min(chunk_rays, B - r0);
-    // per-chunk views (the kernels index rays from 0)
-    h->d_cond = const_cast<float*>(cond_all) + (size_t)r0 * h->cond_stride;
-    h->d_dcond = dcond_all + (size_t)r0 * h->cond_stride;
+    // the chunk's rays (the kernels index them from 0)
+    const float* cond = h->d_cond + (size_t)r0 * h->cond_layout.stride;
+    float* dcond = h->d_dcond + (size_t)r0 * h->cond_layout.stride;
     const float* o = origins + (size_t)r0 * 3;
     const float* d = directions + (size_t)r0 * 3;
     const float* tg = rgb_target + (size_t)r0 * 3;
     float* zc = h->d_zc + (size_t)r0 * nc;
     float* wc = h->d_tr_w;
-    int rc = train_level(h, 0, R, nc, zc, o, d, tg, scale, use_warp, h->d_tr_out, wc, h->d_loss, s, rcfg);
-    if (rc == 0 && fine) {
+    if (train_level(h, 0, R, nc, zc, o, d, tg, cond, dcond, scale, use_warp, h->d_tr_out, wc,
+                    h->d_loss + nfb::train::kSlotRgbCoarse, s, rcfg))
+      return -1;
+    if (fine) {
       float* zf = h->d_zf + (size_t)r0 * nfine;
-      rc = run_resample(h, R, zc, wc, u_rand ? u_rand + (size_t)r0 * c.num_fine_samples : nullptr, zf, s);
-      if (rc == 0)
-        rc = train_level(h, 1, R, nfine, zf, o, d, tg, scale, use_warp, h->d_tr_out + 6 * (size_t)R, h->d_tr_w,
-                         h->d_loss + 1, s, rcfg);
+      if (run_resample(h, R, zc, wc, u_rand ? u_rand + (size_t)r0 * c.num_fine_samples : nullptr, zf, s) ||
+          train_level(h, 1, R, nfine, zf, o, d, tg, cond, dcond, scale, use_warp, h->d_tr_out + 6 * (size_t)R,
+                      h->d_tr_w, h->d_loss + nfb::train::kSlotRgbFine, s, rcfg))
+        return -1;
     }
-    h->d_cond = const_cast<float*>(cond_all);
-    h->d_dcond = dcond_all;
-    if (rc) return -1;
   }
-  // embedding gradients
-  {
-    nfb::train::CondBwdArgs a{};
-    a.dcond = h->d_dcond; a.stride = h->cond_stride; a.num_rays = B;
-    a.warp_id = warp_id; a.app_id = app_id; a.cam_id = cam_id;
-    a.d_warp_table = h->d_gwarp; a.d_app_table = h->d_gapp; a.d_cam_table = h->d_gcam;
-    a.n_warp = c.num_warp_embeddings; a.n_app = c.num_appearance_embeddings; a.n_cam = c.num_camera_embeddings;
-    a.G = h->prog[0].G; a.A = c.num_appearance_features; a.C = c.num_camera_features; a.Fv = c.num_nerf_viewdir_freqs;
-    a.use_viewdirs = c.use_viewdirs; a.use_app = c.use_appearance_metadata; a.use_cam = c.use_camera_metadata;
-    a.use_trunk_c = c.use_trunk_condition; a.use_alpha_c = c.use_alpha_condition;
-    const long long total = (long long)B * a.stride;
-    nfb::train::cond_bwd_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(a);
-    if (launch_check(h, "cond_bwd_kernel")) return -1;
-  }
+  if (run_cond_bwd(h, B, h->d_dcond, warp_id, app_id, cam_id, s)) return -1;
   // background loss (training.py:118-135, 246-257): warp_field.apply on free points
   const int P = (reg && reg->use_background_loss) ? reg->num_background_points : 0;
   if (P > 0) {
@@ -580,7 +553,9 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
     nfb::train::unpack_grad_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(base + p.dst_off, grads[i], p.rows, p.cols, p.ld, p.c_off);
     if (launch_check(h, "unpack_grad_kernel")) return -1;
   }
-  NFB_CUDA(cudaMemcpyAsync(loss_out, h->d_loss, (reg ? 16 : 2) * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  // without regularisers, loss_out holds the two rgb losses only
+  const int slots = reg ? nfb::train::kLossSlots : nfb::train::kSlotRgbFine + 1;
+  NFB_CUDA(cudaMemcpyAsync(loss_out, h->d_loss, slots * sizeof(float), cudaMemcpyDeviceToDevice, s));
   return 0;
 }
 

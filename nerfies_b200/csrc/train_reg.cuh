@@ -359,14 +359,25 @@ __global__ void add_noise_kernel(const float* __restrict__ p, const float* __res
   if (i < n) o[i] = p[i] + (noise ? noise[i] : 0.f);
 }
 
+// Slots of nfb_train_value_and_grad_reg's loss_out (documented in include/nerfies_b200.h).
+// jac_elastic_kernel writes five consecutive slots from kSlotElasticLoss, warp_mag_loss_kernel two.
+enum LossSlot {
+  kSlotRgbCoarse = 0, kSlotRgbFine = 1,
+  kSlotElasticLoss = 2, kSlotElasticResidual = 3, kSlotJacDet = 4, kSlotJacDiv = 5, kSlotJacCurl = 6,
+  kSlotWarpRegCoarse = 7, kSlotWarpRegResidualCoarse = 8, kSlotWarpRegFine = 9, kSlotWarpRegResidualFine = 10,
+  kSlotBackground = 11, kSlotBackgroundResidual = 12,
+  kLossSlots = 16
+};
+
 // sums -> the means the reference reports (training.py:190-193, 201-206, 216-222, 254-257)
 __global__ void finalize_stats_kernel(float* st, float inv_rays, float inv_jac_rows, float inv_bg) {
   if (threadIdx.x != 0) return;
-  st[2] *= inv_rays;                    // loss/elastic: sum over the samples, mean over the rays
-  st[3] *= inv_jac_rows;                // residual/elastic
-  st[4] *= inv_jac_rows; st[5] *= inv_jac_rows; st[6] *= inv_jac_rows;   // metric/jacobian_{det,div,curl}
-  st[7] *= inv_rays; st[8] *= inv_rays; st[9] *= inv_rays; st[10] *= inv_rays;   // warp_reg loss / residual, coarse | fine
-  st[11] *= inv_bg; st[12] *= inv_bg;   // background loss / residual
+  st[kSlotElasticLoss] *= inv_rays;     // sum over the samples, mean over the rays
+  st[kSlotElasticResidual] *= inv_jac_rows;
+  st[kSlotJacDet] *= inv_jac_rows; st[kSlotJacDiv] *= inv_jac_rows; st[kSlotJacCurl] *= inv_jac_rows;
+  st[kSlotWarpRegCoarse] *= inv_rays; st[kSlotWarpRegResidualCoarse] *= inv_rays;
+  st[kSlotWarpRegFine] *= inv_rays; st[kSlotWarpRegResidualFine] *= inv_rays;
+  st[kSlotBackground] *= inv_bg; st[kSlotBackgroundResidual] *= inv_bg;
 }
 
 }  // namespace train
