@@ -210,6 +210,15 @@ __global__ void __launch_bounds__(kWgThreads, 1)
 field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, const uint8_t* __restrict__ wpack,
                 const float* __restrict__ aux, int num_tiles) {
   constexpr int kSlots = kX3 ? 2 : 4, kSlotBytes = kRingBytes / kSlots;
+  // When a consumer warp frees the slot of unit u-1 (see the MMA loop):
+  //   after issuing unit u (bf16): the MMAs of u-1 and u overlap, but the slot is only freed once
+  //     unit u has arrived, so the copy of unit u+kSlots-1 cannot start before that;
+  //   before waiting for unit u (fp16x3): the warp first waits for its MMAs of u-1, then frees the
+  //     slot.  With two slots this lets the copies of u and u+1 be in flight together instead of
+  //     one after the other, which pays more than the lost overlap of two units' MMAs (a unit is
+  //     1536 tensor cycles in fp16x3).  bf16 has four slots and units a third as long: there the
+  //     overlap is worth more.
+  constexpr bool kReleaseFirst = kX3;
   extern __shared__ __align__(1024) uint8_t base[];
   if ((smem_u32(base) & 1023u) != 0) {
     if (threadIdx.x == 0) printf("nfb: dynamic shared memory is not 1024-byte aligned\n");
@@ -353,13 +362,17 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
           const uint32_t a_hi = src == kSrcIn ? in_a : act_a + (uint32_t)src * kABlockBytes;
           const uint32_t a_lo = a_hi + (src == kSrcIn ? kABlockBytes : kActLoOff);
           const uint32_t b_hi = ring_a + sg * kSlotBytes, b_lo = b_hi + (uint32_t)st.chunk_n * kRowBytes;
+          if (kReleaseFirst && u > 0) {
+            wg_wait<0>();
+            if (lane == 0) mbar_arrive(&bars->empty[prev_sg]);
+          }
           mbar_wait(&bars->full[sg], ph, dead);
           wg_fence();
           if (!hidden) wg_unit<kX3, 16>(acc16, a_hi, a_lo, b_hi, b_lo, kb);
           else if (c == 0) wg_unit<kX3, 128>(acc0, a_hi, a_lo, b_hi, b_lo, kb);
           else wg_unit<kX3, 128>(acc1, a_hi, a_lo, b_hi, b_lo, kb);
           wg_commit();
-          if (u > 0) {
+          if (!kReleaseFirst && u > 0) {
             wg_wait<1>();
             if (lane == 0) mbar_arrive(&bars->empty[prev_sg]);
           }
