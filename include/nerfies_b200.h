@@ -287,6 +287,36 @@ int nfb_camera_rays(const nfb_camera* cam, long long first_pixel, long long coun
 int nfb_pixels_to_rays(const nfb_camera* cam, const float* pixels, long long n,
                        float* directions, void* stream);
 
+/* ---- preloaded capture -> ray batches (datasets/core.py:392-447) -------------
+ * A capture of num_images items, their pixels concatenated image after image in
+ * row-major order: ray r of image k is pixel r - pixel_offsets[k] of that image.
+ * Every pointer is a device pointer.  pixel_offsets[0] == 0 and
+ * pixel_offsets[num_images] == num_rays == the sum of the images' w * h. */
+typedef struct nfb_ray_table {
+  int num_images;
+  const nfb_camera* cameras;         /* (num_images)                                */
+  const long long* pixel_offsets;    /* (num_images + 1)                            */
+  const unsigned char* rgb;          /* (num_rays, 3) uint8 RGB; nullable           */
+  const int* appearance;             /* (num_images) metadata indices; nullable     */
+  const int* camera;
+  const int* warp;
+  const float* time;                 /* (num_images); nullable                      */
+  const void* order;                 /* (num_rays) permutation; NULL = identity     */
+  int order_is_64;                   /* order is int64 (else int32)                 */
+  long long num_rays;
+} nfb_ray_table;
+
+/* Output i (0 <= i < count) is ray r = order[(first + i) mod num_rays] of the table:
+ * origins (count,3) = its camera position, directions (count,3) unit (as
+ * nfb_camera_rays), pixels (count,2) centres, rgb (count,3) = u8 / 255.f, and the
+ * image's appearance / camera / warp (count) int32 and time (count) float32.
+ * Every output is nullable; an output whose source is NULL in the table is an
+ * error.  Needs no handle, allocates nothing, is ordered on `stream`; the outputs
+ * do not depend on the launch (no atomics). */
+int nfb_gather_rays(const nfb_ray_table* table, long long first, long long count,
+                    float* origins, float* directions, float* pixels, float* rgb,
+                    int* appearance, int* camera, int* warp, float* time, void* stream);
+
 /* ---- per-frame image metrics of eval.py:process_batch ------------------------
  * Images are (num_images, height, width, channels) float32, channels interleaved (what
  * render_frame returns for 'rgb'), channels in 1..4, height and width >= 161 (MS-SSIM's five

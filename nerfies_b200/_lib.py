@@ -20,7 +20,7 @@ SYMBOLS = [
     'nfb_camera_rays', 'nfb_pixels_to_rays', 'nfb_selftest_gemm3',
     'nfb_debug_provoke_timeout', 'nfb_set_time_alpha', 'nfb_train_value_and_grad', 'nfb_adam_step',
     'nfb_train_value_and_grad_reg', 'nfb_warp_jacobian', 'nfb_check_abort', 'nfb_reset_abort',
-    'nfb_image_metrics_workspace_size', 'nfb_image_metrics',
+    'nfb_image_metrics_workspace_size', 'nfb_image_metrics', 'nfb_gather_rays',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -107,6 +107,23 @@ class NfbCamera(ctypes.Structure):
   ]
 
 
+class NfbRayTable(ctypes.Structure):
+  """struct nfb_ray_table - field order must match the header."""
+  _fields_ = [
+      ('num_images', ctypes.c_int),
+      ('cameras', ctypes.c_void_p),
+      ('pixel_offsets', ctypes.c_void_p),
+      ('rgb', ctypes.c_void_p),
+      ('appearance', ctypes.c_void_p),
+      ('camera', ctypes.c_void_p),
+      ('warp', ctypes.c_void_p),
+      ('time', ctypes.c_void_p),
+      ('order', ctypes.c_void_p),
+      ('order_is_64', ctypes.c_int),
+      ('num_rays', ctypes.c_longlong),
+  ]
+
+
 class NfbError(RuntimeError):
   pass
 
@@ -183,6 +200,8 @@ def load():
   lib.nfb_camera_rays.restype = ci
   lib.nfb_pixels_to_rays.argtypes = [ctypes.POINTER(NfbCamera), vp, ll, vp, vp]
   lib.nfb_pixels_to_rays.restype = ci
+  lib.nfb_gather_rays.argtypes = [ctypes.POINTER(NfbRayTable), ll, ll] + [vp] * 9
+  lib.nfb_gather_rays.restype = ci
   lib.nfb_image_metrics_workspace_size.argtypes = [ci, ci, ci, ci]
   lib.nfb_image_metrics_workspace_size.restype = ll
   lib.nfb_image_metrics.argtypes = [ci, ci, ci, ci, vp, vp, vp, vp, vp, ll, vp, vp, vp, vp]

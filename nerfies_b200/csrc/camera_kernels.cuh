@@ -52,23 +52,26 @@ __device__ __forceinline__ void undistort_point(float xd, float yd, float k1, fl
   xo = x; yo = y;
 }
 
-// One pixel: unit world-space direction and the pixel position used.
-__device__ __forceinline__ void camera_ray_of_pixel(const CameraArgs& a, long long i, float* out_d, float* out_p) {
-  const nfb_camera& c = a.cam;
-  float px, py;
-  if (a.pixels_in) {
-    px = __ldg(a.pixels_in + 2 * i);
-    py = __ldg(a.pixels_in + 2 * i + 1);
-  } else {
-    const long long p = a.first + i;                       // row-major pixel index
-    const long long row = p / c.image_size[0];
-    px = (float)(p - row * c.image_size[0]) + 0.5f;        // camera.py:319-321
-    py = (float)row + 0.5f;
-  }
+// camera.py:201-207: undistortion runs only when a coefficient is non-zero.
+__host__ __device__ __forceinline__ int camera_has_distortion(const nfb_camera& c) {
+  return c.radial_distortion[0] != 0.f || c.radial_distortion[1] != 0.f || c.radial_distortion[2] != 0.f ||
+         c.tangential_distortion[0] != 0.f || c.tangential_distortion[1] != 0.f;
+}
+
+// Pixel centre of row-major pixel p (camera.py:319-321).
+__device__ __forceinline__ void camera_pixel_center(const nfb_camera& c, long long p, float& px, float& py) {
+  const long long row = p / c.image_size[0];
+  px = (float)(p - row * c.image_size[0]) + 0.5f;
+  py = (float)row + 0.5f;
+}
+
+// Unit world-space direction of the pixel position (px, py) (camera.py:225-269).
+__device__ __forceinline__ void camera_pixel_direction(const nfb_camera& c, int has_distortion, float px, float py,
+                                                       float* out_d) {
   const float sy = c.focal_length * c.pixel_aspect_ratio;  // camera.py:186-187
   float y = (py - c.principal_point[1]) / sy;              // camera.py:227
   float x = (px - c.principal_point[0] - y * c.skew) / c.focal_length;   // camera.py:228-229
-  if (a.has_distortion)
+  if (has_distortion)
     undistort_point(x, y, c.radial_distortion[0], c.radial_distortion[1], c.radial_distortion[2],
                     c.tangential_distortion[0], c.tangential_distortion[1], x, y);
   // camera.py:241-242: dirs / ||dirs||, dirs = (x, y, 1)
@@ -83,6 +86,18 @@ __device__ __forceinline__ void camera_ray_of_pixel(const CameraArgs& a, long lo
 #pragma unroll
   for (int j = 0; j < 3; ++j) d[j] = d[j] / n2;
   out_d[0] = d[0]; out_d[1] = d[1]; out_d[2] = d[2];
+}
+
+// One pixel of CameraArgs: unit world-space direction and the pixel position used.
+__device__ __forceinline__ void camera_ray_of_pixel(const CameraArgs& a, long long i, float* out_d, float* out_p) {
+  float px, py;
+  if (a.pixels_in) {
+    px = __ldg(a.pixels_in + 2 * i);
+    py = __ldg(a.pixels_in + 2 * i + 1);
+  } else {
+    camera_pixel_center(a.cam, a.first + i, px, py);
+  }
+  camera_pixel_direction(a.cam, a.has_distortion, px, py, out_d);
   out_p[0] = px; out_p[1] = py;
 }
 
@@ -123,6 +138,55 @@ __global__ void __launch_bounds__(256) camera_rays_kernel(const CameraArgs a) {
       if (a.origins) a.origins[block0 * 3 + e] = a.cam.position[e % 3];
     }
   }
+}
+
+// Training batches and eval items of a preloaded capture (datasets/core.py:392-447 with flatten
+// and shuffle, then repeat + batch): output i is ray order[(first + i) mod num_rays] of the
+// image-after-image, row-major concatenation of the table's items.  Every output is nullable.
+struct GatherArgs {
+  nfb_ray_table t;
+  long long first, count;
+  float* origins;      // (count,3)
+  float* directions;   // (count,3)
+  float* pixels;       // (count,2)
+  float* rgb;          // (count,3)
+  int *appearance, *camera, *warp;   // (count)
+  float* time;         // (count)
+};
+
+__global__ void __launch_bounds__(256) gather_rays_kernel(const GatherArgs a) {
+  const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (i >= a.count) return;
+  const nfb_ray_table& t = a.t;
+  const long long g = (a.first + i) % t.num_rays;
+  long long r = g;
+  if (t.order)
+    r = t.order_is_64 ? __ldg(static_cast<const long long*>(t.order) + g) : __ldg(static_cast<const int*>(t.order) + g);
+  // image k: pixel_offsets[k] <= r < pixel_offsets[k + 1]
+  int lo = 0, hi = t.num_images;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(t.pixel_offsets + mid) <= r) lo = mid; else hi = mid;
+  }
+  const nfb_camera& c = t.cameras[lo];
+  if (a.origins || a.directions || a.pixels) {
+    float px, py;
+    camera_pixel_center(c, r - __ldg(t.pixel_offsets + lo), px, py);
+    if (a.directions) {
+      float d[3];
+      camera_pixel_direction(c, camera_has_distortion(c), px, py, d);
+      for (int j = 0; j < 3; ++j) a.directions[3 * i + j] = d[j];
+    }
+    if (a.pixels) { a.pixels[2 * i] = px; a.pixels[2 * i + 1] = py; }
+    if (a.origins)
+      for (int j = 0; j < 3; ++j) a.origins[3 * i + j] = c.position[j];   // datasets/core.py:176
+  }
+  if (a.rgb)   // datasets/nerfies.py:62: float32(u8) / 255.0, an IEEE division
+    for (int j = 0; j < 3; ++j) a.rgb[3 * i + j] = (float)__ldg(t.rgb + 3 * r + j) / 255.f;
+  if (a.appearance) a.appearance[i] = __ldg(t.appearance + lo);
+  if (a.camera) a.camera[i] = __ldg(t.camera + lo);
+  if (a.warp) a.warp[i] = __ldg(t.warp + lo);
+  if (a.time) a.time[i] = __ldg(t.time + lo);
 }
 
 }  // namespace nfb

@@ -574,12 +574,36 @@ static int launch_camera(const nfb_camera* cam, const float* pixels_in, long lon
   nfb::CameraArgs a{};
   a.cam = *cam; a.pixels_in = pixels_in; a.first = first; a.count = count;
   a.origins = origins; a.directions = directions; a.pixels_out = pixels_out;
-  a.has_distortion = 0;                                   // camera.py:201-207
-  for (int i = 0; i < 3; ++i) a.has_distortion |= cam->radial_distortion[i] != 0.f;
-  for (int i = 0; i < 2; ++i) a.has_distortion |= cam->tangential_distortion[i] != 0.f;
+  a.has_distortion = nfb::camera_has_distortion(*cam);
   nfb::camera_rays_kernel<<<(unsigned)((count + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail("camera_rays_kernel launch failed: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+int nfb_gather_rays(const nfb_ray_table* table, long long first, long long count, float* origins,
+                    float* directions, float* pixels, float* rgb, int* appearance, int* camera, int* warp,
+                    float* time, void* stream) {
+  if (!table) return fail("null ray table");
+  const nfb_ray_table& t = *table;
+  if (t.num_images < 1) return fail("ray table has %d images", t.num_images);
+  if (t.num_rays < 1) return fail("ray table has %lld rays", t.num_rays);
+  if (count < 0 || first < 0) return fail("negative ray range (first %lld, count %lld)", first, count);
+  if (!t.cameras || !t.pixel_offsets) return fail("ray table needs cameras and pixel_offsets");
+  if (rgb && !t.rgb) return fail("rgb requested but the ray table has none");
+  if ((appearance && !t.appearance) || (camera && !t.camera) || (warp && !t.warp) || (time && !t.time))
+    return fail("metadata requested but the ray table has none of that kind");
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
+    return fail("no CUDA device: nerfies_b200 has no CPU path");
+  if (count == 0) return 0;
+  nfb::GatherArgs a{};
+  a.t = t; a.first = first; a.count = count;
+  a.origins = origins; a.directions = directions; a.pixels = pixels; a.rgb = rgb;
+  a.appearance = appearance; a.camera = camera; a.warp = warp; a.time = time;
+  nfb::gather_rays_kernel<<<(unsigned)((count + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("gather_rays_kernel launch failed: %s", cudaGetErrorString(e));
   return 0;
 }
 
