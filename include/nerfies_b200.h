@@ -372,6 +372,24 @@ int nfb_selftest_gemm(int K, int N, const float* A, const float* W, float* C,
 int nfb_selftest_gemm3(int K, int N, const float* A, const float* W, float* C, int reps,
                        long long* out, void* stream);
 
+/* Self-test of the training tier's GEMM: one Dense layer's GEMM through the same launch and
+ * element functors nfb_train_value_and_grad uses.  The layer maps [X | IN] (rows x (k_x + k_in);
+ * X: rows x k_x, ld ldx; IN: rows x k_in, ld ldin) to n outputs; W (k_x + k_in, ldw), bias (n),
+ * Y and dY (rows, ldw), act an activation of nfb_config.  X may be NULL when k_x == 0, IN when k_in == 0.
+ *   NFB_SGEMM_FORWARD: y = act([X | IN] W + bias), written to columns [0, n) of y.
+ *   NFB_SGEMM_DX:      dZ = dY * act'(Y) (Y read from y);  dx += dZ W^T[:, :k_x] (rows, ldx),
+ *                      din += dZ W^T[:, k_x:] (rows, ldin).
+ *   NFB_SGEMM_DW:      dw (k_x + k_in, ldw) += [X | IN]^T dZ, the reduction over the rows split into slices
+ *                      of k_split rows (0: the split the training step picks for this shape), partial sums
+ *                      atomically added.
+ * k_split must be 0 for the other modes.  k_split_used (host, nullable) receives the rows per slice.
+ * Device pointers; allocates nothing; asynchronous on `stream`.  No reference analogue. */
+enum { NFB_SGEMM_FORWARD = 0, NFB_SGEMM_DX = 1, NFB_SGEMM_DW = 2 };
+int nfb_selftest_sgemm(int mode, long long rows, int n, int k_x, int k_in, int act,
+                       const float* x, int ldx, const float* in, int ldin, const float* w, int ldw,
+                       const float* bias, float* y, const float* dy, float* dx, float* din, float* dw,
+                       long long k_split, long long* k_split_used, void* stream);
+
 /* Number of CUDA kernels this handle has launched so far (bench accounting). */
 long long nfb_kernel_launches(const nfb_handle* h);
 /* Thread-local description of the last error returned on this thread. */

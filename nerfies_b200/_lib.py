@@ -20,7 +20,7 @@ SYMBOLS = [
     'nfb_camera_rays', 'nfb_pixels_to_rays', 'nfb_selftest_gemm3',
     'nfb_debug_provoke_timeout', 'nfb_set_time_alpha', 'nfb_train_value_and_grad', 'nfb_adam_step',
     'nfb_train_value_and_grad_reg', 'nfb_warp_jacobian', 'nfb_check_abort', 'nfb_reset_abort',
-    'nfb_image_metrics_workspace_size', 'nfb_image_metrics', 'nfb_gather_rays',
+    'nfb_image_metrics_workspace_size', 'nfb_image_metrics', 'nfb_gather_rays', 'nfb_selftest_sgemm',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -208,6 +208,9 @@ def load():
   lib.nfb_image_metrics.restype = ci
   lib.nfb_selftest_gemm3.argtypes = [ci, ci, vp, vp, vp, ci, vp, vp]
   lib.nfb_selftest_gemm3.restype = ci
+  lib.nfb_selftest_sgemm.argtypes = [ci, ll, ci, ci, ci, ci, vp, ci, vp, ci, vp, ci] + [vp] * 6 + [
+      ll, ctypes.POINTER(ll), vp]
+  lib.nfb_selftest_sgemm.restype = ci
   lib.nfb_debug_provoke_timeout.argtypes = [vp, ci]
   lib.nfb_debug_provoke_timeout.restype = ci
   lib.nfb_last_error.argtypes = []

@@ -611,4 +611,45 @@ int nfb_adam_step(float* params, const float* grads, float* m, float* v, long lo
   return 0;
 }
 
+// The three launches of net_forward / net_backward for one layer, with their functors.
+int nfb_selftest_sgemm(int mode, long long rows, int n, int k_x, int k_in, int act, const float* x, int ldx,
+                       const float* in, int ldin, const float* w, int ldw, const float* bias, float* y,
+                       const float* dy, float* dx, float* din, float* dw, long long k_split,
+                       long long* k_split_used, void* stream) {
+  using namespace nfb::train;
+  const int K = k_x + k_in;
+  if (rows < 1 || n < 1 || k_x < 0 || k_in < 0 || K < 1) return fail("selftest_sgemm: empty shape");
+  if (ldx < k_x || ldin < k_in || ldw < n) return fail("selftest_sgemm: a leading dimension is below its width");
+  if (act < nfb::kNone || act > nfb::kSoftplus) return fail("selftest_sgemm: bad activation %d", act);
+  if (k_split < 0 || (k_split > 0 && mode != NFB_SGEMM_DW)) return fail("selftest_sgemm: k_split applies to dW only");
+  if (!w || (mode != NFB_SGEMM_DX && ((k_x > 0 && !x) || (k_in > 0 && !in))))
+    return fail("selftest_sgemm: null operand");
+  // launch_gemm reads the SM count (dw_split) and counts launches in a handle; this call has none
+  nfb_handle h;
+  int dev = 0;
+  NFB_CUDA(cudaGetDevice(&dev));
+  NFB_CUDA(cudaDeviceGetAttribute(&h.sm_count, cudaDevAttrMultiProcessorCount, dev));
+  cudaStream_t s = (cudaStream_t)stream;
+  const ConcatA a{x, ldx, k_x, in, ldin};
+  const DZ dz{dy, y, ldw, act};
+  long long per = 0;
+  int rc;
+  if (mode == NFB_SGEMM_FORWARD) {
+    if (!bias || !y) return fail("selftest_sgemm: null bias / y");
+    rc = launch_gemm(&h, rows, n, K, a, WeightB{w, ldw}, StoreBiasAct{y, ldw, bias, act}, 0, s, "sgemm (forward)");
+  } else if (mode == NFB_SGEMM_DX) {
+    if (!y || !dy || (k_x > 0 && !dx) || (k_in > 0 && !din)) return fail("selftest_sgemm: null y / dy / dx / din");
+    rc = launch_gemm<true, false>(&h, rows, K, n, dz, WeightBT{w, ldw}, AccumSplit{dx, ldx, k_x, din, ldin}, 0, s,
+                                  "sgemm (dX)");
+  } else if (mode == NFB_SGEMM_DW) {
+    if (!y || !dy || !dw) return fail("selftest_sgemm: null y / dy / dw");
+    per = k_split > 0 ? k_split : dw_split(&h, K, n, rows);
+    rc = launch_gemm<false, true>(&h, K, n, rows, ConcatAT{a}, DZB{dz}, AtomicAdd{dw, ldw}, per, s, "sgemm (dW)");
+  } else {
+    return fail("selftest_sgemm: bad mode %d", mode);
+  }
+  if (k_split_used) *k_split_used = per;
+  return rc;
+}
+
 }  // extern "C"
