@@ -90,7 +90,8 @@ __device__ __forceinline__ void cond_to_block(uint8_t* block, int r, const float
 
 // One 128-column accumulator chunk of a hidden layer (this thread's fragment: rows
 // arow, arow + 8; columns c*128 + 8j + 2*lq + {0, 1}) -> + bias, activation, (alpha
-// head dot product in fp32) -> the activation image of the next layer, in place.
+// head dot product in fp32) -> the activation image of the next layer, in place; in
+// fp16x3 the lo half goes to this thread's register operand `lo` (x3_lo_reg) instead.
 // `inv_s` undoes the fp16x3 power-of-two weight scale (x3_weight_scale; 1 in bf16
 // mode): acc * inv_s is exact, so fma(acc, inv_s, bias) rounds like acc + bias.
 // fp16x3 split: hi = v with the fp32 mantissa truncated to fp16's 11 significant bits
@@ -101,7 +102,7 @@ __device__ __forceinline__ void cond_to_block(uint8_t* block, int r, const float
 template <bool kX3>
 __device__ __forceinline__ void epi_chunk(const float* acc, int c, const float* __restrict__ bias, float inv_s,
                                           bool relu, bool adot, const float* __restrict__ aw, float& al0,
-                                          float& al1, uint8_t* act_hi, uint8_t* act_lo, int arow, int lq) {
+                                          float& al1, uint8_t* act_hi, uint32_t* lo, int arow, int lq) {
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     const int col = c * 128 + 8 * j + 2 * lq;
@@ -122,19 +123,19 @@ __device__ __forceinline__ void epi_chunk(const float* acc, int c, const float* 
     for (int h = 0; h < 2; ++h) {
       const uint32_t off = blk + swz_off(arow + 8 * h, j & 7);
       const float a = v[2 * h], bb = v[2 * h + 1];
-      uint32_t hi, lo;
+      uint32_t hi;
       if constexpr (kX3) {
         const float ta = __uint_as_float(__float_as_uint(a) & 0xFFFFE000u);
         const float tb = __uint_as_float(__float_as_uint(bb) & 0xFFFFE000u);
         const float da = a - ta, db = bb - tb;
+        uint32_t& l = lo[x3_lo_reg(2 * c + (j >> 3), j & 7, h)];
         if (relu) {
           asm("cvt.rn.relu.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(tb), "f"(ta));
-          asm("cvt.rn.relu.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(db), "f"(da));
+          asm("cvt.rn.relu.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(l) : "f"(db), "f"(da));
         } else {
           asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(tb), "f"(ta));
-          asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(db), "f"(da));
+          asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(l) : "f"(db), "f"(da));
         }
-        *reinterpret_cast<uint32_t*>(act_lo + off) = lo;
       } else {
         if (relu) asm("cvt.rn.relu.bf16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(bb), "f"(a));
         else asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(bb), "f"(a));
@@ -172,32 +173,64 @@ struct RowState {
 //
 // Persistent, one CTA per SM, 384 threads, one 128-row tile at a time:
 //   warpgroup 0     : warp 0 streams the weight units (one cp.async.bulk per unit into a
-//                     ring of mbarrier-guarded slots: 2 x 32 KB fp16x3 [W_hi | W_lo], 4 x 16 KB
-//                     bf16); the other warps idle (setmaxnreg 40 / 232).
+//                     ring of four mbarrier-guarded slots: 32 KB fp16x3 [W_hi | W_lo], 16 KB
+//                     bf16); the other warps idle (setmaxnreg 24 / 240).
 //   warpgroups 1, 2 : rows 0-63 / 64-127.  Each issues its own wgmma (M = 64, N = 128 per
 //                     chunk, fp32 accumulators in registers: a 256-wide layer is 128 of them
 //                     per thread), A = its rows of the activation image in shared memory,
 //                     B = the weight slot shared by both.  A layer's epilogue writes the
 //                     next layer's activation image in place once the warpgroup's MMAs of
-//                     the layer are complete, so no second image is needed.
-// Shared memory (225 KB): activation image 4 K-blocks x (hi | lo) = 128 KB | input block
-// (the encoded points / conditions) hi | lo = 32 KB | weight ring 64 KB | alpha partials |
-// composite scratch | barriers.  (bf16 mode leaves the lo images unused.)
+//                     the layer are complete, so no second image is needed.  fp16x3: the
+//                     x_lo operand of the activations is not in shared memory but in the
+//                     registers of the thread whose accumulators produced it (64 per thread,
+//                     epi_chunk -> lo -> the register-A form of wgmma), under the same rule.
+// Shared memory (225 KB), in 16 KB K-blocks:
+//   fp16x3: activation image hi, 4 blocks | input block (the encoded points / conditions)
+//           hi | lo, 2 blocks | weight ring 4 x 32 KB, 8 blocks;
+//   bf16  : activation image, 4 blocks | 4 unused blocks | input block, 2 blocks (its lo
+//           half unused) | weight ring 4 x 16 KB, 4 blocks;
+// then for both alpha partials | composite scratch | barriers.
 // Per-row work (positional encodings, SE(3) exp-map, sigmoid / sigma activation, fused
 // volumetric rendering) is done by "row threads": two per row (hs = which half of the
 // input block's columns), thread t of warpgroup w owns row 64 (w - 1) + (t & 63).
 // Head layers (N = 16) leave their accumulators in a per-warpgroup scratch inside
 // activation block 0 (free at that point: the step after a head reads the input block only).
 constexpr int kWgThreads = 384;
-constexpr int kActLoOff = 4 * kABlockBytes;
-constexpr int kInOff = 8 * kABlockBytes;
-constexpr int kRingOff = 10 * kABlockBytes;
-constexpr int kRingBytes = 4 * kABlockBytes;
-constexpr int kAlphaOff = kRingOff + kRingBytes;      // per-row alpha-head partial (128 floats)
+constexpr int kWgSlots = 4;
+template <bool kX3>
+struct WgSmem {
+  static constexpr int kInOff = (kX3 ? 4 : 8) * kABlockBytes;
+  static constexpr int kRingOff = kInOff + 2 * kABlockBytes;
+  static constexpr int kSlotBytes = (kX3 ? 2 : 1) * kABlockBytes;
+};
+constexpr int kAlphaOff = 14 * kABlockBytes;          // per-row alpha-head partial (128 floats)
 constexpr int kScanOff = kAlphaOff + 512;             // fused composite: cross-warp partials (40 floats)
 constexpr int kBarOff = kScanOff + 256;
 constexpr int kWgSmemBytes = kBarOff + 256;
+static_assert(WgSmem<true>::kRingOff + kWgSlots * WgSmem<true>::kSlotBytes == kAlphaOff &&
+              WgSmem<false>::kRingOff + kWgSlots * WgSmem<false>::kSlotBytes == kAlphaOff,
+              "each precision's ring ends where the alpha partials begin");
 static_assert(kWgSmemBytes <= 232448, "shared memory");
+
+// One weight unit of a layer into the accumulators d, A = K-block `src` (an activation
+// block or kSrcIn).  fp16x3 takes x_lo of an activation block from the registers `lo`, that
+// of the input block (written by the row threads) from its shared image at in_lo; the switch
+// keeps every register index a compile-time constant.
+template <bool kX3, int N>
+__device__ __forceinline__ void wg_layer_unit(float* d, int src, uint32_t a_hi, uint32_t in_lo, const uint32_t* lo,
+                                              uint32_t b_hi, uint32_t b_lo, uint32_t accumulate) {
+  if constexpr (kX3) {
+    switch (src) {
+      case 0: wg_unit<true, N>(d, a_hi, lo + x3_lo_reg(0, 0, 0), b_hi, b_lo, accumulate); break;
+      case 1: wg_unit<true, N>(d, a_hi, lo + x3_lo_reg(1, 0, 0), b_hi, b_lo, accumulate); break;
+      case 2: wg_unit<true, N>(d, a_hi, lo + x3_lo_reg(2, 0, 0), b_hi, b_lo, accumulate); break;
+      case 3: wg_unit<true, N>(d, a_hi, lo + x3_lo_reg(3, 0, 0), b_hi, b_lo, accumulate); break;
+      default: wg_unit<true, N>(d, a_hi, in_lo, b_hi, b_lo, accumulate); break;
+    }
+  } else {
+    wg_unit<false, N>(d, a_hi, 0u, b_hi, b_lo, accumulate);
+  }
+}
 
 struct WgBars {
   uint64_t full[4];
@@ -209,16 +242,15 @@ template <bool kX3>
 __global__ void __launch_bounds__(kWgThreads, 1)
 field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, const uint8_t* __restrict__ wpack,
                 const float* __restrict__ aux, int num_tiles) {
-  constexpr int kSlots = kX3 ? 2 : 4, kSlotBytes = kRingBytes / kSlots;
-  // When a consumer warp frees the slot of unit u-1 (see the MMA loop):
-  //   after issuing unit u (bf16): the MMAs of u-1 and u overlap, but the slot is only freed once
-  //     unit u has arrived, so the copy of unit u+kSlots-1 cannot start before that;
-  //   before waiting for unit u (fp16x3): the warp first waits for its MMAs of u-1, then frees the
-  //     slot.  With two slots this lets the copies of u and u+1 be in flight together instead of
-  //     one after the other, which pays more than the lost overlap of two units' MMAs (a unit is
-  //     1536 tensor cycles in fp16x3).  bf16 has four slots and units a third as long: there the
-  //     overlap is worth more.
-  constexpr bool kReleaseFirst = kX3;
+  using Smem = WgSmem<kX3>;
+  constexpr int kSlots = kWgSlots, kSlotBytes = Smem::kSlotBytes;
+  // Registers per thread: 128 * producer + 256 * consumer <= 64 K.  fp16x3 consumers hold 64
+  // x_lo registers on top of a 256-wide layer's 128 accumulators.
+  constexpr int kProducerRegs = kX3 ? 24 : 40, kConsumerRegs = kX3 ? 240 : 232;
+  // A consumer warp frees the slot of unit u-1 after issuing unit u, so the MMAs of u-1 and u
+  // overlap; with four slots the copies of u+1 .. u+3 can be in flight meanwhile.  (Freeing it
+  // before waiting for unit u, which drains the MMA pipeline on every unit, measured slower in
+  // both precisions: DESIGN 5.1.)
   extern __shared__ __align__(1024) uint8_t base[];
   if ((smem_u32(base) & 1023u) != 0) {
     if (threadIdx.x == 0) printf("nfb: dynamic shared memory is not 1024-byte aligned\n");
@@ -256,11 +288,11 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
 
   if (wg == 0) {
     // ===================== weight producer =====================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(40));
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
     if (warp == 0) {
       uint32_t sg = 0, ph = 0, dead = 0;
       if (args.debug & 8) mbar_wait(&bars->never, 0, dead);   // test hook: provoke a wait time-out
-      uint8_t* ring = base + kRingOff;
+      uint8_t* ring = base + Smem::kRingOff;
       for (int ti = 0; ti < n_my; ++ti) {
         for (int si = first_step; si <= last_step; ++si) {
           const TcStep& st = prog.steps[si];
@@ -281,22 +313,23 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
     }
   } else {
     // ===================== consumers: MMAs + epilogue of 64 rows =====================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(232));
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
     const int cw = wg - 1, t = tid & 127, wq = t >> 5, lq = lane & 3;
     const int arow = 64 * cw + 16 * wq + (lane >> 2);    // accumulator rows arow, arow + 8
     const int r = 64 * cw + (t & 63), hs = t >> 6;       // row thread: row r, input-block half hs
     const int cb = hs * 4, ce = cb + 4;                  // input-block chunks this thread writes
     const int lr = t & 63;                               // row within the warpgroup
     uint8_t* act_hi = base;
-    uint8_t* act_lo = base + kActLoOff;
-    uint8_t* inh = base + kInOff;
+    uint8_t* inh = base + Smem::kInOff;
     uint8_t* inl = inh + kABlockBytes;
     float* alpha_s = reinterpret_cast<float*>(base + kAlphaOff);
     float* scan_s = reinterpret_cast<float*>(base + kScanOff);
     float* scr = reinterpret_cast<float*>(base + cw * 8192);        // head accumulators, 64 x 16
     const uint32_t rows_off = (uint32_t)cw * 8192u;                 // this warpgroup's rows in a K-block
-    const uint32_t ring_a = smem_u32(base + kRingOff);
+    const uint32_t ring_a = smem_u32(base + Smem::kRingOff);
     const uint32_t act_a = smem_u32(act_hi) + rows_off, in_a = smem_u32(inh) + rows_off;
+    // fp16x3: x_lo of the activation image of this thread's accumulator rows, see epi_chunk
+    uint32_t lo[kX3 ? 64 : 1];
     const float alpha_b = __ldg(aux + prog.alpha_b_off);
     const int S = args.samples_per_ray;
     uint32_t sg = 0, ph = 0, dead = 0;
@@ -352,7 +385,8 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
         const float* bias = aux + st.b_off;
         const float inv_s = kX3 ? 1.f / x3_weight_scale(__ldg(aux + prog.scale_off + si)) : 1.f;
         const bool hidden = st.epi == kEpiHidden;
-        float acc0[64], acc1[64], acc16[8];
+        float acc0[64], acc1[64];
+        float* const acc16 = acc0;     // a head (N = 16) accumulates into acc0[0..7]
         // ---- the layer's MMAs: one weight unit per (chunk, K-block), one unit in flight ----
         uint32_t prev_sg = 0;
         const int n_units = st.n_chunks * st.nkb;
@@ -360,19 +394,15 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
           const int c = u >= st.nkb ? 1 : 0, kb = u - c * st.nkb;
           const int src = st.src[kb];
           const uint32_t a_hi = src == kSrcIn ? in_a : act_a + (uint32_t)src * kABlockBytes;
-          const uint32_t a_lo = a_hi + (src == kSrcIn ? kABlockBytes : kActLoOff);
           const uint32_t b_hi = ring_a + sg * kSlotBytes, b_lo = b_hi + (uint32_t)st.chunk_n * kRowBytes;
-          if (kReleaseFirst && u > 0) {
-            wg_wait<0>();
-            if (lane == 0) mbar_arrive(&bars->empty[prev_sg]);
-          }
           mbar_wait(&bars->full[sg], ph, dead);
           wg_fence();
-          if (!hidden) wg_unit<kX3, 16>(acc16, a_hi, a_lo, b_hi, b_lo, kb);
-          else if (c == 0) wg_unit<kX3, 128>(acc0, a_hi, a_lo, b_hi, b_lo, kb);
-          else wg_unit<kX3, 128>(acc1, a_hi, a_lo, b_hi, b_lo, kb);
+          const uint32_t in_lo = in_a + kABlockBytes;
+          if (!hidden) wg_layer_unit<kX3, 16>(acc16, src, a_hi, in_lo, lo, b_hi, b_lo, kb);
+          else if (c == 0) wg_layer_unit<kX3, 128>(acc0, src, a_hi, in_lo, lo, b_hi, b_lo, kb);
+          else wg_layer_unit<kX3, 128>(acc1, src, a_hi, in_lo, lo, b_hi, b_lo, kb);
           wg_commit();
-          if (!kReleaseFirst && u > 0) {
+          if (u > 0) {
             wg_wait<1>();
             if (lane == 0) mbar_arrive(&bars->empty[prev_sg]);
           }
@@ -380,7 +410,7 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
           if (++sg == kSlots) { sg = 0; ph ^= 1; }
         }
         wg_wait<0>();
-        wg_fence_regs<64>(acc0); wg_fence_regs<64>(acc1); wg_fence_regs<8>(acc16);
+        wg_fence_regs<64>(acc0); wg_fence_regs<64>(acc1);
         if (lane == 0) mbar_arrive(&bars->empty[prev_sg]);
         wg_sync();      // every MMA of the warpgroup is complete: its activation rows may be overwritten
 
@@ -389,8 +419,8 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
           const bool relu = st.relu != 0, adot = st.alpha_dot != 0;
           const float* aw = aux + prog.alpha_w_off;
           float al0 = 0.f, al1 = 0.f;
-          epi_chunk<kX3>(acc0, 0, bias, inv_s, relu, adot, aw, al0, al1, act_hi, act_lo, arow, lq);
-          if (st.n_chunks == 2) epi_chunk<kX3>(acc1, 1, bias, inv_s, relu, adot, aw, al0, al1, act_hi, act_lo, arow, lq);
+          epi_chunk<kX3>(acc0, 0, bias, inv_s, relu, adot, aw, al0, al1, act_hi, lo, arow, lq);
+          if (st.n_chunks == 2) epi_chunk<kX3>(acc1, 1, bias, inv_s, relu, adot, aw, al0, al1, act_hi, lo, arow, lq);
           if (adot) {
             // the four threads of a quad hold the row's columns
             al0 += __shfl_xor_sync(0xffffffffu, al0, 1); al0 += __shfl_xor_sync(0xffffffffu, al0, 2);
@@ -516,6 +546,13 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
               bar128();   // scan_s is read by every row thread before the next tile writes it
             }
             if (has_next) begin_tile(tile_of(ti + 1));
+          }
+          // The step after a head reads the input block only (build_tc_program), so the head was
+          // the last reader of the x_lo registers.  Redefining them here, after the row-thread work,
+          // lets the compiler see that they are dead during it (64 registers for the fp64 encoder).
+          if constexpr (kX3) {
+#pragma unroll
+            for (int i = 0; i < 64; ++i) lo[i] = 0u;
           }
         }
         fence_proxy_async();   // this thread's shared-memory stores are visible to the next MMAs ...

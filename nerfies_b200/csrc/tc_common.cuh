@@ -15,6 +15,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 namespace nfb {
 namespace tc {
 
@@ -164,17 +166,50 @@ __device__ __forceinline__ void wg_mma_n128(float* d, uint64_t a, uint64_t b, ui
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
                  "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " NFB_WG_N128_REGS NFB_WG_N128_OPS);
 }
+// D (+)= A * B^T with the fp16 A operand (64 x 16) in registers: 4 x b32 per thread,
+// a[0] = (row, k = 2 lq + {0,1}), a[1] = (row + 8, same k), a[2] / a[3] = the same at k + 8,
+// row = 16 * warp + lane / 4.  That is the accumulator fragment layout of columns
+// 8j + 2lq + {0,1}, j = 0, 1: see x3_lo_reg.
+// Always accumulates (it is never the first product of a K-block).
+__device__ __forceinline__ void wg_mma_n16_rs(float* d, const uint32_t* a, uint64_t b) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}"
+               : NFB_WG_D8(0) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(1u));
+}
+__device__ __forceinline__ void wg_mma_n128_rs(float* d, const uint32_t* a, uint64_t b) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+               "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+               "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+               "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+               "{%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+               : NFB_WG_D8(0), NFB_WG_D8(8), NFB_WG_D8(16), NFB_WG_D8(24), NFB_WG_D8(32), NFB_WG_D8(40),
+                 NFB_WG_D8(48), NFB_WG_D8(56)
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(1u));
+}
 #undef NFB_WG_N128_REGS
 #undef NFB_WG_N128_OPS
 #undef NFB_WG_D8
 
+// fp16x3: index in a thread's register copy of a 64-row activation operand (uint32_t[16 per
+// K-block], fp16 pairs) of the pair at row arow + 8h, columns 64 kb + 8j + 2lq + {0, 1}
+// (j = 0..7) - the pair an accumulator fragment holds as elements 4j + 2h + {0, 1}.  Entries
+// 16 kb + 4 ks .. + 3 are the register A operand of K step ks of K-block kb.
+__host__ __device__ constexpr int x3_lo_reg(int kb, int j, int h) { return 16 * kb + 2 * j + h; }
+
 // One K-block (64 columns = 4 K-steps) of a warpgroup's 64 rows against one weight
 // unit.  bf16: x W.  fp16x3: per K step x_hi W_hi, x_hi W_lo, x_lo W_hi into the same
-// accumulator.  a_* / b_* are shared-memory byte addresses of the K-block images.
-template <bool kX3, int N>
-__device__ __forceinline__ void wg_unit(float* d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+// accumulator.  a_hi / b_* are shared-memory byte addresses of the K-block images; a_lo
+// is either that of the x_lo image (uint32_t) or this thread's 16 registers of x_lo
+// (const uint32_t*, fp16x3 only, see x3_lo_reg).
+template <bool kX3, int N, typename ALo>
+__device__ __forceinline__ void wg_unit(float* d, uint32_t a_hi, ALo a_lo, uint32_t b_hi, uint32_t b_lo,
                                         uint32_t accumulate) {
-  const uint64_t ah = make_wg_desc(a_hi), al = make_wg_desc(a_lo);
+  constexpr bool kLoRegs = !std::is_integral<ALo>::value;
+  static_assert(kX3 || !kLoRegs, "register x_lo operand is fp16x3 only");
+  const uint64_t ah = make_wg_desc(a_hi);
   const uint64_t bh = make_wg_desc(b_hi), bl = make_wg_desc(b_lo);
 #pragma unroll
   for (int ks = 0; ks < 4; ++ks) {
@@ -182,10 +217,18 @@ __device__ __forceinline__ void wg_unit(float* d, uint32_t a_hi, uint32_t a_lo, 
     const uint32_t acc = (accumulate || ks) ? 1u : 0u;
     if constexpr (N == 16) {
       wg_mma_n16<!kX3>(d, ah + o, bh + o, acc);
-      if constexpr (kX3) { wg_mma_n16<false>(d, ah + o, bl + o, 1u); wg_mma_n16<false>(d, al + o, bh + o, 1u); }
+      if constexpr (kX3) {
+        wg_mma_n16<false>(d, ah + o, bl + o, 1u);
+        if constexpr (kLoRegs) wg_mma_n16_rs(d, a_lo + 4 * ks, bh + o);
+        else wg_mma_n16<false>(d, make_wg_desc(a_lo) + o, bh + o, 1u);
+      }
     } else {
       wg_mma_n128<!kX3>(d, ah + o, bh + o, acc);
-      if constexpr (kX3) { wg_mma_n128<false>(d, ah + o, bl + o, 1u); wg_mma_n128<false>(d, al + o, bh + o, 1u); }
+      if constexpr (kX3) {
+        wg_mma_n128<false>(d, ah + o, bl + o, 1u);
+        if constexpr (kLoRegs) wg_mma_n128_rs(d, a_lo + 4 * ks, bh + o);
+        else wg_mma_n128<false>(d, make_wg_desc(a_lo) + o, bh + o, 1u);
+      }
     }
   }
 }

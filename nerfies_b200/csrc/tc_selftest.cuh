@@ -5,7 +5,9 @@
 // field kernel's weight ring receives them), N in 16-column chunks.
 //   kX3 = false: bf16 operands (nfb_selftest_gemm).
 //   kX3 = true : the fp16x3 chains x_hi W_hi + x_hi W_lo + x_lo W_hi of the field
-//                kernel, A split by round-to-nearest (nfb_selftest_gemm3).
+//                kernel, A split by round-to-nearest (nfb_selftest_gemm3).  As in the
+//                field kernel's hidden layers, x_lo is the register A operand: each
+//                thread loads its values in the accumulator fragment layout (x3_lo_reg).
 #pragma once
 #include "field_tc3.cuh"
 #include "tc_common.cuh"
@@ -49,18 +51,34 @@ tc_selftest_kernel(const float* __restrict__ A, int K, const uint8_t* __restrict
     __syncthreads();
     for (int mt = 0; mt < 2; ++mt) {
       float d[8];
+      const int row = mt * 64 + 16 * wq + (lane >> 2);
+      uint32_t lo[kX3 ? kSelfMaxKb * 16 : 1];
+      if constexpr (kX3) {
+#pragma unroll
+        for (int kb = 0; kb < kSelfMaxKb; ++kb)
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int k = kb * kBlockK + 8 * j + 2 * lq;
+              const float* ar = A + (size_t)(row + 8 * h) * K;
+              uint32_t hi;
+              tc3::split_pair(k < K ? ar[k] : 0.f, k + 1 < K ? ar[k + 1] : 0.f, hi, lo[x3_lo_reg(kb, j, h)]);
+            }
+      }
       wg_fence();
       for (int rep = 0; rep < reps; ++rep)
-        for (int kb = 0; kb < nkb; ++kb) {
+#pragma unroll
+        for (int kb = 0; kb < kSelfMaxKb; ++kb) {
+          if (kb >= nkb) break;
           const uint32_t a0 = smem_u32(a_hi + kb * kABlockBytes) + mt * 8192;
-          const uint32_t a1 = smem_u32(a_lo + kb * kABlockBytes) + mt * 8192;
           const uint32_t b0 = smem_u32(ws + kb * parts * 2048);
-          wg_unit<kX3, 16>(d, a0, a1, b0, b0 + 2048, (rep | kb) != 0);
+          if constexpr (kX3) wg_unit<true, 16>(d, a0, lo + x3_lo_reg(kb, 0, 0), b0, b0 + 2048, (rep | kb) != 0);
+          else wg_unit<false, 16>(d, a0, 0u, b0, b0 + 2048, (rep | kb) != 0);
         }
       wg_commit();
       wg_wait<0>();
       wg_fence_regs<8>(d);
-      const int row = mt * 64 + 16 * wq + (lane >> 2);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const int rr = row + 8 * ((i >> 1) & 1), col = nc * 16 + 8 * (i >> 2) + 2 * lq + (i & 1);
