@@ -390,6 +390,25 @@ int nfb_selftest_sgemm(int mode, long long rows, int n, int k_x, int k_in, int a
                        const float* bias, float* y, const float* dy, float* dx, float* din, float* dw,
                        long long k_split, long long* k_split_used, void* stream);
 
+/* Training precision of a handle: the kernel of every GEMM of nfb_train_value_and_grad(_reg) and
+ * nfb_warp_jacobian (Dense layer forward, dX and dW; the tangent rows of the warp Jacobian).
+ *   NFB_TRAIN_FP32   (default): fp32 CUDA-core GEMMs.
+ *   NFB_TRAIN_TF32X3: tensor-core GEMMs with every operand split into two tf32 parts, three wgmma
+ *                     chains (A_small B_big, A_big B_small, A_big B_big) per k-block of 32 into an
+ *                     fp32 partial, the partials summed in fp32: about 3 x 2^-22 relative per product
+ *                     beside fp32's accumulation error.
+ * Independent of nfb_config.precision (the render kernels).  Any other value fails (nfb_last_error)
+ * and leaves the handle's precision as it was.  No reference analogue. */
+enum { NFB_TRAIN_FP32 = 0, NFB_TRAIN_TF32X3 = 1 };
+int nfb_set_train_precision(nfb_handle* h, int train_precision);
+
+/* nfb_selftest_sgemm in a given training precision (NFB_TRAIN_*): the same arguments, launch and
+ * functors; k_split = 0 picks the split that precision's training step uses. */
+int nfb_selftest_train_gemm(int train_precision, int mode, long long rows, int n, int k_x, int k_in, int act,
+                            const float* x, int ldx, const float* in, int ldin, const float* w, int ldw,
+                            const float* bias, float* y, const float* dy, float* dx, float* din, float* dw,
+                            long long k_split, long long* k_split_used, void* stream);
+
 /* Number of CUDA kernels this handle has launched so far (bench accounting). */
 long long nfb_kernel_launches(const nfb_handle* h);
 /* Thread-local description of the last error returned on this thread. */

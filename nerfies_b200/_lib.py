@@ -21,6 +21,7 @@ SYMBOLS = [
     'nfb_debug_provoke_timeout', 'nfb_set_time_alpha', 'nfb_train_value_and_grad', 'nfb_adam_step',
     'nfb_train_value_and_grad_reg', 'nfb_warp_jacobian', 'nfb_check_abort', 'nfb_reset_abort',
     'nfb_image_metrics_workspace_size', 'nfb_image_metrics', 'nfb_gather_rays', 'nfb_selftest_sgemm',
+    'nfb_set_train_precision', 'nfb_selftest_train_gemm',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -41,6 +42,7 @@ ACTIVATIONS = {'none': 0, 'relu': 1, 'elu': 2, 'leaky_relu': 3, 'tanh': 4,
 WARP_TYPES = {None: 0, 'none': 0, 'translation': 1, 'se3': 2}
 WARP_ENCODERS = {'glo': 0, 'time': 1, 'blend': 2}
 PRECISIONS = {'fp32': 0, 'bf16': 1, 'fp16x3': 2}
+TRAIN_PRECISIONS = {'fp32': 0, 'tf32x3': 1}
 FLAG_COARSE_ONLY = 1
 FLAG_NO_WARP = 2
 FLAG_METADATA_ENCODED = 4
@@ -211,6 +213,10 @@ def load():
   lib.nfb_selftest_sgemm.argtypes = [ci, ll, ci, ci, ci, ci, vp, ci, vp, ci, vp, ci] + [vp] * 6 + [
       ll, ctypes.POINTER(ll), vp]
   lib.nfb_selftest_sgemm.restype = ci
+  lib.nfb_selftest_train_gemm.argtypes = [ci] + lib.nfb_selftest_sgemm.argtypes
+  lib.nfb_selftest_train_gemm.restype = ci
+  lib.nfb_set_train_precision.argtypes = [vp, ci]
+  lib.nfb_set_train_precision.restype = ci
   lib.nfb_debug_provoke_timeout.argtypes = [vp, ci]
   lib.nfb_debug_provoke_timeout.restype = ci
   lib.nfb_last_error.argtypes = []

@@ -189,6 +189,25 @@ __device__ __forceinline__ void wg_mma_n128_rs(float* d, const uint32_t* a, uint
                  NFB_WG_D8(48), NFB_WG_D8(56)
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(1u));
 }
+// D(64 x 128, fp32 registers) (+)= A(64 x 8, smem) * B(128 x 8, smem)^T with tf32 operands (the
+// top 19 bits of each fp32 word).  PTX allows no transpose for .tf32: both operands are K-major.  A
+// 128-byte swizzle row holds 32 fp32 and one K step of 8 is 32 bytes, the same step as the k16
+// forms above, so make_wg_desc and its +2 (16-byte units) per step apply unchanged.
+__device__ __forceinline__ void wg_mma_n128_tf32(float* d, uint64_t a, uint64_t b, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+               "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+               "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+               "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+               "%64, %65, p, 1, 1;\n\t}" NFB_WG_N128_OPS);
+}
+// x rounded to tf32 (round to nearest, ties away; the low 13 bits of the result are zero).
+__device__ __forceinline__ float round_tf32(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return __uint_as_float(r);
+}
 #undef NFB_WG_N128_REGS
 #undef NFB_WG_N128_OPS
 #undef NFB_WG_D8

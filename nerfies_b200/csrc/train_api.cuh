@@ -4,6 +4,7 @@
 #pragma once
 #include "train.cuh"
 #include "train_reg.cuh"
+#include "train_tc.cuh"
 
 namespace {
 
@@ -61,7 +62,21 @@ inline long long dw_split(const nfb_handle* h, long long M, int N, long long K) 
   per = (per + 7) / 8 * 8;
   return std::min<long long>(4096, std::max<long long>(256, per));
 }
-// kAKFast / kBNFast: see sgemm128_kernel (which functor index is contiguous in memory).
+// The same for tf32x3_gemm_kernel, which holds one CTA per SM (two 64 KB stages of shared memory): ~4 CTAs
+// per SM, slices of whole k-blocks (32 rows).
+inline long long dw_split_tf32x3(const nfb_handle* h, long long M, int N, long long K) {
+  const long long tiles = ((M + nfb::train::kT2 - 1) / nfb::train::kT2) * ((N + nfb::train::kT2 - 1) / nfb::train::kT2);
+  const long long want = std::max<long long>(1, (4LL * h->sm_count) / tiles);
+  long long per = (K + want - 1) / want;
+  per = (per + nfb::train::kTcBK - 1) / nfb::train::kTcBK * nfb::train::kTcBK;
+  return std::min<long long>(8192, std::max<long long>(256, per));
+}
+// Rows per slice of a weight-gradient reduction in the handle's training precision.
+inline long long dw_split_for(const nfb_handle* h, long long M, int N, long long K) {
+  return h->train_precision == NFB_TRAIN_TF32X3 ? dw_split_tf32x3(h, M, N, K) : dw_split(h, M, N, K);
+}
+// kAKFast / kBNFast: see sgemm128_kernel (which functor index is contiguous in memory).  The handle's training
+// precision picks the kernel: sgemm128_kernel (fp32) or tf32x3_gemm_kernel (train_tc.cuh).
 template <bool kAKFast = true, bool kBNFast = true, class FA, class FB, class FC>
 int launch_gemm(nfb_handle* h, long long M, int N, long long K, FA fa, FB fb, FC fc, long long k_split,
                 cudaStream_t s, const char* what) {
@@ -69,7 +84,13 @@ int launch_gemm(nfb_handle* h, long long M, int N, long long K, FA fa, FB fb, FC
   const long long per = k_split > 0 ? k_split : K;
   dim3 grid((unsigned)((M + nfb::train::kT2 - 1) / nfb::train::kT2),
             (unsigned)((N + nfb::train::kT2 - 1) / nfb::train::kT2), (unsigned)((K + per - 1) / per));
-  nfb::train::sgemm128_kernel<kAKFast, kBNFast><<<grid, 256, 0, s>>>(nfb::train::GemmShape{M, N, K}, fa, fb, fc, per);
+  if (h->train_precision == NFB_TRAIN_TF32X3) {
+    auto kernel = nfb::train::tf32x3_gemm_kernel<kAKFast, kBNFast, FA, FB, FC>;
+    NFB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, nfb::train::kTcSmem));
+    kernel<<<grid, 256, nfb::train::kTcSmem, s>>>(nfb::train::GemmShape{M, N, K}, fa, fb, fc, per);
+  } else {
+    nfb::train::sgemm128_kernel<kAKFast, kBNFast><<<grid, 256, 0, s>>>(nfb::train::GemmShape{M, N, K}, fa, fb, fc, per);
+  }
   return launch_check(h, what);
 }
 
@@ -103,7 +124,7 @@ int net_backward(nfb_handle* h, const Net& net, const float* in, float* d_in, in
     nfb::train::ConcatA a{x, ldx, st.k_x, in + st.in_off, ld_in};
     // dW += [X | IN]^T dZ   (reduction over the rows, split)
     if (launch_gemm<false, true>(h, K, st.n, rows, nfb::train::ConcatAT{a}, nfb::train::DZB{dz},
-                                 nfb::train::AtomicAdd{h->d_gpacked + st.w_off, st.npad}, dw_split(h, K, st.n, rows), s, "sgemm (dW)")) return -1;
+                                 nfb::train::AtomicAdd{h->d_gpacked + st.w_off, st.npad}, dw_split_for(h, K, st.n, rows), s, "sgemm (dW)")) return -1;
     // db += colsum(dZ)
     {
       dim3 grid((unsigned)((st.n + 31) / 32), (unsigned)std::min<long long>((rows + 255) / 256, 128));
@@ -179,7 +200,7 @@ int tnet_backward(nfb_handle* h, const Net& net, const float* tin, float* d_tin,
     const int ldx = producer[i] >= 0 ? net.steps[producer[i]].npad : ld_in;
     nfb::train::ConcatA a{x, ldx, st.k_x, tin + st.in_off, ld_in};
     if (launch_gemm<false, true>(h, K, st.n, trows, nfb::train::ConcatAT{a}, nfb::train::DZTB{dz},
-                                 nfb::train::AtomicAdd{h->d_gpacked + st.w_off, st.npad}, dw_split(h, K, st.n, trows), s, "sgemm (tangent dW)")) return -1;
+                                 nfb::train::AtomicAdd{h->d_gpacked + st.w_off, st.npad}, dw_split_for(h, K, st.n, trows), s, "sgemm (tangent dW)")) return -1;
     if (i == 0 && st.k_x == 0) break;             // nothing upstream of the encoded input carries a parameter
     float* dx = producer[i] >= 0 ? tarena + d_out_t[producer[i]] : d_tin;
     nfb::train::AccumSplit acc{dx, ldx, st.k_x, d_tin + st.in_off, ld_in};
@@ -611,11 +632,27 @@ int nfb_adam_step(float* params, const float* grads, float* m, float* v, long lo
   return 0;
 }
 
-// The three launches of net_forward / net_backward for one layer, with their functors.
+int nfb_set_train_precision(nfb_handle* h, int train_precision) {
+  if (!h) return fail("null handle");
+  if (train_precision != NFB_TRAIN_FP32 && train_precision != NFB_TRAIN_TF32X3)
+    return fail("train precision %d is not NFB_TRAIN_FP32 (0) or NFB_TRAIN_TF32X3 (1)", train_precision);
+  h->train_precision = train_precision;
+  return 0;
+}
+
 int nfb_selftest_sgemm(int mode, long long rows, int n, int k_x, int k_in, int act, const float* x, int ldx,
                        const float* in, int ldin, const float* w, int ldw, const float* bias, float* y,
                        const float* dy, float* dx, float* din, float* dw, long long k_split,
                        long long* k_split_used, void* stream) {
+  return nfb_selftest_train_gemm(NFB_TRAIN_FP32, mode, rows, n, k_x, k_in, act, x, ldx, in, ldin, w, ldw, bias, y,
+                                 dy, dx, din, dw, k_split, k_split_used, stream);
+}
+
+// The three launches of net_forward / net_backward for one layer, with their functors.
+int nfb_selftest_train_gemm(int train_precision, int mode, long long rows, int n, int k_x, int k_in, int act,
+                            const float* x, int ldx, const float* in, int ldin, const float* w, int ldw,
+                            const float* bias, float* y, const float* dy, float* dx, float* din, float* dw,
+                            long long k_split, long long* k_split_used, void* stream) {
   using namespace nfb::train;
   const int K = k_x + k_in;
   if (rows < 1 || n < 1 || k_x < 0 || k_in < 0 || K < 1) return fail("selftest_sgemm: empty shape");
@@ -626,6 +663,7 @@ int nfb_selftest_sgemm(int mode, long long rows, int n, int k_x, int k_in, int a
     return fail("selftest_sgemm: null operand");
   // launch_gemm reads the SM count (dw_split) and counts launches in a handle; this call has none
   nfb_handle h;
+  if (nfb_set_train_precision(&h, train_precision)) return -1;
   int dev = 0;
   NFB_CUDA(cudaGetDevice(&dev));
   NFB_CUDA(cudaDeviceGetAttribute(&h.sm_count, cudaDevAttrMultiProcessorCount, dev));
@@ -643,7 +681,7 @@ int nfb_selftest_sgemm(int mode, long long rows, int n, int k_x, int k_in, int a
                                   "sgemm (dX)");
   } else if (mode == NFB_SGEMM_DW) {
     if (!y || !dy || !dw) return fail("selftest_sgemm: null y / dy / dw");
-    per = k_split > 0 ? k_split : dw_split(&h, K, n, rows);
+    per = k_split > 0 ? k_split : dw_split_for(&h, K, n, rows);
     rc = launch_gemm<false, true>(&h, K, n, rows, ConcatAT{a}, DZB{dz}, AtomicAdd{dw, ldw}, per, s, "sgemm (dW)");
   } else {
     return fail("selftest_sgemm: bad mode %d", mode);

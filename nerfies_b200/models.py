@@ -145,7 +145,7 @@ class NerfModel:
                use_warp_jacobian=False, use_weights=False,
                use_trunk_condition=False, use_alpha_condition=False,
                use_rgb_condition=False, warp_kwargs=None, precision='fp32',
-               batch_size=8192, device=None):
+               batch_size=8192, device=None, train_precision='fp32'):
     self.num_coarse_samples = int(num_coarse_samples)
     self.num_fine_samples = int(num_fine_samples)
     self.use_viewdirs = bool(use_viewdirs)
@@ -186,6 +186,7 @@ class NerfModel:
     self.use_rgb_condition = bool(use_rgb_condition)
     self.warp_kwargs = dict(warp_kwargs or {})
     self.precision = precision
+    self.train_precision = train_precision
     self.batch_size = int(batch_size)
     if device is None:
       # parameters may be built without a GPU (host-logic tests); apply() needs one.
@@ -219,6 +220,19 @@ class NerfModel:
             'depths > 0, min/max_freq_log2, use_identity_map=False, custom initialisers)')
     if precision not in _lib.PRECISIONS:
       raise ValueError(f'precision must be one of {list(_lib.PRECISIONS)}')
+
+  @property
+  def train_precision(self):
+    """The training GEMMs' kernel (value_and_grad, train_step, the warp Jacobian): 'fp32' (CUDA
+    cores, the default) or 'tf32x3' (tensor cores, three tf32 chains per product).  Independent of
+    `precision`, which picks the render kernels."""
+    return self._train_precision
+
+  @train_precision.setter
+  def train_precision(self, name):
+    if name not in _lib.TRAIN_PRECISIONS:
+      raise ValueError(f'train_precision must be one of {list(_lib.TRAIN_PRECISIONS)}, got {name!r}')
+    self._train_precision = name
 
   # Same derived attributes as the reference (models.py:121-131).
   @property
@@ -314,6 +328,8 @@ class NerfModel:
       if self._handle is not None:
         self._handle.close()
       self._handle = _Handle(self.nfb_config(), want, self.device)
+    _lib.check(self._handle.lib.nfb_set_train_precision(
+        self._handle.h, _lib.TRAIN_PRECISIONS[self.train_precision]))
     return self._handle
 
   def invalidate_params(self):
@@ -717,9 +733,10 @@ def construct_nerf(key, config: configs.ModelConfig, batch_size: int,
                    appearance_ids: Sequence[int], camera_ids: Sequence[int],
                    warp_ids: Sequence[int], near: float, far: float,
                    use_warp_jacobian: bool = False, use_weights: bool = False,
-                   precision: str = 'fp32', device=None):
+                   precision: str = 'fp32', device=None, train_precision: str = 'fp32'):
   """Same signature and return value as models.construct_nerf
-  (models.py:378-489) plus the nerfies_b200-only keywords `precision` and `device`.
+  (models.py:378-489) plus the nerfies_b200-only keywords `precision`, `device` and
+  `train_precision` ('fp32' or 'tf32x3', see NerfModel.train_precision).
 
   Note: like the reference, `use_trunk_condition` is NOT forwarded from the
   config (models.py:424-463)."""
@@ -752,6 +769,6 @@ def construct_nerf(key, config: configs.ModelConfig, batch_size: int,
       warp_field_type=config.warp_field_type,
       warp_metadata_encoder_type=config.warp_metadata_encoder_type,
       warp_kwargs=dict(config.warp_kwargs), precision=precision,
-      batch_size=batch_size, device=device)
+      batch_size=batch_size, device=device, train_precision=train_precision)
   params = init_params(model, key)
   return model, params
