@@ -300,8 +300,11 @@ int launch_check(nfb_handle* h, const char* what) {
   return 0;
 }
 
+// `time_encoder` false leaves the TimeEncoder's share of the warp block to the caller (the training tier runs
+// it on a tape of its own: time_forward, train_api.cuh).
 int run_cond(nfb_handle* h, int B, const float* viewdirs, const unsigned* warp_id,
-             const unsigned* app_id, const unsigned* cam_id, cudaStream_t s, bool encoded = false) {
+             const unsigned* app_id, const unsigned* cam_id, cudaStream_t s, bool encoded = false,
+             bool time_encoder = true) {
   const nfb_config& c = h->cfg;
   nfb::CondArgs a{};
   a.viewdirs = viewdirs; a.warp_id = warp_id; a.app_id = app_id; a.cam_id = cam_id;
@@ -316,7 +319,7 @@ int run_cond(nfb_handle* h, int B, const float* viewdirs, const unsigned* warp_i
   if (enc == NFB_WARP_ENC_TIME && !encoded) a.warp_id = nullptr;   // `warp_id` carries float timestamps
   nfb::ray_cond_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(a);
   if (launch_check(h, "ray_cond_kernel")) return -1;
-  if (enc != NFB_WARP_ENC_GLO && !encoded && warp_id) {
+  if (enc != NFB_WARP_ENC_GLO && !encoded && warp_id && time_encoder) {
     // TimeEncoder on metadata['time'] ('time') or on float(id) ('blend', alpha = None)
     nfb::TimeArgs t{};
     t.params = h->d_packed; t.net = h->time_net;
@@ -811,7 +814,7 @@ void nfb_destroy(nfb_handle* h) {
                    h->d_wc, h->d_samples, h->d_out_c, h->d_out_f, h->d_in};
   for (float* p : bufs) if (p) cudaFree(p);
   float* tbufs[] = {h->d_tape, h->d_gpacked, h->d_gwarp, h->d_gapp, h->d_gcam, h->d_dcond, h->d_tr_out, h->d_tr_w, h->d_loss,
-                    h->d_ttape, reinterpret_cast<float*>(h->d_sel)};
+                    h->d_ttape, reinterpret_cast<float*>(h->d_sel), h->d_time_tape};
   for (float* p : tbufs) if (p) cudaFree(p);
   if (h->d_ids) cudaFree(h->d_ids);
   for (int l = 0; l < 2; ++l)

@@ -97,6 +97,7 @@ struct nfb_handle {
   float *d_gpacked = nullptr, *d_gwarp = nullptr, *d_gapp = nullptr, *d_gcam = nullptr;
   float *d_dcond = nullptr, *d_tr_out = nullptr, *d_tr_w = nullptr, *d_loss = nullptr;
   float* d_ttape = nullptr; long long ttape_floats = 0;     // tangent tape (train_reg.cuh)
+  float* d_time_tape = nullptr; long long time_tape_floats = 0;  // TimeEncoder tape, max_rays rows (time_forward)
   int* d_sel = nullptr; long long sel_cap = 0;              // selected tape rows (median-depth samples)
   int train_precision = NFB_TRAIN_FP32;                     // the training GEMMs' kernel (launch_gemm)
   int debug_bits = 0;                 // FieldArgs::debug bits set through the test hook (abort-path test)

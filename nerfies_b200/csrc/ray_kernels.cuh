@@ -112,6 +112,17 @@ constexpr int kTimeRays = 8;
 constexpr int kTimeThreads = 128;
 constexpr int kTimeMaxIn = 40;     // 1 + 2 F, F <= 19
 
+// Input k of the TimeEncoder at timestamp t (its input stage, shared by time_embed_kernel and the training
+// tier's time_encode_kernel so that both see bitwise the same encoding): t itself, then per frequency f
+// window[f] sin(2^f t) and window[f] sin(2^f t + pi/2) (modules.py:213-228 with C = 1).
+__device__ __forceinline__ float time_encoding(float t, int k, const float* window) {
+  if (k == 0) return t;
+  const int f = (k - 1) >> 1, which = (k - 1) & 1;
+  float ang = t * exp2f((float)f);
+  if (which) ang = ang + kHalfPiF;
+  return window[f] * sinf(ang);
+}
+
 struct TimeArgs {
   const float* params;           // packed dense buffer
   Net net;                       // hidden layers + output layer
@@ -136,17 +147,7 @@ time_embed_kernel(const __grid_constant__ TimeArgs a) {
     const int r = i / din, k = i - r * din;
     const int ray = min(ray0 + r, a.num_rays - 1);
     const float t = a.time_f ? a.time_f[ray] : (float)a.time_id[ray];
-    float v;
-    if (k == 0) {
-      v = t;
-    } else {
-      // features [sin(2^f t)]_f, then... per frequency: sin, sin(. + pi/2) (modules.py:213-228 with C = 1)
-      const int f = (k - 1) >> 1, which = (k - 1) & 1;
-      float ang = t * exp2f((float)f);
-      if (which) ang = ang + kHalfPiF;
-      v = a.window[f] * sinf(ang);
-    }
-    in[r][k] = v;
+    in[r][k] = time_encoding(t, k, a.window);
   }
   __syncthreads();
   int cur = 0;

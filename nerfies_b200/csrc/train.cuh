@@ -10,7 +10,8 @@
 //       backward  dX = dZ W^T         (dZ = dY * act'(Y), formed while loading)
 //                 dW = [X | IN]^T dZ  (reduction over the rows: split + atomicAdd)
 //   * colsum_kernel (bias gradients), encode / se3 / raw-activation kernels and their
-//     adjoints, the adjoint of volumetric_rendering, embedding scatter-add, Adam.
+//     adjoints, the adjoint of volumetric_rendering, embedding scatter-add, the TimeEncoder's input and
+//     output stages and their adjoint ('time' / 'blend' warp metadata encoders), Adam.
 // 80 GB of HBM holds the tape of a whole gpu_fullhd training batch (~31 GB); the
 // caller may still process a batch in ray chunks (gradients accumulate).
 // z_fine is a constant of the fine level (lax.stop_gradient, model_utils.py:211).
@@ -502,6 +503,8 @@ struct CondBwdArgs {
   float* d_warp_table; float* d_app_table; float* d_cam_table;
   int n_warp, n_app, n_cam;
   CondLayout layout;
+  // d(warp block) / d(GLO row): 1 ('glo'), 1 - time_alpha ('blend'), 0 ('time': no table; nothing is scattered)
+  float warp_scale;
 };
 __global__ void cond_bwd_kernel(const CondBwdArgs a) {
   const CondLayout& L = a.layout;
@@ -512,10 +515,59 @@ __global__ void cond_bwd_kernel(const CondBwdArgs a) {
   if (v == 0.f) return;
   int j;
   const CondSource src = cond_source(L, (int)(idx - (long long)ray * L.stride), j);
-  if (src == kCondWarp) atomicAdd(a.d_warp_table + embed_row(a.warp_id, ray, a.n_warp) * L.G + j, v);
-  else if (src == kCondApp) atomicAdd(a.d_app_table + embed_row(a.app_id, ray, a.n_app) * L.A + j, v);
+  if (src == kCondWarp) {
+    if (a.warp_scale != 0.f) atomicAdd(a.d_warp_table + embed_row(a.warp_id, ray, a.n_warp) * L.G + j, a.warp_scale * v);
+  } else if (src == kCondApp) atomicAdd(a.d_app_table + embed_row(a.app_id, ray, a.n_app) * L.A + j, v);
   else if (src == kCondCam) atomicAdd(a.d_cam_table + embed_row(a.cam_id, ray, a.n_cam) * L.C + j, v);
   // view directions carry no parameter
+}
+
+// ---------------------------------------------------------------------------
+// The TimeEncoder of the 'time' / 'blend' warp metadata encoders on the time tape (train_api.cuh,
+// time_forward / time_backward): its Dense layers run through net_forward / net_backward like every other
+// MLP; these kernels are the stages around them.  The timestamp is a constant (it is data), so nothing is
+// differentiated below the first layer.
+// ---------------------------------------------------------------------------
+struct TimeEncodeArgs {
+  const float* time_f;        // (n) timestamps, or null
+  const unsigned* time_id;    // (n) ids used as timestamps (float(id)), or null
+  float window[20];           // cosine_easing_window(F, alpha)
+  float* in;                  // (n, ld): the tape's input rows
+  int din, ld, n;             // din = 1 + 2 F
+};
+__global__ void time_encode_kernel(const __grid_constant__ TimeEncodeArgs a) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)a.n * a.din) return;
+  const int r = (int)(idx / a.din), k = (int)(idx - (long long)r * a.din);
+  const float t = a.time_f ? a.time_f[r] : (float)a.time_id[r];
+  a.in[(long long)r * a.ld + k] = time_encoding(t, k, a.window);
+}
+
+// cond[:, 0:G] = Y ('time'), or (1 - time_alpha) cond + time_alpha Y over the GLO rows already there
+// ('blend', warping.py:132-133): the output stage of time_embed_kernel.
+struct TimeCondArgs {
+  const float* y; int ld;     // (n, ld): the TimeEncoder's output layer
+  float* cond; int stride, G, n;
+  int blend; float time_alpha;
+};
+__global__ void time_cond_kernel(const TimeCondArgs a) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)a.n * a.G) return;
+  const int r = (int)(idx / a.G), q = (int)(idx - (long long)r * a.G);
+  float v = a.y[(long long)r * a.ld + q];
+  float* c = a.cond + (long long)r * a.stride + q;
+  if (a.blend) v = (1.0f - a.time_alpha) * *c + a.time_alpha * v;
+  *c = v;
+}
+
+// Its adjoint towards the TimeEncoder: dY = dcond[:, 0:G] ('time'), time_alpha dcond[:, 0:G] ('blend').
+// (The GLO rows' share, (1 - time_alpha) dcond, is cond_bwd_kernel's warp_scale.)
+__global__ void time_cond_bwd_kernel(const float* __restrict__ dcond, int stride, int G, float scale,
+                                     float* __restrict__ dy, int ld, int n) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)n * G) return;
+  const int r = (int)(idx / G), q = (int)(idx - (long long)r * G);
+  dy[(long long)r * ld + q] = scale * dcond[(long long)r * stride + q];
 }
 
 // packed (K x ld, column offset) gradient -> the caller's dense (rows x cols) tensor (+=).

@@ -131,11 +131,13 @@ int net_backward(nfb_handle* h, const Net& net, const float* in, float* d_in, in
       nfb::train::colsum_kernel<<<grid, 256, 0, s>>>(dz, rows, st.n, h->d_gpacked + st.b_off);
       if (launch_check(h, "colsum_kernel")) return -1;
     }
-    // dX, dIN += dZ W^T
+    // dX, dIN += dZ W^T; without d_in (an input that is not differentiated) dX only
+    if (!d_in && producer[i] < 0) continue;
     float* dx = producer[i] >= 0 ? arena + d_out_off[producer[i]] : d_in;
-    nfb::train::AccumSplit acc{dx, ldx, st.k_x, d_in + st.in_off, ld_in};
-    if (launch_gemm<true, false>(h, rows, K, st.n, dz, nfb::train::WeightBT{h->d_packed + st.w_off, st.npad}, acc, 0, s,
-                                 "sgemm (dX)")) return -1;
+    nfb::train::AccumSplit acc{dx, ldx, st.k_x, d_in ? d_in + st.in_off : nullptr, ld_in};
+    if (launch_gemm<true, false>(h, rows, d_in ? K : st.k_x, st.n, dz,
+                                 nfb::train::WeightBT{h->d_packed + st.w_off, st.npad}, acc, 0, s, "sgemm (dX)"))
+      return -1;
   }
   return 0;
 }
@@ -299,6 +301,84 @@ int warp_backward(nfb_handle* h, const nfb::FieldProgram& p, const TapeLayout& t
   return launch_check(h, "encode_bwd_kernel");
 }
 
+// ---- TimeEncoder tape ('time' / 'blend' warp metadata encoders): max_rays rows, one per ray or free point ----
+struct TimeTapeLayout {
+  long long in = 0, grad_begin = 0, total = 0;
+  long long out[nfb::kMaxSteps], d_out[nfb::kMaxSteps];
+  int ld = 0;
+};
+TimeTapeLayout time_tape_layout(const Net& net, int F, long long rows) {
+  TimeTapeLayout t;
+  long long off = 0;
+  auto take = [&](long long n) { long long o = off; off += (n + 63) / 64 * 64; return o; };
+  t.ld = pad32(1 + 2 * F);
+  t.in = take(rows * t.ld);
+  for (int s = 0; s < net.n_steps; ++s) t.out[s] = take(rows * net.steps[s].npad);
+  t.grad_begin = off;
+  for (int s = 0; s < net.n_steps; ++s) t.d_out[s] = take(rows * net.steps[s].npad);
+  t.total = off;
+  return t;
+}
+
+bool has_time_encoder(const nfb_handle* h) {
+  return h->cfg.warp_field_type != NFB_WARP_NONE && h->cfg.warp_metadata_encoder != NFB_WARP_ENC_GLO;
+}
+
+// The TimeEncoder's share of the warp block of the condition vectors of `n` rays / points: its Dense layers
+// through net_forward on the time tape, so that time_backward differentiates the activations used here.  The
+// timestamps are `time_f` or, when it is null, float(`time_id`) (the 'blend' encoder and the background loss).
+// Writes (or blends into the GLO rows already there) cond[:, 0:G], as time_embed_kernel does when rendering.
+int time_forward(nfb_handle* h, int n, const float* time_f, const unsigned* time_id, cudaStream_t s) {
+  using namespace nfb::train;
+  if (!has_time_encoder(h)) return 0;
+  const nfb_config& c = h->cfg;
+  const Net& net = h->time_net;
+  const TimeTapeLayout t = time_tape_layout(net, c.time_encoder_num_freqs, n);
+  float* T = h->d_time_tape;
+  const bool blend = c.warp_metadata_encoder == NFB_WARP_ENC_BLEND;
+  TimeEncodeArgs e{};
+  e.time_f = time_f; e.time_id = time_id;
+  e.din = 1 + 2 * c.time_encoder_num_freqs; e.ld = t.ld; e.n = n; e.in = T + t.in;
+  easing_window(blend ? (float)c.time_encoder_num_freqs : h->time_alpha, c.time_encoder_num_freqs, e.window);
+  time_encode_kernel<<<(unsigned)(((long long)n * e.din + 255) / 256), 256, 0, s>>>(e);
+  if (launch_check(h, "time_encode_kernel")) return -1;
+  if (net_forward(h, net, T + t.in, t.ld, t.out, T, n, s)) return -1;
+  const int last = net.n_steps - 1;
+  TimeCondArgs w{T + t.out[last], net.steps[last].npad, h->d_cond, h->cond_layout.stride, h->cond_layout.G, n,
+                 blend, h->time_alpha};
+  time_cond_kernel<<<(unsigned)(((long long)n * w.G + 255) / 256), 256, 0, s>>>(w);
+  return launch_check(h, "time_cond_kernel");
+}
+
+// Adjoint of time_forward: the condition-vector gradient of the same `n` rows -> the TimeEncoder's parameter
+// gradients (d_gpacked).  time_alpha is a constant of the step.
+int time_backward(nfb_handle* h, int n, const float* dcond, cudaStream_t s) {
+  using namespace nfb::train;
+  if (!has_time_encoder(h)) return 0;
+  const nfb_config& c = h->cfg;
+  const Net& net = h->time_net;
+  const TimeTapeLayout t = time_tape_layout(net, c.time_encoder_num_freqs, n);
+  float* T = h->d_time_tape;
+  NFB_CUDA(cudaMemsetAsync(T + t.grad_begin, 0, (size_t)(t.total - t.grad_begin) * sizeof(float), s));
+  const int last = net.n_steps - 1, G = h->cond_layout.G;
+  const float scale = c.warp_metadata_encoder == NFB_WARP_ENC_BLEND ? h->time_alpha : 1.f;
+  time_cond_bwd_kernel<<<(unsigned)(((long long)n * G + 255) / 256), 256, 0, s>>>(
+      dcond, h->cond_layout.stride, G, scale, T + t.d_out[last], net.steps[last].npad, n);
+  if (launch_check(h, "time_cond_bwd_kernel")) return -1;
+  return net_backward(h, net, T + t.in, nullptr, t.ld, t.out, t.d_out, T, n, s);
+}
+
+// The condition vectors of `n` rays / points for the training tier (run_cond + time_forward).  `warp_id`
+// holds float timestamps when `float_time` ('time' encoder on rays or Jacobian points), uint32 ids otherwise.
+int train_cond(nfb_handle* h, int n, const float* viewdirs, const unsigned* warp_id, bool float_time,
+               const unsigned* app_id, const unsigned* cam_id, cudaStream_t s) {
+  if (has_time_encoder(h) && !warp_id)
+    return fail("training: the 'time' / 'blend' warp metadata encoders need per-ray metadata (warp_id is null)");
+  if (run_cond(h, n, viewdirs, warp_id, app_id, cam_id, s, false, false)) return -1;
+  return time_forward(h, n, float_time ? reinterpret_cast<const float*>(warp_id) : nullptr,
+                      float_time ? nullptr : warp_id, s);
+}
+
 // forward + loss + backward of one level for `R` rays (rows = R * S) on the tape; `cond` / `dcond` are
 // the R rays' condition vectors and their gradient accumulator.
 int train_level(nfb_handle* h, int level, int R, int S, const float* z, const float* origins,
@@ -409,6 +489,12 @@ int train_prepare(nfb_handle* h, int chunk_rays) {
         dm(&h->d_loss, nfb::train::kLossSlots))
       return -1;
   }
+  // the TimeEncoder's tape holds a whole batch: the batch's condition vectors are built before the chunk loop
+  // and differentiated after it
+  if (has_time_encoder(h) &&
+      grow(&h->d_time_tape, &h->time_tape_floats,
+           time_tape_layout(h->time_net, c.time_encoder_num_freqs, h->max_rays).total, "TimeEncoder tape"))
+    return -1;
   return 0;
 }
 
@@ -420,26 +506,30 @@ int train_prepare_rows(nfb_handle* h, long long rows) {
 
 // warp_field.apply on `n` free points (+ optional noise) on the tape of level 0: condition
 // vectors per point, then warp_forward.  The points land in tape.pts, the warped points in tape.warped.
+// `warp_id`: see train_cond.
 int warp_points_forward(nfb_handle* h, int n, const float* points, const float* noise, const unsigned* warp_id,
-                        cudaStream_t s) {
+                        bool float_time, cudaStream_t s) {
   const nfb::FieldProgram& p = h->prog[0];
   const TapeLayout t = tape_layout(p, n);
   float* A = h->d_tape;
   nfb::train::add_noise_kernel<<<(unsigned)(((long long)n * 3 + 255) / 256), 256, 0, s>>>(points, noise, A + t.warped,
                                                                                         (long long)n * 3);
   if (launch_check(h, "add_noise_kernel")) return -1;
-  if (run_cond(h, n, A + t.warped, warp_id, nullptr, nullptr, s)) return -1;      // the "view direction" columns are unused here
+  // the "view direction" columns are unused here
+  if (train_cond(h, n, A + t.warped, warp_id, float_time, nullptr, nullptr, s)) return -1;
   return warp_forward(h, p, t, nullptr, nullptr, nullptr, 1, A + t.warped, h->d_cond, s);
 }
 
 // Embedding gradients: the condition-vector gradients dcond of B rays, scattered into the tables' gradients
-// (the adjoint of run_cond).
+// (the adjoint of run_cond; time_backward is the TimeEncoder's).
 int run_cond_bwd(nfb_handle* h, int B, const float* dcond, const unsigned* warp_id, const unsigned* app_id,
                  const unsigned* cam_id, cudaStream_t s) {
   const nfb_config& c = h->cfg;
   nfb::train::CondBwdArgs a{};
   a.dcond = dcond; a.num_rays = B;
-  a.warp_id = warp_id; a.app_id = app_id; a.cam_id = cam_id;
+  const int enc = has_time_encoder(h) ? c.warp_metadata_encoder : NFB_WARP_ENC_GLO;
+  a.warp_scale = enc == NFB_WARP_ENC_GLO ? 1.f : enc == NFB_WARP_ENC_BLEND ? 1.f - h->time_alpha : 0.f;
+  a.warp_id = enc == NFB_WARP_ENC_TIME ? nullptr : warp_id; a.app_id = app_id; a.cam_id = cam_id;
   a.d_warp_table = h->d_gwarp; a.d_app_table = h->d_gapp; a.d_cam_table = h->d_gcam;
   a.n_warp = c.num_warp_embeddings; a.n_app = c.num_appearance_embeddings; a.n_cam = c.num_camera_embeddings;
   a.layout = h->cond_layout;
@@ -459,7 +549,10 @@ int train_background(nfb_handle* h, int P, const float* points, const unsigned* 
     const int n = std::min(chunk, P - p0);
     const TapeLayout t = tape_layout(p, n);
     float* A = h->d_tape;
-    if (warp_points_forward(h, n, points + (size_t)p0 * 3, noise ? noise + (size_t)p0 * 3 : nullptr, warp_ids + p0, s)) return -1;
+    // the ids are the timestamps of a 'time' encoder too: float(id) (training.py:120-131)
+    if (warp_points_forward(h, n, points + (size_t)p0 * 3, noise ? noise + (size_t)p0 * 3 : nullptr, warp_ids + p0,
+                            false, s))
+      return -1;
     NFB_CUDA(cudaMemsetAsync(A + t.grad_begin, 0, (size_t)(t.grad_end - t.grad_begin) * sizeof(float), s));
     NFB_CUDA(cudaMemsetAsync(h->d_dcond, 0, (size_t)n * h->cond_layout.stride * sizeof(float), s));
     // alpha = -2, scale = 0.001: the defaults of compute_background_loss, which train_step does not override
@@ -468,7 +561,8 @@ int train_background(nfb_handle* h, int P, const float* points, const unsigned* 
     warp_mag_loss_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(wm);
     if (launch_check(h, "warp_mag_loss_kernel")) return -1;
     if (warp_backward(h, p, t, 1, h->d_dcond, s)) return -1;
-    if (run_cond_bwd(h, n, h->d_dcond, warp_ids + p0, nullptr, nullptr, s)) return -1;
+    if (run_cond_bwd(h, n, h->d_dcond, warp_ids + p0, nullptr, nullptr, s) || time_backward(h, n, h->d_dcond, s))
+      return -1;
   }
   return 0;
 }
@@ -488,8 +582,6 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
   if (count != (int)h->specs.size()) return fail("expected %d gradient tensors, got %d", (int)h->specs.size(), count);
   if (flags & NFB_FLAG_METADATA_ENCODED) return fail("training with metadata_encoded=True is not supported");
   const nfb_config& c = h->cfg;
-  if (c.warp_field_type != NFB_WARP_NONE && c.warp_metadata_encoder != NFB_WARP_ENC_GLO)
-    return fail("training supports the 'glo' warp metadata encoder only (no TimeEncoder backward)");
   for (int i = 0; i < count; ++i)
     if (numels[i] != h->specs[i].rows * h->specs[i].cols)
       return fail("gradient %d (%s): expected %lld elements", i, h->specs[i].name.c_str(), h->specs[i].rows * h->specs[i].cols);
@@ -509,7 +601,8 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
   NFB_CUDA(cudaMemsetAsync(h->d_gcam, 0, (size_t)std::max(1, c.num_camera_embeddings * c.num_camera_features) * sizeof(float), s));
   NFB_CUDA(cudaMemsetAsync(h->d_loss, 0, nfb::train::kLossSlots * sizeof(float), s));
   // condition vectors of the whole batch (per ray), their gradient accumulator
-  if (run_cond(h, B, viewdirs ? viewdirs : directions, warp_id, app_id, cam_id, s)) return -1;
+  const bool float_time = has_time_encoder(h) && c.warp_metadata_encoder == NFB_WARP_ENC_TIME;
+  if (train_cond(h, B, viewdirs ? viewdirs : directions, warp_id, float_time, app_id, cam_id, s)) return -1;
   NFB_CUDA(cudaMemsetAsync(h->d_dcond, 0, (size_t)B * h->cond_layout.stride * sizeof(float), s));
   if (nfb_coarse_z_vals(h, B, t_rand, h->d_zc, stream)) return -1;
   const float scale = 1.f / ((float)B * 3.f);       // mean over the local batch (training.py:173)
@@ -549,7 +642,7 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
         return -1;
     }
   }
-  if (run_cond_bwd(h, B, h->d_dcond, warp_id, app_id, cam_id, s)) return -1;
+  if (run_cond_bwd(h, B, h->d_dcond, warp_id, app_id, cam_id, s) || time_backward(h, B, h->d_dcond, s)) return -1;
   // background loss (training.py:118-135, 246-257): warp_field.apply on free points
   const int P = (reg && reg->use_background_loss) ? reg->num_background_points : 0;
   if (P > 0) {
@@ -598,7 +691,6 @@ int nfb_warp_jacobian(nfb_handle* h, int P, const float* points, const unsigned*
   if (check_call(h, std::min(P, h->max_rays))) return -1;
   const nfb_config& c = h->cfg;
   if (h->prog[0].warp_type == 0) return fail("the model has no warp field");
-  if (c.warp_metadata_encoder != NFB_WARP_ENC_GLO) return fail("warp Jacobian: 'glo' warp metadata encoder only");
   cudaStream_t s = (cudaStream_t)stream;
   if (enter_stream(h, s)) return -1;
   if (P == 0) return 0;
@@ -607,7 +699,9 @@ int nfb_warp_jacobian(nfb_handle* h, int P, const float* points, const unsigned*
   if (train_prepare_rows(h, chunk)) return -1;
   for (int p0 = 0; p0 < P; p0 += chunk) {
     const int n = std::min(chunk, P - p0);
-    if (warp_points_forward(h, n, points + (size_t)p0 * 3, nullptr, warp_id ? warp_id + p0 : nullptr, s)) return -1;
+    if (warp_points_forward(h, n, points + (size_t)p0 * 3, nullptr, warp_id ? warp_id + p0 : nullptr,
+                            c.warp_metadata_encoder == NFB_WARP_ENC_TIME, s))
+      return -1;
     const nfb::FieldProgram& p = h->prog[0];
     const TapeLayout t = tape_layout(p, n);
     if (warped_out)

@@ -140,7 +140,11 @@ def value_and_grad(model, params, batch, warp_extra, rngs=None, chunk_rays=256, 
   B = origins.shape[0]
   viewdirs = _prep_f32(batch['viewdirs'], dev) if 'viewdirs' in batch else None
   md = batch.get('metadata', {})
-  warp_id = _prep_ids(md.get('warp'), dev) if model.use_warp else None
+  if model.use_warp and model.warp_metadata_encoder_type == 'time':
+    # models.py:252-254: the TimeEncoder reads metadata['time'] (B,1) float32
+    warp_id = None if md.get('time') is None else _prep_f32(md['time'], dev).reshape(-1)
+  else:
+    warp_id = _prep_ids(md.get('warp'), dev) if model.use_warp else None
   app_id = _prep_ids(md.get('appearance'), dev) if model.use_appearance_metadata else None
   cam_id = _prep_ids(md.get('camera'), dev) if model.use_camera_metadata else None
   target = _prep_f32(batch['rgb'], dev)[..., :3].contiguous()
@@ -150,6 +154,7 @@ def value_and_grad(model, params, batch, warp_extra, rngs=None, chunk_rays=256, 
   u_rand = None if u_rand is None else _prep_f32(u_rand, dev)
   hd = model.handle(B)
   hd.set_params(params)
+  model._set_time_alpha(hd, (warp_extra or {'time_alpha': 0.0}).get('time_alpha'))
   n = len(hd.param_specs)
   numels = [r * c for _, r, c in hd.param_specs]
   if grads is None:
