@@ -37,6 +37,9 @@ struct FieldArgs {
   const float* origins;      // (B,3)
   const float* directions;   // (B,3)
   const float* z_vals;       // (B,S) or nullptr (= 0: free-point mode)
+  const float* points;       // (B*S, 3) already-warped sample points, or nullptr.  When set, a row's
+                             // point is read from here instead of o + z d and the warp net is skipped;
+                             // z_vals still gives the composite's dists and depth.
   const float* cond;         // (B, cond_stride) per-ray [glo | tc | ac | rc]
   const float* window;       // (Fw) cosine-easing window
   float* samples;            // (B*S, 4) out: r,g,b,sigma  (nullable)
@@ -193,9 +196,12 @@ field_simt_kernel(const __grid_constant__ FieldProgram prog, const FieldArgs arg
   const int S = args.samples_per_ray;
   const long long ray = m / S;
 
-  // Sample point x = o + z d.
+  // Sample point x = o + z d, or the given (warped) point.
   float x[3];
-  {
+  if (args.points) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) x[c] = __ldg(args.points + m * 3 + c);
+  } else {
     const float z = args.z_vals ? __ldg(args.z_vals + m) : 0.f;
 #pragma unroll
     for (int c = 0; c < 3; ++c)
@@ -203,7 +209,7 @@ field_simt_kernel(const __grid_constant__ FieldProgram prog, const FieldArgs arg
   }
   const float* cond = args.cond + ray * prog.cond_stride;
 
-  const bool do_warp = args.use_warp && prog.warp_type != 0;
+  const bool do_warp = args.use_warp && prog.warp_type != 0 && !args.points;
   if (do_warp) {
     // Warp-field inputs: identity, windowed posenc, GLO code (warping.py:325-326,
     // modules.py:240-272).

@@ -264,7 +264,7 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
     fence_barrier_init();
   }
   __syncthreads();
-  const bool do_warp = args.use_warp && prog.warp_type != 0;
+  const bool do_warp = args.use_warp && prog.warp_type != 0 && !args.points;
   int first_step = 0;
   if (!do_warp) {
     while (first_step < prog.n_steps && prog.steps[first_step].epi != kEpiWarpHeads) ++first_step;
@@ -337,7 +337,8 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
     RowState row;
 
     // Row state of tile `tile` (model_utils.py:72-73) and this thread's half of its first
-    // input block (warping.py:325-326 / models.py:270).
+    // input block (warping.py:325-326 / models.py:270).  With FieldArgs::points the row's point
+    // is the given (already warped) one and the NeRF net's inputs come first.
     auto begin_tile = [&](int tile) {
       long long m = (long long)tile * kTileRows + r;
       row.valid = m < args.num_rows;
@@ -351,8 +352,13 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
         dir[c] = __ldg(args.directions + row.ray * 3 + c);
         org[c] = __ldg(args.origins + row.ray * 3 + c);
       }
+      if (args.points) {
 #pragma unroll
-      for (int c = 0; c < 3; ++c) row.x[c] = org[c] + z * dir[c];
+        for (int c = 0; c < 3; ++c) row.x[c] = __ldg(args.points + m * 3 + c);
+      } else {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) row.x[c] = org[c] + z * dir[c];
+      }
       if (fuse) {
         // dists of volumetric_rendering (model_utils.py:98-104)
         row.z = z;

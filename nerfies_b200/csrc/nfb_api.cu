@@ -342,19 +342,23 @@ bool can_fuse_composite(const nfb_handle* h, int S) {
   return h->cfg.precision == NFB_PREC_FP16X3 && S % 128 == 0 && S <= nfb::kMaxSamples;
 }
 
+// Profiled launches (nfb_set_profiling) record the level's event pair around the field kernel.
+// Warp-only passes and passes on given points are not timed here: on the fine level they are
+// parts of render_fine_reusing_warp, which times them together.
 int run_field(nfb_handle* h, int level, long long rows, int S, const float* origins,
               const float* directions, const float* z, float* samples, float* warped,
               bool use_warp, bool warp_only, cudaStream_t s, float* ray_out = nullptr,
-              float* ray_weights = nullptr) {
+              float* ray_weights = nullptr, const float* points = nullptr) {
   if (rows == 0) return 0;
   nfb::FieldArgs a{};
   a.ray_out = ray_out; a.ray_weights = ray_weights;
   a.white_bg = h->cfg.use_white_background; a.sample_at_infinity = h->cfg.use_sample_at_infinity;
   a.params = h->d_packed; a.origins = origins; a.directions = directions; a.z_vals = z;
+  a.points = points;
   a.cond = h->d_cond; a.window = h->d_window; a.samples = samples; a.warped = warped;
   a.num_rows = rows; a.samples_per_ray = S; a.use_warp = use_warp; a.warp_only = warp_only;
   a.debug = h->debug_bits;
-  const bool prof = h->profiling && !warp_only;
+  const bool prof = h->profiling && !warp_only && !points;
   if (prof) NFB_CUDA(cudaEventRecord(h->ev[level][0], s));
   int rc;
   if (h->cfg.precision == NFB_PREC_FP32) {
@@ -384,31 +388,72 @@ int run_composite(nfb_handle* h, int B, int S, const float* samples, const float
   return launch_check(h, "composite_kernel");
 }
 
+// `z_new` and `src` (both or neither): see ResampleArgs.
 int run_resample(nfb_handle* h, int B, const float* zc, const float* wc, const float* u_rand,
-                 float* zf, cudaStream_t s) {
+                 float* zf, cudaStream_t s, float* z_new = nullptr, uint16_t* src = nullptr) {
   const nfb_config& c = h->cfg;
   nfb::ResampleArgs a{};
   a.z_coarse = zc; a.w_coarse = wc; a.u_rand = u_rand; a.u_lin = h->d_ulin; a.z_fine = zf;
+  a.z_new = z_new; a.src = src;
   a.num_rays = B; a.nc = c.num_coarse_samples; a.nf = c.num_fine_samples;
   int p = 1;
   while (p < a.nc + a.nf) p <<= 1;
   a.npow2 = p;
   if (a.nc < 3) return fail("hierarchical sampling needs >= 3 coarse samples");
   const int blocks = (B + nfb::kRaysPerBlock - 1) / nfb::kRaysPerBlock;
-  const size_t smem = (size_t)nfb::kRaysPerBlock * (2 * a.nc + p) * sizeof(float);
+  size_t smem = (size_t)nfb::kRaysPerBlock * (2 * a.nc + p) * sizeof(float);
+  if (src) smem += (size_t)nfb::kRaysPerBlock * p * sizeof(uint16_t);
   nfb::resample_kernel<<<blocks, 32 * nfb::kRaysPerBlock, smem, s>>>(a);
   return launch_check(h, "resample_kernel");
 }
 
 // One level of nfb_render_forward: the field at the S samples of every ray, then volumetric
-// rendering into `out` (and `weights`, if not null).
+// rendering into `out` (and `weights`, if not null).  `warped` (nullable) receives the warped
+// points; `points` (nullable) gives them instead of warping (FieldArgs::points).
 int render_level(nfb_handle* h, int level, int B, int S, const float* origins, const float* directions,
-                 const float* z, bool use_warp, float* out, float* weights, cudaStream_t s) {
+                 const float* z, bool use_warp, float* out, float* weights, cudaStream_t s,
+                 float* warped = nullptr, const float* points = nullptr) {
   const long long rows = (long long)B * S;
   if (can_fuse_composite(h, S))   // field + volumetric rendering in one kernel: 24 B per ray (+ the weights) leave the SM
-    return run_field(h, level, rows, S, origins, directions, z, nullptr, nullptr, use_warp, false, s, out, weights);
-  if (run_field(h, level, rows, S, origins, directions, z, h->d_samples, nullptr, use_warp, false, s)) return -1;
+    return run_field(h, level, rows, S, origins, directions, z, nullptr, warped, use_warp, false, s, out, weights,
+                     points);
+  if (run_field(h, level, rows, S, origins, directions, z, h->d_samples, warped, use_warp, false, s, nullptr, nullptr,
+                points))
+    return -1;
   return run_composite(h, B, S, h->d_samples, z, directions, out, weights, s);
+}
+
+// True when nfb_render_forward's fine level reuses the coarse level's warped points.
+bool reuses_warp(const nfb_handle* h, bool use_warp) {
+  return use_warp && h->d_warped_c != nullptr;
+}
+
+// The fine level of nfb_render_forward for a warped model.  Its Nc + Nf samples are the Nc coarse
+// samples, whose warped points the coarse pass kept in d_warped_c, and the Nf new ones: only those
+// are warped (a warp-only pass in draw order), the two sets are gathered in z_fine's order, and the
+// NeRF pass reads the gathered points.  A warped point depends on its z bits, its ray, the warp
+// weights and the kernel alone, so this computes what warping all Nc + Nf samples computes.
+// Profiling times the three launches as the level's field time.
+int render_fine_reusing_warp(nfb_handle* h, int B, const float* origins, const float* directions,
+                             const float* zf, float* out, float* weights, cudaStream_t s) {
+  const nfb_config& c = h->cfg;
+  const int nc = c.num_coarse_samples, nf = c.num_fine_samples, n = nc + nf;
+  const bool prof = h->profiling;
+  if (prof) NFB_CUDA(cudaEventRecord(h->ev[1][0], s));
+  if (run_field(h, 1, (long long)B * nf, nf, origins, directions, h->d_znew, nullptr, h->d_warped_new, true, true, s))
+    return -1;
+  nfb::GatherWarpedArgs g{};
+  g.warped_c = h->d_warped_c; g.warped_new = h->d_warped_new; g.src = h->d_src; g.warped_fine = h->d_warped_fine;
+  g.num_rays = B; g.nc = nc; g.nf = nf;
+  const long long total = (long long)B * n;
+  nfb::gather_warped_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(g);
+  if (launch_check(h, "gather_warped_kernel")) return -1;
+  if (render_level(h, 1, B, n, origins, directions, zf, true, out, weights, s, nullptr, h->d_warped_fine)) return -1;
+  if (prof) {
+    NFB_CUDA(cudaEventRecord(h->ev[1][1], s));
+    h->ev_valid[1] = true;
+  }
+  return 0;
 }
 
 // The tensor-core kernels never trap on a protocol error (see tc_common.cuh,
@@ -795,6 +840,14 @@ int nfb_create(const nfb_config* cfg, int max_rays, nfb_handle** out) {
       dmalloc(&h->d_out_f, B * 6) || dmalloc(&h->d_in, B * 9))
     return bail(-1);
   if (cudaMalloc(&h->d_ids, (size_t)B * 3 * sizeof(unsigned)) != cudaSuccess) return bail(fail("cudaMalloc ids failed"));
+  if (c.warp_field_type != NFB_WARP_NONE && c.num_fine_samples > 0) {   // render_fine_reusing_warp
+    const int nf = c.num_fine_samples;
+    if (dmalloc(&h->d_warped_c, B * nc * 3) || dmalloc(&h->d_warped_new, B * nf * 3) ||
+        dmalloc(&h->d_warped_fine, B * nfine * 3) || dmalloc(&h->d_znew, B * nf))
+      return bail(-1);
+    if (cudaMalloc(&h->d_src, (size_t)B * nfine * sizeof(uint16_t)) != cudaSuccess)
+      return bail(fail("cudaMalloc of %lld sample indices failed", B * nfine));
+  }
   if (cudaMemset(h->d_packed, 0, (size_t)h->packed_floats * sizeof(float)) != cudaSuccess) return bail(fail("cudaMemset failed"));
   if (cudaFuncSetAttribute(nfb::field_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            nfb::kSimtSmemBytes) != cudaSuccess)
@@ -811,8 +864,10 @@ void nfb_destroy(nfb_handle* h) {
   nfb::tc::destroy_tc(h);
   float* bufs[] = {h->d_packed, h->d_warp_table, h->d_app_table, h->d_cam_table, h->d_zlin,
                    h->d_lower, h->d_upper, h->d_ulin, h->d_window, h->d_cond, h->d_zc, h->d_zf,
-                   h->d_wc, h->d_samples, h->d_out_c, h->d_out_f, h->d_in};
+                   h->d_wc, h->d_samples, h->d_out_c, h->d_out_f, h->d_in, h->d_warped_c,
+                   h->d_warped_new, h->d_warped_fine, h->d_znew};
   for (float* p : bufs) if (p) cudaFree(p);
+  if (h->d_src) cudaFree(h->d_src);
   float* tbufs[] = {h->d_tape, h->d_gpacked, h->d_gwarp, h->d_gapp, h->d_gcam, h->d_dcond, h->d_tr_out, h->d_tr_w, h->d_loss,
                     h->d_ttape, reinterpret_cast<float*>(h->d_sel), h->d_time_tape};
   for (float* p : tbufs) if (p) cudaFree(p);
@@ -927,17 +982,23 @@ int nfb_render_forward(nfb_handle* h, int B, const float* origins, const float* 
   if (set_window(h, warp_alpha, s)) return -1;
   if (run_cond(h, B, viewdirs ? viewdirs : directions, warp_id, app_id, cam_id, s,
                (flags & NFB_FLAG_METADATA_ENCODED) != 0)) return -1;
+  // With a warp field the fine level warps only its new samples (render_fine_reusing_warp).
+  const bool reuse = fine && reuses_warp(h, use_warp);
   // coarse level (models.py:332-349)
   if (nfb_coarse_z_vals(h, B, t_rand, h->d_zc, stream)) return -1;
   float* wc = w_coarse ? w_coarse : h->d_wc;
   if (render_level(h, 0, B, nc, origins, directions, h->d_zc, use_warp, out_coarse ? out_coarse : h->d_out_c,
-                   wc, s)) return -1;
+                   wc, s, reuse ? h->d_warped_c : nullptr)) return -1;
   if (!fine) return 0;
   // hierarchical resampling + fine level (models.py:352-370)
   float* zf = z_fine ? z_fine : h->d_zf;
+  float* of = out_fine ? out_fine : h->d_out_f;
+  if (reuse) {
+    if (run_resample(h, B, h->d_zc, wc, u_rand, zf, s, h->d_znew, h->d_src)) return -1;
+    return render_fine_reusing_warp(h, B, origins, directions, zf, of, w_fine, s);
+  }
   if (run_resample(h, B, h->d_zc, wc, u_rand, zf, s)) return -1;
-  return render_level(h, 1, B, nfine, origins, directions, zf, use_warp, out_fine ? out_fine : h->d_out_f,
-                      w_fine, s);
+  return render_level(h, 1, B, nfine, origins, directions, zf, use_warp, of, w_fine, s);
 }
 
 int nfb_render_forward_host(nfb_handle* h, int B, const float* origins, const float* directions,

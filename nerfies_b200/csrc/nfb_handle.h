@@ -78,6 +78,10 @@ struct nfb_handle {
   float *d_cond = nullptr, *d_zc = nullptr, *d_zf = nullptr, *d_wc = nullptr;
   float* d_samples = nullptr;
   float *d_out_c = nullptr, *d_out_f = nullptr;
+  // fine level on reused warped points (render_fine_reusing_warp): models with a warp field and
+  // a fine level only
+  float *d_warped_c = nullptr, *d_warped_new = nullptr, *d_warped_fine = nullptr, *d_znew = nullptr;
+  uint16_t* d_src = nullptr;
   // device + pinned staging for the *_host entry point
   float *d_in = nullptr, *h_in = nullptr, *h_out = nullptr;
   unsigned *d_ids = nullptr, *h_ids = nullptr;

@@ -309,8 +309,33 @@ struct ResampleArgs {
   const float* u_rand;     // (B,Nf) or null
   const float* u_lin;      // (Nf) linspace(0,1,Nf)
   float* z_fine;           // (B,Nc+Nf) sorted
+  // Optional, together: the new samples in draw order, and where each entry of z_fine came
+  // from, as its index in concat(z_coarse, z_new) (gather_warped_kernel).
+  float* z_new;            // (B,Nf) or null
+  uint16_t* src;           // (B,Nc+Nf) or null
   int num_rays, nc, nf, npow2;
 };
+
+// One warp sorts keys[0, npow2) ascending (bitonic network); with kIdx, idx[] follows its keys.
+template <bool kIdx>
+__device__ __forceinline__ void bitonic_sort(float* keys, uint16_t* idx, int npow2, int lane) {
+  for (int k = 2; k <= npow2; k <<= 1) {
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = lane; i < npow2; i += 32) {
+        const int p = i ^ j;
+        if (p > i) {
+          const float x = keys[i], y = keys[p];
+          const bool up = (i & k) == 0;
+          if ((x > y) == up) {
+            keys[i] = y; keys[p] = x;
+            if constexpr (kIdx) { const uint16_t q = idx[i]; idx[i] = idx[p]; idx[p] = q; }
+          }
+        }
+      }
+      __syncwarp();
+    }
+  }
+}
 
 __global__ void __launch_bounds__(32 * kRaysPerBlock)
 resample_kernel(const ResampleArgs a) {
@@ -358,27 +383,53 @@ resample_kernel(const ResampleArgs a) {
     float denom = c1 - c0;
     if (denom < 1e-5f) denom = 1.f;
     const float t = (u - c0) / denom;
-    zs[nc + j] = b0 + t * (b1 - b0);
+    const float z = b0 + t * (b1 - b0);
+    zs[nc + j] = z;
+    if (a.z_new) a.z_new[(size_t)ray * nf + j] = z;
   }
   const int n = nc + nf;
   for (int i = n + lane; i < a.npow2; i += 32) zs[i] = CUDART_INF_F;
+  // with `src`: the sort carries each key's index in concat(z_coarse, z_new) along; the swaps
+  // depend on the keys alone, so z_fine is the same either way.  (Entries past n are the +inf
+  // padding; index 0 keeps them in range should a non-finite key sort behind one.)
+  uint16_t* si = a.src ? reinterpret_cast<uint16_t*>(sh + kRaysPerBlock * (2 * nc + a.npow2)) + warp * a.npow2
+                       : nullptr;
+  if (si)
+    for (int i = lane; i < a.npow2; i += 32) si[i] = (uint16_t)(i < n ? i : 0);
   __syncwarp();
   // jnp.sort(concat([z_vals, z_samples])) (model_utils.py:213): bitonic network.
-  for (int k = 2; k <= a.npow2; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = lane; i < a.npow2; i += 32) {
-        const int p = i ^ j;
-        if (p > i) {
-          const float x = zs[i], y = zs[p];
-          const bool up = (i & k) == 0;
-          if ((x > y) == up) { zs[i] = y; zs[p] = x; }
-        }
-      }
-      __syncwarp();
-    }
-  }
+  if (si) bitonic_sort<true>(zs, si, a.npow2, lane);
+  else bitonic_sort<false>(zs, nullptr, a.npow2, lane);
   float* out = a.z_fine + (size_t)ray * n;
   for (int i = lane; i < n; i += 32) out[i] = zs[i];
+  if (si)
+    for (int i = lane; i < n; i += 32) a.src[(size_t)ray * n + i] = si[i];
+}
+
+// ---------------------------------------------------------------------------
+// The fine level's sample points from work already done (nfb_render_forward): the
+// warped point of fine sample i of a ray is that of the coarse sample or of the new
+// sample it was sorted from (ResampleArgs::src).  Both were warped from the same z
+// bits by the same kernel and weights, so the result is what warping z_fine gives.
+// One thread per fine sample.
+// ---------------------------------------------------------------------------
+struct GatherWarpedArgs {
+  const float* warped_c;     // (B,Nc,3)  the coarse level's warped points
+  const float* warped_new;   // (B,Nf,3)  the new samples' warped points, draw order
+  const uint16_t* src;       // (B,Nc+Nf) index in concat(z_coarse, z_new)
+  float* warped_fine;        // (B,Nc+Nf,3)
+  int num_rays, nc, nf;
+};
+
+__global__ void gather_warped_kernel(const GatherWarpedArgs a) {
+  const int n = a.nc + a.nf;
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)a.num_rays * n) return;
+  const long long ray = idx / n;
+  const int s = a.src[idx];
+  const float* p = s < a.nc ? a.warped_c + (ray * a.nc + s) * 3 : a.warped_new + (ray * a.nf + (s - a.nc)) * 3;
+  float* o = a.warped_fine + idx * 3;
+  o[0] = p[0]; o[1] = p[1]; o[2] = p[2];
 }
 
 }  // namespace nfb
