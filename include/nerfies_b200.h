@@ -354,6 +354,11 @@ int nfb_image_metrics(int num_images, int height, int width, int channels,
  * launches afterwards.  No reference analogue. */
 int nfb_debug_provoke_timeout(nfb_handle* h, int enabled);
 
+/* Test hook: while enabled, the tensor-core warp pass runs in 128-row tiles even where the warp
+ * MLP (no layer wider than 128) fits the 256-row tiles it otherwise uses, so that tests can compare
+ * the two bit for bit.  No reference analogue. */
+int nfb_debug_one_row_block(nfb_handle* h, int enabled);
+
 /* The asynchronous entry points (nfb_render_forward, nfb_render_samples, nfb_warp_forward, ...) return
  * before their kernels finish, so a tensor-core kernel's protocol time-out (see the conventions above)
  * is only seen by a LATER call.  nfb_check_abort reports it for the work already submitted: with

@@ -21,7 +21,7 @@ SYMBOLS = [
     'nfb_debug_provoke_timeout', 'nfb_set_time_alpha', 'nfb_train_value_and_grad', 'nfb_adam_step',
     'nfb_train_value_and_grad_reg', 'nfb_warp_jacobian', 'nfb_check_abort', 'nfb_reset_abort',
     'nfb_image_metrics_workspace_size', 'nfb_image_metrics', 'nfb_gather_rays', 'nfb_selftest_sgemm',
-    'nfb_set_train_precision', 'nfb_selftest_train_gemm',
+    'nfb_set_train_precision', 'nfb_selftest_train_gemm', 'nfb_debug_one_row_block',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -219,6 +219,8 @@ def load():
   lib.nfb_set_train_precision.restype = ci
   lib.nfb_debug_provoke_timeout.argtypes = [vp, ci]
   lib.nfb_debug_provoke_timeout.restype = ci
+  lib.nfb_debug_one_row_block.argtypes = [vp, ci]
+  lib.nfb_debug_one_row_block.restype = ci
   lib.nfb_last_error.argtypes = []
   lib.nfb_last_error.restype = ctypes.c_char_p
   lib.nfb_version.argtypes = []

@@ -32,6 +32,11 @@ constexpr int kSimtSmemFloats =
     + 3 * kTM;               // warped points
 constexpr int kSimtSmemBytes = kSimtSmemFloats * 4;
 
+// FieldArgs::debug bits.  kDebugTimeout: the weight producer of the tensor-core kernel first waits
+// on a barrier that never completes.  kDebugOneRowBlock: the tensor-core warp pass runs in 128-row
+// tiles (kMB = 1) even where the warp net fits 256-row tiles.
+constexpr int kDebugTimeout = 8, kDebugOneRowBlock = 16;
+
 struct FieldArgs {
   const float* params;       // packed weights/biases
   const float* origins;      // (B,3)
@@ -48,8 +53,8 @@ struct FieldArgs {
   int samples_per_ray;       // S
   int use_warp;              // run the warp net
   int warp_only;             // stop after the warp (nfb_warp_forward)
-  int debug;                 // test hook (nfb_debug_provoke_timeout): bit 8 = the weight producer of the
-                             // tensor-core kernel first waits on a barrier that never completes
+  int debug;                 // test hooks: kDebugTimeout (nfb_debug_provoke_timeout), kDebugOneRowBlock
+                             // (nfb_debug_one_row_block)
   // fp16x3 kernel: volumetric rendering fused into the rgb epilogue (samples_per_ray a multiple
   // of 128): per-ray (rgb3, depth, med_depth, acc) and, optionally, the weights.
   float* ray_out;            // (B,6) or nullptr = no fused composite

@@ -62,14 +62,15 @@ __device__ __forceinline__ void posenc_fast_to_block(uint8_t* block, int r, cons
 }
 // This thread's half `hs` (32 columns) of row r of the input block, [x | window * posenc(x) | extra | 0...],
 // in the kernel's precision: fp16 hi / lo images (kX3) or bf16.  Inlined: a call with a literal null `extra`
-// and n_extra = 0 carries no extra-column code (register pressure).
-template <bool kX3>
+// and n_extra = 0 carries no extra-column code (register pressure).  The lo image follows the hi
+// image at kBlkBytes.
+template <bool kX3, uint32_t kBlkBytes>
 __device__ __forceinline__ void encode_input(uint8_t* in_block, int r, int hs, const float* x, int F,
                                              const float* __restrict__ window,
                                              const float* __restrict__ extra, int n_extra) {
   if constexpr (kX3) {
-    if (hs == 0) tc3::posenc_block_x3<0>(in_block, in_block + kABlockBytes, r, x, F, window, extra, n_extra);
-    else tc3::posenc_block_x3<1>(in_block, in_block + kABlockBytes, r, x, F, window, extra, n_extra);
+    if (hs == 0) tc3::posenc_block_x3<0>(in_block, in_block + kBlkBytes, r, x, F, window, extra, n_extra);
+    else tc3::posenc_block_x3<1>(in_block, in_block + kBlkBytes, r, x, F, window, extra, n_extra);
   } else {
     posenc_fast_to_block(in_block, r, x, F, window, extra, n_extra, 4 * hs, 4 * hs + 4);
   }
@@ -98,8 +99,9 @@ __device__ __forceinline__ void cond_to_block(uint8_t* block, int r, const float
 // (the conversion is then exact), lo = fp16(v - hi) (exact subtraction):
 // v - (hi + lo) <= 2^-23 |v|, the bound of a round-to-nearest split.  ReLU rides on the
 // conversions: for v < 0 both hi and v - hi are <= 0 and convert to +0.  Conversions
-// saturate: |v| > 65504 does not become inf.
-template <bool kX3>
+// saturate: |v| > 65504 does not become inf.  kBlkBytes: bytes of one K-block of the tile's
+// activation image (128 or 256 rows).
+template <bool kX3, uint32_t kBlkBytes>
 __device__ __forceinline__ void epi_chunk(const float* acc, int c, const float* __restrict__ bias, float inv_s,
                                           bool relu, bool adot, const float* __restrict__ aw, float& al0,
                                           float& al1, uint8_t* act_hi, uint32_t* lo, int arow, int lq) {
@@ -118,7 +120,7 @@ __device__ __forceinline__ void epi_chunk(const float* acc, int c, const float* 
       al1 = fmaf(relu ? fmaxf(v[2], 0.f) : v[2], w.x, al1);
       al1 = fmaf(relu ? fmaxf(v[3], 0.f) : v[3], w.y, al1);
     }
-    const uint32_t blk = (uint32_t)(2 * c + (j >> 3)) * kABlockBytes + 4 * lq;
+    const uint32_t blk = (uint32_t)(2 * c + (j >> 3)) * kBlkBytes + 4 * lq;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const uint32_t off = blk + swz_off(arow + 8 * h, j & 7);
@@ -171,10 +173,20 @@ struct RowState {
 // Fused per-sample field evaluation on the Hopper tensor cores (wgmma), one kernel for
 // both tensor-core precisions (kX3: fp16x3, else bf16).
 //
-// Persistent, one CTA per SM, 384 threads, one 128-row tile at a time:
+// A launch runs one of the program's two nets (TcProgram::n_warp): the warp pass (FieldArgs::
+// warp_only) evaluates the warp MLP and the SE(3) / translation tail and writes the warped
+// points; the NeRF pass reads them (FieldArgs::points), or forms o + z d without a warp.
+//
+// Persistent, one CTA per SM, 384 threads, one tile of 128 kMB rows at a time:
 //   warpgroup 0     : warp 0 streams the weight units (one cp.async.bulk per unit into a
-//                     ring of four mbarrier-guarded slots: 32 KB fp16x3 [W_hi | W_lo], 16 KB
+//                     ring of mbarrier-guarded slots: 32 KB fp16x3 [W_hi | W_lo], 16 KB
 //                     bf16); the other warps idle (setmaxnreg 24 / 240).
+//   kMB = 2         : (warp pass of a warp MLP no wider than 128) each consumer warpgroup
+//                     owns two 64-row blocks, rows 128 cw + {0..63, 64..127}, with one
+//                     accumulator set (acc0 / acc1) and 32 x_lo registers per block; every
+//                     unit issues block 0's chain, then block 1's, so a row sees the same
+//                     products in the same order as at kMB = 1, and each weight unit feeds
+//                     256 rows.  One row thread per row.  Below, the kMB = 1 kernel:
 //   warpgroups 1, 2 : rows 0-63 / 64-127.  Each issues its own wgmma (M = 64, N = 128 per
 //                     chunk, fp32 accumulators in registers: a 256-wide layer is 128 of them
 //                     per thread), A = its rows of the activation image in shared memory,
@@ -184,47 +196,59 @@ struct RowState {
 //                     x_lo operand of the activations is not in shared memory but in the
 //                     registers of the thread whose accumulators produced it (64 per thread,
 //                     epi_chunk -> lo -> the register-A form of wgmma), under the same rule.
-// Shared memory (225 KB), in 16 KB K-blocks:
-//   fp16x3: activation image hi, 4 blocks | input block (the encoded points / conditions)
-//           hi | lo, 2 blocks | weight ring 4 x 32 KB, 8 blocks;
-//   bf16  : activation image, 4 blocks | 4 unused blocks | input block, 2 blocks (its lo
-//           half unused) | weight ring 4 x 16 KB, 4 blocks;
-// then for both alpha partials | composite scratch | barriers.
+// Shared memory (225 KB), in 16 KB units; the activation image is 64 KB at both kMB (4 K-blocks
+// of 128 rows or 2 of 256), an input-block K-block is 128 kMB rows:
+//   fp16x3 kMB = 1: activation image hi 64 KB | input block (the encoded points / conditions)
+//                   hi | lo, 32 KB | weight ring 4 x 32 KB;
+//   fp16x3 kMB = 2: activation image hi 64 KB | input block hi | lo, 64 KB (the skip layer reads
+//                   it again, so it stays resident) | weight ring 3 x 32 KB;
+//   bf16   kMB = 1: activation image 64 KB | 64 KB unused | input block 32 KB (its lo half
+//                   unused) | weight ring 4 x 16 KB;
+//   bf16   kMB = 2: activation image 64 KB | 32 KB unused | input block 64 KB (lo unused) |
+//                   weight ring 4 x 16 KB;
+// then for all alpha partials | composite scratch | barriers.  The weight units are 128-column
+// N-chunks at both kMB, so a 256-row fp16x3 tile keeps 32 KB slots and drops to three of them.
 // Per-row work (positional encodings, SE(3) exp-map, sigmoid / sigma activation, fused
-// volumetric rendering) is done by "row threads": two per row (hs = which half of the
-// input block's columns), thread t of warpgroup w owns row 64 (w - 1) + (t & 63).
+// volumetric rendering) is done by "row threads".  kMB = 1: two per row (hs = which half of the
+// input block's columns), thread t of warpgroup w owns row 64 (w - 1) + (t & 63); kMB = 2: one
+// per row, thread t owns row 128 (w - 1) + t and writes both halves.
 // Head layers (N = 16) leave their accumulators in a per-warpgroup scratch inside
 // activation block 0 (free at that point: the step after a head reads the input block only).
 constexpr int kWgThreads = 384;
-constexpr int kWgSlots = 4;
-template <bool kX3>
-struct WgSmem {
-  static constexpr int kInOff = (kX3 ? 4 : 8) * kABlockBytes;
-  static constexpr int kRingOff = kInOff + 2 * kABlockBytes;
-  static constexpr int kSlotBytes = (kX3 ? 2 : 1) * kABlockBytes;
-};
 constexpr int kAlphaOff = 14 * kABlockBytes;          // per-row alpha-head partial (128 floats)
 constexpr int kScanOff = kAlphaOff + 512;             // fused composite: cross-warp partials (40 floats)
 constexpr int kBarOff = kScanOff + 256;
 constexpr int kWgSmemBytes = kBarOff + 256;
-static_assert(WgSmem<true>::kRingOff + kWgSlots * WgSmem<true>::kSlotBytes == kAlphaOff &&
-              WgSmem<false>::kRingOff + kWgSlots * WgSmem<false>::kSlotBytes == kAlphaOff,
-              "each precision's ring ends where the alpha partials begin");
+template <bool kX3, int kMB>
+struct WgSmem {
+  static constexpr int kRows = kMB * kTileRows;                 // rows of a tile
+  static constexpr uint32_t kBlkBytes = kRows * kRowBytes;      // one K-block of the tile
+  static constexpr int kSlots = (kX3 && kMB == 2) ? 3 : 4;
+  static constexpr int kSlotBytes = (kX3 ? 2 : 1) * kABlockBytes;
+  static constexpr int kRingOff = kAlphaOff - kSlots * kSlotBytes;   // the ring ends at the alpha partials
+  static constexpr int kInOff = kRingOff - 2 * (int)kBlkBytes;
+  static_assert(kInOff >= 4 * kABlockBytes, "input block overlaps the activation image");
+};
 static_assert(kWgSmemBytes <= 232448, "shared memory");
 
 // One weight unit of a layer into the accumulators d, A = K-block `src` (an activation
 // block or kSrcIn).  fp16x3 takes x_lo of an activation block from the registers `lo`, that
 // of the input block (written by the row threads) from its shared image at in_lo; the switch
-// keeps every register index a compile-time constant.
-template <bool kX3, int N>
+// keeps every register index a compile-time constant.  kActKb: K-blocks of the activation image
+// (4, or 2 in a 256-row tile, whose `lo` holds 32 registers per row block).
+template <bool kX3, int N, int kActKb>
 __device__ __forceinline__ void wg_layer_unit(float* d, int src, uint32_t a_hi, uint32_t in_lo, const uint32_t* lo,
                                               uint32_t b_hi, uint32_t b_lo, uint32_t accumulate) {
   if constexpr (kX3) {
     switch (src) {
       case 0: wg_unit<true, N>(d, a_hi, lo + x3_lo_reg(0, 0, 0), b_hi, b_lo, accumulate); break;
       case 1: wg_unit<true, N>(d, a_hi, lo + x3_lo_reg(1, 0, 0), b_hi, b_lo, accumulate); break;
-      case 2: wg_unit<true, N>(d, a_hi, lo + x3_lo_reg(2, 0, 0), b_hi, b_lo, accumulate); break;
-      case 3: wg_unit<true, N>(d, a_hi, lo + x3_lo_reg(3, 0, 0), b_hi, b_lo, accumulate); break;
+      case 2:
+        if constexpr (kActKb > 2) wg_unit<true, N>(d, a_hi, lo + x3_lo_reg(2, 0, 0), b_hi, b_lo, accumulate);
+        break;
+      case 3:
+        if constexpr (kActKb > 2) wg_unit<true, N>(d, a_hi, lo + x3_lo_reg(3, 0, 0), b_hi, b_lo, accumulate);
+        break;
       default: wg_unit<true, N>(d, a_hi, in_lo, b_hi, b_lo, accumulate); break;
     }
   } else {
@@ -238,12 +262,15 @@ struct WgBars {
   uint64_t never;          // never completes: the abort-path test hook waits on it
 };
 
-template <bool kX3>
+template <bool kX3, int kMB>
 __global__ void __launch_bounds__(kWgThreads, 1)
 field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, const uint8_t* __restrict__ wpack,
                 const float* __restrict__ aux, int num_tiles) {
-  using Smem = WgSmem<kX3>;
-  constexpr int kSlots = kWgSlots, kSlotBytes = Smem::kSlotBytes;
+  static_assert(kMB == 1 || kMB == 2, "one or two 64-row blocks per consumer warpgroup");
+  using Smem = WgSmem<kX3, kMB>;
+  constexpr int kSlots = Smem::kSlots, kSlotBytes = Smem::kSlotBytes, kRows = Smem::kRows;
+  constexpr uint32_t kBlk = Smem::kBlkBytes;
+  constexpr int kActKb = 4 / kMB;                 // K-blocks of the activation image
   // Registers per thread: 128 * producer + 256 * consumer <= 64 K.  fp16x3 consumers hold 64
   // x_lo registers on top of a 256-wide layer's 128 accumulators.
   constexpr int kProducerRegs = kX3 ? 24 : 40, kConsumerRegs = kX3 ? 240 : 232;
@@ -264,21 +291,13 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
     fence_barrier_init();
   }
   __syncthreads();
-  const bool do_warp = args.use_warp && prog.warp_type != 0 && !args.points;
-  int first_step = 0;
-  if (!do_warp) {
-    while (first_step < prog.n_steps && prog.steps[first_step].epi != kEpiWarpHeads) ++first_step;
-    first_step = (first_step < prog.n_steps) ? first_step + 1 : 0;   // skip the warp net
-  }
-  int last_step = prog.n_steps - 1;
-  if (args.warp_only) {
-    last_step = 0;
-    while (prog.steps[last_step].epi != kEpiWarpHeads) ++last_step;
-  }
+  // the warp pass runs steps [0, n_warp), the NeRF pass the rest (build_tc_program)
+  const bool warp_pass = args.warp_only != 0;
+  const int first_step = warp_pass ? 0 : prog.n_warp, end_step = warp_pass ? prog.n_warp : prog.n_steps;
   // Tiles of this CTA: blockIdx.x, + gridDim.x, ...  With the fused composite a CTA takes whole
   // rays - the S / 128 tiles of a ray back to back - so that transmittance and the partial sums
   // are carried in registers from tile to tile.
-  const bool fuse = args.ray_out != nullptr && !args.warp_only;
+  const bool fuse = kMB == 1 && args.ray_out != nullptr && !warp_pass;
   const int tpr = fuse ? args.samples_per_ray / kTileRows : 1;          // tiles per group
   const int groups = num_tiles / tpr;
   const int bid = (int)blockIdx.x;
@@ -291,10 +310,10 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
     if (warp == 0) {
       uint32_t sg = 0, ph = 0, dead = 0;
-      if (args.debug & 8) mbar_wait(&bars->never, 0, dead);   // test hook: provoke a wait time-out
+      if (args.debug & kDebugTimeout) mbar_wait(&bars->never, 0, dead);   // test hook: provoke a wait time-out
       uint8_t* ring = base + Smem::kRingOff;
       for (int ti = 0; ti < n_my; ++ti) {
-        for (int si = first_step; si <= last_step; ++si) {
+        for (int si = first_step; si < end_step; ++si) {
           const TcStep& st = prog.steps[si];
           const uint32_t bytes = (kX3 ? 2u : 1u) * (uint32_t)st.chunk_n * kRowBytes;
           const uint8_t* src = wpack + st.w_off;
@@ -312,23 +331,30 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
       }
     }
   } else {
-    // ===================== consumers: MMAs + epilogue of 64 rows =====================
+    // ===================== consumers: MMAs + epilogue of 64 kMB rows =====================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+    constexpr int kWgRows = 64 * kMB;                    // rows of a consumer warpgroup
     const int cw = wg - 1, t = tid & 127, wq = t >> 5, lq = lane & 3;
-    const int arow = 64 * cw + 16 * wq + (lane >> 2);    // accumulator rows arow, arow + 8
-    const int r = 64 * cw + (t & 63), hs = t >> 6;       // row thread: row r, input-block half hs
-    const int cb = hs * 4, ce = cb + 4;                  // input-block chunks this thread writes
-    const int lr = t & 63;                               // row within the warpgroup
+    // accumulator rows arow, arow + 8 of block 0; block b adds 64 b
+    const int arow = kWgRows * cw + 16 * wq + (lane >> 2);
+    // row thread: row r, input-block halves [h0, h1)
+    const int lr = kMB == 2 ? t : (t & 63);              // row within the warpgroup
+    const int r = kWgRows * cw + lr;
+    const int h0 = kMB == 2 ? 0 : t >> 6, h1 = kMB == 2 ? 2 : h0 + 1;
+    const int cb = h0 * 4, ce = cb + 4;                  // input-block chunks this thread writes (kMB = 1)
     uint8_t* act_hi = base;
     uint8_t* inh = base + Smem::kInOff;
-    uint8_t* inl = inh + kABlockBytes;
+    uint8_t* inl = inh + kBlk;
     float* alpha_s = reinterpret_cast<float*>(base + kAlphaOff);
     float* scan_s = reinterpret_cast<float*>(base + kScanOff);
-    float* scr = reinterpret_cast<float*>(base + cw * 8192);        // head accumulators, 64 x 16
-    const uint32_t rows_off = (uint32_t)cw * 8192u;                 // this warpgroup's rows in a K-block
+    const uint32_t rows_off = (uint32_t)(kWgRows * cw * kRowBytes); // this warpgroup's rows in a K-block
+    // head accumulators, kWgRows x 16 floats over this warpgroup's own rows of activation block 0
+    // (the other warpgroup's MMAs may still read its rows)
+    float* scr = reinterpret_cast<float*>(base + rows_off);
     const uint32_t ring_a = smem_u32(base + Smem::kRingOff);
     const uint32_t act_a = smem_u32(act_hi) + rows_off, in_a = smem_u32(inh) + rows_off;
     // fp16x3: x_lo of the activation image of this thread's accumulator rows, see epi_chunk
+    // (kMB = 2: lo[32 b ..] for block b)
     uint32_t lo[kX3 ? 64 : 1];
     const float alpha_b = __ldg(aux + prog.alpha_b_off);
     const int S = args.samples_per_ray;
@@ -340,7 +366,7 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
     // input block (warping.py:325-326 / models.py:270).  With FieldArgs::points the row's point
     // is the given (already warped) one and the NeRF net's inputs come first.
     auto begin_tile = [&](int tile) {
-      long long m = (long long)tile * kTileRows + r;
+      long long m = (long long)tile * kRows + r;
       row.valid = m < args.num_rows;
       if (!row.valid) m = args.num_rows - 1;
       row.m = m;
@@ -368,14 +394,16 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
         const float d = row.last ? (args.sample_at_infinity ? 1e10f : 1e-19f) : (zn - z);
         row.dist = d * dnorm;
       }
-      if (!do_warp && args.warped && row.valid && hs == 0) {
+      if (!warp_pass && args.warped && row.valid && h0 == 0) {
 #pragma unroll
         for (int c = 0; c < 3; ++c) args.warped[m * 3 + c] = row.x[c];
       }
       const float* cond = args.cond + row.ray * prog.cond_stride;
       // warp net: [posenc | GLO code]; NeRF net: [posenc | trunk condition]
-      encode_input<kX3>(inh, r, hs, row.x, do_warp ? prog.Fw : prog.Fp, do_warp ? args.window : nullptr,
-                        do_warp ? cond : cond + prog.G, do_warp ? prog.G : prog.tc);
+#pragma unroll
+      for (int hs = h0; hs < h1; ++hs)
+        encode_input<kX3, kBlk>(inh, r, hs, row.x, warp_pass ? prog.Fw : prog.Fp, warp_pass ? args.window : nullptr,
+                                warp_pass ? cond : cond + prog.G, warp_pass ? prog.G : prog.tc);
     };
 
     // fused composite: running state of the ray this CTA is on (replicated in every row thread)
@@ -386,27 +414,39 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
     for (int ti = 0; ti < n_my; ++ti) {
       const int tile = tile_of(ti);
       const bool has_next = ti + 1 < n_my;
-      for (int si = first_step; si <= last_step; ++si) {
+      for (int si = first_step; si < end_step; ++si) {
         const TcStep& st = prog.steps[si];
         const float* bias = aux + st.b_off;
         const float inv_s = kX3 ? 1.f / x3_weight_scale(__ldg(aux + prog.scale_off + si)) : 1.f;
         const bool hidden = st.epi == kEpiHidden;
+        // kMB = 1: acc0 / acc1 = N-chunk 0 / 1; kMB = 2: acc0 / acc1 = row block 0 / 1 (one N-chunk).
+        // A head (N = 16) accumulates into acc0[0..7] (and acc1[0..7] for row block 1).
         float acc0[64], acc1[64];
-        float* const acc16 = acc0;     // a head (N = 16) accumulates into acc0[0..7]
         // ---- the layer's MMAs: one weight unit per (chunk, K-block), one unit in flight ----
         uint32_t prev_sg = 0;
         const int n_units = st.n_chunks * st.nkb;
         for (int u = 0; u < n_units; ++u) {
           const int c = u >= st.nkb ? 1 : 0, kb = u - c * st.nkb;
           const int src = st.src[kb];
-          const uint32_t a_hi = src == kSrcIn ? in_a : act_a + (uint32_t)src * kABlockBytes;
+          const uint32_t a_hi = src == kSrcIn ? in_a : act_a + (uint32_t)src * kBlk;
           const uint32_t b_hi = ring_a + sg * kSlotBytes, b_lo = b_hi + (uint32_t)st.chunk_n * kRowBytes;
           mbar_wait(&bars->full[sg], ph, dead);
           wg_fence();
-          const uint32_t in_lo = in_a + kABlockBytes;
-          if (!hidden) wg_layer_unit<kX3, 16>(acc16, src, a_hi, in_lo, lo, b_hi, b_lo, kb);
-          else if (c == 0) wg_layer_unit<kX3, 128>(acc0, src, a_hi, in_lo, lo, b_hi, b_lo, kb);
-          else wg_layer_unit<kX3, 128>(acc1, src, a_hi, in_lo, lo, b_hi, b_lo, kb);
+          const uint32_t in_lo = in_a + kBlk;
+          if constexpr (kMB == 1) {
+            if (!hidden) wg_layer_unit<kX3, 16, kActKb>(acc0, src, a_hi, in_lo, lo, b_hi, b_lo, kb);
+            else if (c == 0) wg_layer_unit<kX3, 128, kActKb>(acc0, src, a_hi, in_lo, lo, b_hi, b_lo, kb);
+            else wg_layer_unit<kX3, 128, kActKb>(acc1, src, a_hi, in_lo, lo, b_hi, b_lo, kb);
+          } else {
+            // row block 1's rows are 64 rows (8 KB) after block 0's in every K-block
+            if (!hidden) {
+              wg_layer_unit<kX3, 16, kActKb>(acc0, src, a_hi, in_lo, lo, b_hi, b_lo, kb);
+              wg_layer_unit<kX3, 16, kActKb>(acc1, src, a_hi + 8192u, in_lo + 8192u, lo + 32, b_hi, b_lo, kb);
+            } else {
+              wg_layer_unit<kX3, 128, kActKb>(acc0, src, a_hi, in_lo, lo, b_hi, b_lo, kb);
+              wg_layer_unit<kX3, 128, kActKb>(acc1, src, a_hi + 8192u, in_lo + 8192u, lo + 32, b_hi, b_lo, kb);
+            }
+          }
           wg_commit();
           if (u > 0) {
             wg_wait<1>();
@@ -424,28 +464,40 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
           // ---- hidden layer: the output overwrites the input in place ----
           const bool relu = st.relu != 0, adot = st.alpha_dot != 0;
           const float* aw = aux + prog.alpha_w_off;
-          float al0 = 0.f, al1 = 0.f;
-          epi_chunk<kX3>(acc0, 0, bias, inv_s, relu, adot, aw, al0, al1, act_hi, lo, arow, lq);
-          if (st.n_chunks == 2) epi_chunk<kX3>(acc1, 1, bias, inv_s, relu, adot, aw, al0, al1, act_hi, lo, arow, lq);
-          if (adot) {
-            // the four threads of a quad hold the row's columns
-            al0 += __shfl_xor_sync(0xffffffffu, al0, 1); al0 += __shfl_xor_sync(0xffffffffu, al0, 2);
-            al1 += __shfl_xor_sync(0xffffffffu, al1, 1); al1 += __shfl_xor_sync(0xffffffffu, al1, 2);
-            if (lq == 0) { alpha_s[arow] = al0; alpha_s[arow + 8] = al1; }
-          }
-          if (st.write_cond) {   // the rgb condition: the input block of the next step
-            const float* cond = args.cond + row.ray * prog.cond_stride + prog.rc_off;
-            if constexpr (kX3) tc3::cond_to_block_x3(inh, inl, r, cond, prog.rc, cb, ce);
-            else cond_to_block(inh, r, cond, prog.rc, cb, ce);
+          if constexpr (kMB == 1) {
+            float al0 = 0.f, al1 = 0.f;
+            epi_chunk<kX3, kBlk>(acc0, 0, bias, inv_s, relu, adot, aw, al0, al1, act_hi, lo, arow, lq);
+            if (st.n_chunks == 2)
+              epi_chunk<kX3, kBlk>(acc1, 1, bias, inv_s, relu, adot, aw, al0, al1, act_hi, lo, arow, lq);
+            if (adot) {
+              // the four threads of a quad hold the row's columns
+              al0 += __shfl_xor_sync(0xffffffffu, al0, 1); al0 += __shfl_xor_sync(0xffffffffu, al0, 2);
+              al1 += __shfl_xor_sync(0xffffffffu, al1, 1); al1 += __shfl_xor_sync(0xffffffffu, al1, 2);
+              if (lq == 0) { alpha_s[arow] = al0; alpha_s[arow + 8] = al1; }
+            }
+            if (st.write_cond) {   // the rgb condition: the input block of the next step
+              const float* cond = args.cond + row.ray * prog.cond_stride + prog.rc_off;
+              if constexpr (kX3) tc3::cond_to_block_x3(inh, inl, r, cond, prog.rc, cb, ce);
+              else cond_to_block(inh, r, cond, prog.rc, cb, ce);
+            }
+          } else {
+            // warp net: one 128-column chunk per row block, no alpha head, no rgb condition
+            float al0 = 0.f, al1 = 0.f;
+            epi_chunk<kX3, kBlk>(acc0, 0, bias, inv_s, relu, false, aw, al0, al1, act_hi, lo, arow, lq);
+            epi_chunk<kX3, kBlk>(acc1, 0, bias, inv_s, relu, false, aw, al0, al1, act_hi, lo + 32, arow + 64, lq);
           }
         } else {
           // ---- heads: N = 16 accumulator columns through the scratch to the row threads ----
           const int l0 = 16 * wq + (lane >> 2);
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            float* sr = scr + (l0 + 8 * h) * 16 + 2 * lq;
-            sr[0] = acc16[2 * h]; sr[1] = acc16[2 * h + 1];
-            sr[8] = acc16[4 + 2 * h]; sr[9] = acc16[5 + 2 * h];
+          for (int b = 0; b < kMB; ++b) {
+            const float* a16 = b == 0 ? acc0 : acc1;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float* sr = scr + (l0 + 64 * b + 8 * h) * 16 + 2 * lq;
+              sr[0] = a16[2 * h]; sr[1] = a16[2 * h + 1];
+              sr[8] = a16[4 + 2 * h]; sr[9] = a16[5 + 2 * h];
+            }
           }
           wg_sync();
           float v[12];
@@ -455,21 +507,12 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
           if (st.epi == kEpiWarpHeads) {
             float y[3];
             warp_tail(prog.warp_type, v, row.x, prog.warp_pivot, prog.warp_trans, y);
-#pragma unroll
-            for (int c = 0; c < 3; ++c) row.x[c] = y[c];
-            if (args.warped && row.valid && hs == 0) {
+            if (row.valid && h0 == 0) {
 #pragma unroll
               for (int c = 0; c < 3; ++c) args.warped[row.m * 3 + c] = y[c];
             }
-            if (args.warp_only) {
-              if (has_next) begin_tile(tile_of(ti + 1));
-            } else if (prog.tc) {   // NeRF net inputs: [posenc | trunk condition]
-              encode_input<kX3>(inh, r, hs, row.x, prog.Fp, nullptr,
-                                args.cond + row.ray * prog.cond_stride + prog.G, prog.tc);
-            } else {                // without one, the encoder's extra columns are compile-time empty
-              encode_input<kX3>(inh, r, hs, row.x, prog.Fp, nullptr, nullptr, 0);
-            }
-          } else {
+            if (has_next) begin_tile(tile_of(ti + 1));
+          } else if constexpr (kMB == 1) {
             float4 o;
             o.x = sigmoidf(v[0]); o.y = sigmoidf(v[1]); o.z = sigmoidf(v[2]);
             // alpha condition (Dense(1) on [bottleneck | alpha condition]): its per-ray part
@@ -477,8 +520,8 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
                                                                aux + prog.alpha_w_off + kAlphaCondOff, prog.ac)
                                          : 0.f;
             o.w = apply_act(alpha_b + (alpha_s[r] + a_cond), prog.sigma_act);
-            if (hs == 0 && row.valid && args.samples) reinterpret_cast<float4*>(args.samples)[row.m] = o;
-            if (fuse && hs == 0) {
+            if (h0 == 0 && row.valid && args.samples) reinterpret_cast<float4*>(args.samples)[row.m] = o;
+            if (fuse && h0 == 0) {
               // ---- volumetric_rendering (model_utils.py:104-136) + median depth (:231-239, 262-263)
               //      over the 128 samples of this tile; one sample per row thread of half 0 ----
               const int qd = r >> 5;
@@ -652,6 +695,12 @@ inline int build_tc_program(nfb_handle* h, int level, long long* wbytes, long lo
     if (add(st, head ? kEpiWarpHeads : kEpiHidden, width)) return -1;
     if (!head) width = st.n;
   }
+  tp.n_warp = tp.n_steps;
+  // A warp net no wider than 128 runs in 256-row tiles: its layers are one N-chunk, so two row
+  // blocks fit the accumulator and x_lo registers of one 256-wide layer.
+  tp.warp_mb = 2;
+  for (int i = 0; i < tp.n_warp; ++i)
+    if (tp.steps[i].n_chunks != 1) tp.warp_mb = 1;
   // nerf net: trunk..., [bottleneck], alpha head (folded), rgb branch
   width = 0;
   int last_hidden = -1;
@@ -709,8 +758,11 @@ inline int create_tc(nfb_handle* h) {
   if (cudaMalloc(&h->d_wpack, (size_t)wbytes) != cudaSuccess) return fail("cudaMalloc wpack failed");
   if (cudaMalloc(&h->d_aux, (size_t)auxf * sizeof(float)) != cudaSuccess) return fail("cudaMalloc aux failed");
   if (cudaMemset(h->d_aux, 0, (size_t)auxf * sizeof(float)) != cudaSuccess) return fail("cudaMemset failed");
-  if (cudaFuncSetAttribute(field_wg_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmemBytes) != cudaSuccess ||
-      cudaFuncSetAttribute(field_wg_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmemBytes) != cudaSuccess)
+  const auto smem_attr = cudaFuncAttributeMaxDynamicSharedMemorySize;
+  if (cudaFuncSetAttribute(field_wg_kernel<true, 1>, smem_attr, kWgSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(field_wg_kernel<true, 2>, smem_attr, kWgSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(field_wg_kernel<false, 1>, smem_attr, kWgSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(field_wg_kernel<false, 2>, smem_attr, kWgSmemBytes) != cudaSuccess)
     return fail("cannot reserve %d bytes of shared memory for the tensor-core kernel", kWgSmemBytes);
   return 0;
 }
@@ -782,18 +834,26 @@ inline int pack_tc(nfb_handle* h, cudaStream_t s) {
   return 0;
 }
 
+// One pass of field_wg_kernel: the warp net (a.warp_only, into a.warped) or the NeRF net.  The NeRF
+// pass of a warped model reads the warp pass's points (a.points); nothing warps inside it.
 inline int run_field_tc(nfb_handle* h, int level, const FieldArgs& a, cudaStream_t s) {
-  const long long tiles = (a.num_rows + kTileRows - 1) / kTileRows;
+  const TcProgram& prog = h->tcprog[level];
+  if (a.warp_only && (prog.n_warp == 0 || !a.warped)) return fail("warp pass without a warp net or an output");
+  if (!a.warp_only && a.use_warp && prog.n_warp > 0 && !a.points)
+    return fail("the NeRF pass of a warped model needs the warp pass's points");
+  const int mb = (a.warp_only && prog.warp_mb == 2 && !(a.debug & kDebugOneRowBlock)) ? 2 : 1;
+  const long long rows_per_tile = (long long)mb * kTileRows;
+  const long long tiles = (a.num_rows + rows_per_tile - 1) / rows_per_tile;
   if (tiles > 0x7fffffffLL) return fail("too many rows for one launch");
   const bool fuse = a.ray_out != nullptr && !a.warp_only;
   if (fuse && (a.samples_per_ray % kTileRows != 0 || a.num_rows % a.samples_per_ray != 0))
     return fail("fused composite needs samples_per_ray to be a multiple of %d", kTileRows);
   const long long groups = fuse ? a.num_rows / a.samples_per_ray : tiles;
   const int grid = (int)std::min<long long>(groups, h->sm_count);
-  if (h->cfg.precision == NFB_PREC_FP16X3)
-    field_wg_kernel<true><<<grid, kWgThreads, kWgSmemBytes, s>>>(h->tcprog[level], a, h->d_wpack, h->d_aux, (int)tiles);
-  else
-    field_wg_kernel<false><<<grid, kWgThreads, kWgSmemBytes, s>>>(h->tcprog[level], a, h->d_wpack, h->d_aux, (int)tiles);
+  const bool x3 = h->cfg.precision == NFB_PREC_FP16X3;
+  auto kernel = x3 ? (mb == 2 ? field_wg_kernel<true, 2> : field_wg_kernel<true, 1>)
+                   : (mb == 2 ? field_wg_kernel<false, 2> : field_wg_kernel<false, 1>);
+  kernel<<<grid, kWgThreads, kWgSmemBytes, s>>>(prog, a, h->d_wpack, h->d_aux, (int)tiles);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail("field_wg_kernel launch failed: %s", cudaGetErrorString(e));
   h->launches++;

@@ -343,8 +343,8 @@ bool can_fuse_composite(const nfb_handle* h, int S) {
 }
 
 // Profiled launches (nfb_set_profiling) record the level's event pair around the field kernel.
-// Warp-only passes and passes on given points are not timed here: on the fine level they are
-// parts of render_fine_reusing_warp, which times them together.
+// Warp passes and passes on given points are not timed here: with a warp field a level's field time
+// spans its warp pass, the NeRF pass and whatever runs between them (prof_begin / prof_end).
 int run_field(nfb_handle* h, int level, long long rows, int S, const float* origins,
               const float* directions, const float* z, float* samples, float* warped,
               bool use_warp, bool warp_only, cudaStream_t s, float* ray_out = nullptr,
@@ -373,6 +373,30 @@ int run_field(nfb_handle* h, int level, long long rows, int S, const float* orig
     h->ev_valid[level] = true;
   }
   return rc;
+}
+
+int prof_begin(nfb_handle* h, int level, cudaStream_t s) {
+  if (h->profiling) NFB_CUDA(cudaEventRecord(h->ev[level][0], s));
+  return 0;
+}
+int prof_end(nfb_handle* h, int level, cudaStream_t s) {
+  if (!h->profiling) return 0;
+  NFB_CUDA(cudaEventRecord(h->ev[level][1], s));
+  h->ev_valid[level] = true;
+  return 0;
+}
+
+// True when the samples are warped: then every level runs a warp pass (FieldArgs::warp_only) that
+// writes the warped points, and the NeRF pass reads them (FieldArgs::points).  In the tensor-core
+// kernel the warp MLP runs in 256-row tiles, the NeRF MLP in 128-row ones (field_tc.cuh).
+bool warps(const nfb_handle* h, bool use_warp) {
+  return use_warp && h->cfg.warp_field_type != NFB_WARP_NONE;
+}
+
+// The warp pass over the S samples of B rays at z (z = nullptr: free points, origins = the points).
+int run_warp(nfb_handle* h, int level, long long B, int S, const float* origins, const float* directions,
+             const float* z, float* warped, cudaStream_t s) {
+  return run_field(h, level, B * S, S, origins, directions, z, nullptr, warped, true, true, s);
 }
 
 int run_composite(nfb_handle* h, int B, int S, const float* samples, const float* z,
@@ -423,14 +447,21 @@ int render_level(nfb_handle* h, int level, int B, int S, const float* origins, c
   return run_composite(h, B, S, h->d_samples, z, directions, out, weights, s);
 }
 
-// True when nfb_render_forward's fine level reuses the coarse level's warped points.
-bool reuses_warp(const nfb_handle* h, bool use_warp) {
-  return use_warp && h->d_warped_c != nullptr;
+// The coarse level of nfb_render_forward for a warped model: the warp pass writes the warped points
+// into d_warped_c, where the NeRF pass and then the fine level (render_fine_reusing_warp) read them.
+// Profiling times both launches as the level's field time.
+int render_coarse_warped(nfb_handle* h, int B, const float* origins, const float* directions, float* out,
+                         float* weights, cudaStream_t s) {
+  const int nc = h->cfg.num_coarse_samples;
+  if (prof_begin(h, 0, s) || run_warp(h, 0, B, nc, origins, directions, h->d_zc, h->d_warped_c, s) ||
+      render_level(h, 0, B, nc, origins, directions, h->d_zc, true, out, weights, s, nullptr, h->d_warped_c))
+    return -1;
+  return prof_end(h, 0, s);
 }
 
 // The fine level of nfb_render_forward for a warped model.  Its Nc + Nf samples are the Nc coarse
-// samples, whose warped points the coarse pass kept in d_warped_c, and the Nf new ones: only those
-// are warped (a warp-only pass in draw order), the two sets are gathered in z_fine's order, and the
+// samples, whose warped points the coarse level kept in d_warped_c, and the Nf new ones: only those
+// are warped (a warp pass in draw order), the two sets are gathered in z_fine's order, and the
 // NeRF pass reads the gathered points.  A warped point depends on its z bits, its ray, the warp
 // weights and the kernel alone, so this computes what warping all Nc + Nf samples computes.
 // Profiling times the three launches as the level's field time.
@@ -438,10 +469,7 @@ int render_fine_reusing_warp(nfb_handle* h, int B, const float* origins, const f
                              const float* zf, float* out, float* weights, cudaStream_t s) {
   const nfb_config& c = h->cfg;
   const int nc = c.num_coarse_samples, nf = c.num_fine_samples, n = nc + nf;
-  const bool prof = h->profiling;
-  if (prof) NFB_CUDA(cudaEventRecord(h->ev[1][0], s));
-  if (run_field(h, 1, (long long)B * nf, nf, origins, directions, h->d_znew, nullptr, h->d_warped_new, true, true, s))
-    return -1;
+  if (prof_begin(h, 1, s) || run_warp(h, 1, B, nf, origins, directions, h->d_znew, h->d_warped_new, s)) return -1;
   nfb::GatherWarpedArgs g{};
   g.warped_c = h->d_warped_c; g.warped_new = h->d_warped_new; g.src = h->d_src; g.warped_fine = h->d_warped_fine;
   g.num_rays = B; g.nc = nc; g.nf = nf;
@@ -449,11 +477,7 @@ int render_fine_reusing_warp(nfb_handle* h, int B, const float* origins, const f
   nfb::gather_warped_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(g);
   if (launch_check(h, "gather_warped_kernel")) return -1;
   if (render_level(h, 1, B, n, origins, directions, zf, true, out, weights, s, nullptr, h->d_warped_fine)) return -1;
-  if (prof) {
-    NFB_CUDA(cudaEventRecord(h->ev[1][1], s));
-    h->ev_valid[1] = true;
-  }
-  return 0;
+  return prof_end(h, 1, s);
 }
 
 // The tensor-core kernels never trap on a protocol error (see tc_common.cuh,
@@ -701,7 +725,13 @@ int nfb_image_metrics(int num_images, int height, int width, int channels, const
 
 int nfb_debug_provoke_timeout(nfb_handle* h, int enabled) {
   if (!h) return fail("null handle");
-  h->debug_bits = enabled ? 8 : 0;
+  h->debug_bits = enabled ? (h->debug_bits | nfb::kDebugTimeout) : (h->debug_bits & ~nfb::kDebugTimeout);
+  return 0;
+}
+
+int nfb_debug_one_row_block(nfb_handle* h, int enabled) {
+  if (!h) return fail("null handle");
+  h->debug_bits = enabled ? (h->debug_bits | nfb::kDebugOneRowBlock) : (h->debug_bits & ~nfb::kDebugOneRowBlock);
   return 0;
 }
 
@@ -840,10 +870,11 @@ int nfb_create(const nfb_config* cfg, int max_rays, nfb_handle** out) {
       dmalloc(&h->d_out_f, B * 6) || dmalloc(&h->d_in, B * 9))
     return bail(-1);
   if (cudaMalloc(&h->d_ids, (size_t)B * 3 * sizeof(unsigned)) != cudaSuccess) return bail(fail("cudaMalloc ids failed"));
+  if (c.warp_field_type != NFB_WARP_NONE && dmalloc(&h->d_warped_c, B * nc * 3)) return bail(-1);   // warp pass
   if (c.warp_field_type != NFB_WARP_NONE && c.num_fine_samples > 0) {   // render_fine_reusing_warp
     const int nf = c.num_fine_samples;
-    if (dmalloc(&h->d_warped_c, B * nc * 3) || dmalloc(&h->d_warped_new, B * nf * 3) ||
-        dmalloc(&h->d_warped_fine, B * nfine * 3) || dmalloc(&h->d_znew, B * nf))
+    if (dmalloc(&h->d_warped_new, B * nf * 3) || dmalloc(&h->d_warped_fine, B * nfine * 3) ||
+        dmalloc(&h->d_znew, B * nf))
       return bail(-1);
     if (cudaMalloc(&h->d_src, (size_t)B * nfine * sizeof(uint16_t)) != cudaSuccess)
       return bail(fail("cudaMalloc of %lld sample indices failed", B * nfine));
@@ -960,8 +991,32 @@ int nfb_render_samples(nfb_handle* h, int level, int B, int S, const float* z_va
                (flags & NFB_FLAG_METADATA_ENCODED) != 0)) return -1;
   float* smp = samples ? samples : h->d_samples;
   const bool use_warp = !(flags & NFB_FLAG_NO_WARP);
-  if (run_field(h, level, (long long)B * S, S, origins, directions, z_vals, smp, warped_points,
-                use_warp, false, s)) return -1;
+  const long long rows = (long long)B * S;
+  if (!warps(h, use_warp)) {
+    if (run_field(h, level, rows, S, origins, directions, z_vals, smp, warped_points, use_warp, false, s)) return -1;
+  } else {
+    // The warp pass writes into the caller's warped_points or into the workspace (d_warped_fine
+    // holds max_rays x (Nc + Nf) points, d_warped_c max_rays x Nc); a caller-sized S beyond it gets a
+    // stream-ordered allocation for this call.
+    float* pts = warped_points;
+    float* tmp = nullptr;
+    if (!pts) {
+      const long long cap = (long long)h->max_rays * (h->d_warped_fine ? smax : h->cfg.num_coarse_samples);
+      if (rows <= cap) {
+        pts = h->d_warped_fine ? h->d_warped_fine : h->d_warped_c;
+      } else {
+        NFB_CUDA(cudaMallocAsync(&tmp, (size_t)rows * 3 * sizeof(float), s));
+        pts = tmp;
+      }
+    }
+    int rc = prof_begin(h, level, s);
+    if (rc == 0) rc = run_warp(h, level, B, S, origins, directions, z_vals, pts, s);
+    if (rc == 0) rc = run_field(h, level, rows, S, origins, directions, z_vals, smp, nullptr, true, false, s,
+                                nullptr, nullptr, pts);
+    if (rc == 0) rc = prof_end(h, level, s);
+    if (tmp) NFB_CUDA(cudaFreeAsync(tmp, s));
+    if (rc) return -1;
+  }
   if (out) return run_composite(h, B, S, smp, z_vals, directions, out, weights, s);
   return 0;
 }
@@ -983,17 +1038,19 @@ int nfb_render_forward(nfb_handle* h, int B, const float* origins, const float* 
   if (run_cond(h, B, viewdirs ? viewdirs : directions, warp_id, app_id, cam_id, s,
                (flags & NFB_FLAG_METADATA_ENCODED) != 0)) return -1;
   // With a warp field the fine level warps only its new samples (render_fine_reusing_warp).
-  const bool reuse = fine && reuses_warp(h, use_warp);
+  const bool warp = warps(h, use_warp);
   // coarse level (models.py:332-349)
   if (nfb_coarse_z_vals(h, B, t_rand, h->d_zc, stream)) return -1;
   float* wc = w_coarse ? w_coarse : h->d_wc;
-  if (render_level(h, 0, B, nc, origins, directions, h->d_zc, use_warp, out_coarse ? out_coarse : h->d_out_c,
-                   wc, s, reuse ? h->d_warped_c : nullptr)) return -1;
+  float* oc = out_coarse ? out_coarse : h->d_out_c;
+  if (warp ? render_coarse_warped(h, B, origins, directions, oc, wc, s)
+           : render_level(h, 0, B, nc, origins, directions, h->d_zc, use_warp, oc, wc, s))
+    return -1;
   if (!fine) return 0;
   // hierarchical resampling + fine level (models.py:352-370)
   float* zf = z_fine ? z_fine : h->d_zf;
   float* of = out_fine ? out_fine : h->d_out_f;
-  if (reuse) {
+  if (warp) {
     if (run_resample(h, B, h->d_zc, wc, u_rand, zf, s, h->d_znew, h->d_src)) return -1;
     return render_fine_reusing_warp(h, B, origins, directions, zf, of, w_fine, s);
   }
@@ -1060,7 +1117,7 @@ int nfb_warp_forward(nfb_handle* h, int P, const float* points, const unsigned* 
   // view-direction block is computed from `points` and ignored.
   if (run_cond(h, P, points, warp_id, nullptr, nullptr, s, (flags & NFB_FLAG_METADATA_ENCODED) != 0)) return -1;
   // Free points: rows = points, z = 0 (x = p + 0 * p = p exactly for finite p).
-  return run_field(h, 0, P, 1, points, points, nullptr, nullptr, warped, true, true, s);
+  return run_warp(h, 0, P, 1, points, points, nullptr, warped, s);
 }
 
 }  // extern "C"

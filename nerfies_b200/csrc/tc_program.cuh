@@ -29,6 +29,8 @@ struct TcStep {
 struct TcProgram {
   int n_steps;
   TcStep steps[kMaxTcSteps];
+  int n_warp;                     // steps [0, n_warp) are the warp net, the rest the NeRF net
+  int warp_mb;                    // 64-row blocks per consumer warpgroup in the warp pass (1 or 2)
   int warp_type, Fw, G, Fp, rc, cond_stride, sigma_act;
   int tc, ac;                     // trunk / alpha condition widths
   int ac_off, rc_off;             // offsets of the alpha / rgb condition in the per-ray condition vector
