@@ -347,6 +347,19 @@ int nfb_image_metrics(int num_images, int height, int width, int channels,
                       void* workspace, long long workspace_bytes,
                       float* ms_ssim, float* mse, float* depth_abs, void* stream);
 
+/* Float frames -> 8- or 16-bit images, value for value what numpy computes in
+ * image_utils.image_to_uint8 / image_to_uint16 (image_utils.py:114-131) and save_depth
+ * (image_utils.py:172-174):
+ *   dst[i] = (uintN) clip(src[i] / scale * max, 0, max),   max = 255 (bits 8) | 65535 (bits 16).
+ * The division and the product are each one IEEE float32 operation, the cast truncates toward
+ * zero (0.999 * 255 -> 254).  Negatives and -inf give 0, values above 1 and +inf give max, and
+ * NaN gives 0: numpy's clip passes NaN and the x86-64 float -> unsigned cast of it is 0.
+ * scale = 1 is image_to_uintN; scale = 1000, bits = 16 is save_depth.  scale must be positive and
+ * finite.  src (n) float32 and dst (n) uint8 / uint16 are device pointers of their natural
+ * alignment; 16-byte aligned pointers take 16-byte loads and stores.  One pass, no workspace, no
+ * handle, ordered on `stream`. */
+int nfb_image_quantize(const float* src, long long n, int bits, float scale, void* dst, void* stream);
+
 /* Test hook for the abort path described in the conventions above: while enabled,
  * the weight producer of the tensor-core kernel first waits on an mbarrier that never
  * completes, so the launch must time out, drain and raise the abort flag

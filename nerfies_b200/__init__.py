@@ -8,6 +8,8 @@ Public surface (mirrors the reference's, SURVEY.md §8b):
   nerfies_b200.training    train_step (value_and_grad + gradient all-reduce + Adam)
   nerfies_b200.datasets    NerfiesDataSource: a capture on the GPU, train.py / eval.py batches
   nerfies_b200.schedules   the annealing schedules of train.py
+  nerfies_b200.train       python -m nerfies_b200.train: the training driver (train.py:100-326)
+  nerfies_b200.eval        python -m nerfies_b200.eval: the evaluation driver (eval.py:225-419)
 The arithmetic lives in libnerfies_b200.so (include/nerfies_b200.h); there is no
 CPU or PyTorch fallback.
 """

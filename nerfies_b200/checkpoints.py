@@ -166,6 +166,8 @@ def restore_checkpoint(ckpt_dir, target=None, step=None, prefix='checkpoint_', d
       warp_alpha=float(np.asarray(state_dict.get('warp_alpha', 0.0)).reshape(-1)[0]),
       time_alpha=float(np.asarray(state_dict.get('time_alpha', 0.0)).reshape(-1)[0]))
   state.step = int(np.asarray(opt.get('state', {}).get('step', 0)).reshape(-1)[0])
+  # Adam's moments, {'model': {...: {'grad_ema', 'grad_sq_ema'}}}: what a resumed run needs
+  state.param_states = _to_torch(opt.get('state', {}).get('param_states') or {}, device)
   return state
 
 
@@ -184,11 +186,14 @@ def _check_same_structure(want, got, where):
 
 
 def save_checkpoint(ckpt_dir, state, step, prefix='checkpoint_', keep=2):
-  """Writes `state` in the reference's layout (training.py:46-53); keeps the newest `keep` files."""
+  """Writes `state` in the reference's layout (training.py:46-53); keeps the newest `keep` files.
+  An optimizer that has `param_states` (training.AdamOptimizer) gets its moments written where flax
+  writes them, so that a run can resume; the plain `model_utils.Optimizer` has none."""
   os.makedirs(ckpt_dir, exist_ok=True)
   tree = {
       'optimizer': {'target': state.optimizer.target,
-                    'state': {'step': np.asarray(step, np.int32), 'param_states': {}}},
+                    'state': {'step': np.asarray(step, np.int32),
+                              'param_states': getattr(state.optimizer, 'param_states', {})}},
       'warp_alpha': np.asarray(state.warp_alpha, np.float32),
       'time_alpha': np.asarray(state.time_alpha, np.float32),
   }

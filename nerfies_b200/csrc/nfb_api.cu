@@ -17,6 +17,7 @@
 #include "ray_kernels.cuh"
 #include "camera_kernels.cuh"
 #include "metrics_kernels.cuh"
+#include "image_kernels.cuh"
 #include "tc_common.cuh"
 #include "tc_selftest.cuh"
 #include "field_tc.cuh"
@@ -720,6 +721,33 @@ int nfb_image_metrics(int num_images, int height, int width, int channels, const
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail("image metrics launch failed: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+int nfb_image_quantize(const float* src, long long n, int bits, float scale, void* dst, void* stream) {
+  if (bits != 8 && bits != 16) return fail("nfb_image_quantize: bits must be 8 or 16, got %d", bits);
+  if (n < 0) return fail("nfb_image_quantize: negative count %lld", n);
+  if (!(scale > 0.0f) || std::isinf(scale)) return fail("nfb_image_quantize: scale must be positive and finite");
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
+    return fail("no CUDA device: nerfies_b200 has no CPU path");
+  if (n == 0) return 0;
+  if (!src || !dst) return fail("null argument");
+  if (reinterpret_cast<uintptr_t>(src) & 3) return fail("src must be 4-byte aligned");
+  if (bits == 16 && (reinterpret_cast<uintptr_t>(dst) & 1)) return fail("a 16-bit dst must be 2-byte aligned");
+  const bool aligned = ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0;
+  const long long vec = aligned ? n / (128 / bits) : 0;
+  const long long threads = std::max(vec, n - vec * (128 / bits));
+  const unsigned blocks = (unsigned)std::min<long long>((threads + nfb::image::kThreads - 1) / nfb::image::kThreads, 1 << 16);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (bits == 8)
+    nfb::image::image_quantize_kernel<unsigned char><<<blocks, nfb::image::kThreads, 0, s>>>(
+        src, n, vec, scale, static_cast<unsigned char*>(dst));
+  else
+    nfb::image::image_quantize_kernel<unsigned short><<<blocks, nfb::image::kThreads, 0, s>>>(
+        src, n, vec, scale, static_cast<unsigned short*>(dst));
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("image_quantize_kernel launch failed: %s", cudaGetErrorString(e));
   return 0;
 }
 

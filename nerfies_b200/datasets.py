@@ -80,10 +80,10 @@ def _rank_slice(batch_size, rank, world_size):
   return rank * per, per
 
 
-def _batch_starts(total, batch_size, repeat):
-  """(start, size) of each batch of a dataset of `total` elements: repeat() then batch(), or
-  batch() alone, which ends with a partial batch."""
-  for step in itertools.count():
+def _batch_starts(total, batch_size, repeat, first_batch=0):
+  """(start, size) of each batch of a dataset of `total` elements from batch `first_batch` on:
+  repeat() then batch(), or batch() alone, which ends with a partial batch."""
+  for step in itertools.count(first_batch):
     start = step * batch_size
     if not repeat and start >= total:
       return
@@ -361,12 +361,14 @@ class NerfiesDataSource:
 
   def create_iterator(self, item_ids, batch_size, repeat=True, flatten=False, shuffle=False,
                       prefetch_size=0, shuffle_buffer_size=1000000, devices=None, rank=None,
-                      world_size=None):
+                      world_size=None, first_batch=0):
     """The batches of core.py:352-372 with preload (see the module docstring).  With
     `batch_size=0`, whole items as (h, w, ·) tensors; otherwise dicts of rank `rank`'s
     batch_size / world_size rays ('metadata' values (b, 1)).  `prefetch_size`,
     `shuffle_buffer_size` and `devices` are accepted for the reference's signature: batches are
-    made on this source's device, in order on the current stream, when next() is called."""
+    made on this source's device, in order on the current stream, when next() is called.
+    `first_batch` (flattened rays only) starts the stream at that batch, at no cost: a resumed
+    run continues where the interrupted one stopped instead of replaying the order's head."""
     del prefetch_size, shuffle_buffer_size, devices
     if not self.preload:
       raise NotImplementedError('preload=False is the lazy tf.data path with shuffle buffers; it has no '
@@ -380,10 +382,12 @@ class NerfiesDataSource:
     host = self.ray_table(item_ids)
     order = self.rng.permutation(host.num_rays)      # core.py:425: drawn on every call
     table = _upload(host, self.device, order if shuffle else None)
+    if first_batch and not (flatten and batch_size > 0):
+      raise NotImplementedError('first_batch is for batches of flattened rays')
     if batch_size <= 0:
       return _item_iterator(table, repeat)
     if flatten:
-      return _ray_iterator(table, batch_size, repeat, rank, world_size)
+      return _ray_iterator(table, batch_size, repeat, rank, world_size, first_batch)
     return _item_batch_iterator(table, batch_size, repeat, rank, world_size)
 
   def create_cameras_dataset(self, cameras, flatten=False, shuffle=False):
@@ -419,8 +423,8 @@ def _item_iterator(table, repeat):
       return
 
 
-def _ray_iterator(table, batch_size, repeat, rank, world_size):
-  for start, size in _batch_starts(table.num_rays, batch_size, repeat):
+def _ray_iterator(table, batch_size, repeat, rank, world_size, first_batch=0):
+  for start, size in _batch_starts(table.num_rays, batch_size, repeat, first_batch):
     offset, count = _rank_slice(size, rank, world_size)
     yield table.gather(start + offset, count)
 
@@ -437,19 +441,22 @@ def _item_batch_iterator(table, batch_size, repeat, rank, world_size):
 
 
 def iterator_from_dataset(dataset, batch_size, repeat=True, prefetch_size=0, devices=None, rank=None,
-                          world_size=None):
+                          world_size=None, first_batch=0):
   """Batches of a device tensor along its first axis (train.py:187-197's background points), with
   core.py:131-160's repeat-then-batch semantics and rank `rank`'s contiguous slice of each batch;
   a batch is at most two device-to-device copies.  With `batch_size=0`, the elements of
-  `dataset` one by one (eval.py's test cameras: `create_cameras_dataset`)."""
+  `dataset` one by one (eval.py's test cameras: `create_cameras_dataset`).  `first_batch` starts
+  the batches of a tensor at that batch (see `create_iterator`)."""
   del prefetch_size, devices
+  if first_batch and batch_size <= 0:
+    raise NotImplementedError('first_batch is for batches of a tensor')
   if batch_size <= 0:
     return _elements(dataset, repeat)
   if not torch.is_tensor(dataset) or not dataset.is_cuda:
     raise ValueError('iterator_from_dataset batches a CUDA tensor (e.g. load_points())')
   rank, world_size = _dist_rank_world(rank, world_size)
   _rank_slice(batch_size, rank, world_size)
-  return _tensor_batches(dataset, batch_size, repeat, rank, world_size)
+  return _tensor_batches(dataset, batch_size, repeat, rank, world_size, first_batch)
 
 
 def _elements(dataset, repeat):
@@ -459,9 +466,9 @@ def _elements(dataset, repeat):
       return
 
 
-def _tensor_batches(points, batch_size, repeat, rank, world_size):
+def _tensor_batches(points, batch_size, repeat, rank, world_size, first_batch=0):
   n = points.shape[0]
-  for start, size in _batch_starts(n, batch_size, repeat):
+  for start, size in _batch_starts(n, batch_size, repeat, first_batch):
     offset, count = _rank_slice(size, rank, world_size)
     out = torch.empty((count,) + tuple(points.shape[1:]), dtype=points.dtype, device=points.device)
     done, src = 0, (start + offset) % n

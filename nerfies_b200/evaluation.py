@@ -17,6 +17,9 @@ h*w/chunk host round trips with a collective each.
 `compute_metrics`, `compute_multiscale_ssim` and `compute_psnr` are the per-frame
 metrics of eval.py:process_batch (eval.py:58-62, 120-122, 140; utils.py:94-103),
 computed on the device by the library's metrics kernels (`nfb_image_metrics`).
+
+`image_to_uint8`, `image_to_uint16` and `depth_to_uint16` are image_utils.py:114-131, 172-174 on
+the device (`nfb_image_quantize`): a frame leaves the GPU as the 8- / 16-bit image that is saved.
 """
 import ctypes
 import math
@@ -162,7 +165,7 @@ def render_frame(model, params, camera, warp_extra, metadata=None, max_rays=6553
   every rank (padding rays past the end repeat the last pixel, like the
   reference's edge padding, and are dropped).
 
-  metadata: {'warp': id, 'appearance': id, 'camera': id} scalars applied to every
+  metadata: {'warp': id, 'appearance': id, 'camera': id, 'time': t} scalars applied to every
   ray (eval.py:344-348 renders one camera with one metadata id per frame).
   timings (optional dict) receives {'render_ms', 'gather_ms'} measured with CUDA
   events on the current stream.  Returns {rgb (h,w,3), depth, med_depth, acc}."""
@@ -185,7 +188,9 @@ def render_frame(model, params, camera, warp_extra, metadata=None, max_rays=6553
     n = min(max_rays, count - done)
     rays = camera_lib.camera_to_rays(camera, dev, first_pixel=first + done, count=n)
     rays_dict = {'origins': rays['origins'], 'directions': rays['directions'],
-                 'metadata': {k: torch.full((n, 1), int(v), dtype=torch.int32, device=dev)
+                 # ids are int32; 'time' (the TimeEncoder's input, models.py:252-254) is float32
+                 'metadata': {k: (torch.full((n, 1), float(v), dtype=torch.float32, device=dev) if k == 'time'
+                                  else torch.full((n, 1), int(v), dtype=torch.int32, device=dev))
                               for k, v in md.items()}}
     out = model.apply({'params': params}, rays_dict, warp_extra=warp_extra, _packed=True)
     if levels_key is None:
@@ -253,6 +258,37 @@ def _image_metrics(image, target, depth=None, depth_target=None):
         ptr(out[0]), ptr(out[1]), ptr(out[2]) if depth is not None else None,
         ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
   return out[0], out[1], (out[2] if depth is not None else None)
+
+
+def _image_quantize(image, bits, scale):
+  """One nfb_image_quantize call; the result has the image's shape."""
+  if not torch.is_tensor(image) or not image.is_cuda:
+    raise ValueError('the image must be a torch tensor on a CUDA device: nerfies_b200 has no CPU path')
+  if image.dtype != torch.float32:
+    raise ValueError(f'Input image should be float32 but is of type {image.dtype}')
+  image = image.contiguous()
+  out = torch.empty(image.shape, dtype=torch.uint8 if bits == 8 else torch.uint16, device=image.device)
+  with torch.cuda.device(image.device):
+    _lib.check(_lib.load().nfb_image_quantize(
+        ctypes.c_void_p(image.data_ptr()), image.numel(), bits, float(scale), ctypes.c_void_p(out.data_ptr()),
+        ctypes.c_void_p(torch.cuda.current_stream(image.device).cuda_stream)))
+  return out
+
+
+def image_to_uint8(image):
+  """image_utils.image_to_uint8 (image_utils.py:114-121) on the device:
+  (image * 255).clip(0, 255).astype(uint8), value for value.  CUDA float32 in, torch.uint8 out."""
+  return _image_quantize(image, 8, 1.0)
+
+
+def image_to_uint16(image):
+  """image_utils.image_to_uint16 (image_utils.py:124-131) on the device; torch.uint16 out."""
+  return _image_quantize(image, 16, 1.0)
+
+
+def depth_to_uint16(depth):
+  """What image_utils.save_depth writes (image_utils.py:172-174): image_to_uint16(depth / 1000.0)."""
+  return _image_quantize(depth, 16, 1000.0)
 
 
 def compute_multiscale_ssim(image1, image2):

@@ -234,18 +234,20 @@ class NerfModel:
       raise ValueError(f'train_precision must be one of {list(_lib.TRAIN_PRECISIONS)}, got {name!r}')
     self._train_precision = name
 
-  # Same derived attributes as the reference (models.py:121-131).
+  # Same derived attributes as the reference (models.py:121-131).  The reference reads them only for
+  # the embeddings the model has; a data source gives () for metadata that is off
+  # (datasets/core.py:276-303), which counts as one unused row here.
   @property
   def num_appearance_embeddings(self):
-    return max(self.appearance_ids) + 1
+    return max(self.appearance_ids, default=0) + 1
 
   @property
   def num_warp_embeddings(self):
-    return max(self.warp_ids) + 1
+    return max(self.warp_ids, default=0) + 1
 
   @property
   def num_camera_embeddings(self):
-    return max(self.camera_ids) + 1
+    return max(self.camera_ids, default=0) + 1
 
   @property
   def warp_trunk_depth(self):

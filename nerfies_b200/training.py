@@ -57,6 +57,41 @@ class AdamOptimizer(model_utils.Optimizer):
     self.step = 0
     self.beta1, self.beta2, self.eps = beta1, beta2, eps
 
+  def _moment_views(self):
+    """(target leaf, m view, v view) per parameter, in `specs` order."""
+    for name, off, numel in self.specs:
+      leaf = self.target['model']
+      for part in name.split('/'):
+        leaf = leaf[part]
+      yield name, leaf, self.m[off:off + numel].view(leaf.shape), self.v[off:off + numel].view(leaf.shape)
+
+  @property
+  def param_states(self):
+    """The moments in the layout flax.optim.Adam serialises (`_AdamParamState` per leaf of the
+    target): {'model': {...: {'grad_ema': m, 'grad_sq_ema': v}}}, views of the flat buffers."""
+    tree = {}
+    for name, _, m, v in self._moment_views():
+      node = tree
+      for part in name.split('/'):
+        node = node.setdefault(part, {})
+      node['grad_ema'], node['grad_sq_ema'] = m, v
+    return {'model': tree}
+
+  def load(self, restored):
+    """Copies a restored TrainState's parameters, moments and step count into the flat buffers
+    (train.py:232-233: the optimizer of the restored state replaces the fresh one)."""
+    states = getattr(restored, 'param_states', None) or {}
+    for name, leaf, m, v in self._moment_views():
+      src, st = restored.optimizer.target['model'], states.get('model', {})
+      for part in name.split('/'):
+        src, st = src[part], st.get(part, {})
+      if 'grad_ema' not in st or 'grad_sq_ema' not in st:
+        raise ValueError(f'the checkpoint has no Adam moments for {name}: training cannot resume from it')
+      leaf.copy_(torch.as_tensor(src).reshape(leaf.shape))
+      m.copy_(torch.as_tensor(st['grad_ema']).reshape(leaf.shape))
+      v.copy_(torch.as_tensor(st['grad_sq_ema']).reshape(leaf.shape))
+    self.step = int(restored.step)
+
   def apply_gradient(self, grad_flat, learning_rate):
     """optimizer.apply_gradient(grad, learning_rate=...) (training.py:268-269); in place."""
     self.step += 1
