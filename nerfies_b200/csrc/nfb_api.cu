@@ -61,6 +61,16 @@ struct Builder {
   }
 };
 
+// Appends one step to `net`, whose step list is a fixed array: a network of more than kMaxSteps
+// Dense layers (trunk, heads and branches together) is refused, never written past its end.
+int push_step(Net& net, const Step& st, const std::string& name) {
+  if (net.n_steps >= nfb::kMaxSteps)
+    return fail("%s: too many layers (a network holds at most kMaxSteps = %d Dense layers)", name.c_str(),
+                nfb::kMaxSteps);
+  net.steps[net.n_steps++] = st;
+  return 0;
+}
+
 int build_mlp(Builder& b, Net& net, const std::string& prefix, int depth, int width,
               unsigned skips, int in_dim, int in_off, int act, int first_src, int first_kx,
               int* cur_buf /* in: buffer holding X (if first_kx>0); out: buffer with result */) {
@@ -78,9 +88,9 @@ int build_mlp(Builder& b, Net& net, const std::string& prefix, int depth, int wi
     }
     const int src = (i == 0) ? first_src : cur;
     int dst = (src == nfb::kB0) ? nfb::kB1 : nfb::kB0;
-    if (net.n_steps >= nfb::kMaxSteps) return fail("too many layers");
-    net.steps[net.n_steps++] = b.dense({prefix + "/hidden_" + std::to_string(i)}, k_x, k_in,
-                                       in_off, {width}, act, src, dst);
+    if (push_step(net, b.dense({prefix + "/hidden_" + std::to_string(i)}, k_x, k_in, in_off, {width}, act, src, dst),
+                  prefix))
+      return -1;
     cur = dst;
   }
   *cur_buf = cur;
@@ -128,7 +138,7 @@ int build_programs(nfb_handle* h) {
       int tcur = nfb::kB0;
       Net tn{};
       if (build_mlp(b, tn, root, 6, 64, 1u << 4, 1 + 2 * F, 0, nfb::kRelu, nfb::kB0, 0, &tcur)) return -1;
-      tn.steps[tn.n_steps++] = b.dense({root + "/logit"}, 64, 0, 0, {G}, nfb::kNone, tcur, nfb::kOut0);
+      if (push_step(tn, b.dense({root + "/logit"}, 64, 0, 0, {G}, nfb::kNone, tcur, nfb::kOut0), root)) return -1;
       h->time_net = tn;
     }
     if (c.warp_field_type != NFB_WARP_SE3 && (c.warp_use_pivot || c.warp_use_translation))
@@ -145,10 +155,12 @@ int build_programs(nfb_handle* h) {
       std::vector<int> ns = {3, 3};
       if (c.warp_use_pivot) { names.push_back("warp_field/branches_p/logit"); ns.push_back(3); }
       if (c.warp_use_translation) { names.push_back("warp_field/branches_t/logit"); ns.push_back(3); }
-      warp.steps[warp.n_steps++] = b.dense(names, c.warp_trunk_width, 0, 0, ns, nfb::kNone, cur, nfb::kOut0);
+      if (push_step(warp, b.dense(names, c.warp_trunk_width, 0, 0, ns, nfb::kNone, cur, nfb::kOut0), mlp_name))
+        return -1;
     } else {
-      warp.steps[warp.n_steps++] = b.dense({"warp_field/mlp/logit"}, c.warp_trunk_width, 0, 0,
-                                           {3}, nfb::kNone, cur, nfb::kOut0);
+      if (push_step(warp, b.dense({"warp_field/mlp/logit"}, c.warp_trunk_width, 0, 0, {3}, nfb::kNone, cur,
+                                  nfb::kOut0), mlp_name))
+        return -1;
     }
   }
   if (c.use_appearance_metadata)
@@ -172,14 +184,14 @@ int build_programs(nfb_handle* h) {
     // execution order is bottleneck, alpha, rgb (alpha must read the trunk output
     // before the rgb branch reuses that buffer).  Specs are re-sorted below.
     const size_t spec_mark = h->specs.size();
-    if (has_cond)
-      nerf.steps[nerf.n_steps++] = b.dense({root + "/bottleneck"}, W, 0, 0, {W}, nfb::kNone, P, Q);
+    if (has_cond && push_step(nerf, b.dense({root + "/bottleneck"}, W, 0, 0, {W}, nfb::kNone, P, Q), root))
+      return -1;
     // alpha branch (depth 0: logit only), modules.py:152-157.
     const size_t alpha_mark = h->specs.size();
-    if (ac > 0)
-      nerf.steps[nerf.n_steps++] = b.dense({root + "/MLP_2/logit"}, W, ac, Dp + tc, {1}, nfb::kNone, Q, nfb::kOut0);
-    else
-      nerf.steps[nerf.n_steps++] = b.dense({root + "/MLP_2/logit"}, W, 0, 0, {1}, nfb::kNone, P, nfb::kOut0);
+    if (push_step(nerf, ac > 0 ? b.dense({root + "/MLP_2/logit"}, W, ac, Dp + tc, {1}, nfb::kNone, Q, nfb::kOut0)
+                               : b.dense({root + "/MLP_2/logit"}, W, 0, 0, {1}, nfb::kNone, P, nfb::kOut0),
+                  root))
+      return -1;
     const size_t rgb_mark = h->specs.size();
     // rgb branch, modules.py:159-164.
     int rsrc = (rc > 0) ? Q : P;
@@ -187,12 +199,13 @@ int build_programs(nfb_handle* h) {
     int kin = rc, inoff = Dp + tc + ac;
     for (int i = 0; i < c.nerf_rgb_branch_depth; ++i) {
       const int dst = (rsrc == nfb::kB0) ? nfb::kB1 : nfb::kB0;
-      if (nerf.n_steps >= nfb::kMaxSteps - 1) return fail("too many layers");
-      nerf.steps[nerf.n_steps++] = b.dense({root + "/MLP_1/hidden_" + std::to_string(i)}, kx, kin,
-                                           inoff, {c.nerf_rgb_branch_width}, c.activation, rsrc, dst);
+      if (push_step(nerf, b.dense({root + "/MLP_1/hidden_" + std::to_string(i)}, kx, kin, inoff,
+                                  {c.nerf_rgb_branch_width}, c.activation, rsrc, dst), root))
+        return -1;
       rsrc = dst; kx = c.nerf_rgb_branch_width; kin = 0;
     }
-    nerf.steps[nerf.n_steps++] = b.dense({root + "/MLP_1/logit"}, kx, kin, inoff, {3}, nfb::kNone, rsrc, nfb::kOut1);
+    if (push_step(nerf, b.dense({root + "/MLP_1/logit"}, kx, kin, inoff, {3}, nfb::kNone, rsrc, nfb::kOut1), root))
+      return -1;
     // Re-order specs to the Flax order: bottleneck, MLP_1..., MLP_2.
     std::vector<ParamSpec> bott(h->specs.begin() + spec_mark, h->specs.begin() + alpha_mark);
     std::vector<ParamSpec> alpha(h->specs.begin() + alpha_mark, h->specs.begin() + rgb_mark);
@@ -337,6 +350,11 @@ int run_cond(nfb_handle* h, int B, const float* viewdirs, const unsigned* warp_i
   return 0;
 }
 
+// Dynamic shared memory composite_kernel and resample_kernel are opted into (nfb_create).
+constexpr int kRaySmemOptIn = 64 * 1024;
+static_assert(nfb::kRaysPerBlock * 3 * nfb::kMaxSamples * sizeof(float) <= (size_t)kRaySmemOptIn,
+              "composite_kernel's shared memory exceeds its opt-in at kMaxSamples");
+
 // The fp16x3 kernel can finish a ray on chip (volumetric rendering fused into its rgb epilogue)
 // when a ray's samples are whole 128-row tiles.
 bool can_fuse_composite(const nfb_handle* h, int S) {
@@ -428,6 +446,10 @@ int run_resample(nfb_handle* h, int B, const float* zc, const float* wc, const f
   const int blocks = (B + nfb::kRaysPerBlock - 1) / nfb::kRaysPerBlock;
   size_t smem = (size_t)nfb::kRaysPerBlock * (2 * a.nc + p) * sizeof(float);
   if (src) smem += (size_t)nfb::kRaysPerBlock * p * sizeof(uint16_t);
+  // nfb_create admits Nc + Nf <= kMaxSamples: Nc < kMaxSamples and npow2 <= kMaxSamples
+  static_assert(nfb::kRaysPerBlock * (3 * nfb::kMaxSamples * sizeof(float) + nfb::kMaxSamples * sizeof(uint16_t)) <=
+                    (size_t)kRaySmemOptIn,
+                "resample_kernel's shared memory exceeds its opt-in at kMaxSamples");
   nfb::resample_kernel<<<blocks, 32 * nfb::kRaysPerBlock, smem, s>>>(a);
   return launch_check(h, "resample_kernel");
 }
@@ -865,6 +887,14 @@ int nfb_create(const nfb_config* cfg, int max_rays, nfb_handle** out) {
   if (max_rays < 1) return fail("max_rays must be >= 1");
   if (cfg->num_coarse_samples < 2) return fail("num_coarse_samples must be >= 2");
   if (cfg->num_fine_samples < 0) return fail("num_fine_samples must be >= 0");
+  // The fine level has Nc + Nf samples per ray: composite_kernel (and its adjoint) hold a ray's samples in
+  // shared memory, up to kMaxSamples.  Within that bound resample_kernel's shared memory always fits its
+  // 64 KiB opt-in (static_assert in run_resample).
+  if (cfg->num_coarse_samples + cfg->num_fine_samples > nfb::kMaxSamples)
+    return fail("num_coarse_samples + num_fine_samples = %d: more than %d samples per ray (kMaxSamples)",
+                cfg->num_coarse_samples + cfg->num_fine_samples, nfb::kMaxSamples);
+  if (cfg->num_fine_samples > 0 && cfg->num_coarse_samples < 3)
+    return fail("hierarchical sampling needs >= 3 coarse samples (num_fine_samples > 0)");
   if (cfg->precision < NFB_PREC_FP32 || cfg->precision > NFB_PREC_FP16X3) return fail("bad precision");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
@@ -911,8 +941,11 @@ int nfb_create(const nfb_config* cfg, int max_rays, nfb_handle** out) {
   if (cudaFuncSetAttribute(nfb::field_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            nfb::kSimtSmemBytes) != cudaSuccess)
     return bail(fail("cannot reserve %d bytes of shared memory", nfb::kSimtSmemBytes));
-  cudaFuncSetAttribute(nfb::composite_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
-  cudaFuncSetAttribute(nfb::resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
+  if (cudaFuncSetAttribute(nfb::composite_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           kRaySmemOptIn) != cudaSuccess ||
+      cudaFuncSetAttribute(nfb::resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           kRaySmemOptIn) != cudaSuccess)
+    return bail(fail("cannot reserve %d bytes of shared memory for the per-ray kernels", kRaySmemOptIn));
   if (c.precision != NFB_PREC_FP32 && nfb::tc::create_tc(h)) return bail(-1);
   *out = h;
   return 0;

@@ -474,7 +474,12 @@ int train_prepare(nfb_handle* h, int chunk_rays) {
     if (grow(&h->d_tape, &h->tape_floats, need, "tape")) return -1;
     NFB_CUDA(cudaMemset(h->d_tape, 0, (size_t)need * sizeof(float)));
   }
-  cudaFuncSetAttribute(nfb::train::composite_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
+  // composite_bwd_kernel holds 4 floats per sample of each of its kRaysPerBlock rays (train_level)
+  static_assert(nfb::kRaysPerBlock * 4 * nfb::kMaxSamples * sizeof(float) <= 96 * 1024,
+                "composite_bwd_kernel's shared memory exceeds its opt-in at kMaxSamples");
+  if (cudaFuncSetAttribute(nfb::train::composite_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024) !=
+      cudaSuccess)
+    return fail("training: cannot reserve 96 KiB of shared memory for composite_bwd_kernel");
   if (!h->d_gpacked) {
     auto dm = [&](float** p, long long n) {
       return cudaMalloc(p, (size_t)std::max<long long>(n, 1) * sizeof(float)) == cudaSuccess ? 0

@@ -355,6 +355,26 @@ def main():
       warp_kwargs={'trunk_width': 32, 'use_pivot': True, 'use_translation': True}),
             num_rays=8, n_app=4, n_cam=1, n_warp=6, near=0.02, far=0.83,
             warp_alpha=8.0, seed=21)
+  # L: widths off every multiple of 32, two skips, elu hidden layers, sigmoid sigma.
+  make_case('arch_odd', dict(
+      use_warp=True, warp_field_type='se3', num_nerf_point_freqs=6,
+      num_warp_freqs=6, use_appearance_metadata=True, nerf_trunk_depth=5,
+      nerf_skips=(1, 3), nerf_trunk_width=100, nerf_rgb_branch_width=72,
+      nerf_rgb_branch_depth=2, activation='elu', sigma_activation='sigmoid',
+      num_coarse_samples=16, num_fine_samples=16, warp_kwargs={'trunk_width': 32}),
+            num_rays=9, n_app=4, n_cam=1, n_warp=5, near=0.02, far=0.83,
+            warp_alpha=5.5, seed=22, oracle_param_seed=22, store_params=False)
+  # M: rgb branch of depth 0 (the rgb logit reads [bottleneck | viewdirs | camera code]),
+  #    leaky_relu hidden layers, translation warp.  (A tanh or elu sigma gives negative densities, and with them
+  #    negative weights, for which the reference's hierarchical resampling has no distribution to
+  #    sample: those are checked on given z in tests/test_architectures_gpu.py.)
+  make_case('arch_rgb0', dict(
+      use_warp=True, warp_field_type='translation', num_warp_freqs=6, num_nerf_point_freqs=8,
+      nerf_trunk_depth=4, nerf_skips=(2,), nerf_trunk_width=64, nerf_rgb_branch_depth=0,
+      use_camera_metadata=True, activation='leaky_relu', sigma_activation='softplus',
+      num_coarse_samples=16, num_fine_samples=16, warp_kwargs={'hidden_channels': 32}),
+            num_rays=10, n_app=1, n_cam=3, n_warp=4, near=0.05, far=1.2,
+            warp_alpha=4.0, seed=23, oracle_param_seed=23, store_params=False)
 
 
 if __name__ == '__main__':

@@ -12,7 +12,7 @@ GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 CASES = ['se3_small', 'translation_small', 'nowarp_variants',
          'alpha_cond_init', 'se3_stratified', 'quarterhd_dims',
          'test_local_dims', 'encoded_small', 'time_small', 'blend_small',
-         'pivot_small']
+         'pivot_small', 'arch_odd', 'arch_rgb0']
 
 
 def unflatten(flat):

@@ -113,10 +113,14 @@ def test_rank_slices_concatenate_to_the_batch(world_size):
     assert torch.equal(torch.cat([next(r) for r in pranks]), next(pwhole))
 
 
-def test_mixed_image_sizes(tmp_path):
+def test_mixed_image_sizes_in_a_writable_copy(tmp_path):
   import cv2
   data = tmp_path / 'capture'
-  shutil.copytree(CAPTURE, data)
+  # contents only: the checkout may be read-only, and copytree's default (copy2) would carry its
+  # file modes into the copy that this test rewrites
+  shutil.copytree(CAPTURE, data, copy_function=shutil.copyfile)
+  for d, _, _ in os.walk(data):
+    os.chmod(d, 0o755)
   with open(data / 'camera' / 'left_003.json') as f:
     cam = json.load(f)
   cam['image_size'] = [80, 62]
