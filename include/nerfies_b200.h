@@ -245,6 +245,40 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
                                  int chunk_rays, const nfb_train_reg* reg, float* const* grads,
                                  const long long* numels, int count, float* loss_out, void* stream);
 
+/* Vector-Jacobian product of one nfb_render_forward call with respect to the parameters: what jax.vjp of
+ * NerfModel.__call__ gives for any loss on its outputs (training.py:228-264 is one such loss).
+ *   origins ... flags: the forward call's arguments (NFB_FLAG_NO_WARP, NFB_FLAG_COARSE_ONLY and
+ *     NFB_FLAG_METADATA_ENCODED as there; with the last, warp_id / appearance_id / camera_id are the (B, G|A|C)
+ *     float codes);
+ *   z_coarse (B,Nc), z_fine (B,Nc+Nf): the z values the forward used (nfb_coarse_z_vals of its t_rand and the
+ *     z_fine output of nfb_render_forward / nfb_sample_pdf).  They are constants (lax.stop_gradient,
+ *     model_utils.py:211): nothing is resampled;
+ *   cotangents, each nullable (a null one is zero; a level with none is skipped):
+ *     d_out_coarse / d_out_fine (B,6) in the forward's out layout (rgb, depth, med_depth, acc; med_depth is
+ *     piecewise constant and its column is ignored), d_weights_coarse (B,Nc) / d_weights_fine (B,Nc+Nf),
+ *     d_warped_coarse (B,Nc,3) / d_warped_fine (B,Nc+Nf,3) of the warped sample points;
+ *   d_warp_code (B,G), d_app_code (B,A), d_cam_code (B,C): with NFB_FLAG_METADATA_ENCODED, nullable, the
+ *     gradients of the codes (+=);
+ *   chunk_rays, grads, numels, count: as nfb_train_value_and_grad (grads ACCUMULATED into, +=).
+ * Per chunk of rays and level, the taped forward of nfb_train_value_and_grad is recomputed at the given z and
+ * walked backwards, seeded from the cotangents; it runs in the handle's training precision
+ * (nfb_set_train_precision) whatever nfb_config.precision is.  Uses the parameters of the last nfb_set_params
+ * and the time_alpha of the last nfb_set_time_alpha. */
+int nfb_render_vjp(nfb_handle* h, int num_rays, const float* origins, const float* directions,
+                   const float* viewdirs, const unsigned* warp_id, const unsigned* appearance_id,
+                   const unsigned* camera_id, float warp_alpha, unsigned flags, const float* z_coarse,
+                   const float* z_fine, const float* d_out_coarse, const float* d_out_fine,
+                   const float* d_weights_coarse, const float* d_weights_fine, const float* d_warped_coarse,
+                   const float* d_warped_fine, float* d_warp_code, float* d_app_code, float* d_cam_code,
+                   int chunk_rays, float* const* grads, const long long* numels, int count, void* stream);
+
+/* The same for nfb_warp_forward (warp_field.apply on free points): d_warped (P,3) -> the warp field's parameter
+ * gradients (+= into grads, laid out as nfb_train_value_and_grad's) and, with NFB_FLAG_METADATA_ENCODED,
+ * d_code (P, num_warp_features), nullable (+=).  Training precision, chunks of max_rays points. */
+int nfb_warp_vjp(nfb_handle* h, int num_points, const float* points, const unsigned* warp_id, float warp_alpha,
+                 unsigned flags, const float* d_warped, float* d_code, float* const* grads,
+                 const long long* numels, int count, void* stream);
+
 /* Jacobian of the warp field at free points: jacobian_out (P,3,3), J[i][j] = d warped_i / d point_j
  * (jax.jacfwd(self.warp, argnums=0), warping.py:196-198, 385-387); warped_out (P,3) nullable.
  * warp_id (P) GLO ids, or with NFB_WARP_ENC_TIME const float* timestamps (P); the metadata embedding is a

@@ -22,7 +22,7 @@ SYMBOLS = [
     'nfb_train_value_and_grad_reg', 'nfb_warp_jacobian', 'nfb_check_abort', 'nfb_reset_abort',
     'nfb_image_metrics_workspace_size', 'nfb_image_metrics', 'nfb_gather_rays', 'nfb_selftest_sgemm',
     'nfb_set_train_precision', 'nfb_selftest_train_gemm', 'nfb_debug_one_row_block',
-    'nfb_image_quantize',
+    'nfb_image_quantize', 'nfb_render_vjp', 'nfb_warp_vjp',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -179,6 +179,12 @@ def load():
   lib.nfb_train_value_and_grad_reg.argtypes = [vp, ci] + [vp] * 6 + [cf, vp, vp, cu, vp, ci, vp, ctypes.POINTER(vp),
                                                ctypes.POINTER(ctypes.c_longlong), ci, vp, vp]
   lib.nfb_train_value_and_grad_reg.restype = ci
+  lib.nfb_render_vjp.argtypes = [vp, ci] + [vp] * 6 + [cf, cu] + [vp] * 11 + [ci, ctypes.POINTER(vp),
+                                                                              ctypes.POINTER(ctypes.c_longlong), ci, vp]
+  lib.nfb_render_vjp.restype = ci
+  lib.nfb_warp_vjp.argtypes = [vp, ci, vp, vp, cf, cu, vp, vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_longlong),
+                               ci, vp]
+  lib.nfb_warp_vjp.restype = ci
   lib.nfb_warp_jacobian.argtypes = [vp, ci, vp, vp, cf, vp, vp, vp]
   lib.nfb_warp_jacobian.restype = ci
   lib.nfb_check_abort.argtypes = [vp, ci]

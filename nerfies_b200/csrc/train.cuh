@@ -493,6 +493,115 @@ __global__ void composite_bwd_kernel(const CompositeBwdArgs a) {
   }
 }
 
+// The adjoint of volumetric_rendering (model_utils.py:104-126) for caller-given cotangents of its outputs:
+// nfb_render_vjp's seed of the backward, where composite_bwd_kernel seeds the photometric loss's.  Per ray
+//   d/dw_i = g_rgb . c_i - [white_bg] sum(g_rgb) + g_depth z_i + g_acc [i < S-1 or !sample_at_infinity] + g_w_i
+// (the white background adds 1 - sum w, the acc before sample_at_infinity drops the last sample), then the same
+// chain as composite_bwd_kernel to the raw rgb and density.  med_depth is piecewise constant: no cotangent.
+struct CompositeVjpArgs {
+  const float4* samples; const float* z; const float* directions;   // the taped forward
+  const float* d_out;         // (R,6) cotangents of rgb, depth, med_depth (ignored), acc; or null
+  const float* d_weights;     // (R,S) or null
+  const float* rgb_raw; int ld_rgb; const float* alpha_raw; int ld_a;
+  float* d_rgb_raw; float* d_alpha_raw;     // same layouts: = (not +=)
+  int num_rays, S, white_bg, sample_at_infinity, sigma_act;
+};
+// Shared memory: three floats per sample of each of kRaysPerBlock rays.
+constexpr size_t composite_vjp_smem(int S) { return (size_t)kRaysPerBlock * 3 * S * sizeof(float); }
+
+// One warp per ray, S <= kMaxSamples.  Lane l owns the contiguous samples [l p, l p + p), p = ceil(S / 32): the
+// transmittance T_i = prod_{j<i} (1 - alpha_j + eps) is an exclusive product scan and sum_{k>i} gw_k w_k an
+// exclusive suffix-sum scan, each as a serial pass over the lane's own samples around one shuffle scan of the
+// 32 lane totals.
+__global__ void __launch_bounds__(32 * kRaysPerBlock) composite_vjp_kernel(const CompositeVjpArgs a) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int ray = blockIdx.x * kRaysPerBlock + warp;
+  if (ray >= a.num_rays) return;
+  extern __shared__ float sh[];
+  const int S = a.S;
+  float* gw = sh + warp * 3 * S;       // d / d w_i
+  float* al = gw + S;                  // alpha_i
+  float* tr = al + S;                  // T_i
+  float g[3] = {0.f, 0.f, 0.f}, gd = 0.f, ga = 0.f;
+  if (a.d_out) {
+    const float* o = a.d_out + (size_t)ray * 6;
+    g[0] = o[0]; g[1] = o[1]; g[2] = o[2]; gd = o[3]; ga = o[5];
+  }
+  const float gsum = g[0] + g[1] + g[2];
+  const float dx = a.directions[ray * 3], dy = a.directions[ray * 3 + 1], dz = a.directions[ray * 3 + 2];
+  const float dnorm = sqrtf(dx * dx + dy * dy + dz * dz);
+  const float last = a.sample_at_infinity ? 1e10f : 1e-19f;
+  const size_t base = (size_t)ray * S;
+  for (int i = lane; i < S; i += 32) {
+    const float4 c = a.samples[base + i];
+    const float z = a.z[base + i];
+    float v = g[0] * c.x + g[1] * c.y + g[2] * c.z;
+    if (a.white_bg) v -= gsum;
+    v += gd * z;
+    if (i + 1 < S || !a.sample_at_infinity) v += ga;
+    if (a.d_weights) v += a.d_weights[base + i];
+    gw[i] = v;
+    const float dist = (i + 1 < S) ? (a.z[base + i + 1] - z) : last;
+    al[i] = -expm1f(-c.w * (dist * dnorm));
+  }
+  __syncwarp();
+  const int per = (S + 31) / 32;
+  const int b = min(S, lane * per), e = min(S, b + per);
+  // T: product of the lane's factors, exclusive scan over the lanes, then the lane's own samples
+  float p = 1.f;
+  for (int i = b; i < e; ++i) p = p * (1.0f - al[i] + 1e-10f);
+  float incl = p;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float u = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl = incl * u;
+  }
+  float t = __shfl_up_sync(0xffffffffu, incl, 1);
+  if (lane == 0) t = 1.f;
+  float s = 0.f;                       // the lane's sum of gw_k w_k
+  for (int i = b; i < e; ++i) {
+    tr[i] = t;
+    s += gw[i] * (al[i] * t);
+    t = t * (1.0f - al[i] + 1e-10f);
+  }
+  // sum over the lanes to the right: an inclusive suffix scan, shifted by one lane.  (Not the inclusive sum minus
+  // the lane's own: dalpha divides this sum by 1 - alpha_i + eps, down to 1e-10 behind an opaque sample, where
+  // the cancellation's error of ~2^-24 |s| would swamp the true, tiny remainder.)
+  float incl_suf = s;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float u = __shfl_down_sync(0xffffffffu, incl_suf, o);
+    if (lane + o < 32) incl_suf += u;
+  }
+  float acc = __shfl_down_sync(0xffffffffu, incl_suf, 1);
+  if (lane == 31) acc = 0.f;
+  for (int i = e - 1; i >= b; --i) {
+    const size_t m = base + i;
+    const float4 c = a.samples[m];
+    const float dist = ((i + 1 < S) ? (a.z[m + 1] - a.z[m]) : last) * dnorm;
+    const float w = al[i] * tr[i];
+    // w_i = alpha_i T_i: dL/dalpha_i = gw_i T_i - (sum_{k>i} gw_k w_k) / (1 - alpha_i + eps)
+    const float dalpha = gw[i] * tr[i] - acc / (1.0f - al[i] + 1e-10f);
+    acc += gw[i] * w;
+    const float dsigma = dalpha * dist * expf(-c.w * dist);      // alpha = 1 - exp(-sigma dist)
+    const float raw = a.alpha_raw[m * a.ld_a];
+    float dact;                                                    // sigma = act(raw)
+    if (a.sigma_act == kSoftplus) dact = 1.f / (1.f + expf(-raw));
+    else if (a.sigma_act == kRelu) dact = raw > 0.f ? 1.f : 0.f;
+    else dact = act_grad_from_output(c.w, a.sigma_act);
+    a.d_alpha_raw[m * a.ld_a] = dsigma * dact;
+    a.d_rgb_raw[m * a.ld_rgb + 0] = g[0] * w * c.x * (1.f - c.x);
+    a.d_rgb_raw[m * a.ld_rgb + 1] = g[1] * w * c.y * (1.f - c.y);
+    a.d_rgb_raw[m * a.ld_rgb + 2] = g[2] * w * c.z * (1.f - c.z);
+  }
+}
+
+// out[i] += x[i]
+__global__ void add_into_kernel(float* __restrict__ out, const float* __restrict__ x, long long n) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] += x[i];
+}
+
 // ---------------------------------------------------------------------------
 // Embedding gradients: dcond (B, stride) -> table rows (glo.py:41-53), the adjoint of
 // ray_cond_kernel over the same layout.
@@ -520,6 +629,36 @@ __global__ void cond_bwd_kernel(const CondBwdArgs a) {
   } else if (src == kCondApp) atomicAdd(a.d_app_table + embed_row(a.app_id, ray, a.n_app) * L.A + j, v);
   else if (src == kCondCam) atomicAdd(a.d_cam_table + embed_row(a.cam_id, ray, a.n_cam) * L.C + j, v);
   // view directions carry no parameter
+}
+
+// The same adjoint with metadata_encoded=True (models.py:198-213, warping.py:186-187): the condition vector holds
+// the caller's per-ray codes, so dcond goes (+=) to the dense code gradients d_warp (B,G), d_app (B,A), d_cam
+// (B,C).  An appearance code feeding several blocks (trunk, alpha and, under the use_alpha_condition quirk of
+// models.py:206-207, rgb) receives their sum.  A code the call did not pass is row 0 of its table
+// (ray_cond_kernel), whose gradient goes to that row; a null gradient pointer drops its code's share.
+struct CondVjpEncodedArgs {
+  const float* dcond; int num_rays;
+  int has_warp, has_app, has_cam;                   // the call passed that code
+  float* d_warp; float* d_app; float* d_cam;        // dense code gradients, or null
+  float* d_warp_table; float* d_app_table; float* d_cam_table;   // row 0 of the tables, or null
+  CondLayout layout;
+};
+__global__ void cond_vjp_encoded_kernel(const CondVjpEncodedArgs a) {
+  const CondLayout& L = a.layout;
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)a.num_rays * L.stride) return;
+  const int ray = (int)(idx / L.stride);
+  const float v = a.dcond[idx];
+  if (v == 0.f) return;
+  int j;
+  const CondSource src = cond_source(L, (int)(idx - (long long)ray * L.stride), j);
+  auto to = [&](int has, float* dense, float* table, int width) {
+    if (has && dense) atomicAdd(dense + (size_t)ray * width + j, v);
+    else if (!has && table) atomicAdd(table + j, v);
+  };
+  if (src == kCondWarp) to(a.has_warp, a.d_warp, a.d_warp_table, L.G);
+  else if (src == kCondApp) to(a.has_app, a.d_app, a.d_app_table, L.A);
+  else if (src == kCondCam) to(a.has_cam, a.d_cam, a.d_cam_table, L.C);
 }
 
 // ---------------------------------------------------------------------------

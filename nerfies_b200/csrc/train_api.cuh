@@ -379,12 +379,12 @@ int train_cond(nfb_handle* h, int n, const float* viewdirs, const unsigned* warp
                       float_time ? nullptr : warp_id, s);
 }
 
-// forward + loss + backward of one level for `R` rays (rows = R * S) on the tape; `cond` / `dcond` are
-// the R rays' condition vectors and their gradient accumulator.
-int train_level(nfb_handle* h, int level, int R, int S, const float* z, const float* origins,
-                const float* directions, const float* target, const float* cond, float* dcond, float scale,
-                bool use_warp, float* out6, float* weights, float* loss, cudaStream_t s,
-                const RegCfg* reg = nullptr) {
+// The taped forward of one level for `R` rays (rows = R * S) at the given z: warp field, encoding, NeRF MLP,
+// raw -> samples, volumetric rendering into out6 (and weights, nullable).  *alpha_step / *rgb_step: the
+// steps whose outputs hold the raw density and rgb.
+int level_forward(nfb_handle* h, int level, int R, int S, const float* z, const float* origins,
+                  const float* directions, const float* cond, bool use_warp, float* out6, float* weights,
+                  cudaStream_t s, int* alpha_step_out, int* rgb_step_out) {
   using namespace nfb::train;
   const nfb::FieldProgram& p = h->prog[level];
   const long long rows = (long long)R * S;
@@ -392,7 +392,6 @@ int train_level(nfb_handle* h, int level, int R, int S, const float* z, const fl
   float* A = h->d_tape;
   const bool warp = use_warp && p.warp_type != 0;
   const unsigned blocks = (unsigned)((rows + 127) / 128);
-  // ---- forward ----
   if (warp && warp_forward(h, p, t, origins, directions, z, S, nullptr, cond, s)) return -1;
   {
     EncodeArgs e{};
@@ -415,7 +414,28 @@ int train_level(nfb_handle* h, int level, int R, int S, const float* z, const fl
   raw_to_samples_kernel<<<blocks, 128, 0, s>>>(A + t.out_n[rgb_step], ld_rgb, A + t.out_n[alpha_step], ld_a,
                                                p.sigma_act, reinterpret_cast<float4*>(A + t.samples), rows);
   if (launch_check(h, "raw_to_samples_kernel")) return -1;
-  if (run_composite(h, R, S, A + t.samples, z, directions, out6, weights, s)) return -1;
+  *alpha_step_out = alpha_step;
+  *rgb_step_out = rgb_step;
+  return run_composite(h, R, S, A + t.samples, z, directions, out6, weights, s);
+}
+
+// forward + loss + backward of one level for `R` rays (rows = R * S) on the tape; `cond` / `dcond` are
+// the R rays' condition vectors and their gradient accumulator.
+int train_level(nfb_handle* h, int level, int R, int S, const float* z, const float* origins,
+                const float* directions, const float* target, const float* cond, float* dcond, float scale,
+                bool use_warp, float* out6, float* weights, float* loss, cudaStream_t s,
+                const RegCfg* reg = nullptr) {
+  using namespace nfb::train;
+  const nfb::FieldProgram& p = h->prog[level];
+  const long long rows = (long long)R * S;
+  const TapeLayout t = tape_layout(p, rows);
+  float* A = h->d_tape;
+  const bool warp = use_warp && p.warp_type != 0;
+  const unsigned blocks = (unsigned)((rows + 127) / 128);
+  int alpha_step = -1, rgb_step = -1;
+  if (level_forward(h, level, R, S, z, origins, directions, cond, use_warp, out6, weights, s, &alpha_step, &rgb_step))
+    return -1;
+  const int ld_a = p.nerf.steps[alpha_step].npad, ld_rgb = p.nerf.steps[rgb_step].npad;
   // ---- loss + backward ----
   NFB_CUDA(cudaMemsetAsync(A + t.grad_begin, 0, (size_t)(t.grad_end - t.grad_begin) * sizeof(float), s));
   {
@@ -463,6 +483,109 @@ int train_level(nfb_handle* h, int level, int R, int S, const float* z, const fl
     if (launch_check(h, "warp_mag_loss_kernel")) return -1;
   }
   return warp ? warp_backward(h, p, t, S, dcond, s) : 0;
+}
+
+// One level of nfb_render_vjp for `R` rays: the taped forward at the given z, then train_level's backward,
+// seeded by composite_vjp_kernel from the cotangents of the level's outputs instead of by the photometric loss.
+// d_out (R,6), d_weights (R,S) and d_warped (R,S,3) are nullable; d_warped joins the gradient of the warped
+// points that the NeRF MLP's encoding leaves in tape.dwarped.
+static_assert(nfb::train::composite_vjp_smem(nfb::kMaxSamples) <= 48 * 1024,
+              "composite_vjp_kernel's shared memory exceeds the default 48 KiB at kMaxSamples");
+int vjp_level(nfb_handle* h, int level, int R, int S, const float* z, const float* origins, const float* directions,
+              const float* cond, float* dcond, bool use_warp, const float* d_out, const float* d_weights,
+              const float* d_warped, cudaStream_t s) {
+  using namespace nfb::train;
+  const nfb::FieldProgram& p = h->prog[level];
+  const long long rows = (long long)R * S;
+  const TapeLayout t = tape_layout(p, rows);
+  float* A = h->d_tape;
+  const bool warp = use_warp && p.warp_type != 0;
+  const unsigned blocks = (unsigned)((rows + 127) / 128);
+  int alpha_step = -1, rgb_step = -1;
+  if (level_forward(h, level, R, S, z, origins, directions, cond, use_warp, h->d_tr_out, nullptr, s, &alpha_step,
+                    &rgb_step))
+    return -1;
+  NFB_CUDA(cudaMemsetAsync(A + t.grad_begin, 0, (size_t)(t.grad_end - t.grad_begin) * sizeof(float), s));
+  {
+    CompositeVjpArgs c{};
+    c.samples = reinterpret_cast<const float4*>(A + t.samples); c.z = z; c.directions = directions;
+    c.d_out = d_out; c.d_weights = d_weights;
+    c.rgb_raw = A + t.out_n[rgb_step]; c.ld_rgb = p.nerf.steps[rgb_step].npad;
+    c.alpha_raw = A + t.out_n[alpha_step]; c.ld_a = p.nerf.steps[alpha_step].npad;
+    c.d_rgb_raw = A + t.d_out_n[rgb_step]; c.d_alpha_raw = A + t.d_out_n[alpha_step];
+    c.num_rays = R; c.S = S;
+    c.white_bg = h->cfg.use_white_background; c.sample_at_infinity = h->cfg.use_sample_at_infinity;
+    c.sigma_act = p.sigma_act;
+    const int nblk = (R + nfb::kRaysPerBlock - 1) / nfb::kRaysPerBlock;
+    composite_vjp_kernel<<<nblk, 32 * nfb::kRaysPerBlock, composite_vjp_smem(S), s>>>(c);
+    if (launch_check(h, "composite_vjp_kernel")) return -1;
+  }
+  if (net_backward(h, p.nerf, A + t.in_n, A + t.d_in_n, t.ld_n, t.out_n, t.d_out_n, A, rows, s)) return -1;
+  {
+    EncodeBwdArgs e{};
+    e.pts = A + t.warped; e.window = nullptr; e.din = A + t.d_in_n; e.F = p.Fp; e.ld = t.ld_n; e.S = S;
+    e.cond_stride = h->cond_layout.stride; e.cond_off = p.G; e.n_cond = p.tc + p.ac + p.rc;
+    e.dpts = warp ? A + t.dwarped : nullptr; e.dcond = dcond; e.rows = rows;
+    encode_bwd_kernel<<<blocks, 128, 0, s>>>(e);
+    if (launch_check(h, "encode_bwd_kernel")) return -1;
+  }
+  if (!warp) return 0;
+  if (d_warped) {
+    add_into_kernel<<<(unsigned)((rows * 3 + 255) / 256), 256, 0, s>>>(A + t.dwarped, d_warped, rows * 3);
+    if (launch_check(h, "add_into_kernel")) return -1;
+  }
+  return warp_backward(h, p, t, S, dcond, s);
+}
+
+// The gradient accumulators of the packed parameters and of the three embedding tables, zeroed.
+int zero_grads(nfb_handle* h, cudaStream_t s) {
+  const nfb_config& c = h->cfg;
+  NFB_CUDA(cudaMemsetAsync(h->d_gpacked, 0, (size_t)h->packed_floats * sizeof(float), s));
+  NFB_CUDA(cudaMemsetAsync(h->d_gwarp, 0, (size_t)std::max(1, c.num_warp_embeddings * c.num_warp_features) * sizeof(float), s));
+  NFB_CUDA(cudaMemsetAsync(h->d_gapp, 0, (size_t)std::max(1, c.num_appearance_embeddings * c.num_appearance_features) * sizeof(float), s));
+  NFB_CUDA(cudaMemsetAsync(h->d_gcam, 0, (size_t)std::max(1, c.num_camera_embeddings * c.num_camera_features) * sizeof(float), s));
+  return 0;
+}
+
+// `count` gradient tensors of `numels` elements: the order and sizes of nfb_param_info.
+int check_grads(const nfb_handle* h, float* const* grads, const long long* numels, int count) {
+  if (!grads || !numels) return fail("null gradient list");
+  if (count != (int)h->specs.size()) return fail("expected %d gradient tensors, got %d", (int)h->specs.size(), count);
+  for (int i = 0; i < count; ++i)
+    if (numels[i] != h->specs[i].rows * h->specs[i].cols)
+      return fail("gradient %d (%s): expected %lld elements", i, h->specs[i].name.c_str(), h->specs[i].rows * h->specs[i].cols);
+  return 0;
+}
+
+// packed layouts -> the caller's tensors (+=), in the order of nfb_param_info
+int unpack_grads(nfb_handle* h, float* const* grads, int count, cudaStream_t s) {
+  for (int i = 0; i < count; ++i) {
+    const ParamSpec& p = h->specs[i];
+    const float* base = p.table == 0 ? h->d_gpacked : p.table == 1 ? h->d_gwarp : p.table == 2 ? h->d_gapp : h->d_gcam;
+    const long long n = p.rows * p.cols;
+    if (n == 0) continue;
+    if (!grads[i]) return fail("gradient %d (%s) is null", i, p.name.c_str());
+    nfb::train::unpack_grad_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(base + p.dst_off, grads[i], p.rows, p.cols, p.ld, p.c_off);
+    if (launch_check(h, "unpack_grad_kernel")) return -1;
+  }
+  return 0;
+}
+
+// The adjoint of run_cond(encoded = true) for `n` rays: dcond -> the dense code gradients (+=), or row 0 of a
+// table for a code the call did not pass.
+int cond_vjp_encoded(nfb_handle* h, int n, const float* dcond, bool has_warp, bool has_app, bool has_cam,
+                     float* d_warp, float* d_app, float* d_cam, cudaStream_t s) {
+  nfb::train::CondVjpEncodedArgs a{};
+  a.dcond = dcond; a.num_rays = n;
+  a.has_warp = has_warp; a.has_app = has_app; a.has_cam = has_cam;
+  a.d_warp = d_warp; a.d_app = d_app; a.d_cam = d_cam;
+  // a 'time' encoder has no table: ray_cond_kernel's row-0 fallback reads memory no parameter owns
+  a.d_warp_table = has_time_encoder(h) && h->cfg.warp_metadata_encoder == NFB_WARP_ENC_TIME ? nullptr : h->d_gwarp;
+  a.d_app_table = h->d_gapp; a.d_cam_table = h->d_gcam;
+  a.layout = h->cond_layout;
+  const long long total = (long long)n * a.layout.stride;
+  nfb::train::cond_vjp_encoded_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(a);
+  return launch_check(h, "cond_vjp_encoded_kernel");
 }
 
 int train_prepare(nfb_handle* h, int chunk_rays) {
@@ -587,9 +710,7 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
   if (count != (int)h->specs.size()) return fail("expected %d gradient tensors, got %d", (int)h->specs.size(), count);
   if (flags & NFB_FLAG_METADATA_ENCODED) return fail("training with metadata_encoded=True is not supported");
   const nfb_config& c = h->cfg;
-  for (int i = 0; i < count; ++i)
-    if (numels[i] != h->specs[i].rows * h->specs[i].cols)
-      return fail("gradient %d (%s): expected %lld elements", i, h->specs[i].name.c_str(), h->specs[i].rows * h->specs[i].cols);
+  if (check_grads(h, grads, numels, count)) return -1;
   cudaStream_t s = (cudaStream_t)stream;
   if (enter_stream(h, s)) return -1;
   if (B == 0) return 0;
@@ -600,10 +721,7 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
   const bool use_warp = !(flags & NFB_FLAG_NO_WARP);
   const bool fine = c.num_fine_samples > 0;
   if (set_window(h, warp_alpha, s)) return -1;
-  NFB_CUDA(cudaMemsetAsync(h->d_gpacked, 0, (size_t)h->packed_floats * sizeof(float), s));
-  NFB_CUDA(cudaMemsetAsync(h->d_gwarp, 0, (size_t)std::max(1, c.num_warp_embeddings * c.num_warp_features) * sizeof(float), s));
-  NFB_CUDA(cudaMemsetAsync(h->d_gapp, 0, (size_t)std::max(1, c.num_appearance_embeddings * c.num_appearance_features) * sizeof(float), s));
-  NFB_CUDA(cudaMemsetAsync(h->d_gcam, 0, (size_t)std::max(1, c.num_camera_embeddings * c.num_camera_features) * sizeof(float), s));
+  if (zero_grads(h, s)) return -1;
   NFB_CUDA(cudaMemsetAsync(h->d_loss, 0, nfb::train::kLossSlots * sizeof(float), s));
   // condition vectors of the whole batch (per ray), their gradient accumulator
   const bool float_time = has_time_encoder(h) && c.warp_metadata_encoder == NFB_WARP_ENC_TIME;
@@ -662,16 +780,7 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
     nfb::train::finalize_stats_kernel<<<1, 32, 0, s>>>(h->d_loss, 1.f / (float)B, 1.f / (float)jrows, P > 0 ? 1.f / (float)P : 0.f);
     if (launch_check(h, "finalize_stats_kernel")) return -1;
   }
-  // packed layouts -> the caller's tensors (+=), in the order of nfb_param_info
-  for (int i = 0; i < count; ++i) {
-    const ParamSpec& p = h->specs[i];
-    const float* base = p.table == 0 ? h->d_gpacked : p.table == 1 ? h->d_gwarp : p.table == 2 ? h->d_gapp : h->d_gcam;
-    const long long n = p.rows * p.cols;
-    if (n == 0) continue;
-    if (!grads[i]) return fail("gradient %d (%s) is null", i, p.name.c_str());
-    nfb::train::unpack_grad_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(base + p.dst_off, grads[i], p.rows, p.cols, p.ld, p.c_off);
-    if (launch_check(h, "unpack_grad_kernel")) return -1;
-  }
+  if (unpack_grads(h, grads, count, s)) return -1;
   // without regularisers, loss_out holds the two rgb losses only
   const int slots = reg ? nfb::train::kLossSlots : nfb::train::kSlotRgbFine + 1;
   NFB_CUDA(cudaMemcpyAsync(loss_out, h->d_loss, slots * sizeof(float), cudaMemcpyDeviceToDevice, s));
@@ -687,6 +796,123 @@ int nfb_train_value_and_grad(nfb_handle* h, int B, const float* origins, const f
   return nfb_train_value_and_grad_reg(h, B, origins, directions, viewdirs, warp_id, app_id, cam_id, warp_alpha, t_rand,
                                       u_rand, flags, rgb_target, chunk_rays, nullptr, grads, numels, count, loss_out,
                                       stream);
+}
+
+int nfb_render_vjp(nfb_handle* h, int B, const float* origins, const float* directions, const float* viewdirs,
+                   const unsigned* warp_id, const unsigned* app_id, const unsigned* cam_id, float warp_alpha,
+                   unsigned flags, const float* z_coarse, const float* z_fine, const float* d_out_coarse,
+                   const float* d_out_fine, const float* d_weights_coarse, const float* d_weights_fine,
+                   const float* d_warped_coarse, const float* d_warped_fine, float* d_warp_code, float* d_app_code,
+                   float* d_cam_code, int chunk_rays, float* const* grads, const long long* numels, int count,
+                   void* stream) {
+  if (check_call(h, B)) return -1;
+  if (check_grads(h, grads, numels, count)) return -1;
+  const nfb_config& c = h->cfg;
+  const bool encoded = (flags & NFB_FLAG_METADATA_ENCODED) != 0;
+  if (!encoded && (d_warp_code || d_app_code || d_cam_code))
+    return fail("render VJP: code gradients need NFB_FLAG_METADATA_ENCODED");
+  const bool use_warp = !(flags & NFB_FLAG_NO_WARP);
+  const bool warp = use_warp && c.warp_field_type != NFB_WARP_NONE;
+  const bool coarse = d_out_coarse || d_weights_coarse || d_warped_coarse;
+  const bool fine = d_out_fine || d_weights_fine || d_warped_fine;
+  if (fine && (c.num_fine_samples == 0 || (flags & NFB_FLAG_COARSE_ONLY)))
+    return fail("render VJP: fine-level cotangents, but the call renders no fine level");
+  if (!warp && (d_warped_coarse || d_warped_fine))
+    return fail("render VJP: warped-point cotangents, but the call does not warp");
+  cudaStream_t s = (cudaStream_t)stream;
+  if (enter_stream(h, s)) return -1;
+  if (B == 0) return 0;
+  if (!origins || !directions) return fail("render VJP: origins / directions are null");
+  if ((coarse && !z_coarse) || (fine && !z_fine)) return fail("render VJP: the z values of a level with cotangents are null");
+  if (chunk_rays < 1) chunk_rays = 256;
+  chunk_rays = std::min(chunk_rays, B);
+  if (train_prepare(h, chunk_rays)) return -1;
+  if (set_window(h, warp_alpha, s) || zero_grads(h, s)) return -1;
+  // condition vectors of the whole batch (per ray), their gradient accumulator
+  const float* vd = viewdirs ? viewdirs : directions;
+  const bool time_enc = warp && !encoded && has_time_encoder(h);
+  if (time_enc ? train_cond(h, B, vd, warp_id, c.warp_metadata_encoder == NFB_WARP_ENC_TIME, app_id, cam_id, s)
+               : run_cond(h, B, vd, warp_id, app_id, cam_id, s, encoded, false))
+    return -1;
+  NFB_CUDA(cudaMemsetAsync(h->d_dcond, 0, (size_t)B * h->cond_layout.stride * sizeof(float), s));
+  const int nc = c.num_coarse_samples, nfine = nc + c.num_fine_samples;
+  auto at = [](const float* p, size_t off) { return p ? p + off : nullptr; };
+  for (int r0 = 0; r0 < B; r0 += chunk_rays) {
+    const int R = std::min(chunk_rays, B - r0);
+    const float* cond = h->d_cond + (size_t)r0 * h->cond_layout.stride;
+    float* dcond = h->d_dcond + (size_t)r0 * h->cond_layout.stride;
+    const float* o = origins + (size_t)r0 * 3;
+    const float* d = directions + (size_t)r0 * 3;
+    if (coarse && vjp_level(h, 0, R, nc, z_coarse + (size_t)r0 * nc, o, d, cond, dcond, use_warp,
+                            at(d_out_coarse, (size_t)r0 * 6), at(d_weights_coarse, (size_t)r0 * nc),
+                            at(d_warped_coarse, (size_t)r0 * nc * 3), s))
+      return -1;
+    if (fine && vjp_level(h, 1, R, nfine, z_fine + (size_t)r0 * nfine, o, d, cond, dcond, use_warp,
+                          at(d_out_fine, (size_t)r0 * 6), at(d_weights_fine, (size_t)r0 * nfine),
+                          at(d_warped_fine, (size_t)r0 * nfine * 3), s))
+      return -1;
+  }
+  if (encoded) {
+    if (cond_vjp_encoded(h, B, h->d_dcond, warp_id, app_id, cam_id, d_warp_code, d_app_code, d_cam_code, s)) return -1;
+  } else if (run_cond_bwd(h, B, h->d_dcond, warp_id, app_id, cam_id, s) ||
+             (time_enc && time_backward(h, B, h->d_dcond, s))) {
+    return -1;
+  }
+  return unpack_grads(h, grads, count, s);
+}
+
+int nfb_warp_vjp(nfb_handle* h, int P, const float* points, const unsigned* warp_id, float warp_alpha,
+                 unsigned flags, const float* d_warped, float* d_code, float* const* grads, const long long* numels,
+                 int count, void* stream) {
+  if (!h) return fail("null handle");
+  if (P < 0) return fail("P must be >= 0");
+  if (check_call(h, std::min(P, h->max_rays))) return -1;
+  if (check_grads(h, grads, numels, count)) return -1;
+  const nfb_config& c = h->cfg;
+  if (h->prog[0].warp_type == 0) return fail("the model has no warp field");
+  const bool encoded = (flags & NFB_FLAG_METADATA_ENCODED) != 0;
+  if (d_code && !encoded) return fail("warp VJP: d_code needs NFB_FLAG_METADATA_ENCODED");
+  cudaStream_t s = (cudaStream_t)stream;
+  if (enter_stream(h, s)) return -1;
+  if (P == 0) return 0;
+  if (!points || !d_warped) return fail("warp VJP: points / d_warped are null");
+  if (set_window(h, warp_alpha, s)) return -1;
+  const int chunk = std::min(P, h->max_rays);
+  if (train_prepare_rows(h, chunk) || zero_grads(h, s)) return -1;
+  const nfb::FieldProgram& p = h->prog[0];
+  const int G = h->cond_layout.G;
+  for (int p0 = 0; p0 < P; p0 += chunk) {
+    const int n = std::min(chunk, P - p0);
+    const TapeLayout t = tape_layout(p, n);
+    float* A = h->d_tape;
+    if (encoded) {
+      // warp_points_forward with the caller's codes as the warp block of the condition vectors
+      const unsigned* codes = warp_id ? reinterpret_cast<const unsigned*>(reinterpret_cast<const float*>(warp_id) +
+                                                                          (size_t)p0 * G) : nullptr;
+      nfb::train::add_noise_kernel<<<(unsigned)(((long long)n * 3 + 255) / 256), 256, 0, s>>>(
+          points + (size_t)p0 * 3, nullptr, A + t.warped, (long long)n * 3);
+      if (launch_check(h, "add_noise_kernel") || run_cond(h, n, A + t.warped, codes, nullptr, nullptr, s, true, false) ||
+          warp_forward(h, p, t, nullptr, nullptr, nullptr, 1, A + t.warped, h->d_cond, s))
+        return -1;
+    } else if (warp_points_forward(h, n, points + (size_t)p0 * 3, nullptr, warp_id ? warp_id + p0 : nullptr,
+                                   c.warp_metadata_encoder == NFB_WARP_ENC_TIME, s)) {
+      return -1;
+    }
+    NFB_CUDA(cudaMemsetAsync(A + t.grad_begin, 0, (size_t)(t.grad_end - t.grad_begin) * sizeof(float), s));
+    NFB_CUDA(cudaMemsetAsync(h->d_dcond, 0, (size_t)n * h->cond_layout.stride * sizeof(float), s));
+    NFB_CUDA(cudaMemcpyAsync(A + t.dwarped, d_warped + (size_t)p0 * 3, (size_t)n * 3 * sizeof(float),
+                             cudaMemcpyDeviceToDevice, s));
+    if (warp_backward(h, p, t, 1, h->d_dcond, s)) return -1;
+    if (encoded) {
+      if (cond_vjp_encoded(h, n, h->d_dcond, warp_id != nullptr, false, false,
+                           d_code ? d_code + (size_t)p0 * G : nullptr, nullptr, nullptr, s))
+        return -1;
+    } else if (run_cond_bwd(h, n, h->d_dcond, warp_id ? warp_id + p0 : nullptr, nullptr, nullptr, s) ||
+               time_backward(h, n, h->d_dcond, s)) {
+      return -1;
+    }
+  }
+  return unpack_grads(h, grads, count, s);
 }
 
 int nfb_warp_jacobian(nfb_handle* h, int P, const float* points, const unsigned* warp_id, float warp_alpha,

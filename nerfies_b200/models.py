@@ -115,7 +115,11 @@ class _Handle:
       if t.numel() != rows * cols:
         raise ValueError(f'parameter {name}: shape {tuple(t.shape)} does not '
                          f'hold {rows}x{cols} elements')
-      tensors.append(t.to(device=self.device, dtype=torch.float32).contiguous())
+      tensors.append(t.detach().to(device=self.device, dtype=torch.float32).contiguous())
+    self.upload(tensors)
+
+  def upload(self, tensors):
+    """nfb_set_params of device fp32 tensors in nfb_param_info order, unless the handle holds them already."""
     key = tuple((t.data_ptr(), t._version) for t in tensors)
     if key == self.param_key:
       return
@@ -125,6 +129,157 @@ class _Handle:
     _lib.check(self.lib.nfb_set_params(self.h, ptrs, numels, n, _stream()))
     self.param_key = key
     self._keepalive = tensors  # until the stream has consumed them
+
+
+# ---------------------------------------------------------------------------
+# torch.autograd for model.apply / warp_field.apply (nfb_render_vjp, nfb_warp_vjp)
+# ---------------------------------------------------------------------------
+class _GradInputs:
+  """The tensors a differentiable call hands to its autograd.Function: the parameter leaves of the pytree
+  (`spec_index`: their index in nfb_param_info order) and then the encoded metadata codes (`code_slot`: 0 warp,
+  1 appearance, 2 camera)."""
+
+  def __init__(self, leaves, codes):
+    self.tensors = [t for _, t in leaves] + [t for _, t in codes]
+    self.spec_index = [i for i, _ in leaves]
+    self.code_slot = [k for k, _ in codes]
+
+
+def _grad_inputs(hd, params, codes, prefix=''):
+  """_GradInputs of a call when a parameter leaf (names starting with `prefix`) or a code requires grad, else
+  None: then the call runs as it would without autograd."""
+  leaves = []
+  for i, (name, _, _) in enumerate(hd.param_specs):
+    if not name.startswith(prefix):
+      continue
+    node = params
+    for part in name.split('/'):
+      node = node.get(part) if isinstance(node, Mapping) else None
+    if torch.is_tensor(node):
+      leaves.append((i, node))
+  codes = [(k, t) for k, t in enumerate(codes) if t is not None]
+  if not any(t.requires_grad for _, t in leaves + codes):
+    return None
+  return _GradInputs(leaves, codes)
+
+
+class _VjpState:
+  """What the backward of a differentiable call needs besides the saved tensors."""
+
+  def __init__(self, model, hd, grad_inputs, **kw):
+    self.model = model
+    self.uploaded = hd._keepalive            # the parameters the forward rendered with
+    self.grad_inputs = grad_inputs
+    self.z_c = self.z_f = None
+    self.__dict__.update(kw)
+
+  def handle(self):
+    """The model's handle, holding the forward's parameters and time_alpha again."""
+    m = self.model
+    hd = m.handle(self.B)
+    hd.upload(self.uploaded)
+    m._set_time_alpha(hd, self.time_alpha)
+    return hd
+
+  def grad_buffers(self, hd):
+    """A zeroed flat gradient of every parameter and its per-tensor pointer / numel arrays."""
+    numels = [r * c for _, r, c in hd.param_specs]
+    flat = torch.zeros(sum(numels), device=self.model.device, dtype=torch.float32)
+    n = len(numels)
+    ptrs, off = (ctypes.c_void_p * n)(), 0
+    for i, k in enumerate(numels):
+      ptrs[i] = flat.data_ptr() + 4 * off
+      off += k
+    return flat, ptrs, (ctypes.c_longlong * n)(*numels), n
+
+  def input_grads(self, ctx, hd, flat, code_grads):
+    """The gradients of the Function's tensor inputs (None where not needed), in their shapes and dtypes."""
+    offs, off = [], 0
+    for _, r, c in hd.param_specs:
+      offs.append(off)
+      off += r * c
+    gi, out = self.grad_inputs, []
+    saved = ctx.saved_tensors
+    for j, t in enumerate(saved):
+      if not ctx.needs_input_grad[2 + j]:
+        out.append(None)
+      elif j < len(gi.spec_index):
+        i = gi.spec_index[j]
+        g = flat[offs[i]:offs[i] + t.numel()].view(t.shape)
+        out.append(g.to(device=t.device, dtype=t.dtype))
+      else:
+        out.append(code_grads[gi.code_slot[j - len(gi.spec_index)]])
+    return out
+
+
+def _contig(t):
+  return None if t is None else t.contiguous()
+
+
+class _RenderVjp(torch.autograd.Function):
+  """model.apply as an autograd.Function: the forward is the call's ordinary launches (same values); the
+  backward is nfb_render_vjp at the z values the forward used.  Outputs: out_c, w_c, out_f, w_f and the
+  warped points of the two levels (staged path), None where the call has none."""
+
+  @staticmethod
+  def forward(ctx, st, render, *inputs):
+    ctx.set_materialize_grads(False)
+    out_c, w_c, out_f, w_f, pts, st.z_c, st.z_f = render(True)
+    wp_c = pts['coarse'][1] if 'coarse' in pts else None
+    wp_f = pts['fine'][1] if 'fine' in pts else None
+    ctx.st = st
+    ctx.save_for_backward(*inputs)
+    return out_c, w_c, out_f, w_f, wp_c, wp_f
+
+  @staticmethod
+  @torch.autograd.function.once_differentiable
+  def backward(ctx, d_out_c, d_w_c, d_out_f, d_w_f, d_wp_c, d_wp_f):
+    st = ctx.st
+    m = st.model
+    hd = st.handle()
+    flat, ptrs, numels, n = st.grad_buffers(hd)
+    widths = (m.num_warp_features, m.num_appearance_features, m.num_camera_features)
+    code_grads = [None, None, None]
+    for j, k in enumerate(st.grad_inputs.code_slot):
+      if ctx.needs_input_grad[2 + len(st.grad_inputs.spec_index) + j]:
+        code_grads[k] = torch.zeros(st.B, widths[k], device=m.device)
+    cot = [_contig(t) for t in (d_out_c, d_out_f, d_w_c, d_w_f)]
+    wp = [_contig(t) if st.warps else None for t in (d_wp_c, d_wp_f)]
+    o, d, v = st.rays
+    with torch.cuda.device(m.device):
+      _lib.check(hd.lib.nfb_render_vjp(
+          hd.h, st.B, _ptr(o), _ptr(d), _ptr(v), *[_ptr(t) for t in st.ids], st.alpha, st.flags,
+          _ptr(st.z_c), _ptr(st.z_f), *[_ptr(t) for t in cot + wp], *[_ptr(t) for t in code_grads],
+          int(m.vjp_chunk_rays), ptrs, numels, n, _stream()))
+    return (None, None, *st.input_grads(ctx, hd, flat, code_grads))
+
+
+class _WarpVjp(torch.autograd.Function):
+  """warp_field.apply on free points as an autograd.Function (nfb_warp_vjp)."""
+
+  @staticmethod
+  def forward(ctx, st, render, *inputs):
+    ctx.set_materialize_grads(False)
+    ctx.st = st
+    ctx.save_for_backward(*inputs)
+    return render()
+
+  @staticmethod
+  @torch.autograd.function.once_differentiable
+  def backward(ctx, d_warped):
+    st = ctx.st
+    m = st.model
+    hd = st.handle()
+    flat, ptrs, numels, n = st.grad_buffers(hd)
+    code_grads = [None, None, None]
+    if st.grad_inputs.code_slot and ctx.needs_input_grad[-1]:
+      code_grads[0] = torch.zeros(st.B, m.num_warp_features, device=m.device)
+    if d_warped is not None:
+      d_warped = d_warped.contiguous()
+      with torch.cuda.device(m.device):
+        _lib.check(hd.lib.nfb_warp_vjp(hd.h, st.B, _ptr(st.points), _ptr(st.ids), st.alpha, st.flags,
+                                       _ptr(d_warped), _ptr(code_grads[0]), ptrs, numels, n, _stream()))
+    return (None, None, *st.input_grads(ctx, hd, flat, code_grads))
 
 
 class NerfModel:
@@ -188,6 +343,8 @@ class NerfModel:
     self.precision = precision
     self.train_precision = train_precision
     self.batch_size = int(batch_size)
+    # rays per tape chunk of the backward of a differentiable apply (nfb_render_vjp's chunk_rays)
+    self.vjp_chunk_rays = 256
     if device is None:
       # parameters may be built without a GPU (host-logic tests); apply() needs one.
       device = 'cuda' if torch.cuda.is_available() else 'cpu'
@@ -388,6 +545,13 @@ class NerfModel:
 
     Extra keyword arguments `t_rand` (B,Nc) / `u_rand` (B,Nf) inject the
     uniform draws of the stratified path (used by the parity tests).
+
+    Differentiable like the reference's Flax module: when grad mode is on and a parameter leaf of `variables`
+    (or, with metadata_encoded=True, a metadata code) requires grad, rgb, depth, acc, weights and
+    warped_points carry a grad_fn and `loss.backward()` runs nfb_render_vjp (in the model's train_precision,
+    at the z values this call used, which are constants as in the reference).  med_depth, points and z_vals
+    have no gradient.  In such a call, rays that require grad, warp Jacobians and a second-order backward
+    raise NotImplementedError; without a parameter or code that requires grad the call is the plain one.
     """
     del deterministic, mutable  # unused by the reference's __call__ as well.
     # models.py:345, 367: the coarse level returns Jacobians when either the call or the
@@ -464,41 +628,77 @@ class NerfModel:
     if metadata_encoded:
       flags |= _lib.FLAG_METADATA_ENCODED
     out = {}
-    with torch.cuda.device(dev):
-      out_c = torch.empty(B, 6, device=dev)
-      w_c = torch.empty(B, nc, device=dev)
-      out_f = torch.empty(B, 6, device=dev) if nf > 0 else None
-      w_f = (torch.empty(B, nc + nf, device=dev)
-             if nf > 0 and return_weights else None)
-      if not return_points:
-        _lib.check(lib.nfb_render_forward(
-            h, B, _ptr(origins), _ptr(directions), _ptr(viewdirs),
-            _ptr(warp_id), _ptr(app_id), _ptr(cam_id), alpha, _ptr(t_rand),
-            _ptr(u_rand), flags, _ptr(out_c), _ptr(out_f), _ptr(w_c),
-            _ptr(w_f), None, _stream()))
-        pts = {}
-      else:
-        # staged path: exposes z_vals / warped points of both levels.
-        pts = {}
-        z_c = torch.empty(B, nc, device=dev)
-        _lib.check(lib.nfb_coarse_z_vals(h, B, _ptr(t_rand), _ptr(z_c),
-                                         _stream()))
-        wp_c = torch.empty(B, nc, 3, device=dev)
-        _lib.check(lib.nfb_render_samples(
-            h, 0, B, nc, _ptr(z_c), _ptr(origins), _ptr(directions),
-            _ptr(viewdirs), _ptr(warp_id), _ptr(app_id), _ptr(cam_id), alpha,
-            flags, _ptr(out_c), _ptr(w_c), None, _ptr(wp_c), _stream()))
-        pts['coarse'] = (z_c, wp_c)
-        if nf > 0:
-          z_f = torch.empty(B, nc + nf, device=dev)
-          _lib.check(lib.nfb_sample_pdf(h, B, _ptr(z_c), _ptr(w_c),
-                                        _ptr(u_rand), _ptr(z_f), _stream()))
-          wp_f = torch.empty(B, nc + nf, 3, device=dev)
+    grad_inputs = None
+    if torch.is_grad_enabled() and not _packed:
+      codes = (warp_id, app_id, cam_id) if metadata_encoded else (None, None, None)
+      grad_inputs = _grad_inputs(hd, params, codes)
+    if grad_inputs is not None:
+      if any(t is not None and t.requires_grad for t in (origins, directions, viewdirs)):
+        raise NotImplementedError('model.apply: gradients with respect to the rays (origins, directions, '
+                                  'viewdirs) are not computed')
+      if jac_levels:
+        raise NotImplementedError('model.apply: warp Jacobians are not differentiated; call it with '
+                                  'return_warp_jacobian=False (and a model without use_warp_jacobian)')
+
+    def render(keep_z):
+      """The launches of the call -> (out_c, w_c, out_f, w_f, pts, z_c, z_f).  keep_z: also return the z
+      values of the fast path (z_fine from nfb_render_forward, z_coarse recomputed from t_rand)."""
+      z_c = z_f = None
+      with torch.cuda.device(dev):
+        out_c = torch.empty(B, 6, device=dev)
+        w_c = torch.empty(B, nc, device=dev)
+        out_f = torch.empty(B, 6, device=dev) if nf > 0 else None
+        w_f = (torch.empty(B, nc + nf, device=dev)
+               if nf > 0 and return_weights else None)
+        if not return_points:
+          if keep_z and nf > 0:
+            z_f = torch.empty(B, nc + nf, device=dev)
+          _lib.check(lib.nfb_render_forward(
+              h, B, _ptr(origins), _ptr(directions), _ptr(viewdirs),
+              _ptr(warp_id), _ptr(app_id), _ptr(cam_id), alpha, _ptr(t_rand),
+              _ptr(u_rand), flags, _ptr(out_c), _ptr(out_f), _ptr(w_c),
+              _ptr(w_f), _ptr(z_f), _stream()))
+          if keep_z:
+            z_c = torch.empty(B, nc, device=dev)
+            _lib.check(lib.nfb_coarse_z_vals(h, B, _ptr(t_rand), _ptr(z_c), _stream()))
+          pts = {}
+        else:
+          # staged path: exposes z_vals / warped points of both levels.
+          pts = {}
+          z_c = torch.empty(B, nc, device=dev)
+          _lib.check(lib.nfb_coarse_z_vals(h, B, _ptr(t_rand), _ptr(z_c),
+                                           _stream()))
+          wp_c = torch.empty(B, nc, 3, device=dev)
           _lib.check(lib.nfb_render_samples(
-              h, 1, B, nc + nf, _ptr(z_f), _ptr(origins), _ptr(directions),
+              h, 0, B, nc, _ptr(z_c), _ptr(origins), _ptr(directions),
               _ptr(viewdirs), _ptr(warp_id), _ptr(app_id), _ptr(cam_id), alpha,
-              flags, _ptr(out_f), _ptr(w_f), None, _ptr(wp_f), _stream()))
-          pts['fine'] = (z_f, wp_f)
+              flags, _ptr(out_c), _ptr(w_c), None, _ptr(wp_c), _stream()))
+          pts['coarse'] = (z_c, wp_c)
+          if nf > 0:
+            z_f = torch.empty(B, nc + nf, device=dev)
+            _lib.check(lib.nfb_sample_pdf(h, B, _ptr(z_c), _ptr(w_c),
+                                          _ptr(u_rand), _ptr(z_f), _stream()))
+            wp_f = torch.empty(B, nc + nf, 3, device=dev)
+            _lib.check(lib.nfb_render_samples(
+                h, 1, B, nc + nf, _ptr(z_f), _ptr(origins), _ptr(directions),
+                _ptr(viewdirs), _ptr(warp_id), _ptr(app_id), _ptr(cam_id), alpha,
+                flags, _ptr(out_f), _ptr(w_f), None, _ptr(wp_f), _stream()))
+            pts['fine'] = (z_f, wp_f)
+      return out_c, w_c, out_f, w_f, pts, z_c, z_f
+
+    if grad_inputs is None:
+      out_c, w_c, out_f, w_f, pts, _, _ = render(False)
+    else:
+      st = _VjpState(self, hd, grad_inputs, B=B, alpha=alpha, time_alpha=time_alpha, flags=flags,
+                     rays=(origins, directions, viewdirs),
+                     ids=tuple(None if t is None else t.detach() for t in (warp_id, app_id, cam_id)),
+                     warps=use_warp)
+      out_c, w_c, out_f, w_f, wp_c, wp_f = _RenderVjp.apply(st, render, *grad_inputs.tensors)
+      pts = {}
+      if return_points:
+        pts['coarse'] = (st.z_c, wp_c)
+        if nf > 0:
+          pts['fine'] = (st.z_f, wp_f)
 
     def pack(o, w, level):
       ret = {'rgb': o[:, 0:3], 'depth': o[:, 3], 'med_depth': o[:, 4],
@@ -618,13 +818,34 @@ class WarpField:
       ids, flags = _prep_ids(torch.as_tensor(metadata).reshape(P, -1), dev), 0
     hd = m.handle(P)
     p = variables['params']
-    hd.set_params(p if 'warp_field' in p else {'warp_field': p}, partial=True)
+    tree = p if 'warp_field' in p else {'warp_field': p}
+    hd.set_params(tree, partial=True)
     m._set_time_alpha(hd, extra.get('time_alpha'))
-    out = torch.empty_like(pts)
+    grad_inputs = None
+    if torch.is_grad_enabled():
+      grad_inputs = _grad_inputs(hd, tree, (ids if metadata_encoded else None,), prefix='warp_field/')
+    if grad_inputs is not None:
+      if pts.requires_grad:
+        raise NotImplementedError('warp_field.apply: gradients with respect to the points are not computed')
+      if return_jacobian:
+        raise NotImplementedError('warp_field.apply: the warp Jacobian is not differentiated; call it with '
+                                  'return_jacobian=False')
+
+    def render():
+      out = torch.empty_like(pts)
+      with torch.cuda.device(dev):
+        _lib.check(hd.lib.nfb_warp_forward(
+            hd.h, P, _ptr(pts), _ptr(ids), float(extra.get('alpha', 0.0)), flags,
+            _ptr(out), _stream()))
+      return out
+
+    if grad_inputs is None:
+      out = render()
+    else:
+      st = _VjpState(m, hd, grad_inputs, B=P, alpha=float(extra.get('alpha', 0.0)),
+                     time_alpha=extra.get('time_alpha'), flags=flags, points=pts.detach(), ids=ids.detach())
+      out = _WarpVjp.apply(st, render, *grad_inputs.tensors)
     with torch.cuda.device(dev):
-      _lib.check(hd.lib.nfb_warp_forward(
-          hd.h, P, _ptr(pts), _ptr(ids), float(extra.get('alpha', 0.0)), flags,
-          _ptr(out), _stream()))
       ret = {'warped_points': out.reshape(shape)}
       if return_jacobian:                                  # warping.py:385-387
         jac = torch.empty(P, 3, 3, device=dev)
