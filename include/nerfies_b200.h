@@ -394,6 +394,40 @@ int nfb_image_metrics(int num_images, int height, int width, int channels,
  * handle, ordered on `stream`. */
 int nfb_image_quantize(const float* src, long long n, int bits, float scale, void* dst, void* stream);
 
+/* Colour maps: visualization.colorize (visualization.py:177-219) on the device, value for value
+ * what numpy 2 computes, as float64 (height, width, 3) or, through image_utils.image_to_uint8
+ * (image_utils.py:114-121), as uint8.  The value of pixel p comes from `source`:
+ *   NFB_VIZ_VALUE       a[p]                                    (a: height * width float32)
+ *   NFB_VIZ_RECIPROCAL  1 / a[p], IEEE                           (disparity, eval.py:94-95)
+ *   NFB_VIZ_ABS_ERROR   (|a0 - b0| + |a1 - b1|) + |a2 - b2|      (a, b: (height, width, 3),
+ *   NFB_VIZ_SQ_ERROR    the same with squares                     eval.py:129-132)
+ *   NFB_VIZ_RGB         not a colour map: a is an (height, width, 3) image written as uint8 with a
+ *                       float64 product, trunc(clip((double) a * 255, 0, 255)) (uint8 output only)
+ * Scale: x = (v - cmin) / d in float32 with cmin rounded to float32.  Without the frame flags,
+ * `d` is the divisor float32(max(cmax - cmin, eps)) computed by the caller (its subtraction is fp64
+ * when the bounds are Python floats) and cmax is unused.  With NFB_VIZ_FRAME_MIN / _MAX the bound is
+ * the frame's min / max of the source (NaN if the frame holds a NaN, as np.min), found by a first
+ * launch into `workspace` (NFB_VIZ_WORKSPACE_BYTES, 4-byte aligned), and `d` must be float32(eps):
+ * the divisor is then max(cmax - cmin, eps) in float32.  NFB_VIZ_INVERT maps 1 - x.  Then
+ * t = 255 * y, a = floor(t), b = min(a + 1, 255), colour = table[a] + (table[b] - table[a]) * (t - a)
+ * in float64; x > 1 gives 1.0 (0.0 inverted), x < 0 gives 0.0 (1.0 inverted), NaN a NaN colour
+ * (0 as uint8).  `table`: device (256, 3) float64, row-major.
+ * Output: out_f64 (height * width * 3, contiguous) or out_u8, exactly one of them.  Row r of out_u8
+ * starts at out_u8 + r * pitch bytes (pitch >= 3 * width; pass the column offset in the pointer).
+ * At most two launches, no allocation, no host synchronisation, ordered on `stream`. */
+#define NFB_VIZ_VALUE      0
+#define NFB_VIZ_RECIPROCAL 1
+#define NFB_VIZ_ABS_ERROR  2
+#define NFB_VIZ_SQ_ERROR   3
+#define NFB_VIZ_RGB        4
+#define NFB_VIZ_INVERT     1
+#define NFB_VIZ_FRAME_MIN  2
+#define NFB_VIZ_FRAME_MAX  4
+#define NFB_VIZ_WORKSPACE_BYTES 2048
+int nfb_colorize(const float* a, const float* b, int height, int width, int source, const double* table,
+                 float cmin, float cmax, float d, int flags, void* workspace, double* out_f64,
+                 unsigned char* out_u8, long long pitch, void* stream);
+
 /* Test hook for the abort path described in the conventions above: while enabled,
  * the weight producer of the tensor-core kernel first waits on an mbarrier that never
  * completes, so the launch must time out, drain and raise the abort flag

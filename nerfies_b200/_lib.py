@@ -22,7 +22,7 @@ SYMBOLS = [
     'nfb_train_value_and_grad_reg', 'nfb_warp_jacobian', 'nfb_check_abort', 'nfb_reset_abort',
     'nfb_image_metrics_workspace_size', 'nfb_image_metrics', 'nfb_gather_rays', 'nfb_selftest_sgemm',
     'nfb_set_train_precision', 'nfb_selftest_train_gemm', 'nfb_debug_one_row_block',
-    'nfb_image_quantize', 'nfb_render_vjp', 'nfb_warp_vjp',
+    'nfb_image_quantize', 'nfb_render_vjp', 'nfb_warp_vjp', 'nfb_colorize',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -217,6 +217,8 @@ def load():
   lib.nfb_image_metrics.restype = ci
   lib.nfb_image_quantize.argtypes = [vp, ll, ci, cf, vp, vp]
   lib.nfb_image_quantize.restype = ci
+  lib.nfb_colorize.argtypes = [vp, vp, ci, ci, ci, vp, cf, cf, cf, ci, vp, vp, vp, ll, vp]
+  lib.nfb_colorize.restype = ci
   lib.nfb_selftest_gemm3.argtypes =[ci, ci, vp, vp, vp, ci, vp, vp]
   lib.nfb_selftest_gemm3.restype = ci
   lib.nfb_selftest_sgemm.argtypes = [ci, ll, ci, ci, ci, ci, vp, ci, vp, ci, vp, ci] + [vp] * 6 + [

@@ -18,6 +18,7 @@
 #include "camera_kernels.cuh"
 #include "metrics_kernels.cuh"
 #include "image_kernels.cuh"
+#include "viz_kernels.cuh"
 #include "tc_common.cuh"
 #include "tc_selftest.cuh"
 #include "field_tc.cuh"
@@ -770,6 +771,42 @@ int nfb_image_quantize(const float* src, long long n, int bits, float scale, voi
         src, n, vec, scale, static_cast<unsigned short*>(dst));
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail("image_quantize_kernel launch failed: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+int nfb_colorize(const float* a, const float* b, int height, int width, int source, const double* table,
+                 float cmin, float cmax, float d, int flags, void* workspace, double* out_f64,
+                 unsigned char* out_u8, long long pitch, void* stream) {
+  using namespace nfb::viz;
+  if (source < NFB_VIZ_VALUE || source > NFB_VIZ_RGB) return fail("nfb_colorize: unknown source %d", source);
+  if (height < 0 || width < 0) return fail("nfb_colorize: negative shape %d x %d", height, width);
+  if (flags & ~(kInvert | kFrameMin | kFrameMax)) return fail("nfb_colorize: unknown flags 0x%x", flags);
+  if ((long long)height * width == 0) return 0;
+  if ((out_f64 == nullptr) == (out_u8 == nullptr)) return fail("nfb_colorize: pass exactly one of out_f64 and out_u8");
+  if (source == NFB_VIZ_RGB && out_f64) return fail("nfb_colorize: the rgb source writes uint8 only");
+  if (out_u8 && pitch < 3ll * width) return fail("nfb_colorize: pitch %lld is below 3 * width = %lld", pitch, 3ll * width);
+  if ((long long)height * (3 * width / 16 + 2) >= (1ll << 31)) return fail("nfb_colorize: frame too large");
+  const bool frame = flags & (kFrameMin | kFrameMax);
+  if (source != NFB_VIZ_RGB && !(d > 0.0f)) return fail("nfb_colorize: d must be positive (it is a divisor or eps)");
+  int dev = 0, sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return fail("no CUDA device: nerfies_b200 has no CPU path");
+  const bool two = source == NFB_VIZ_ABS_ERROR || source == NFB_VIZ_SQ_ERROR;
+  if (!a || (two && !b) || (source != NFB_VIZ_RGB && !table) || (frame && !workspace)) return fail("null argument");
+  if (((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(workspace)) & 3) ||
+      (reinterpret_cast<uintptr_t>(table) | reinterpret_cast<uintptr_t>(out_f64)) & 7)
+    return fail("nfb_colorize: misaligned pointer");
+  float* partials = static_cast<float*>(workspace);
+  cudaStream_t s = (cudaStream_t)stream;
+  switch (source) {
+    case NFB_VIZ_VALUE: nfb::viz::launch<kValue>(a, b, height, width, table, cmin, cmax, d, flags, partials, out_f64, out_u8, pitch, sms, s); break;
+    case NFB_VIZ_RECIPROCAL: nfb::viz::launch<kReciprocal>(a, b, height, width, table, cmin, cmax, d, flags, partials, out_f64, out_u8, pitch, sms, s); break;
+    case NFB_VIZ_ABS_ERROR: nfb::viz::launch<kAbsError>(a, b, height, width, table, cmin, cmax, d, flags, partials, out_f64, out_u8, pitch, sms, s); break;
+    case NFB_VIZ_SQ_ERROR: nfb::viz::launch<kSqError>(a, b, height, width, table, cmin, cmax, d, flags, partials, out_f64, out_u8, pitch, sms, s); break;
+    default: nfb::viz::launch<kRgb>(a, b, height, width, table, cmin, cmax, d, flags & kInvert, partials, out_f64, out_u8, pitch, sms, s); break;
+  }
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("colorize launch failed: %s", cudaGetErrorString(e));
   return 0;
 }
 

@@ -8,16 +8,21 @@ sets renders the chosen items with `evaluation.render_frame`, scores them with
 `metrics-eval/{mse,psnr,ssim}/{tag}` (eval.py:205-214).  With `EvalConfig.save_output`,
 `rgb_<id>.png` (8 bit) and `depth_expected_<id>.png`, `depth_median_<id>.png` (16 bit, depth / 1000
 as image_utils.save_depth) go to `<exp_dir>/renders/<step, 8 digits>/<tag>/` (eval.py:97-109, 166).
+With `--save_viz`, each frame also writes the colour-mapped images of eval.py:87-109, 129-132
+(`visualization.colorize_uint8`, magma): `depth_expected_viz_`, `depth_median_viz_` (the reference's
+two files), and the images the reference sends to TensorBoard, `disparity_expected_viz_`,
+`disparity_median_viz_`, `acc_viz_` and, for items with a target, `rgb_abs_error_viz_` and
+`rgb_sq_error_viz_<id>.png`.
 Frames are quantised on the device (`nfb_image_quantize`), copied to pinned host memory without
 blocking, and PNG-encoded by a worker thread while the next frame renders; every worker is joined
 before `evaluate` returns.
 
-Not written: the colour-mapped `*_viz` files (visualization.colorize needs matplotlib's colour
-tables) and TensorBoard images and scalars (TensorBoard is not a dependency; the scalars are in
-eval.jsonl).  Test cameras are rendered and saved but not scored, as in the reference.  Frames
+Not written: TensorBoard images and scalars (TensorBoard is not a dependency; the scalars are in
+eval.jsonl).  The colour tables are OpenCV's (see `visualization`).  Test cameras are rendered and saved but not scored, as in the reference.  Frames
 smaller than 161 pixels on a side have no MS-SSIM: `ssim` is left out for them, with one notice.
 """
 import concurrent.futures
+import functools
 import os
 import shutil
 import sys
@@ -32,6 +37,7 @@ from nerfies_b200 import driver_utils
 from nerfies_b200 import evaluation
 from nerfies_b200 import model_utils
 from nerfies_b200 import models
+from nerfies_b200 import visualization
 
 
 def strided_subset(sequence, count):
@@ -77,14 +83,30 @@ def choose_test_metadata(datasource, step):
   return metadata
 
 
-def render_and_score(model, params, camera, warp_extra, metadata, rgb_target):
+def viz_images(render, rgb_target, near, far):
+  """The colour-mapped images of eval.py:87-96, 129-132 as uint8 device images, by file stem."""
+  viz = visualization.colorize_uint8
+  images = {'depth_expected_viz': viz(render['depth'], near, far, invert=True),
+            'depth_median_viz': viz(render['med_depth'], near, far, invert=True),
+            'disparity_expected_viz': viz(render['depth'], source='reciprocal'),
+            'disparity_median_viz': viz(render['med_depth'], source='reciprocal'),
+            'acc_viz': viz(render['acc'], 0.0, 1.0)}
+  if rgb_target is not None:
+    images['rgb_abs_error_viz'] = viz(rgb_target, 0, 1, source='abs_error', target=render['rgb'])
+    images['rgb_sq_error_viz'] = viz(rgb_target, 0, 1, source='sq_error', target=render['rgb'])
+  return images
+
+
+def render_and_score(model, params, camera, warp_extra, metadata, rgb_target, viz_range=None):
   """One frame on the GPU: ({file stem: uint8 / uint16 device image}, {metric: 0-d device tensor}).
-  The images are what eval.py:99-108 saves; the metrics eval.py:118-125's, without `ssim` for
-  frames MS-SSIM cannot take."""
+  The images are what eval.py:99-108 saves, plus `viz_images` when `viz_range` is the scene's
+  (near, far); the metrics eval.py:118-125's, without `ssim` for frames MS-SSIM cannot take."""
   render = evaluation.render_frame(model, params, camera, warp_extra, metadata)
   images = {'rgb': evaluation.image_to_uint8(render['rgb']),
             'depth_expected': evaluation.depth_to_uint16(render['depth']),
             'depth_median': evaluation.depth_to_uint16(render['med_depth'])}
+  if viz_range is not None:
+    images.update(viz_images(render, rgb_target, *viz_range))
   metrics = {}
   if rgb_target is not None:
     if min(rgb_target.shape[:2]) >= evaluation.MIN_METRICS_SIZE:
@@ -162,10 +184,11 @@ def delete_old_renders(render_dir, max_renders):
 
 def evaluate(exp_config, model_config, train_config, eval_config, base_folder, data_dir=None,
              precision='fp16x3', poll_seconds=10.0, datasource=None, construct_fn=models.construct_nerf,
-             frame_fn=render_and_score, log=print):
+             frame_fn=render_and_score, log=print, save_viz=False):
   """Renders and scores checkpoints until `eval_once` is set or step `max_steps` has been rendered.
   Returns the list of steps handled.  `datasource`, `construct_fn` and `frame_fn` replace the data
-  source, the model constructor and the renderer (tests run the loop without a GPU that way)."""
+  source, the model constructor and the renderer (tests run the loop without a GPU that way).
+  `save_viz` passes `viz_range=(near, far)` to `frame_fn`, which then adds the colour-mapped images."""
   rank, world, own_group = driver_utils.init_distributed()
   pool = concurrent.futures.ThreadPoolExecutor(max_workers=2)
   writer = None
@@ -177,6 +200,8 @@ def evaluate(exp_config, model_config, train_config, eval_config, base_folder, d
       writer = driver_utils.ScalarWriter(dirs['summaries'] / 'eval.jsonl')
     if datasource is None:
       datasource = driver_utils.make_datasource(exp_config, model_config, data_dir)
+    if save_viz:
+      frame_fn = functools.partial(frame_fn, viz_range=(datasource.near, datasource.far))
 
     def items_of(ids):                                                           # eval.py:297-300
       return [(i, datasource.load_camera(i), item['metadata'], item['rgb'])
@@ -225,6 +250,8 @@ def evaluate(exp_config, model_config, train_config, eval_config, base_folder, d
 def main(argv=None, poll_seconds=10.0):
   parser = driver_utils.make_parser('nerfies_b200.eval', 'fp16x3')
   parser.add_argument('--eval_once', action='store_true', help='sets EvalConfig.eval_once')
+  parser.add_argument('--save_viz', action='store_true',
+                      help='also write the colour-mapped depth, disparity, accumulation and error images')
   args = parser.parse_args(argv)
   driver_utils.parse_configs(args.gin_configs, args.gin_bindings)
   exp_config = configs.ExperimentConfig()                                        # eval.py:238-241
@@ -236,7 +263,7 @@ def main(argv=None, poll_seconds=10.0):
   if args.eval_once:
     eval_config.eval_once = True
   evaluate(exp_config, model_config, train_config, eval_config, args.base_folder, args.data_dir,
-           precision=args.precision, poll_seconds=poll_seconds)
+           precision=args.precision, poll_seconds=poll_seconds, save_viz=args.save_viz)
   return 0
 
 
