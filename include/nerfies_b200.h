@@ -428,6 +428,47 @@ int nfb_colorize(const float* a, const float* b, int height, int width, int sour
                  float cmin, float cmax, float d, int flags, void* workspace, double* out_f64,
                  unsigned char* out_u8, long long pitch, void* stream);
 
+/* ---- capture processing (notebooks/Nerfies_Capture_Processing.ipynb) ----------------------
+ * No handle, no allocation, ordered on `stream`.
+ *
+ * Image pyramid of one uint8 RGB frame (the notebook's "Resize images into different scales"):
+ * src is (height, width, 3) with rows `src_pitch` bytes apart, already cropped to a multiple of the
+ * largest scale (make_divisible: pass the crop's height and width with the full frame's pitch).
+ * Level l is dst[l] (height / scales[l], width / scales[l], 3), contiguous: scale 1 copies the
+ * frame; an even scale s gives each output pixel (a + b + c + d + 2) >> 2 over the 2x2 source block
+ * at offsets s/2 - 1 and s/2, byte for byte what cv2.resize(image, (w, h)) with its default
+ * INTER_LINEAR writes.  Every scale must divide the largest; at most 8 levels.  `scales` and `dst`
+ * are host arrays (the pointers in dst are device pointers).  One launch; the frame is read once. */
+int nfb_frame_pyramid(const unsigned char* src, int height, int width, long long src_pitch, int num_levels,
+                      const int* scales, unsigned char* const* dst, void* stream);
+
+/* Blur scores of num_frames (height, width, 3) uint8 RGB frames, contiguous: per frame,
+ * cv2.Laplacian(cv2.cvtColor(rgb, COLOR_RGB2GRAY), CV_64F).var() into scores (num_frames) float64.
+ * The Laplacian's integer sum and sum of squares are exact (int64), the variance one fp64 division
+ * of an exact 128-bit numerator.  workspace: device, 8-byte aligned, at least
+ * nfb_blur_scores_workspace_size bytes.  Two launches and one memset. */
+long long nfb_blur_scores_workspace_size(int num_frames);
+int nfb_blur_scores(const unsigned char* frames, int num_frames, int height, int width, void* workspace,
+                    long long workspace_bytes, double* scores, void* stream);
+
+/* Camera.project (camera.py:283-315) of float32 points (n, 3) -> pixels (n, 2), in float32
+ * arithmetic operation for operation as numpy evaluates it.  `cam` is a host struct. */
+int nfb_camera_project(const nfb_camera* cam, const float* points, long long n, float* pixels, void* stream);
+
+/* Per-camera near/far planes of the notebook's estimate_near_far_for_image: for camera c, the
+ * float64 points (num_points, 3) are projected in fp64 (the camera's float32 fields widened, as numpy
+ * promotes them); those with 0 <= px <= width, 0 <= py <= height and depth > 0 are kept, and
+ *   near[c] = np.quantile(depths, q_near), far[c] = np.quantile(depths, q_far)   ('linear' rule)
+ * counts[c] = the number kept; near and far are NaN where it is 0.  `cameras` is a DEVICE array of
+ * num_cameras structs.  The quantiles come from exact order statistics (radix select over the depths'
+ * bit patterns), so no depth array is formed: the workspace (device, 256-byte aligned, at least
+ * nfb_near_far_workspace_size bytes) grows with the cameras only.  17 launches and one memset; no
+ * host synchronisation. */
+long long nfb_near_far_workspace_size(int num_cameras);
+int nfb_near_far(const nfb_camera* cameras, int num_cameras, const double* points, long long num_points,
+                 double q_near, double q_far, void* workspace, long long workspace_bytes, double* near,
+                 double* far, long long* counts, void* stream);
+
 /* Test hook for the abort path described in the conventions above: while enabled,
  * the weight producer of the tensor-core kernel first waits on an mbarrier that never
  * completes, so the launch must time out, drain and raise the abort flag

@@ -23,6 +23,8 @@ SYMBOLS = [
     'nfb_image_metrics_workspace_size', 'nfb_image_metrics', 'nfb_gather_rays', 'nfb_selftest_sgemm',
     'nfb_set_train_precision', 'nfb_selftest_train_gemm', 'nfb_debug_one_row_block',
     'nfb_image_quantize', 'nfb_render_vjp', 'nfb_warp_vjp', 'nfb_colorize',
+    'nfb_frame_pyramid', 'nfb_blur_scores_workspace_size', 'nfb_blur_scores', 'nfb_camera_project',
+    'nfb_near_far_workspace_size', 'nfb_near_far',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -219,6 +221,18 @@ def load():
   lib.nfb_image_quantize.restype = ci
   lib.nfb_colorize.argtypes = [vp, vp, ci, ci, ci, vp, cf, cf, cf, ci, vp, vp, vp, ll, vp]
   lib.nfb_colorize.restype = ci
+  lib.nfb_frame_pyramid.argtypes = [vp, ci, ci, ll, ci, ctypes.POINTER(ci), ctypes.POINTER(vp), vp]
+  lib.nfb_frame_pyramid.restype = ci
+  lib.nfb_blur_scores_workspace_size.argtypes = [ci]
+  lib.nfb_blur_scores_workspace_size.restype = ll
+  lib.nfb_blur_scores.argtypes = [vp, ci, ci, ci, vp, ll, vp, vp]
+  lib.nfb_blur_scores.restype = ci
+  lib.nfb_camera_project.argtypes = [ctypes.POINTER(NfbCamera), vp, ll, vp, vp]
+  lib.nfb_camera_project.restype = ci
+  lib.nfb_near_far_workspace_size.argtypes = [ci]
+  lib.nfb_near_far_workspace_size.restype = ll
+  lib.nfb_near_far.argtypes = [vp, ci, vp, ll, ctypes.c_double, ctypes.c_double, vp, ll, vp, vp, vp, vp]
+  lib.nfb_near_far.restype = ci
   lib.nfb_selftest_gemm3.argtypes =[ci, ci, vp, vp, vp, ci, vp, vp]
   lib.nfb_selftest_gemm3.restype = ci
   lib.nfb_selftest_sgemm.argtypes = [ci, ll, ci, ci, ci, ci, vp, ci, vp, ci, vp, ci] + [vp] * 6 + [

@@ -90,6 +90,34 @@ class Camera:
     params['image_size'] = np.array([int(round(float(n) * scale)) for n in self.image_size])
     return Camera(**params)
 
+  def points_to_local_points(self, points):
+    """World points (..., 3) in the camera frame, on the host (camera.py:279-282)."""
+    points = np.asarray(points)
+    return np.matmul(self.orientation, (points - self.position).reshape(-1, 3).T).T.reshape(points.shape)
+
+  def look_at(self, position, look_at, up, eps=1e-6):
+    """A copy of the camera at `position` looking at `look_at` with `up` along the image's -y
+    (camera.py:342-387).  The rotation is computed in float64 and stored as float32."""
+    position = np.asarray(position, np.float64)
+    optical_axis = np.asarray(look_at, np.float64) - position
+    norm = np.linalg.norm(optical_axis)
+    if norm < eps:
+      raise ValueError('The camera center and look at position are too close.')
+    optical_axis /= norm
+    right_vector = np.cross(optical_axis, up)
+    norm = np.linalg.norm(right_vector)
+    if norm < eps:
+      raise ValueError('The up-vector is parallel to the optical axis.')
+    right_vector /= norm
+    camera_rotation = np.identity(3)
+    camera_rotation[0, :] = right_vector
+    camera_rotation[1, :] = np.cross(optical_axis, right_vector)
+    camera_rotation[2, :] = optical_axis
+    look_at_camera = self.copy()
+    look_at_camera.position = position.astype(np.float32)
+    look_at_camera.orientation = camera_rotation.astype(np.float32)
+    return look_at_camera
+
   # ---- the C-ABI view ----
   def _struct(self):
     c = _lib.NfbCamera()
@@ -125,6 +153,26 @@ class Camera:
       _lib.check(lib.nfb_pixels_to_rays(ctypes.byref(self._struct()), _ptr(flat), flat.shape[0],
                                         _ptr(out), _stream(pixels.device)))
     return out.reshape(*batch_shape, 3)
+
+  def project(self, points):
+    """Pixel positions (..., 2) of float32 world points (..., 3) on a CUDA device
+    (camera.py:283-315), in float32 arithmetic as the reference's numpy computes it."""
+    if not torch.is_tensor(points):
+      raise TypeError('points must be a torch tensor on a CUDA device')
+    if points.shape[-1] != 3:
+      raise ValueError('The last dimension of points must be 3.')
+    if points.dtype != torch.float32:
+      raise ValueError(f'points dtype ({points.dtype!r}) must match camera dtype (float32)')
+    if not points.is_cuda:
+      raise ValueError('points must live on a CUDA device: nerfies_b200 has no CPU path')
+    lib = _lib.load()
+    batch_shape = points.shape[:-1]
+    flat = points.reshape(-1, 3).contiguous()
+    out = torch.empty(flat.shape[0], 2, dtype=torch.float32, device=points.device)
+    with torch.cuda.device(points.device):
+      _lib.check(lib.nfb_camera_project(ctypes.byref(self._struct()), _ptr(flat), flat.shape[0], _ptr(out),
+                                        _stream(points.device)))
+    return out.reshape(*batch_shape, 2)
 
   def get_pixel_centers(self, device):
     """Pixel centres (H, W, 2) on `device` (camera.py:317-321)."""

@@ -88,6 +88,48 @@ __device__ __forceinline__ void camera_pixel_direction(const nfb_camera& c, int 
   out_d[0] = d[0]; out_d[1] = d[1]; out_d[2] = d[2];
 }
 
+// Camera.project (camera.py:279-315) of the world point (X, Y, Z) in arithmetic T, written operation
+// for operation as numpy evaluates it: T = float is float32 numpy on float32 points; T = double is
+// float64 points against the camera's float32 fields, which numpy widens per operation.  Products of
+// two camera fields (2 * p1, focal * aspect) stay float32 as numpy computes them on float32 scalars.
+// Returns the pixel position and the local depth (points_to_local_points(.)[..., 2]).  The elementwise
+// operations keep each a*b+c at two roundings (the build's -fmad=false), as numpy's ufuncs do.  The
+// rotation is np.matmul, which numpy hands to BLAS: OpenBLAS's x86-64 GEMM kernels accumulate the
+// three products as fma(o2, t2, fma(o1, t1, o0 * t0)), and that chain reproduces the recorded
+// projections (tests/golden/camera_*.npz) bit for bit where two roundings per step miss by up to 384 ulp.
+template <typename T>
+__device__ __forceinline__ void camera_project_point(const nfb_camera& c, T X, T Y, T Z, T& px, T& py,
+                                                     T& depth) {
+  const T t0 = X - (T)c.position[0], t1 = Y - (T)c.position[1], t2 = Z - (T)c.position[2];   // camera.py:280
+  T l[3];
+#pragma unroll
+  for (int i = 0; i < 3; ++i)                                                               // camera.py:281
+    l[i] = fma((T)c.orientation[3 * i + 2], t2, fma((T)c.orientation[3 * i + 1], t1, (T)c.orientation[3 * i] * t0));
+  const T x = l[0] / l[2], y = l[1] / l[2];                                                 // camera.py:291-292
+  const T r2 = x * x + y * y;
+  const T k1 = (T)c.radial_distortion[0], k2 = (T)c.radial_distortion[1], k3 = (T)c.radial_distortion[2];
+  const T d = (T)1 + r2 * (k1 + r2 * (k2 + k3 * r2));                                       // camera.py:296-298
+  const T xy = x * y;
+  const float p1 = c.tangential_distortion[0], p2 = c.tangential_distortion[1];
+  const T xd = x * d + (T)(2.f * p1) * xy + (T)p2 * (r2 + (T)2 * (x * x));                  // camera.py:302-304
+  const T yd = y * d + (T)(2.f * p2) * xy + (T)p1 * (r2 + (T)2 * (y * y));                  // camera.py:305-307
+  px = (T)c.focal_length * xd + (T)c.skew * yd + (T)c.principal_point[0];                   // camera.py:310
+  py = (T)(c.focal_length * c.pixel_aspect_ratio) * yd + (T)c.principal_point[1];           // camera.py:311-312
+  depth = l[2];
+}
+
+// Camera.project of float32 points (n, 3) -> pixels (n, 2), float32 throughout.
+__global__ void __launch_bounds__(256) camera_project_kernel(const nfb_camera c, const float* __restrict__ points,
+                                                             long long n, float* __restrict__ pixels) {
+  const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (i >= n) return;
+  float px, py, depth;
+  camera_project_point<float>(c, __ldg(points + 3 * i), __ldg(points + 3 * i + 1), __ldg(points + 3 * i + 2),
+                              px, py, depth);
+  pixels[2 * i] = px;
+  pixels[2 * i + 1] = py;
+}
+
 // One pixel of CameraArgs: unit world-space direction and the pixel position used.
 __device__ __forceinline__ void camera_ray_of_pixel(const CameraArgs& a, long long i, float* out_d, float* out_p) {
   float px, py;

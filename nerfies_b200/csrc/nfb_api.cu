@@ -19,6 +19,7 @@
 #include "metrics_kernels.cuh"
 #include "image_kernels.cuh"
 #include "viz_kernels.cuh"
+#include "capture_kernels.cuh"
 #include "tc_common.cuh"
 #include "tc_selftest.cuh"
 #include "field_tc.cuh"
@@ -771,6 +772,138 @@ int nfb_image_quantize(const float* src, long long n, int bits, float scale, voi
         src, n, vec, scale, static_cast<unsigned short*>(dst));
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail("image_quantize_kernel launch failed: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+static int device_sms(int* sms) {
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return fail("no CUDA device: nerfies_b200 has no CPU path");
+  return 0;
+}
+
+int nfb_frame_pyramid(const unsigned char* src, int height, int width, long long src_pitch, int num_levels,
+                      const int* scales, unsigned char* const* dst, void* stream) {
+  using namespace nfb::capture;
+  if (num_levels < 1 || num_levels > kMaxLevels)
+    return fail("nfb_frame_pyramid: num_levels=%d outside [1, %d]", num_levels, kMaxLevels);
+  if (!src || !scales || !dst) return fail("null argument");
+  PyramidArgs a{};
+  a.src = src; a.src_pitch = src_pitch; a.height = height; a.width = width; a.num_levels = num_levels;
+  int S = 0;
+  for (int l = 0; l < num_levels; ++l) {
+    const int s = scales[l];
+    if (s < 1 || (s != 1 && s % 2)) return fail("nfb_frame_pyramid: scale %d is neither 1 nor even", s);
+    if (!dst[l]) return fail("null argument");
+    a.scale[l] = s; a.dst[l] = dst[l];
+    S = std::max(S, s);
+  }
+  for (int l = 0; l < num_levels; ++l)
+    if (S % a.scale[l]) return fail("nfb_frame_pyramid: scale %d does not divide the largest scale %d", a.scale[l], S);
+  if (height < S || width < S || height % S || width % S)
+    return fail("nfb_frame_pyramid: frame %d x %d is not a positive multiple of the largest scale %d", height, width, S);
+  if (src_pitch < 3ll * width) return fail("nfb_frame_pyramid: src_pitch %lld is below 3 * width", src_pitch);
+  a.max_scale = S;
+  int sms = 0;
+  if (device_sms(&sms)) return -1;
+  const long long blocks = ((long long)(height / S) * (width / S) + 255) / 256;
+  nfb::capture::frame_pyramid_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("frame_pyramid_kernel launch failed: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+long long nfb_blur_scores_workspace_size(int num_frames) {
+  if (num_frames < 0) return fail("nfb_blur_scores: negative frame count %d", num_frames);
+  return 16ll * num_frames;
+}
+
+int nfb_blur_scores(const unsigned char* frames, int num_frames, int height, int width, void* workspace,
+                    long long workspace_bytes, double* scores, void* stream) {
+  using namespace nfb::capture;
+  if (num_frames < 0 || num_frames > 65535) return fail("nfb_blur_scores: num_frames=%d outside [0, 65535]", num_frames);
+  if (height < 1 || width < 1) return fail("nfb_blur_scores: frame size %d x %d must be positive", height, width);
+  if (num_frames == 0) return 0;
+  if (!frames || !scores || !workspace) return fail("null argument");
+  if (workspace_bytes < 16ll * num_frames)
+    return fail("nfb_blur_scores: workspace of %lld bytes is smaller than the %lld bytes needed", workspace_bytes,
+                16ll * num_frames);
+  if ((reinterpret_cast<uintptr_t>(workspace) | reinterpret_cast<uintptr_t>(scores)) & 7)
+    return fail("nfb_blur_scores: workspace and scores must be 8-byte aligned");
+  int sms = 0;
+  if (device_sms(&sms)) return -1;
+  cudaStream_t s = (cudaStream_t)stream;
+  BlurArgs a{};
+  a.frames = frames; a.num_frames = num_frames; a.height = height; a.width = width;
+  a.sums = static_cast<unsigned long long*>(workspace); a.scores = scores;
+  cudaError_t e = cudaMemsetAsync(workspace, 0, 16ll * num_frames, s);
+  if (e != cudaSuccess) return fail("nfb_blur_scores: memset failed: %s", cudaGetErrorString(e));
+  const long long pixels = (long long)height * width;
+  const long long per_frame = std::max(1ll, std::min((pixels + 2047) / 2048, std::max(1ll, 8ll * sms / num_frames)));
+  blur_sums_kernel<<<dim3((unsigned)per_frame, num_frames), 256, 0, s>>>(a);
+  blur_finalize_kernel<<<(num_frames + 127) / 128, 128, 0, s>>>(a);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("blur score launch failed: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+int nfb_camera_project(const nfb_camera* cam, const float* points, long long n, float* pixels, void* stream) {
+  if (!cam) return fail("null argument");
+  if (n < 0) return fail("nfb_camera_project: negative point count %lld", n);
+  int sms = 0;
+  if (device_sms(&sms)) return -1;
+  if (n == 0) return 0;
+  if (!points || !pixels) return fail("null argument");
+  nfb::camera_project_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(*cam, points, n, pixels);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("camera_project_kernel launch failed: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+// Workspace of nfb_near_far: the histograms, then the selection state, each 256-byte aligned.
+static long long near_far_hist_bytes(int C) {
+  using namespace nfb::capture;
+  return ((long long)C * kRanks * kBins * sizeof(unsigned int) + 255) / 256 * 256;
+}
+
+long long nfb_near_far_workspace_size(int num_cameras) {
+  if (num_cameras < 1 || num_cameras > 65535) return fail("nfb_near_far: num_cameras=%d outside [1, 65535]", num_cameras);
+  return near_far_hist_bytes(num_cameras) + ((long long)num_cameras * sizeof(nfb::capture::NearFarState) + 255) / 256 * 256;
+}
+
+int nfb_near_far(const nfb_camera* cameras, int num_cameras, const double* points, long long num_points,
+                 double q_near, double q_far, void* workspace, long long workspace_bytes, double* near,
+                 double* far, long long* counts, void* stream) {
+  using namespace nfb::capture;
+  const long long need = nfb_near_far_workspace_size(num_cameras);
+  if (need < 0) return -1;
+  if (num_points < 0) return fail("nfb_near_far: negative point count %lld", num_points);
+  if (!(q_near >= 0.0 && q_near <= 1.0 && q_far >= 0.0 && q_far <= 1.0))
+    return fail("nfb_near_far: quantiles must lie in [0, 1]");
+  if (!cameras || (num_points && !points) || !near || !far || !counts || !workspace) return fail("null argument");
+  if (workspace_bytes < need)
+    return fail("nfb_near_far: workspace of %lld bytes is smaller than the %lld bytes nfb_near_far_workspace_size returns",
+                workspace_bytes, need);
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail("nfb_near_far: workspace must be 256-byte aligned");
+  int sms = 0;
+  if (device_sms(&sms)) return -1;
+  cudaStream_t s = (cudaStream_t)stream;
+  NearFarArgs a{};
+  a.cameras = cameras; a.num_cameras = num_cameras; a.points = points; a.num_points = num_points;
+  a.q[0] = q_near; a.q[1] = q_far;
+  a.hist = static_cast<unsigned int*>(workspace);
+  a.state = reinterpret_cast<NearFarState*>(static_cast<char*>(workspace) + near_far_hist_bytes(num_cameras));
+  a.near = near; a.far = far; a.counts = counts;
+  cudaError_t e = cudaMemsetAsync(a.hist, 0, near_far_hist_bytes(num_cameras), s);
+  if (e != cudaSuccess) return fail("nfb_near_far: memset failed: %s", cudaGetErrorString(e));
+  // Enough blocks per camera to fill the device twice over, each at least 256 points.
+  const long long per_camera = std::max(1ll, std::min((num_points + 255) / 256, (2ll * 8 * sms + num_cameras - 1) / num_cameras));
+  for (int pass = 0; pass < kPasses; ++pass) {
+    near_far_hist_kernel<<<dim3((unsigned)per_camera, num_cameras), 256, 0, s>>>(a, pass);
+    near_far_select_kernel<<<num_cameras, 32, 0, s>>>(a, pass);
+  }
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("near/far launch failed: %s", cudaGetErrorString(e));
   return 0;
 }
 
