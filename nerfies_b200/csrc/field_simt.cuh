@@ -60,6 +60,10 @@ struct FieldArgs {
   float* ray_out;            // (B,6) or nullptr = no fused composite
   float* ray_weights;        // (B,S) or nullptr
   int white_bg, sample_at_infinity;
+  // tensor-core NeRF pass of a model with a bottleneck (ray_bias_kernel): the bias of the layer with
+  // TcStep::ray_bias, (B, 128 n_chunks), and with an alpha condition the alpha head's constant, (B)
+  const float* ray_bias;
+  const float* ray_alpha;
 };
 
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {

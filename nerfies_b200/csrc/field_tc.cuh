@@ -75,19 +75,6 @@ __device__ __forceinline__ void encode_input(uint8_t* in_block, int r, int hs, c
     posenc_fast_to_block(in_block, r, x, F, window, extra, n_extra, 4 * hs, 4 * hs + 4);
   }
 }
-__device__ __forceinline__ void cond_to_block(uint8_t* block, int r, const float* __restrict__ cond,
-                                              int n, int c_begin = 0, int c_end = 8) {
-#pragma unroll 1
-  for (int c = c_begin; c < c_end; ++c) {
-    float v[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int k = c * 8 + j;
-      v[j] = k < n ? __ldg(cond + k) : 0.f;
-    }
-    store_chunk(block, r, c, v);
-  }
-}
 
 // One 128-column accumulator chunk of a hidden layer (this thread's fragment: rows
 // arow, arow + 8; columns c*128 + 8j + 2*lq + {0, 1}) -> + bias, activation, (alpha
@@ -100,8 +87,9 @@ __device__ __forceinline__ void cond_to_block(uint8_t* block, int r, const float
 // v - (hi + lo) <= 2^-23 |v|, the bound of a round-to-nearest split.  ReLU rides on the
 // conversions: for v < 0 both hi and v - hi are <= 0 and convert to +0.  Conversions
 // saturate: |v| > 65504 does not become inf.  kBlkBytes: bytes of one K-block of the tile's
-// activation image (128 or 256 rows).
-template <bool kX3, uint32_t kBlkBytes>
+// activation image (128 or 256 rows).  kRows: bit h set = write row arow + 8h (a layer whose two rows
+// take different biases runs one call per row, so only one bias pointer is live at a time).
+template <bool kX3, uint32_t kBlkBytes, int kRows = 3>
 __device__ __forceinline__ void epi_chunk(const float* acc, int c, const float* __restrict__ bias, float inv_s,
                                           bool relu, bool adot, const float* __restrict__ aw, float& al0,
                                           float& al1, uint8_t* act_hi, uint32_t* lo, int arow, int lq) {
@@ -123,6 +111,7 @@ __device__ __forceinline__ void epi_chunk(const float* acc, int c, const float* 
     const uint32_t blk = (uint32_t)(2 * c + (j >> 3)) * kBlkBytes + 4 * lq;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
+      if (!((kRows >> h) & 1)) continue;
       const uint32_t off = blk + swz_off(arow + 8 * h, j & 7);
       const float a = v[2 * h], bb = v[2 * h + 1];
       uint32_t hi;
@@ -147,16 +136,26 @@ __device__ __forceinline__ void epi_chunk(const float* acc, int c, const float* 
   }
 }
 
-// Per-ray part of the alpha head with an alpha condition: cond . w (bf16 mode: bf16-rounded weights).
+// bf16: the rgb condition into chunks [c_begin, c_end) of row r of the input block.
+__device__ __forceinline__ void cond_to_block(uint8_t* block, int r, const float* __restrict__ cond,
+                                              int n, int c_begin, int c_end) {
+#pragma unroll 1
+  for (int c = c_begin; c < c_end; ++c) {
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int k = c * 8 + j;
+      v[j] = k < n ? __ldg(cond + k) : 0.f;
+    }
+    store_chunk(block, r, c, v);
+  }
+}
+
+// bf16: the per-ray part of the alpha head with an alpha condition, cond . w with bf16-rounded weights.
 // Out of line: it runs once per row and tile, and inlined it costs the hot loop registers.
-template <bool kX3>
 __device__ __noinline__ float alpha_cond_dot(const float* __restrict__ cond, const float* __restrict__ w, int n) {
   float a = 0.f;
-  for (int j = 0; j < n; ++j) {
-    float wj = __ldg(w + j);
-    if constexpr (!kX3) wj = __bfloat162float(__float2bfloat16_rn(wj));
-    a = fmaf(__ldg(cond + j), wj, a);
-  }
+  for (int j = 0; j < n; ++j) a = fmaf(__ldg(cond + j), __bfloat162float(__float2bfloat16_rn(__ldg(w + j))), a);
   return a;
 }
 
@@ -217,7 +216,8 @@ struct RowState {
 constexpr int kWgThreads = 384;
 constexpr int kAlphaOff = 14 * kABlockBytes;          // per-row alpha-head partial (128 floats)
 constexpr int kScanOff = kAlphaOff + 512;             // fused composite: cross-warp partials (40 floats)
-constexpr int kBarOff = kScanOff + 256;
+constexpr int kRayOff = kScanOff + 256;               // NeRF pass: each row's ray (128 ints, TcStep::ray_bias)
+constexpr int kBarOff = kRayOff + 512;
 constexpr int kWgSmemBytes = kBarOff + 256;
 template <bool kX3, int kMB>
 struct WgSmem {
@@ -341,12 +341,11 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
     const int lr = kMB == 2 ? t : (t & 63);              // row within the warpgroup
     const int r = kWgRows * cw + lr;
     const int h0 = kMB == 2 ? 0 : t >> 6, h1 = kMB == 2 ? 2 : h0 + 1;
-    const int cb = h0 * 4, ce = cb + 4;                  // input-block chunks this thread writes (kMB = 1)
     uint8_t* act_hi = base;
     uint8_t* inh = base + Smem::kInOff;
-    uint8_t* inl = inh + kBlk;
     float* alpha_s = reinterpret_cast<float*>(base + kAlphaOff);
     float* scan_s = reinterpret_cast<float*>(base + kScanOff);
+    int* ray_s = reinterpret_cast<int*>(base + kRayOff);
     const uint32_t rows_off = (uint32_t)(kWgRows * cw * kRowBytes); // this warpgroup's rows in a K-block
     // head accumulators, kWgRows x 16 floats over this warpgroup's own rows of activation block 0
     // (the other warpgroup's MMAs may still read its rows)
@@ -371,6 +370,7 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
       if (!row.valid) m = args.num_rows - 1;
       row.m = m;
       row.ray = m / S;
+      if (!warp_pass && h0 == 0) ray_s[r] = (int)row.ray;   // read by the ray_bias epilogue
       const float z = args.z_vals ? __ldg(args.z_vals + m) : 0.f;
       float org[3], dir[3];
 #pragma unroll
@@ -466,19 +466,32 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
           const float* aw = aux + prog.alpha_w_off;
           if constexpr (kMB == 1) {
             float al0 = 0.f, al1 = 0.f;
-            epi_chunk<kX3, kBlk>(acc0, 0, bias, inv_s, relu, adot, aw, al0, al1, act_hi, lo, arow, lq);
-            if (st.n_chunks == 2)
-              epi_chunk<kX3, kBlk>(acc1, 1, bias, inv_s, relu, adot, aw, al0, al1, act_hi, lo, arow, lq);
+            if (kX3 && st.ray_bias) {
+              // the bias of each accumulator row's own ray: a tile of the staged path with S % 128 != 0
+              // spans rays (with the fused composite the tile is one ray)
+              const int cols = 128 * st.n_chunks;
+              const float* rb = args.ray_bias + (size_t)ray_s[arow] * cols;
+              epi_chunk<kX3, kBlk, 1>(acc0, 0, rb, inv_s, relu, false, aw, al0, al1, act_hi, lo, arow, lq);
+              if (st.n_chunks == 2) epi_chunk<kX3, kBlk, 1>(acc1, 1, rb, inv_s, relu, false, aw, al0, al1, act_hi, lo, arow, lq);
+              rb = args.ray_bias + (size_t)ray_s[arow + 8] * cols;
+              epi_chunk<kX3, kBlk, 2>(acc0, 0, rb, inv_s, relu, false, aw, al0, al1, act_hi, lo, arow, lq);
+              if (st.n_chunks == 2) epi_chunk<kX3, kBlk, 2>(acc1, 1, rb, inv_s, relu, false, aw, al0, al1, act_hi, lo, arow, lq);
+            } else {
+              epi_chunk<kX3, kBlk>(acc0, 0, bias, inv_s, relu, adot, aw, al0, al1, act_hi, lo, arow, lq);
+              if (st.n_chunks == 2)
+                epi_chunk<kX3, kBlk>(acc1, 1, bias, inv_s, relu, adot, aw, al0, al1, act_hi, lo, arow, lq);
+            }
             if (adot) {
               // the four threads of a quad hold the row's columns
               al0 += __shfl_xor_sync(0xffffffffu, al0, 1); al0 += __shfl_xor_sync(0xffffffffu, al0, 2);
               al1 += __shfl_xor_sync(0xffffffffu, al1, 1); al1 += __shfl_xor_sync(0xffffffffu, al1, 2);
               if (lq == 0) { alpha_s[arow] = al0; alpha_s[arow + 8] = al1; }
             }
-            if (st.write_cond) {   // the rgb condition: the input block of the next step
-              const float* cond = args.cond + row.ray * prog.cond_stride + prog.rc_off;
-              if constexpr (kX3) tc3::cond_to_block_x3(inh, inl, r, cond, prog.rc, cb, ce);
-              else cond_to_block(inh, r, cond, prog.rc, cb, ce);
+            if constexpr (!kX3) {
+              if (st.write_cond) {   // bf16: the rgb condition, the input block of the next step
+                const float* cond = args.cond + row.ray * prog.cond_stride + prog.rc_off;
+                cond_to_block(inh, r, cond, prog.rc, 4 * h0, 4 * h0 + 4);
+              }
             }
           } else {
             // warp net: one 128-column chunk per row block, no alpha head, no rgb condition
@@ -515,11 +528,19 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
           } else if constexpr (kMB == 1) {
             float4 o;
             o.x = sigmoidf(v[0]); o.y = sigmoidf(v[1]); o.z = sigmoidf(v[2]);
-            // alpha condition (Dense(1) on [bottleneck | alpha condition]): its per-ray part
-            const float a_cond = prog.ac ? alpha_cond_dot<kX3>(args.cond + row.ray * prog.cond_stride + prog.ac_off,
-                                                               aux + prog.alpha_w_off + kAlphaCondOff, prog.ac)
-                                         : 0.f;
-            o.w = apply_act(alpha_b + (alpha_s[r] + a_cond), prog.sigma_act);
+            float a;
+            if constexpr (kX3) {
+              // with an alpha condition the head's bias, the bottleneck's and the condition's terms are one
+              // per-ray constant
+              a = (prog.ac ? __ldg(args.ray_alpha + row.ray) : alpha_b) + alpha_s[r];
+            } else {
+              // bf16: the alpha condition's part of Dense(1) on [bottleneck | alpha condition]
+              const float a_cond = prog.ac ? alpha_cond_dot(args.cond + row.ray * prog.cond_stride + prog.ac_off,
+                                                            aux + prog.alpha_w_off + kAlphaCondOff, prog.ac)
+                                           : 0.f;
+              a = alpha_b + (alpha_s[r] + a_cond);
+            }
+            o.w = apply_act(a, prog.sigma_act);
             if (h0 == 0 && row.valid && args.samples) reinterpret_cast<float4*>(args.samples)[row.m] = o;
             if (fuse && h0 == 0) {
               // ---- volumetric_rendering (model_utils.py:104-136) + median depth (:231-239, 262-263)
@@ -620,17 +641,21 @@ inline int tc_fail(const char* what) {
   return fail("the tensor-core paths (precision bf16 / fp16x3) do not support this model: %s; use precision fp32", what);
 }
 
-inline int build_tc_program(nfb_handle* h, int level, long long* wbytes, long long* aux_floats) {
+inline int build_tc_program(nfb_handle* h, int level, long long* wbytes, long long* aux_floats,
+                            long long* fold_floats) {
   const FieldProgram& fp = h->prog[level];
   TcProgram& tp = h->tcprog[level];
   memset(&tp, 0, sizeof(tp));
+  TcFold& fo = h->tc_fold[level];
+  memset(&fo, 0, sizeof(fo));
   // fp16x3: every unit is [W_hi | W_lo]
   const int wparts = h->cfg.precision == NFB_PREC_FP16X3 ? 2 : 1;
   tp.warp_pivot = fp.warp_pivot; tp.warp_trans = fp.warp_trans;
-  tp.warp_type = fp.warp_type; tp.Fw = fp.Fw; tp.G = fp.G; tp.Fp = fp.Fp; tp.rc = fp.rc;
+  tp.warp_type = fp.warp_type; tp.Fw = fp.Fw; tp.G = fp.G; tp.Fp = fp.Fp;
   tp.cond_stride = fp.cond_stride; tp.sigma_act = fp.sigma_act;
+  tp.tc = fp.tc; tp.ac = fp.ac; tp.rc = fp.rc; tp.ac_off = fp.G + fp.tc; tp.rc_off = fp.G + fp.tc + fp.ac;
   // per-ray condition vector: [glo | trunk | alpha | rgb] (nfb_api.cu: build_programs)
-  tp.tc = fp.tc; tp.ac = fp.ac; tp.ac_off = fp.G + fp.tc; tp.rc_off = fp.G + fp.tc + fp.ac;
+  fo.ac_off = fp.G + fp.tc; fo.rc_off = fp.G + fp.tc + fp.ac;
   if (fp.rc > kBlockK) return tc_fail("rgb condition wider than 64 channels");
   if (fp.ac > kBlockK) return tc_fail("alpha condition wider than 64 channels");
   if (fp.Dp + fp.tc > kBlockK || (fp.warp_type && fp.Dw > kBlockK)) return tc_fail("encoded inputs wider than 64");
@@ -641,8 +666,12 @@ inline int build_tc_program(nfb_handle* h, int level, long long* wbytes, long lo
     h->tc_aux_jobs.push_back({st.b_off, st.n, 1, off});
     return off;
   };
-  auto add = [&](const Step& st, int epi, int cur_width) -> int {
-    if (tp.n_steps >= kMaxTcSteps) return tc_fail("too many layers");
+  // The folded bottleneck still counts against kMaxTcSteps, so the fold does not change which models
+  // the tensor-core paths accept.
+  int folded = 0;
+  // fold: the layer that reads the bottleneck, its weights W_b W_r[:W] in d_fold and its bias per ray
+  auto add = [&](const Step& st, int epi, int cur_width, bool fold = false) -> int {
+    if (tp.n_steps + folded >= kMaxTcSteps) return tc_fail("too many layers");
     TcStep& t = tp.steps[tp.n_steps];
     memset(&t, 0, sizeof(t));
     if (st.k_x > 256 || st.k_in > kBlockK) return tc_fail("layer wider than 256 or inputs wider than 64");
@@ -665,7 +694,8 @@ inline int build_tc_program(nfb_handle* h, int level, long long* wbytes, long lo
       if (st.n > 12) return tc_fail("head wider than 12");
       if (st.k_in) return tc_fail("head reading the encoded inputs");
     }
-    t.b_off = new_bias(st);
+    if (fold) t.ray_bias = 1;
+    else t.b_off = new_bias(st);
     // weight units: for chunk c, for kb: wparts x chunk_n rows x 128 B
     t.w_off = (uint32_t)*wbytes;
     for (int c = 0; c < t.n_chunks; ++c) {
@@ -673,6 +703,7 @@ inline int build_tc_program(nfb_handle* h, int level, long long* wbytes, long lo
       job.level = level; job.step = tp.n_steps; job.chunk = c;
       job.simt_w_off = st.w_off; job.ld = st.npad; job.n = st.n; job.n0 = c * t.chunk_n;
       job.k_total = st.k_x + st.k_in;
+      job.fold = fold;
       job.k_map.assign((size_t)t.nkb * kBlockK, -1);
       for (int kb = 0; kb < t.nkb; ++kb)
         for (int j = 0; j < kBlockK; ++j) {
@@ -701,40 +732,81 @@ inline int build_tc_program(nfb_handle* h, int level, long long* wbytes, long lo
   tp.warp_mb = 2;
   for (int i = 0; i < tp.n_warp; ++i)
     if (tp.steps[i].n_chunks != 1) tp.warp_mb = 1;
-  // nerf net: trunk..., [bottleneck], alpha head (folded), rgb branch
+  // nerf net: trunk..., alpha head (an epilogue dot product), rgb branch.  A bottleneck (a Dense(W) with no
+  // activation, present when there is an alpha or rgb condition, modules.py:149-161) is linear, so it is
+  // folded into the layers that read it and has no step: the rgb branch's first layer reads
+  //   relu([x W_b + b_b | cond] W_r + b_r) = relu(x (W_b W_r[:W]) + (b_b W_r[:W] + b_r + cond W_r[W:])),
+  // x = the trunk's last activation; the second term is one vector per ray (ray_bias_kernel).  With an
+  // alpha condition the alpha head is folded the same way: weights W_b w_a[:W] over x, and a per-ray
+  // constant b_a + b_b w_a[:W] + cond w_a[W:].
+  // bf16 keeps the bottleneck as a layer: that mode's arithmetic is bf16 operands per layer (the rgb
+  // condition enters as a K-block the bottleneck's epilogue writes, the alpha condition's dot product is
+  // added by the row threads), which a folded product cannot reproduce.
+  const bool fold = h->cfg.precision == NFB_PREC_FP16X3;
   width = 0;
   int last_hidden = -1;
-  bool seen_alpha = false, seen_bottleneck = false;
+  bool seen_alpha = false, fold_pending = false, seen_bottleneck = false;
   for (int i = 0; i < fp.nerf.n_steps; ++i) {
     const Step& st = fp.nerf.steps[i];
     if (st.dst == fp.alpha_slot && st.n == 1 && !seen_alpha) {
       // alpha = Dense(1)(trunk_out), or with an alpha condition Dense(1)([bottleneck_out | alpha_cond])
-      // (models.py:206-207, modules.py:152-157): the dot product over the layer output is folded into
-      // the epilogue of the layer it reads, the per-ray condition part is added by the row threads.
+      // (models.py:206-207, modules.py:152-157): the dot product over the trunk's last layer is folded into
+      // that layer's epilogue.
       if (st.k_in != fp.ac) return tc_fail("alpha head inputs");
       seen_alpha = true;
-      // The SIMT program runs bottleneck before alpha: without an alpha condition the alpha head
+      // Unfolded, the program runs the bottleneck before alpha: without an alpha condition the alpha head
       // reads the trunk's last layer, the hidden step before the bottleneck.
-      const int src_step = (seen_bottleneck && !st.k_in) ? last_hidden - 1 : last_hidden;
+      const int src_step = (!fold && seen_bottleneck && !st.k_in) ? last_hidden - 1 : last_hidden;
       if (src_step < 0) return tc_fail("alpha head without a trunk layer");
       tp.steps[src_step].alpha_dot = 1;
       tp.alpha_w_off = (int)*aux_floats; *aux_floats += kAlphaCondOff + kBlockK;
       tp.alpha_b_off = (int)*aux_floats; *aux_floats += 4;
-      h->tc_aux_jobs.push_back({st.w_off, st.k_x, st.npad, tp.alpha_w_off});
-      if (st.k_in)
-        h->tc_aux_jobs.push_back({st.w_off + st.k_x * st.npad, st.k_in, st.npad, tp.alpha_w_off + kAlphaCondOff});
-      h->tc_aux_jobs.push_back({st.b_off, 1, 1, tp.alpha_b_off});
+      if (st.k_in && !fold) {
+        h->tc_aux_jobs.push_back({st.w_off, st.k_x, st.npad, tp.alpha_w_off, false});
+        h->tc_aux_jobs.push_back({st.w_off + st.k_x * st.npad, st.k_in, st.npad, tp.alpha_w_off + kAlphaCondOff, false});
+      } else if (st.k_in) {
+        fo.ac = st.k_in; fo.lda = st.npad; fo.wa = st.w_off; fo.ba = st.b_off;
+        h->tc_aux_jobs.push_back({fo.fwa, st.k_x, 1, tp.alpha_w_off, true});
+      } else {
+        h->tc_aux_jobs.push_back({st.w_off, st.k_x, st.npad, tp.alpha_w_off, false});
+      }
+      h->tc_aux_jobs.push_back({st.b_off, 1, 1, tp.alpha_b_off, false});
       continue;
     }
     const bool out = st.dst == fp.rgb_slot;
-    if (!out && st.act == kNone) {                 // bottleneck
+    if (!out && st.act == kNone && !fold) {        // bottleneck, bf16
       seen_bottleneck = true;
+      if (add(st, kEpiHidden, width)) return -1;
+      last_hidden = tp.n_steps - 1;
+      tp.steps[last_hidden].write_cond = 1;
+      continue;
+    }
+    if (!out && st.act == kNone) {                 // bottleneck, fp16x3
+      fo.active = 1; fo.W = st.n; fo.ldb = st.npad; fo.wb = st.w_off; fo.bb = st.b_off;
+      // d_fold: [W_b w_a[:W] (W) | constant (4) | rgb constant (256) | W_b W_r[:W] (W x ldr)]
+      fo.fwa = (int)*fold_floats; fo.fca = fo.fwa + (fo.W + 3) / 4 * 4; fo.fc = fo.fca + 4; fo.fw = fo.fc + 256;
+      *fold_floats = fo.fw;
+      ++folded;
+      fold_pending = true;
+      continue;
+    }
+    if (fold_pending) {                            // the layer that reads the bottleneck
+      fold_pending = false;
+      if (out) return tc_fail(st.k_in ? "head reading the encoded inputs" : "rgb logit reading the bottleneck");
+      fo.nr = st.n; fo.ldr = st.npad; fo.rc = st.k_in; fo.wr = st.w_off; fo.br = st.b_off;
+      fo.cols = 128 * ((st.n + 127) / 128);
+      *fold_floats += (long long)fo.W * fo.ldr;
+      Step f = st;
+      f.k_in = 0; f.w_off = fo.fw;
+      if (add(f, kEpiHidden, width, true)) return -1;
+      last_hidden = tp.n_steps - 1;
+      width = st.n;
+      continue;
     }
     if (add(st, out ? kEpiRgbOut : kEpiHidden, width)) return -1;
     if (!out) {
       last_hidden = tp.n_steps - 1;
       width = st.n;
-      if (st.act == kNone) tp.steps[last_hidden].write_cond = 1;
     }
   }
   if (!seen_alpha) return tc_fail("model without alpha head");
@@ -748,16 +820,23 @@ inline int build_tc_program(nfb_handle* h, int level, long long* wbytes, long lo
 }
 
 inline int create_tc(nfb_handle* h) {
-  long long wbytes = 0, auxf = 0;
+  long long wbytes = 0, auxf = 0, foldf = 0;
   h->tc_jobs.clear(); h->tc_aux_jobs.clear();
   const int levels = h->cfg.num_fine_samples > 0 ? 2 : 1;
   for (int lv = 0; lv < levels; ++lv)
-    if (build_tc_program(h, lv, &wbytes, &auxf)) return -1;
-  if (levels == 1) h->tcprog[1] = h->tcprog[0];
+    if (build_tc_program(h, lv, &wbytes, &auxf, &foldf)) return -1;
+  if (levels == 1) { h->tcprog[1] = h->tcprog[0]; h->tc_fold[1] = h->tc_fold[0]; }
   h->wpack_bytes = wbytes; h->aux_floats = auxf;
   if (cudaMalloc(&h->d_wpack, (size_t)wbytes) != cudaSuccess) return fail("cudaMalloc wpack failed");
   if (cudaMalloc(&h->d_aux, (size_t)auxf * sizeof(float)) != cudaSuccess) return fail("cudaMalloc aux failed");
   if (cudaMemset(h->d_aux, 0, (size_t)auxf * sizeof(float)) != cudaSuccess) return fail("cudaMemset failed");
+  if (h->tc_fold[0].active) {
+    // both levels have the same widths, so one per-ray buffer serves both
+    const size_t rb = (size_t)h->max_rays * (h->tc_fold[0].cols + 1);
+    if (cudaMalloc(&h->d_fold, (size_t)foldf * sizeof(float)) != cudaSuccess ||
+        cudaMalloc(&h->d_ray_bias, rb * sizeof(float)) != cudaSuccess)
+      return fail("cudaMalloc of the bottleneck fold buffers failed");
+  }
   const auto smem_attr = cudaFuncAttributeMaxDynamicSharedMemorySize;
   if (cudaFuncSetAttribute(field_wg_kernel<true, 1>, smem_attr, kWgSmemBytes) != cudaSuccess ||
       cudaFuncSetAttribute(field_wg_kernel<true, 2>, smem_attr, kWgSmemBytes) != cudaSuccess ||
@@ -770,13 +849,36 @@ inline int create_tc(nfb_handle* h) {
 inline void destroy_tc(nfb_handle* h) {
   if (h->d_wpack) cudaFree(h->d_wpack);
   if (h->d_aux) cudaFree(h->d_aux);
-  h->d_wpack = nullptr; h->d_aux = nullptr;
+  if (h->d_fold) cudaFree(h->d_fold);
+  if (h->d_ray_bias) cudaFree(h->d_ray_bias);
+  h->d_wpack = nullptr; h->d_aux = nullptr; h->d_fold = nullptr; h->d_ray_bias = nullptr;
 }
 
 __global__ void aux_copy_kernel(const float* __restrict__ src, int count, int stride,
                                 float* __restrict__ dst) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < count) dst[i] = src[(size_t)i * stride];
+}
+
+// The bottleneck fold of one level (TcFold) from the fp32 parameters p, in fp64, each output rounded once.
+// Thread (i, j) of (W + 1) x (ldr + 1): row i < W is the bottleneck's weight row i (its output is row i of
+// the folded weights), row W its bias (the folded constants); column j < ldr is column j of the rgb layer
+// (zero past nr), column ldr the alpha head (alpha condition only).
+__global__ void fold_kernel(const float* __restrict__ p, const TcFold f, float* __restrict__ out) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  const int cols = f.ldr + 1;
+  if (idx >= (f.W + 1) * cols) return;
+  const int i = idx / cols, j = idx - i * cols;
+  const bool alpha = j == f.ldr, bias = i == f.W;
+  if (alpha && !f.ac) return;
+  float* o = alpha ? out + (bias ? f.fca : f.fwa + i) : out + (bias ? f.fc : f.fw + i * f.ldr) + j;
+  if (!alpha && j >= f.nr) { *o = 0.f; return; }
+  const float* x = bias ? p + f.bb : p + f.wb + (size_t)i * f.ldb;
+  const float* y = alpha ? p + f.wa : p + f.wr + j;
+  const int ldy = alpha ? f.lda : f.ldr;
+  double v = bias ? (double)p[alpha ? f.ba : f.br + j] : 0.0;
+  for (int k = 0; k < f.W; ++k) v = fma((double)x[k], (double)y[(size_t)k * ldy], v);
+  *o = (float)v;
 }
 
 // Called from nfb_set_params after the fp32 layout has been filled.
@@ -794,6 +896,15 @@ inline int pack_tc(nfb_handle* h, cudaStream_t s) {
   if (e != cudaSuccess) { cudaFree(d_maps); return fail("k_map upload failed: %s", cudaGetErrorString(e)); }
   size_t map_off = 0;
   const bool x3 = h->cfg.precision == NFB_PREC_FP16X3;
+  // the folded weights first: the pack jobs of the layers that read the bottleneck read them
+  for (int lv = 0; lv < (h->cfg.num_fine_samples > 0 ? 2 : 1); ++lv) {
+    const TcFold& f = h->tc_fold[lv];
+    if (!f.active) continue;
+    const int n = (f.W + 1) * (f.ldr + 1);
+    fold_kernel<<<(n + 127) / 128, 128, 0, s>>>(h->d_packed, f, h->d_fold);
+    h->launches++;
+  }
+  auto src = [&](bool fold) { return fold ? h->d_fold : h->d_packed; };
   if (x3) {
     // per-layer max |W| -> power-of-two scale (x3_weight_scale), computed on the device
     for (int lv = 0; lv < 2; ++lv)
@@ -802,7 +913,7 @@ inline int pack_tc(nfb_handle* h, cudaStream_t s) {
       if (j.chunk != 0) continue;
       const long long n = (long long)j.k_total * j.ld;
       absmax_kernel<<<(unsigned)std::min<long long>((n + 255) / 256, 64), 256, 0, s>>>(
-          h->d_packed + j.simt_w_off, n, h->d_aux + h->tcprog[j.level].scale_off + j.step);
+          src(j.fold) + j.simt_w_off, n, h->d_aux + h->tcprog[j.level].scale_off + j.step);
       h->launches++;
     }
   }
@@ -813,17 +924,17 @@ inline int pack_tc(nfb_handle* h, cudaStream_t s) {
     // source columns n0.. of the fp32 (K x npad) matrix: shift the base pointer.
     if (x3)
       pack_weight_x3_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(
-          h->d_packed + j.simt_w_off + j.n0, j.ld, d_maps + map_off, t.nkb, j.n - j.n0, t.chunk_n,
+          src(j.fold) + j.simt_w_off + j.n0, j.ld, d_maps + map_off, t.nkb, j.n - j.n0, t.chunk_n,
           h->d_aux + h->tcprog[j.level].scale_off + j.step, dst);
     else
       pack_weight_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(
-          h->d_packed + j.simt_w_off + j.n0, j.ld, d_maps + map_off, t.nkb, j.n - j.n0, t.chunk_n,
+          src(j.fold) + j.simt_w_off + j.n0, j.ld, d_maps + map_off, t.nkb, j.n - j.n0, t.chunk_n,
           reinterpret_cast<__nv_bfloat16*>(dst));
     h->launches++;
     map_off += j.k_map.size();
   }
   for (auto& a : h->tc_aux_jobs) {
-    aux_copy_kernel<<<(a.count + 127) / 128, 128, 0, s>>>(h->d_packed + a.src_off, a.count, a.stride,
+    aux_copy_kernel<<<(a.count + 127) / 128, 128, 0, s>>>(src(a.fold) + a.src_off, a.count, a.stride,
                                                           h->d_aux + a.dst_off);
     h->launches++;
   }
@@ -835,9 +946,28 @@ inline int pack_tc(nfb_handle* h, cudaStream_t s) {
 }
 
 // One pass of field_wg_kernel: the warp net (a.warp_only, into a.warped) or the NeRF net.  The NeRF
-// pass of a warped model reads the warp pass's points (a.points); nothing warps inside it.
-inline int run_field_tc(nfb_handle* h, int level, const FieldArgs& a, cudaStream_t s) {
+// pass of a warped model reads the warp pass's points (a.points); nothing warps inside it.  The NeRF pass
+// of a model with a bottleneck first forms its rays' folded bias (ray_bias_kernel, from a.cond).
+inline int run_field_tc(nfb_handle* h, int level, const FieldArgs& args, cudaStream_t s) {
   const TcProgram& prog = h->tcprog[level];
+  FieldArgs a = args;
+  const TcFold& f = h->tc_fold[level];
+  if (!a.warp_only && f.active && a.num_rows > 0) {
+    RayBiasArgs r{};
+    r.num_rays = (int)((a.num_rows + a.samples_per_ray - 1) / a.samples_per_ray);
+    r.cond = a.cond; r.stride = prog.cond_stride;
+    r.w_rc = h->d_packed + f.wr + (size_t)f.W * f.ldr; r.ldr = f.ldr; r.rc = f.rc; r.rc_off = f.rc_off;
+    r.c_r = h->d_fold + f.fc; r.nr = f.nr; r.cols = f.cols;
+    r.w_ac = h->d_packed + f.wa + (size_t)f.W * f.lda; r.lda = f.lda; r.ac = f.ac; r.ac_off = f.ac_off;
+    r.c_a = h->d_fold + f.fca;
+    r.bias = h->d_ray_bias; r.alpha = h->d_ray_bias + (size_t)h->max_rays * f.cols;
+    const long long n = (long long)r.num_rays * (f.cols + (f.ac > 0));
+    ray_bias_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(r);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail("ray_bias_kernel launch failed: %s", cudaGetErrorString(e));
+    h->launches++;
+    a.ray_bias = r.bias; a.ray_alpha = r.alpha;
+  }
   if (a.warp_only && (prog.n_warp == 0 || !a.warped)) return fail("warp pass without a warp net or an output");
   if (!a.warp_only && a.use_warp && prog.n_warp > 0 && !a.points)
     return fail("the NeRF pass of a warped model needs the warp pass's points");

@@ -110,9 +110,17 @@ struct nfb_handle {
   unsigned char* d_wpack = nullptr;   // weight units, shared-memory image (bf16, or fp16 hi | lo)
   float* d_aux = nullptr;             // fp32 biases + alpha head
   long long wpack_bytes = 0, aux_floats = 0;
-  struct TcPackJob { int level, step, chunk; int simt_w_off, ld, n, n0, k_total; std::vector<int> k_map; };
+  // fold: simt_w_off is in d_fold, not d_packed
+  struct TcPackJob { int level, step, chunk; int simt_w_off, ld, n, n0, k_total; bool fold; std::vector<int> k_map; };
   std::vector<TcPackJob> tc_jobs;
-  struct TcAuxJob { int src_off, count, stride, dst_off; };
+  struct TcAuxJob { int src_off, count, stride, dst_off; bool fold; };   // fold: src_off is in d_fold
   std::vector<TcAuxJob> tc_aux_jobs;
+  // The bottleneck folded into the rgb branch (and, with an alpha condition, the alpha head), per level:
+  // fold_kernel writes W_b W_r[:W] and b_b W_r[:W] + b_r (and W_b w_a[:W], b_a + b_b w_a[:W]) into d_fold at
+  // every nfb_set_params; ray_bias_kernel adds the per-ray condition terms into d_ray_bias before each
+  // tensor-core NeRF pass.
+  nfb::tc::TcFold tc_fold[2];
+  float* d_fold = nullptr;
+  float* d_ray_bias = nullptr;        // (max_rays, 128 n_chunks) rgb bias, then (max_rays) alpha constants
 };
 

@@ -101,6 +101,49 @@ __global__ void ray_cond_kernel(const CondArgs a) {
 }
 
 // ---------------------------------------------------------------------------
+// The per-ray terms of a NeRF level whose bottleneck the tensor-core program folds (TcFold,
+// field_tc.cuh), from the condition vector, for the field pass that follows:
+//   bias[ray, j] = c_r[j] + cond_rgb . W_r[W:, j]    (j < nr; zero up to cols)
+//   alpha[ray]   = c_a + cond_alpha . w_a[W:]        (with an alpha condition)
+// c_r = b_b W_r[:W] + b_r and c_a = b_a + b_b w_a[:W] come from fold_kernel.  fp64 sums of the exact
+// fp32 products, rounded once.  One thread per output; consecutive threads write consecutive columns.
+// ---------------------------------------------------------------------------
+struct RayBiasArgs {
+  const float* cond;              // (B, stride)
+  int stride, num_rays;
+  const float* w_rc;              // W_r[W:], rc rows of ldr
+  int ldr, rc, rc_off, nr, cols;
+  const float* c_r;               // (nr)
+  const float* w_ac;              // w_a[W:], ac rows of lda (column 0)
+  int lda, ac, ac_off;
+  const float* c_a;               // (1)
+  float* bias;                    // (B, cols)
+  float* alpha;                   // (B)
+};
+
+__global__ void ray_bias_kernel(const RayBiasArgs a) {
+  const int per = a.cols + (a.ac > 0);
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)a.num_rays * per) return;
+  const long long ray = idx / per;
+  const int j = (int)(idx - ray * per);
+  const float* cond = a.cond + ray * a.stride;
+  if (j < a.cols) {
+    double v = 0.0;
+    if (j < a.nr) {
+      v = (double)a.c_r[j];
+      for (int q = 0; q < a.rc; ++q)
+        v = fma((double)cond[a.rc_off + q], (double)a.w_rc[(size_t)q * a.ldr + j], v);
+    }
+    a.bias[ray * a.cols + j] = (float)v;
+  } else {
+    double v = (double)a.c_a[0];
+    for (int q = 0; q < a.ac; ++q) v = fma((double)cond[a.ac_off + q], (double)a.w_ac[(size_t)q * a.lda], v);
+    a.alpha[ray] = (float)v;
+  }
+}
+
+// ---------------------------------------------------------------------------
 // modules.TimeEncoder (modules.py:297-322) per ray: annealed positional encoding
 // of the timestamp, MLP(depth 6, width 64, skips (4,)) + `features`-wide output
 // layer; writes (or, 'blend' encoder of TranslationField, warping.py:128-133,
