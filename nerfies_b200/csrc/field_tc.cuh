@@ -408,6 +408,7 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
 
     // fused composite: running state of the ray this CTA is on (replicated in every row thread)
     float c_T = 1.f, c_cw = 0.f, a_r = 0.f, a_g = 0.f, a_b = 0.f, a_d = 0.f, a_w = 0.f, a_wnl = 0.f, a_med = 0.f;
+    bool c_med = false;   // the ray's median sample has been found
     if (n_my > 0) begin_tile(tile_of(0));
     fence_proxy_async();
     wg_sync();
@@ -547,7 +548,9 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
               //      over the 128 samples of this tile; one sample per row thread of half 0 ----
               const int qd = r >> 5;
               auto bar128 = [&]() { asm volatile("bar.sync 3, 128;" ::: "memory"); };
-              if ((tile % tpr) == 0) { c_T = 1.f; c_cw = 0.f; a_r = a_g = a_b = a_d = a_w = a_wnl = a_med = 0.f; }
+              if ((tile % tpr) == 0) {
+                c_T = 1.f; c_cw = 0.f; a_r = a_g = a_b = a_d = a_w = a_wnl = a_med = 0.f; c_med = false;
+              }
               // alpha = 1 - exp(-sigma * dist) as -expm1(-x) (see composite_kernel)
               const float al = -expm1f(-o.w * row.dist);
               const float tf = 1.0f - al + 1e-10f;
@@ -595,15 +598,20 @@ field_wg_kernel(const __grid_constant__ TcProgram prog, const FieldArgs args, co
                 for (int k = 0; k < 6; ++k) tot[k] += scan_s[8 + q * 8 + k];
               }
               const float cwt = pre + C;                       // cumsum over the ray up to this sample
-              float prev = __shfl_up_sync(0xffffffffu, cwt, 1);
-              if (lane == 0) prev = pre;
-              // first sample whose cumulative weight reaches 0.5 (opaque xor shifted, :231-238)
-              float med = (cwt >= 0.5f && !(prev >= 0.5f)) ? row.z : 0.f;
-#pragma unroll
-              for (int sh = 16; sh > 0; sh >>= 1) med += __shfl_xor_sync(0xffffffffu, med, sh);
-              if (lane == 0) scan_s[4 + qd] = med;
+              // Median depth: the first sample in ray order whose cumulative weight reaches 0.5
+              // (opaque xor shifted, :231-238).  cwt is summed in three associations (the shfl_up scan,
+              // the quarter totals, the tile carry), so it is not monotone across lanes, quarters and
+              // tiles: comparing each sample with its predecessor can fire no sample or two near 0.5.
+              // The median is the lowest firing lane of the lowest firing quarter of the ray's first
+              // firing tile, taken once.
+              const unsigned hit = __ballot_sync(0xffffffffu, cwt >= 0.5f);
+              const float zhit = __shfl_sync(0xffffffffu, row.z, hit ? __ffs(hit) - 1 : 0);
+              if (lane == 0) { scan_s[4 + qd] = zhit; scan_s[8 + qd * 8 + 6] = hit ? 1.f : 0.f; }
               bar128();
-              a_med += scan_s[4] + scan_s[5] + scan_s[6] + scan_s[7];
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                if (!c_med && scan_s[8 + q * 8 + 6] != 0.f) { a_med = scan_s[4 + q]; c_med = true; }
+              }
               a_r += tot[0]; a_g += tot[1]; a_b += tot[2]; a_d += tot[3]; a_w += tot[4]; a_wnl += tot[5];
               c_T = c_T * Wall; c_cw += tot[4];
               if ((tile % tpr) == tpr - 1 && r == 0) {

@@ -167,16 +167,32 @@ def tree_to_device(tree, device):
   return tree.to(device)
 
 
+def med_depth_rule_ok(got, weights, z_vals, window=1e-6):
+  """Per ray: med_depth is exactly the z of the first sample whose cumulative
+  weight reaches 0.5 (model_utils.py:231-239) - in fp64 over the kernel's own
+  `weights`, or any sample whose cumulative weight is within `window` of 0.5 -
+  or 0 when the ray's total weight is below 0.5 + window."""
+  got, w, z = got.cpu().double(), weights.cpu().double(), z_vals.cpu().double()
+  cum = torch.cumsum(w, -1)
+  reach = cum >= 0.5
+  allowed = (cum - 0.5).abs() <= window
+  has = reach.any(-1)
+  allowed[has, reach.int().argmax(-1)[has]] = True
+  ok = ((got[:, None] == z) & allowed).any(-1)
+  return ok | ((got == 0) & (cum[:, -1] < 0.5 + window))
+
+
 def med_depth_ok(got, ref_out, z_vals, tol=1e-4):
   """med_depth is a step function of the weights (first sample with
   cumsum >= 0.5, model_utils.py:231-239): equal to the reference except where
   the cumulative weight passes within `tol` of 0.5, where the neighbouring
-  sample may be picked instead."""
+  sample may be picked instead, and 0 only where the total weight is within
+  `tol` of 0.5."""
   got = got.cpu()
   ref = ref_out['med_depth']
   exact = (got - ref).abs() <= 1e-6 * (1 + ref.abs())
   cum = torch.cumsum(ref_out['weights'].double(), -1)
   near_half = ((cum - 0.5).abs() < tol).any(-1)
   in_z = (got[:, None] - z_vals).abs().min(-1).values <= 1e-6
-  in_z = in_z | (got == 0)
+  in_z = in_z | ((got == 0) & ((cum[:, -1] - 0.5).abs() < tol))
   return bool((exact | (near_half & in_z)).all())
