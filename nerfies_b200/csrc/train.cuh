@@ -404,7 +404,7 @@ __global__ void warp_tail_bwd_kernel(const WarpTailBwdArgs a) {
 }
 
 // ---------------------------------------------------------------------------
-// R8: raw -> (sigmoid(rgb), sigma_act(alpha)); R9 adjoint + the photometric loss.
+// R8: raw -> (sigmoid(rgb), sigma_act(alpha)); the photometric loss; R9 adjoint.
 // ---------------------------------------------------------------------------
 __global__ void raw_to_samples_kernel(const float* __restrict__ rgb_raw, int ld_rgb,
                                       const float* __restrict__ alpha_raw, int ld_a, int sigma_act,
@@ -417,87 +417,30 @@ __global__ void raw_to_samples_kernel(const float* __restrict__ rgb_raw, int ld_
   samples[m] = o;
 }
 
-// One warp per ray: loss = mean((rgb - target)^2) over the LOCAL batch (training.py:173),
-// d(loss)/d(raw) through volumetric_rendering (model_utils.py:104-126).
-struct CompositeBwdArgs {
-  const float4* samples; const float* z; const float* directions;   // forward results
-  const float* out;           // (B,6) forward rgb...
-  const float* target;        // (B,3)
-  const float* rgb_raw; int ld_rgb; const float* alpha_raw; int ld_a;
-  float* d_rgb_raw; float* d_alpha_raw;     // same layouts: = (not +=)
-  float* loss;                // += this level's loss (scalar)
-  float scale;                // 1 / (batch_rays * 3)
-  int num_rays, S, white_bg, sample_at_infinity, sigma_act;
-};
-__global__ void composite_bwd_kernel(const CompositeBwdArgs a) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int ray = blockIdx.x * kRaysPerBlock + warp;
-  if (ray >= a.num_rays) return;
-  extern __shared__ float sh[];
-  const int S = a.S;
-  float* gw = sh + warp * 4 * S;       // d loss / d w_i
-  float* suf = gw + S;                 // sum_{k>i} gw_k w_k
-  float* al = suf + S;                 // alpha_i
-  float* tr = al + S;                  // T_i
-  float g[3];
+// loss = mean((rgb - target)^2) over the LOCAL batch (training.py:173), one thread per ray: adds the ray's share
+// to *loss and writes its row of d_out (R,6), the cotangents of rgb, depth, med_depth and acc that seed
+// composite_vjp_kernel.
+__global__ void photometric_loss_kernel(const float* __restrict__ out, const float* __restrict__ target, float scale,
+                                        int num_rays, float* __restrict__ d_out, float* __restrict__ loss) {
+  const int ray = blockIdx.x * blockDim.x + threadIdx.x;
+  if (ray >= num_rays) return;
   float l = 0.f;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    const float diff = a.out[ray * 6 + c] - a.target[ray * 3 + c];
-    g[c] = 2.f * diff * a.scale;
-    l += diff * diff * a.scale;
+    const float diff = out[ray * 6 + c] - target[ray * 3 + c];
+    d_out[ray * 6 + c] = 2.f * diff * scale;
+    l += diff * diff * scale;
   }
-  if (lane == 0) atomicAdd(a.loss, l);
-  const float dx = a.directions[ray * 3], dy = a.directions[ray * 3 + 1], dz = a.directions[ray * 3 + 2];
-  const float dnorm = sqrtf(dx * dx + dy * dy + dz * dz);
-  const float last = a.sample_at_infinity ? 1e10f : 1e-19f;
-  const float gsum = g[0] + g[1] + g[2];
-  for (int i = lane; i < S; i += 32) {
-    const size_t m = (size_t)ray * S + i;
-    const float4 c = a.samples[m];
-    // rgb = sum w c (+ (1 - sum w) on a white background, model_utils.py:121-122)
-    float v = g[0] * c.x + g[1] * c.y + g[2] * c.z;
-    if (a.white_bg) v -= gsum;
-    gw[i] = v;
-    float dist = (i + 1 < S) ? (a.z[m + 1] - a.z[m]) : last;
-    al[i] = -expm1f(-c.w * (dist * dnorm));
-  }
-  __syncwarp();
-  if (lane == 0) {
-    // w_i = alpha_i T_i, T_i = prod_{j<i} (1 - alpha_j + eps)  (model_utils.py:108-114):
-    // dL/dalpha_i = gw_i T_i - (sum_{k>i} gw_k w_k) / (1 - alpha_i + eps)
-    float t = 1.f;
-    for (int i = 0; i < S; ++i) { tr[i] = t; t = t * (1.0f - al[i] + 1e-10f); }
-    float acc = 0.f;
-    for (int i = S - 1; i >= 0; --i) { suf[i] = acc; acc += gw[i] * (al[i] * tr[i]); }
-  }
-  __syncwarp();
-  for (int i = lane; i < S; i += 32) {
-    const size_t m = (size_t)ray * S + i;
-    const float4 c = a.samples[m];
-    float dist = (i + 1 < S) ? (a.z[m + 1] - a.z[m]) : last;
-    dist = dist * dnorm;
-    const float dalpha = gw[i] * tr[i] - suf[i] / (1.0f - al[i] + 1e-10f);
-    const float dsigma = dalpha * dist * expf(-c.w * dist);      // alpha = 1 - exp(-sigma dist)
-    const float raw = a.alpha_raw[m * a.ld_a];
-    float dact;                                                    // sigma = act(raw)
-    if (a.sigma_act == kSoftplus) dact = 1.f / (1.f + expf(-raw));
-    else if (a.sigma_act == kRelu) dact = raw > 0.f ? 1.f : 0.f;
-    else dact = act_grad_from_output(c.w, a.sigma_act);
-    a.d_alpha_raw[m * a.ld_a] = dsigma * dact;
-    const float w = al[i] * tr[i];
-    // rgb_i = sigmoid(raw): d/draw = c (1 - c)
-    a.d_rgb_raw[m * a.ld_rgb + 0] = g[0] * w * c.x * (1.f - c.x);
-    a.d_rgb_raw[m * a.ld_rgb + 1] = g[1] * w * c.y * (1.f - c.y);
-    a.d_rgb_raw[m * a.ld_rgb + 2] = g[2] * w * c.z * (1.f - c.z);
-  }
+#pragma unroll
+  for (int c = 3; c < 6; ++c) d_out[ray * 6 + c] = 0.f;
+  atomicAdd(loss, l);
 }
 
-// The adjoint of volumetric_rendering (model_utils.py:104-126) for caller-given cotangents of its outputs:
-// nfb_render_vjp's seed of the backward, where composite_bwd_kernel seeds the photometric loss's.  Per ray
+// The adjoint of volumetric_rendering (model_utils.py:104-126) for given cotangents of its outputs: the seed of
+// every backward (the caller's cotangents in nfb_render_vjp, photometric_loss_kernel's in training).  Per ray
 //   d/dw_i = g_rgb . c_i - [white_bg] sum(g_rgb) + g_depth z_i + g_acc [i < S-1 or !sample_at_infinity] + g_w_i
-// (the white background adds 1 - sum w, the acc before sample_at_infinity drops the last sample), then the same
-// chain as composite_bwd_kernel to the raw rgb and density.  med_depth is piecewise constant: no cotangent.
+// (the white background adds 1 - sum w, the acc before sample_at_infinity drops the last sample), then through
+// w_i = alpha_i T_i to the raw rgb and density.  med_depth is piecewise constant: no cotangent.
 struct CompositeVjpArgs {
   const float4* samples; const float* z; const float* directions;   // the taped forward
   const float* d_out;         // (R,6) cotangents of rgb, depth, med_depth (ignored), acc; or null

@@ -419,12 +419,16 @@ int level_forward(nfb_handle* h, int level, int R, int S, const float* z, const 
   return run_composite(h, R, S, A + t.samples, z, directions, out6, weights, s);
 }
 
-// forward + loss + backward of one level for `R` rays (rows = R * S) on the tape; `cond` / `dcond` are
-// the R rays' condition vectors and their gradient accumulator.
-int train_level(nfb_handle* h, int level, int R, int S, const float* z, const float* origins,
-                const float* directions, const float* target, const float* cond, float* dcond, float scale,
-                bool use_warp, float* out6, float* weights, float* loss, cudaStream_t s,
-                const RegCfg* reg = nullptr) {
+// The backward of one level for `R` rays (rows = R * S) on the tape that level_forward filled at the same z:
+// composite_vjp_kernel seeded by the cotangents d_out (R,6) and d_weights (R,S) of the level's outputs, the
+// regularisers of `reg` (on the level's `weights`), the NeRF MLP and its encoding, then the warp field, whose
+// warped points also receive d_warped (R,S,3).  d_out, d_weights, d_warped and reg are nullable; `dcond` is the R
+// rays' condition-vector gradient accumulator.
+static_assert(nfb::train::composite_vjp_smem(nfb::kMaxSamples) <= 48 * 1024,
+              "composite_vjp_kernel's shared memory exceeds the default 48 KiB at kMaxSamples");
+int level_backward(nfb_handle* h, int level, int R, int S, const float* z, const float* directions, float* dcond,
+                   bool use_warp, int alpha_step, int rgb_step, const float* d_out, const float* d_weights,
+                   const float* d_warped, const float* weights, const RegCfg* reg, cudaStream_t s) {
   using namespace nfb::train;
   const nfb::FieldProgram& p = h->prog[level];
   const long long rows = (long long)R * S;
@@ -432,25 +436,20 @@ int train_level(nfb_handle* h, int level, int R, int S, const float* z, const fl
   float* A = h->d_tape;
   const bool warp = use_warp && p.warp_type != 0;
   const unsigned blocks = (unsigned)((rows + 127) / 128);
-  int alpha_step = -1, rgb_step = -1;
-  if (level_forward(h, level, R, S, z, origins, directions, cond, use_warp, out6, weights, s, &alpha_step, &rgb_step))
-    return -1;
-  const int ld_a = p.nerf.steps[alpha_step].npad, ld_rgb = p.nerf.steps[rgb_step].npad;
-  // ---- loss + backward ----
   NFB_CUDA(cudaMemsetAsync(A + t.grad_begin, 0, (size_t)(t.grad_end - t.grad_begin) * sizeof(float), s));
   {
-    CompositeBwdArgs c{};
+    CompositeVjpArgs c{};
     c.samples = reinterpret_cast<const float4*>(A + t.samples); c.z = z; c.directions = directions;
-    c.out = out6; c.target = target;
-    c.rgb_raw = A + t.out_n[rgb_step]; c.ld_rgb = ld_rgb; c.alpha_raw = A + t.out_n[alpha_step]; c.ld_a = ld_a;
+    c.d_out = d_out; c.d_weights = d_weights;
+    c.rgb_raw = A + t.out_n[rgb_step]; c.ld_rgb = p.nerf.steps[rgb_step].npad;
+    c.alpha_raw = A + t.out_n[alpha_step]; c.ld_a = p.nerf.steps[alpha_step].npad;
     c.d_rgb_raw = A + t.d_out_n[rgb_step]; c.d_alpha_raw = A + t.d_out_n[alpha_step];
-    c.loss = loss; c.scale = scale; c.num_rays = R; c.S = S;
+    c.num_rays = R; c.S = S;
     c.white_bg = h->cfg.use_white_background; c.sample_at_infinity = h->cfg.use_sample_at_infinity;
     c.sigma_act = p.sigma_act;
     const int nblk = (R + nfb::kRaysPerBlock - 1) / nfb::kRaysPerBlock;
-    const size_t smem = (size_t)nfb::kRaysPerBlock * 4 * S * sizeof(float);
-    composite_bwd_kernel<<<nblk, 32 * nfb::kRaysPerBlock, smem, s>>>(c);
-    if (launch_check(h, "composite_bwd_kernel")) return -1;
+    composite_vjp_kernel<<<nblk, 32 * nfb::kRaysPerBlock, composite_vjp_smem(S), s>>>(c);
+    if (launch_check(h, "composite_vjp_kernel")) return -1;
   }
   const bool want_sel = reg && warp && ((reg->elastic && level == 0 && reg->reduce == 0) || reg->warp_reg);
   if (want_sel) {
@@ -474,7 +473,9 @@ int train_level(nfb_handle* h, int level, int R, int S, const float* z, const fl
     encode_bwd_kernel<<<blocks, 128, 0, s>>>(e);
     if (launch_check(h, "encode_bwd_kernel")) return -1;
   }
-  if (warp && reg && reg->warp_reg) {
+  if (!warp) return 0;
+  // encode_bwd_kernel has set tape.dwarped; the warp-reg loss and d_warped add to it
+  if (reg && reg->warp_reg) {
     // training.py:194-207: robust loss of |points - warped_points|^2 at the median-depth sample
     WarpMagArgs wm{A + t.pts, A + t.warped, h->d_sel, A + t.dwarped,
                    reg->stats + (level == 0 ? kSlotWarpRegCoarse : kSlotWarpRegFine),
@@ -482,54 +483,6 @@ int train_level(nfb_handle* h, int level, int R, int S, const float* z, const fl
     warp_mag_loss_kernel<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(wm);
     if (launch_check(h, "warp_mag_loss_kernel")) return -1;
   }
-  return warp ? warp_backward(h, p, t, S, dcond, s) : 0;
-}
-
-// One level of nfb_render_vjp for `R` rays: the taped forward at the given z, then train_level's backward,
-// seeded by composite_vjp_kernel from the cotangents of the level's outputs instead of by the photometric loss.
-// d_out (R,6), d_weights (R,S) and d_warped (R,S,3) are nullable; d_warped joins the gradient of the warped
-// points that the NeRF MLP's encoding leaves in tape.dwarped.
-static_assert(nfb::train::composite_vjp_smem(nfb::kMaxSamples) <= 48 * 1024,
-              "composite_vjp_kernel's shared memory exceeds the default 48 KiB at kMaxSamples");
-int vjp_level(nfb_handle* h, int level, int R, int S, const float* z, const float* origins, const float* directions,
-              const float* cond, float* dcond, bool use_warp, const float* d_out, const float* d_weights,
-              const float* d_warped, cudaStream_t s) {
-  using namespace nfb::train;
-  const nfb::FieldProgram& p = h->prog[level];
-  const long long rows = (long long)R * S;
-  const TapeLayout t = tape_layout(p, rows);
-  float* A = h->d_tape;
-  const bool warp = use_warp && p.warp_type != 0;
-  const unsigned blocks = (unsigned)((rows + 127) / 128);
-  int alpha_step = -1, rgb_step = -1;
-  if (level_forward(h, level, R, S, z, origins, directions, cond, use_warp, h->d_tr_out, nullptr, s, &alpha_step,
-                    &rgb_step))
-    return -1;
-  NFB_CUDA(cudaMemsetAsync(A + t.grad_begin, 0, (size_t)(t.grad_end - t.grad_begin) * sizeof(float), s));
-  {
-    CompositeVjpArgs c{};
-    c.samples = reinterpret_cast<const float4*>(A + t.samples); c.z = z; c.directions = directions;
-    c.d_out = d_out; c.d_weights = d_weights;
-    c.rgb_raw = A + t.out_n[rgb_step]; c.ld_rgb = p.nerf.steps[rgb_step].npad;
-    c.alpha_raw = A + t.out_n[alpha_step]; c.ld_a = p.nerf.steps[alpha_step].npad;
-    c.d_rgb_raw = A + t.d_out_n[rgb_step]; c.d_alpha_raw = A + t.d_out_n[alpha_step];
-    c.num_rays = R; c.S = S;
-    c.white_bg = h->cfg.use_white_background; c.sample_at_infinity = h->cfg.use_sample_at_infinity;
-    c.sigma_act = p.sigma_act;
-    const int nblk = (R + nfb::kRaysPerBlock - 1) / nfb::kRaysPerBlock;
-    composite_vjp_kernel<<<nblk, 32 * nfb::kRaysPerBlock, composite_vjp_smem(S), s>>>(c);
-    if (launch_check(h, "composite_vjp_kernel")) return -1;
-  }
-  if (net_backward(h, p.nerf, A + t.in_n, A + t.d_in_n, t.ld_n, t.out_n, t.d_out_n, A, rows, s)) return -1;
-  {
-    EncodeBwdArgs e{};
-    e.pts = A + t.warped; e.window = nullptr; e.din = A + t.d_in_n; e.F = p.Fp; e.ld = t.ld_n; e.S = S;
-    e.cond_stride = h->cond_layout.stride; e.cond_off = p.G; e.n_cond = p.tc + p.ac + p.rc;
-    e.dpts = warp ? A + t.dwarped : nullptr; e.dcond = dcond; e.rows = rows;
-    encode_bwd_kernel<<<blocks, 128, 0, s>>>(e);
-    if (launch_check(h, "encode_bwd_kernel")) return -1;
-  }
-  if (!warp) return 0;
   if (d_warped) {
     add_into_kernel<<<(unsigned)((rows * 3 + 255) / 256), 256, 0, s>>>(A + t.dwarped, d_warped, rows * 3);
     if (launch_check(h, "add_into_kernel")) return -1;
@@ -597,12 +550,6 @@ int train_prepare(nfb_handle* h, int chunk_rays) {
     if (grow(&h->d_tape, &h->tape_floats, need, "tape")) return -1;
     NFB_CUDA(cudaMemset(h->d_tape, 0, (size_t)need * sizeof(float)));
   }
-  // composite_bwd_kernel holds 4 floats per sample of each of its kRaysPerBlock rays (train_level)
-  static_assert(nfb::kRaysPerBlock * 4 * nfb::kMaxSamples * sizeof(float) <= 96 * 1024,
-                "composite_bwd_kernel's shared memory exceeds its opt-in at kMaxSamples");
-  if (cudaFuncSetAttribute(nfb::train::composite_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024) !=
-      cudaSuccess)
-    return fail("training: cannot reserve 96 KiB of shared memory for composite_bwd_kernel");
   if (!h->d_gpacked) {
     auto dm = [&](float** p, long long n) {
       return cudaMalloc(p, (size_t)std::max<long long>(n, 1) * sizeof(float)) == cudaSuccess ? 0
@@ -613,7 +560,8 @@ int train_prepare(nfb_handle* h, int chunk_rays) {
         dm(&h->d_gapp, (long long)c.num_appearance_embeddings * c.num_appearance_features) ||
         dm(&h->d_gcam, (long long)c.num_camera_embeddings * c.num_camera_features) ||
         dm(&h->d_dcond, (long long)h->max_rays * h->cond_layout.stride) ||
-        dm(&h->d_tr_out, (long long)h->max_rays * 12) || dm(&h->d_tr_w, (long long)h->max_rays * smax) ||
+        // d_tr_out: a chunk's coarse outputs, fine outputs and photometric-loss cotangents, (R,6) each
+        dm(&h->d_tr_out, (long long)h->max_rays * 18) || dm(&h->d_tr_w, (long long)h->max_rays * smax) ||
         dm(&h->d_loss, nfb::train::kLossSlots))
       return -1;
   }
@@ -634,9 +582,9 @@ int train_prepare_rows(nfb_handle* h, long long rows) {
 
 // warp_field.apply on `n` free points (+ optional noise) on the tape of level 0: condition
 // vectors per point, then warp_forward.  The points land in tape.pts, the warped points in tape.warped.
-// `warp_id`: see train_cond.
+// `warp_id`: see train_cond; with `encoded`, the points' warp codes (n, G floats).
 int warp_points_forward(nfb_handle* h, int n, const float* points, const float* noise, const unsigned* warp_id,
-                        bool float_time, cudaStream_t s) {
+                        bool float_time, bool encoded, cudaStream_t s) {
   const nfb::FieldProgram& p = h->prog[0];
   const TapeLayout t = tape_layout(p, n);
   float* A = h->d_tape;
@@ -644,7 +592,9 @@ int warp_points_forward(nfb_handle* h, int n, const float* points, const float* 
                                                                                         (long long)n * 3);
   if (launch_check(h, "add_noise_kernel")) return -1;
   // the "view direction" columns are unused here
-  if (train_cond(h, n, A + t.warped, warp_id, float_time, nullptr, nullptr, s)) return -1;
+  if (encoded ? run_cond(h, n, A + t.warped, warp_id, nullptr, nullptr, s, true, false)
+              : train_cond(h, n, A + t.warped, warp_id, float_time, nullptr, nullptr, s))
+    return -1;
   return warp_forward(h, p, t, nullptr, nullptr, nullptr, 1, A + t.warped, h->d_cond, s);
 }
 
@@ -666,6 +616,17 @@ int run_cond_bwd(nfb_handle* h, int B, const float* dcond, const unsigned* warp_
   return launch_check(h, "cond_bwd_kernel");
 }
 
+// Adjoint of warp_points_forward, from the gradient of the warped points that the caller has seeded in
+// tape.dwarped (after zeroing the tape's gradient region and h->d_dcond): the warp MLP's parameter gradients,
+// then those of the codes: the tables' rows and the TimeEncoder's parameters or, with `encoded`, d_code
+// (n, G; nullable).
+int warp_points_backward(nfb_handle* h, int n, const unsigned* warp_id, bool encoded, float* d_code, cudaStream_t s) {
+  const nfb::FieldProgram& p = h->prog[0];
+  if (warp_backward(h, p, tape_layout(p, n), 1, h->d_dcond, s)) return -1;
+  if (encoded) return cond_vjp_encoded(h, n, h->d_dcond, warp_id != nullptr, false, false, d_code, nullptr, nullptr, s);
+  return run_cond_bwd(h, n, h->d_dcond, warp_id, nullptr, nullptr, s) || time_backward(h, n, h->d_dcond, s) ? -1 : 0;
+}
+
 // compute_background_loss (training.py:118-135) and its gradient, in chunks of max_rays points.
 int train_background(nfb_handle* h, int P, const float* points, const unsigned* warp_ids, const float* noise,
                      float weight, cudaStream_t s) {
@@ -679,7 +640,7 @@ int train_background(nfb_handle* h, int P, const float* points, const unsigned* 
     float* A = h->d_tape;
     // the ids are the timestamps of a 'time' encoder too: float(id) (training.py:120-131)
     if (warp_points_forward(h, n, points + (size_t)p0 * 3, noise ? noise + (size_t)p0 * 3 : nullptr, warp_ids + p0,
-                            false, s))
+                            false, false, s))
       return -1;
     NFB_CUDA(cudaMemsetAsync(A + t.grad_begin, 0, (size_t)(t.grad_end - t.grad_begin) * sizeof(float), s));
     NFB_CUDA(cudaMemsetAsync(h->d_dcond, 0, (size_t)n * h->cond_layout.stride * sizeof(float), s));
@@ -687,9 +648,7 @@ int train_background(nfb_handle* h, int P, const float* points, const unsigned* 
     WarpMagArgs wm{A + t.pts, A + t.warped, nullptr, A + t.dwarped, h->d_loss + kSlotBackground, -2.0f, 0.001f,
                    weight / (float)P, n};
     warp_mag_loss_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(wm);
-    if (launch_check(h, "warp_mag_loss_kernel")) return -1;
-    if (warp_backward(h, p, t, 1, h->d_dcond, s)) return -1;
-    if (run_cond_bwd(h, n, h->d_dcond, warp_ids + p0, nullptr, nullptr, s) || time_backward(h, n, h->d_dcond, s))
+    if (launch_check(h, "warp_mag_loss_kernel") || warp_points_backward(h, n, warp_ids + p0, false, nullptr, s))
       return -1;
   }
   return 0;
@@ -752,16 +711,24 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
     const float* o = origins + (size_t)r0 * 3;
     const float* d = directions + (size_t)r0 * 3;
     const float* tg = rgb_target + (size_t)r0 * 3;
+    float* d_out = h->d_tr_out + 12 * (size_t)R;
+    float* w = h->d_tr_w;
+    // forward, photometric loss and backward of one level at z
+    auto level = [&](int lv, int S, const float* z, float* out, int loss_slot) {
+      int alpha_step = -1, rgb_step = -1;
+      if (level_forward(h, lv, R, S, z, o, d, cond, use_warp, out, w, s, &alpha_step, &rgb_step)) return -1;
+      nfb::train::photometric_loss_kernel<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(out, tg, scale, R, d_out,
+                                                                                     h->d_loss + loss_slot);
+      if (launch_check(h, "photometric_loss_kernel")) return -1;
+      return level_backward(h, lv, R, S, z, d, dcond, use_warp, alpha_step, rgb_step, d_out, nullptr, nullptr, w,
+                            rcfg, s);
+    };
     float* zc = h->d_zc + (size_t)r0 * nc;
-    float* wc = h->d_tr_w;
-    if (train_level(h, 0, R, nc, zc, o, d, tg, cond, dcond, scale, use_warp, h->d_tr_out, wc,
-                    h->d_loss + nfb::train::kSlotRgbCoarse, s, rcfg))
-      return -1;
+    if (level(0, nc, zc, h->d_tr_out, nfb::train::kSlotRgbCoarse)) return -1;
     if (fine) {
       float* zf = h->d_zf + (size_t)r0 * nfine;
-      if (run_resample(h, R, zc, wc, u_rand ? u_rand + (size_t)r0 * c.num_fine_samples : nullptr, zf, s) ||
-          train_level(h, 1, R, nfine, zf, o, d, tg, cond, dcond, scale, use_warp, h->d_tr_out + 6 * (size_t)R,
-                      h->d_tr_w, h->d_loss + nfb::train::kSlotRgbFine, s, rcfg))
+      if (run_resample(h, R, zc, w, u_rand ? u_rand + (size_t)r0 * c.num_fine_samples : nullptr, zf, s) ||
+          level(1, nfine, zf, h->d_tr_out + 6 * (size_t)R, nfb::train::kSlotRgbFine))
         return -1;
     }
   }
@@ -843,13 +810,19 @@ int nfb_render_vjp(nfb_handle* h, int B, const float* origins, const float* dire
     float* dcond = h->d_dcond + (size_t)r0 * h->cond_layout.stride;
     const float* o = origins + (size_t)r0 * 3;
     const float* d = directions + (size_t)r0 * 3;
-    if (coarse && vjp_level(h, 0, R, nc, z_coarse + (size_t)r0 * nc, o, d, cond, dcond, use_warp,
-                            at(d_out_coarse, (size_t)r0 * 6), at(d_weights_coarse, (size_t)r0 * nc),
-                            at(d_warped_coarse, (size_t)r0 * nc * 3), s))
+    // the taped forward of one level at z, then its backward from the caller's cotangents
+    auto level = [&](int lv, int S, const float* z, const float* d_out, const float* d_weights, const float* d_warped) {
+      int alpha_step = -1, rgb_step = -1;
+      if (level_forward(h, lv, R, S, z, o, d, cond, use_warp, h->d_tr_out, nullptr, s, &alpha_step, &rgb_step))
+        return -1;
+      return level_backward(h, lv, R, S, z, d, dcond, use_warp, alpha_step, rgb_step, d_out, d_weights, d_warped,
+                            nullptr, nullptr, s);
+    };
+    if (coarse && level(0, nc, z_coarse + (size_t)r0 * nc, at(d_out_coarse, (size_t)r0 * 6),
+                        at(d_weights_coarse, (size_t)r0 * nc), at(d_warped_coarse, (size_t)r0 * nc * 3)))
       return -1;
-    if (fine && vjp_level(h, 1, R, nfine, z_fine + (size_t)r0 * nfine, o, d, cond, dcond, use_warp,
-                          at(d_out_fine, (size_t)r0 * 6), at(d_weights_fine, (size_t)r0 * nfine),
-                          at(d_warped_fine, (size_t)r0 * nfine * 3), s))
+    if (fine && level(1, nfine, z_fine + (size_t)r0 * nfine, at(d_out_fine, (size_t)r0 * 6),
+                      at(d_weights_fine, (size_t)r0 * nfine), at(d_warped_fine, (size_t)r0 * nfine * 3)))
       return -1;
   }
   if (encoded) {
@@ -885,32 +858,18 @@ int nfb_warp_vjp(nfb_handle* h, int P, const float* points, const unsigned* warp
     const int n = std::min(chunk, P - p0);
     const TapeLayout t = tape_layout(p, n);
     float* A = h->d_tape;
-    if (encoded) {
-      // warp_points_forward with the caller's codes as the warp block of the condition vectors
-      const unsigned* codes = warp_id ? reinterpret_cast<const unsigned*>(reinterpret_cast<const float*>(warp_id) +
-                                                                          (size_t)p0 * G) : nullptr;
-      nfb::train::add_noise_kernel<<<(unsigned)(((long long)n * 3 + 255) / 256), 256, 0, s>>>(
-          points + (size_t)p0 * 3, nullptr, A + t.warped, (long long)n * 3);
-      if (launch_check(h, "add_noise_kernel") || run_cond(h, n, A + t.warped, codes, nullptr, nullptr, s, true, false) ||
-          warp_forward(h, p, t, nullptr, nullptr, nullptr, 1, A + t.warped, h->d_cond, s))
-        return -1;
-    } else if (warp_points_forward(h, n, points + (size_t)p0 * 3, nullptr, warp_id ? warp_id + p0 : nullptr,
-                                   c.warp_metadata_encoder == NFB_WARP_ENC_TIME, s)) {
+    // the chunk's ids, or with `encoded` its codes (G floats per point)
+    const unsigned* ids = !warp_id ? nullptr
+        : encoded ? reinterpret_cast<const unsigned*>(reinterpret_cast<const float*>(warp_id) + (size_t)p0 * G)
+                  : warp_id + p0;
+    if (warp_points_forward(h, n, points + (size_t)p0 * 3, nullptr, ids, c.warp_metadata_encoder == NFB_WARP_ENC_TIME,
+                            encoded, s))
       return -1;
-    }
     NFB_CUDA(cudaMemsetAsync(A + t.grad_begin, 0, (size_t)(t.grad_end - t.grad_begin) * sizeof(float), s));
     NFB_CUDA(cudaMemsetAsync(h->d_dcond, 0, (size_t)n * h->cond_layout.stride * sizeof(float), s));
     NFB_CUDA(cudaMemcpyAsync(A + t.dwarped, d_warped + (size_t)p0 * 3, (size_t)n * 3 * sizeof(float),
                              cudaMemcpyDeviceToDevice, s));
-    if (warp_backward(h, p, t, 1, h->d_dcond, s)) return -1;
-    if (encoded) {
-      if (cond_vjp_encoded(h, n, h->d_dcond, warp_id != nullptr, false, false,
-                           d_code ? d_code + (size_t)p0 * G : nullptr, nullptr, nullptr, s))
-        return -1;
-    } else if (run_cond_bwd(h, n, h->d_dcond, warp_id ? warp_id + p0 : nullptr, nullptr, nullptr, s) ||
-               time_backward(h, n, h->d_dcond, s)) {
-      return -1;
-    }
+    if (warp_points_backward(h, n, ids, encoded, d_code ? d_code + (size_t)p0 * G : nullptr, s)) return -1;
   }
   return unpack_grads(h, grads, count, s);
 }
@@ -931,7 +890,7 @@ int nfb_warp_jacobian(nfb_handle* h, int P, const float* points, const unsigned*
   for (int p0 = 0; p0 < P; p0 += chunk) {
     const int n = std::min(chunk, P - p0);
     if (warp_points_forward(h, n, points + (size_t)p0 * 3, nullptr, warp_id ? warp_id + p0 : nullptr,
-                            c.warp_metadata_encoder == NFB_WARP_ENC_TIME, s))
+                            c.warp_metadata_encoder == NFB_WARP_ENC_TIME, false, s))
       return -1;
     const nfb::FieldProgram& p = h->prog[0];
     const TapeLayout t = tape_layout(p, n);

@@ -294,7 +294,7 @@ def test_gradients_vs_autograd(name, train_precision):
 
 
 def test_training_step_at_max_samples():
-  """Both levels of a training step with Nc + Nf = kMaxSamples: the fine level's composite_bwd_kernel
+  """Both levels of a training step with Nc + Nf = kMaxSamples: the fine level's composite_vjp_kernel
   holds 1024 samples per ray in shared memory."""
   from nerfies_b200 import training
   spec, p, rays, _, ref = _reference('samples_max')

@@ -492,7 +492,7 @@ def test_sample_pdf_on_hand_built_weights(sizes, draws):
 
 
 # ---------------------------------------------------------------------------
-# 4. Backward at fixed z: composite_bwd_kernel and composite_vjp_kernel
+# 4. Backward at fixed z: composite_vjp_kernel seeded by the photometric loss and by given cotangents
 # ---------------------------------------------------------------------------
 def _grad_case(regime):
   S = 128

@@ -7,9 +7,9 @@ Measured, alternating R times after W warm-up calls each, with CUDA events on th
   value_and_grad: training.value_and_grad (photometric loss, fp32 training GEMMs);
   apply_backward: model.apply of the fp16x3 render kernels with the parameters requiring grad, torch's
     mean((rgb - target)^2) of both levels, and backward() (nfb_render_vjp, fp32 training GEMMs).
-Then one call of each under torch.profiler: the device time of composite_vjp_kernel (the VJP's seed)
-against composite_bwd_kernel (the training step's).  Reported: median, min and max of each, and the card's
-name, power limit and maximum SM clock (nvidia-smi, read-only query).
+Then one call of each under torch.profiler: the device time of composite_vjp_kernel, which seeds both
+backwards, and of photometric_loss_kernel, which writes its cotangents in the training step.  Reported: median,
+min and max of each, and the card's name, power limit and maximum SM clock (nvidia-smi, read-only query).
 """
 import argparse
 import json
@@ -108,15 +108,15 @@ def main():
   result['apply_backward_minus_value_and_grad_ms_median'] = (result['apply_backward_ms']['median'] -
                                                              result['value_and_grad_ms']['median'])
   kernels = {}
-  for fn in fns.values():
+  for key, fn in fns.items():
     torch.cuda.synchronize()
     with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
       fn(c)
       torch.cuda.synchronize()
     for e in prof.key_averages():
-      for name in ('composite_vjp_kernel', 'composite_bwd_kernel'):
+      for name in ('composite_vjp_kernel', 'photometric_loss_kernel'):
         if name in e.key:
-          k = kernels.setdefault(name, {'calls': 0, 'device_ms': 0.0})
+          k = kernels.setdefault(key, {}).setdefault(name, {'calls': 0, 'device_ms': 0.0})
           k['calls'] += e.count
           k['device_ms'] += e.device_time_total / 1000.0
   result['kernels'] = kernels
