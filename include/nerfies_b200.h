@@ -469,6 +469,51 @@ int nfb_near_far(const nfb_camera* cameras, int num_cameras, const double* point
                  double q_near, double q_far, void* workspace, long long workspace_bytes, double* near,
                  double* far, long long* counts, void* stream);
 
+/* ---- surface extraction: marching cubes (no reference analogue) -----------------------------
+ * grid: (nz, ny, nx) float32, C-contiguous, x fastest; value [k][j][i] lies at
+ * origin + (i, j, k) * spacing.  Every side lies in [2, 1024].  No handle, ordered on `stream`.
+ *   - a point is inside iff value > level, so NaN is outside (the mesh stays closed around
+ *     non-finite cells) and value == level is outside;
+ *   - one vertex per grid edge whose endpoints lie on different sides, shared by the cubes around the
+ *     edge: the mesh is indexed and watertight.  Vertices are ordered by (edge axis, linear index of
+ *     the edge's lower endpoint); faces by cube (linear index of its lowest corner), then table order;
+ *   - vertex on the edge p0 -> p1 (values v0, v1; p1 one step along the edge's axis), in float32,
+ *     each operation rounded once, no fused multiply-add:
+ *       t = (level - v0) / (v1 - v0)                      (t = 0.5 when v0 or v1 is NaN)
+ *       x0 = origin + float(index) * spacing, x1 = origin + float(index + 1) * spacing
+ *       x  = x0 + t * (x1 - x0) along the edge's axis, x0 across it;
+ *   - normal: the central-difference gradient of the grid over the spacing (one-sided on the border)
+ *     at both endpoints, interpolated with the same t, normalised and negated (it points toward lower
+ *     values, out of the surface).  A zero or non-finite gradient gives a zero normal;
+ *   - triangles are counter-clockwise seen from outside (from lower values): the signed volume of a
+ *     closed surface around a dense region is positive;
+ *   - the mesh is open where the surface leaves the grid; it is not capped.
+ * Two calls on the same grid write bitwise-equal meshes (no atomics).
+ *
+ * Bytes of device workspace for this grid (< 0: invalid size, or no device): 16 bytes per grid point
+ * (a 32-bit vertex id per edge, a 32-bit face offset per cube) plus CUB's scan scratch. */
+long long nfb_marching_cubes_workspace_size(int nx, int ny, int nz);
+/* Classifies the grid into the workspace (device, 256-byte aligned, at least
+ * nfb_marching_cubes_workspace_size bytes) and writes counts_out (device, 4 int64): the number of
+ * vertices, the number of faces, and the ids of the first vertex on a y-edge and on a z-edge (vertices
+ * before the first are on x-edges).  Asynchronous: two kernels and three CUB passes, no host
+ * synchronisation. */
+int nfb_marching_cubes_count(const float* grid, int nx, int ny, int nz, float level, void* workspace,
+                             long long workspace_bytes, long long* counts_out, void* stream);
+/* Writes the mesh the preceding nfb_marching_cubes_count call on the same grid, level and workspace
+ * counted: vertices (V, 3) float32, normals (V, 3) float32 (nullable) and faces (F, 3) int32 vertex
+ * indices.  origin and spacing are HOST arrays of 3 floats.  It first reads the two totals back (one
+ * small copy and a stream synchronisation) and fails when either exceeds INT32_MAX. */
+int nfb_marching_cubes(const float* grid, int nx, int ny, int nz, float level, const float* origin,
+                       const float* spacing, void* workspace, long long workspace_bytes, float* vertices,
+                       float* normals, int* faces, void* stream);
+/* The case table, host only (needs no device).  Corner c of a cube sits at offset
+ * (c & 1, c >> 1 & 1, c >> 2 & 1); edge e = 4 * axis + u + 2 v runs along `axis` from the corner whose
+ * coordinates along the other two axes, the lower axis first, are (u, v).  Case bits: bit c set iff
+ * corner c is inside.  Returns the largest triangle count of any case (M) and, when out is not NULL,
+ * writes 256 rows of 1 + 3 M ints: the case's triangle count, then its triangles' edges (-1 padded). */
+int nfb_marching_cubes_table(int* out);
+
 /* Test hook for the abort path described in the conventions above: while enabled,
  * the weight producer of the tensor-core kernel first waits on an mbarrier that never
  * completes, so the launch must time out, drain and raise the abort flag

@@ -24,7 +24,8 @@ SYMBOLS = [
     'nfb_set_train_precision', 'nfb_selftest_train_gemm', 'nfb_debug_one_row_block',
     'nfb_image_quantize', 'nfb_render_vjp', 'nfb_warp_vjp', 'nfb_colorize',
     'nfb_frame_pyramid', 'nfb_blur_scores_workspace_size', 'nfb_blur_scores', 'nfb_camera_project',
-    'nfb_near_far_workspace_size', 'nfb_near_far',
+    'nfb_near_far_workspace_size', 'nfb_near_far', 'nfb_marching_cubes_workspace_size',
+    'nfb_marching_cubes_count', 'nfb_marching_cubes', 'nfb_marching_cubes_table',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -233,6 +234,15 @@ def load():
   lib.nfb_near_far_workspace_size.restype = ll
   lib.nfb_near_far.argtypes = [vp, ci, vp, ll, ctypes.c_double, ctypes.c_double, vp, ll, vp, vp, vp, vp]
   lib.nfb_near_far.restype = ci
+  lib.nfb_marching_cubes_workspace_size.argtypes = [ci, ci, ci]
+  lib.nfb_marching_cubes_workspace_size.restype = ll
+  lib.nfb_marching_cubes_count.argtypes = [vp, ci, ci, ci, cf, vp, ll, vp, vp]
+  lib.nfb_marching_cubes_count.restype = ci
+  lib.nfb_marching_cubes.argtypes = [vp, ci, ci, ci, cf, ctypes.POINTER(cf), ctypes.POINTER(cf), vp, ll, vp, vp,
+                                     vp, vp]
+  lib.nfb_marching_cubes.restype = ci
+  lib.nfb_marching_cubes_table.argtypes = [ctypes.POINTER(ci)]
+  lib.nfb_marching_cubes_table.restype = ci
   lib.nfb_selftest_gemm3.argtypes =[ci, ci, vp, vp, vp, ci, vp, vp]
   lib.nfb_selftest_gemm3.restype = ci
   lib.nfb_selftest_sgemm.argtypes = [ci, ll, ci, ci, ci, ci, vp, ci, vp, ci, vp, ci] + [vp] * 6 + [

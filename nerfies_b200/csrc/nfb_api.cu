@@ -20,6 +20,7 @@
 #include "image_kernels.cuh"
 #include "viz_kernels.cuh"
 #include "capture_kernels.cuh"
+#include "mesh_kernels.cuh"
 #include "tc_common.cuh"
 #include "tc_selftest.cuh"
 #include "field_tc.cuh"
@@ -905,6 +906,126 @@ int nfb_near_far(const nfb_camera* cameras, int num_cameras, const double* point
   e = cudaGetLastError();
   if (e != cudaSuccess) return fail("near/far launch failed: %s", cudaGetErrorString(e));
   return 0;
+}
+
+// Workspace of marching cubes: edge ids (3n + 1), triangle offsets (n + 1), the two int64 totals and
+// CUB's scratch, each 256-byte aligned.
+struct MeshPlan {
+  long long n, ids_off, tris_off, totals_off, temp_off, temp_bytes, bytes;
+};
+
+static int mesh_plan(const char* fn, int nx, int ny, int nz, MeshPlan* p) {
+  using nfb::mesh::kMaxSide;
+  if (nx < 2 || ny < 2 || nz < 2 || nx > kMaxSide || ny > kMaxSide || nz > kMaxSide)
+    return fail("%s: grid %d x %d x %d (nx, ny, nz): every side must lie in [2, %d]", fn, nx, ny, nz, kMaxSide);
+  auto align = [](long long b) { return (b + 255) / 256 * 256; };
+  p->n = (long long)nx * ny * nz;
+  p->ids_off = 0;
+  p->tris_off = align((3 * p->n + 1) * (long long)sizeof(unsigned));
+  p->totals_off = p->tris_off + align((p->n + 1) * (long long)sizeof(unsigned));
+  p->temp_off = p->totals_off + 256;
+  size_t scan_edges = 0, scan_cubes = 0, reduce = 0;
+  unsigned* u = nullptr;
+  long long* ll = nullptr;
+  if (cub::DeviceScan::ExclusiveSum(nullptr, scan_edges, u, u, 3 * p->n + 1) != cudaSuccess ||
+      cub::DeviceScan::ExclusiveSum(nullptr, scan_cubes, u, u, p->n + 1) != cudaSuccess ||
+      cub::DeviceReduce::Sum(nullptr, reduce, u, ll, p->n + 1) != cudaSuccess) {
+    cudaGetLastError();
+    return fail("%s: no CUDA device: nerfies_b200 has no CPU path", fn);
+  }
+  p->temp_bytes = align((long long)std::max(scan_edges, std::max(scan_cubes, reduce)));
+  p->bytes = p->temp_off + p->temp_bytes;
+  return 0;
+}
+
+static nfb::mesh::MeshArgs mesh_args(const float* grid, int nx, int ny, int nz, float level, void* workspace,
+                                     const MeshPlan& p) {
+  nfb::mesh::MeshArgs a{};
+  char* ws = static_cast<char*>(workspace);
+  a.grid = grid; a.nx = nx; a.ny = ny; a.nz = nz; a.n = p.n; a.level = level;
+  a.edge_ids = reinterpret_cast<unsigned*>(ws + p.ids_off);
+  a.tri_offsets = reinterpret_cast<unsigned*>(ws + p.tris_off);
+  a.totals = reinterpret_cast<long long*>(ws + p.totals_off);
+  return a;
+}
+
+static int mesh_check(const char* fn, const float* grid, void* workspace, long long workspace_bytes,
+                      const MeshPlan& p) {
+  if (!grid || !workspace) return fail("%s: null argument", fn);
+  if (workspace_bytes < p.bytes)
+    return fail("%s: workspace of %lld bytes is smaller than the %lld bytes nfb_marching_cubes_workspace_size returns",
+                fn, workspace_bytes, p.bytes);
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail("%s: workspace must be 256-byte aligned", fn);
+  if (reinterpret_cast<uintptr_t>(grid) & 3) return fail("%s: grid must be 4-byte aligned", fn);
+  return 0;
+}
+
+long long nfb_marching_cubes_workspace_size(int nx, int ny, int nz) {
+  MeshPlan p;
+  return mesh_plan("nfb_marching_cubes_workspace_size", nx, ny, nz, &p) ? -1 : p.bytes;
+}
+
+int nfb_marching_cubes_count(const float* grid, int nx, int ny, int nz, float level, void* workspace,
+                             long long workspace_bytes, long long* counts_out, void* stream) {
+  using namespace nfb::mesh;
+  const char* fn = "nfb_marching_cubes_count";
+  MeshPlan p;
+  if (mesh_plan(fn, nx, ny, nz, &p) || mesh_check(fn, grid, workspace, workspace_bytes, p)) return -1;
+  if (!counts_out) return fail("%s: null argument", fn);
+  cudaStream_t s = (cudaStream_t)stream;
+  MeshArgs a = mesh_args(grid, nx, ny, nz, level, workspace, p);
+  void* temp = static_cast<char*>(workspace) + p.temp_off;
+  size_t temp_bytes = (size_t)p.temp_bytes;
+  classify_kernel<<<(unsigned)((p.n + kThreads - 1) / kThreads), kThreads, 0, s>>>(a);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = cub::DeviceReduce::Sum(temp, temp_bytes, a.tri_offsets, a.totals + 1, p.n + 1, s);
+  if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(temp, temp_bytes, a.edge_ids, a.edge_ids, 3 * p.n + 1, s);
+  if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(temp, temp_bytes, a.tri_offsets, a.tri_offsets, p.n + 1, s);
+  if (e == cudaSuccess) {
+    finish_counts_kernel<<<1, 1, 0, s>>>(a, counts_out);
+    e = cudaGetLastError();
+  }
+  if (e != cudaSuccess) return fail("%s: launch failed: %s", fn, cudaGetErrorString(e));
+  return 0;
+}
+
+int nfb_marching_cubes(const float* grid, int nx, int ny, int nz, float level, const float* origin,
+                       const float* spacing, void* workspace, long long workspace_bytes, float* vertices,
+                       float* normals, int* faces, void* stream) {
+  using namespace nfb::mesh;
+  const char* fn = "nfb_marching_cubes";
+  MeshPlan p;
+  if (mesh_plan(fn, nx, ny, nz, &p) || mesh_check(fn, grid, workspace, workspace_bytes, p)) return -1;
+  if (!origin || !spacing) return fail("%s: null argument", fn);
+  cudaStream_t s = (cudaStream_t)stream;
+  MeshArgs a = mesh_args(grid, nx, ny, nz, level, workspace, p);
+  long long totals[2] = {0, 0};
+  NFB_CUDA(cudaMemcpyAsync(totals, a.totals, sizeof(totals), cudaMemcpyDeviceToHost, s));
+  NFB_CUDA(cudaStreamSynchronize(s));
+  if (totals[0] > INT32_MAX || totals[1] > INT32_MAX)
+    return fail("%s: %lld vertices and %lld faces: int32 indices hold at most %d", fn, totals[0], totals[1],
+                INT32_MAX);
+  if ((totals[0] && !vertices) || (totals[1] && !faces)) return fail("%s: null argument", fn);
+  for (int d = 0; d < 3; ++d) { a.origin[d] = origin[d]; a.spacing[d] = spacing[d]; }
+  a.vertices = vertices; a.normals = normals; a.faces = faces;
+  if (totals[0]) vertex_kernel<<<(unsigned)((3 * p.n + kThreads - 1) / kThreads), kThreads, 0, s>>>(a);
+  if (totals[1]) face_kernel<<<(unsigned)((p.n + kThreads - 1) / kThreads), kThreads, 0, s>>>(a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("%s: launch failed: %s", fn, cudaGetErrorString(e));
+  return 0;
+}
+
+int nfb_marching_cubes_table(int* out) {
+  using namespace nfb::mesh;
+  if (out) {
+    const int row = 1 + 3 * kMaxTriangles;
+    for (int cs = 0; cs < 256; ++cs) {
+      const int n = kCaseTable.count[cs];
+      out[cs * row] = n;
+      for (int i = 0; i < 3 * kMaxTriangles; ++i) out[cs * row + 1 + i] = i < 3 * n ? kCaseTable.edge[cs][i] : -1;
+    }
+  }
+  return kMaxTriangles;
 }
 
 int nfb_colorize(const float* a, const float* b, int height, int width, int source, const double* table,
