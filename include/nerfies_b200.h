@@ -286,6 +286,30 @@ int nfb_warp_vjp(nfb_handle* h, int num_points, const float* points, const unsig
 int nfb_warp_jacobian(nfb_handle* h, int P, const float* points, const unsigned* warp_id, float warp_alpha,
                       float* warped_out, float* jacobian_out, void* stream);
 
+/* Per-point outcome of nfb_warp_invert. */
+enum { NFB_INVERT_CONVERGED = 0,   /* |W(x) - target| <= tol                                         */
+       NFB_INVERT_MAX_ITERS = 1,   /* still improving when the iterations ran out                     */
+       NFB_INVERT_SINGULAR = 2,    /* J at the best iterate is singular or not finite                 */
+       NFB_INVERT_STALLED = 3,     /* no step down to 2^-10 of the Newton step lowered the residual   */
+       NFB_INVERT_NONFINITE = 4 }; /* W at the starting point is not finite                           */
+
+/* Solve W(x) = target for x at free points, where W is the warp field of the frame that warp_id names
+ * (nfb_warp_jacobian's W, ids or NFB_WARP_ENC_TIME timestamps; encoded metadata is not supported).
+ *   targets (P,3): template points; init (P,3) nullable: starting points (NULL: the targets);
+ *   max_iters in [1, 64]; tol > 0 (absolute, in scene units);
+ *   points_out (P,3): the best iterate; residual_out (P): |W(points_out) - target|_2;
+ *   jacobian_out (P,3,3) nullable: J at points_out; status_out (P) nullable int32 (NFB_INVERT_*).
+ * Damped Newton: each of the max_iters iterations evaluates W and J at every point's candidate (the
+ * tape kernels of nfb_warp_jacobian) and then, per point in fp64, accepts a candidate whose residual is
+ * finite and below the best so far and takes the full Newton step from it (3x3 LU, partial pivoting), or
+ * halves the step from the best iterate.  Converged, singular, stalled and non-finite points are frozen.
+ * A fixed iteration count and no atomics: the call never synchronises with the host, and a point's
+ * results do not depend on the other points.  Chunks of max_rays points; the handle's training precision
+ * (fp32 or tf32x3), whatever nfb_config.precision is. */
+int nfb_warp_invert(nfb_handle* h, int P, const float* targets, const float* init, const unsigned* warp_id,
+                    float warp_alpha, int max_iters, float tol, float* points_out, float* residual_out,
+                    float* jacobian_out, int* status_out, void* stream);
+
 /* flax.optim.Adam.apply_gradient (training.py:268; beta1 0.9, beta2 0.999, eps 1e-8, no
  * weight decay are the Flax defaults the reference uses, train.py:219) on flat device
  * vectors of n floats; `step` counts from 1 (bias correction 1 - beta^step).  No handle. */

@@ -25,7 +25,7 @@ SYMBOLS = [
     'nfb_image_quantize', 'nfb_render_vjp', 'nfb_warp_vjp', 'nfb_colorize',
     'nfb_frame_pyramid', 'nfb_blur_scores_workspace_size', 'nfb_blur_scores', 'nfb_camera_project',
     'nfb_near_far_workspace_size', 'nfb_near_far', 'nfb_marching_cubes_workspace_size',
-    'nfb_marching_cubes_count', 'nfb_marching_cubes', 'nfb_marching_cubes_table',
+    'nfb_marching_cubes_count', 'nfb_marching_cubes', 'nfb_marching_cubes_table', 'nfb_warp_invert',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -50,6 +50,8 @@ TRAIN_PRECISIONS = {'fp32': 0, 'tf32x3': 1}
 FLAG_COARSE_ONLY = 1
 FLAG_NO_WARP = 2
 FLAG_METADATA_ENCODED = 4
+# nfb_warp_invert's per-point status (NFB_INVERT_*)
+INVERT_STATUS = {'converged': 0, 'max_iters': 1, 'singular': 2, 'stalled': 3, 'nonfinite': 4}
 
 
 class NfbConfig(ctypes.Structure):
@@ -190,6 +192,8 @@ def load():
   lib.nfb_warp_vjp.restype = ci
   lib.nfb_warp_jacobian.argtypes = [vp, ci, vp, vp, cf, vp, vp, vp]
   lib.nfb_warp_jacobian.restype = ci
+  lib.nfb_warp_invert.argtypes = [vp, ci, vp, vp, vp, cf, ci, cf, vp, vp, vp, vp, vp]
+  lib.nfb_warp_invert.restype = ci
   lib.nfb_check_abort.argtypes = [vp, ci]
   lib.nfb_check_abort.restype = ci
   lib.nfb_reset_abort.argtypes = []

@@ -1255,6 +1255,7 @@ void nfb_destroy(nfb_handle* h) {
                     h->d_ttape, reinterpret_cast<float*>(h->d_sel), h->d_time_tape};
   for (float* p : tbufs) if (p) cudaFree(p);
   if (h->d_ids) cudaFree(h->d_ids);
+  if (h->d_invert) cudaFree(h->d_invert);
   for (int l = 0; l < 2; ++l)
     for (int i = 0; i < 2; ++i) if (h->ev[l][i]) cudaEventDestroy(h->ev[l][i]);
   if (h->h_in) cudaFreeHost(h->h_in);

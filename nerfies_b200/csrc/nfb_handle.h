@@ -103,6 +103,7 @@ struct nfb_handle {
   float* d_ttape = nullptr; long long ttape_floats = 0;     // tangent tape (train_reg.cuh)
   float* d_time_tape = nullptr; long long time_tape_floats = 0;  // TimeEncoder tape, max_rays rows (time_forward)
   int* d_sel = nullptr; long long sel_cap = 0;              // selected tape rows (median-depth samples)
+  void* d_invert = nullptr;           // nfb_warp_invert's per-point state, max_rays rows (allocated on first use)
   int train_precision = NFB_TRAIN_FP32;                     // the training GEMMs' kernel (launch_gemm)
   int debug_bits = 0;                 // FieldArgs::debug bits set through the test hook (abort-path test)
   // tensor-core path (precision != fp32)

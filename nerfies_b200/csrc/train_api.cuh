@@ -5,6 +5,7 @@
 #include "train.cuh"
 #include "train_reg.cuh"
 #include "train_tc.cuh"
+#include "warp_invert.cuh"
 
 namespace {
 
@@ -220,14 +221,20 @@ struct RegCfg {
   float* stats = nullptr;         // device: nfb_train_value_and_grad_reg's loss_out layout
 };
 
+// The warp Jacobian's restriction: the tangent rows take the activation masks of a piecewise-linear MLP.
+int check_relu_warp(const nfb::FieldProgram& p, const char* what) {
+  for (int i = 0; i < p.warp.n_steps - 1; ++i)
+    if (p.warp.steps[i].act != nfb::kRelu && p.warp.steps[i].act != nfb::kNone)
+      return fail("%s: the warp MLP must use relu (piecewise-linear) activations", what);
+  return 0;
+}
+
 // Jacobian (+ elastic loss and its adjoint when `with_grad`) at `sel_rows` tape rows of the warp tape in `A`.
 int warp_jacobian_on_tape(nfb_handle* h, const nfb::FieldProgram& p, const TapeLayout& t, float* A, const int* sel,
                           long long sel_rows, const float* row_w, const RegCfg* reg, bool with_grad, float* jac_out,
                           cudaStream_t s) {
   using namespace nfb::train;
-  for (int i = 0; i < p.warp.n_steps - 1; ++i)
-    if (p.warp.steps[i].act != nfb::kRelu && p.warp.steps[i].act != nfb::kNone)
-      return fail("warp Jacobian: the warp MLP must use relu (piecewise-linear) activations");
+  if (check_relu_warp(p, "warp Jacobian")) return -1;
   const TTapeLayout tt = ttape_layout(p, sel_rows);
   if (grow(&h->d_ttape, &h->ttape_floats, tt.total, "tangent tape")) return -1;
   float* T = h->d_ttape;
@@ -627,6 +634,27 @@ int warp_points_backward(nfb_handle* h, int n, const unsigned* warp_id, bool enc
   return run_cond_bwd(h, n, h->d_dcond, warp_id, nullptr, nullptr, s) || time_backward(h, n, h->d_dcond, s) ? -1 : 0;
 }
 
+// nfb_warp_invert's per-point state for max_rays points, carved from one allocation made on first use.
+constexpr long long kInvertRowBytes = 4 * sizeof(double) + 25 * sizeof(float) + sizeof(int);   // 136
+int invert_state(nfb_handle* h, nfb::train::InvertState* st) {
+  const long long R = h->max_rays;
+  if (!h->d_invert && cudaMalloc(&h->d_invert, (size_t)(R * kInvertRowBytes)) != cudaSuccess) {
+    h->d_invert = nullptr;
+    return fail("warp invert: cannot allocate its %lld-byte workspace", R * kInvertRowBytes);
+  }
+  char* b = static_cast<char*>(h->d_invert);
+  auto take = [&](long long bytes) { char* p = b; b += bytes; return p; };
+  st->dx = reinterpret_cast<double*>(take(R * 3 * sizeof(double)));
+  st->rb = reinterpret_cast<double*>(take(R * sizeof(double)));
+  st->cand = reinterpret_cast<float*>(take(R * 3 * sizeof(float)));
+  st->jac = reinterpret_cast<float*>(take(R * 9 * sizeof(float)));
+  st->xb = reinterpret_cast<float*>(take(R * 3 * sizeof(float)));
+  st->jb = reinterpret_cast<float*>(take(R * 9 * sizeof(float)));
+  st->lam = reinterpret_cast<float*>(take(R * sizeof(float)));
+  st->status = reinterpret_cast<int*>(take(R * sizeof(int)));
+  return 0;
+}
+
 // compute_background_loss (training.py:118-135) and its gradient, in chunks of max_rays points.
 int train_background(nfb_handle* h, int P, const float* points, const unsigned* warp_ids, const float* noise,
                      float weight, cudaStream_t s) {
@@ -899,6 +927,50 @@ int nfb_warp_jacobian(nfb_handle* h, int P, const float* points, const unsigned*
                                cudaMemcpyDeviceToDevice, s));
     if (warp_jacobian_on_tape(h, p, t, h->d_tape, nullptr, n, nullptr, nullptr, false, jacobian_out + (size_t)p0 * 9, s))
       return -1;
+  }
+  return 0;
+}
+
+int nfb_warp_invert(nfb_handle* h, int P, const float* targets, const float* init, const unsigned* warp_id,
+                    float warp_alpha, int max_iters, float tol, float* points_out, float* residual_out,
+                    float* jacobian_out, int* status_out, void* stream) {
+  if (!h || !targets || !points_out || !residual_out) return fail("null argument");
+  if (P < 0) return fail("P must be >= 0");
+  if (check_call(h, std::min(P, h->max_rays))) return -1;
+  const nfb_config& c = h->cfg;
+  const nfb::FieldProgram& p = h->prog[0];
+  if (p.warp_type == 0) return fail("the model has no warp field");
+  if (check_relu_warp(p, "warp invert")) return -1;
+  if (max_iters < 1 || max_iters > 64) return fail("warp invert: max_iters=%d outside [1, 64]", max_iters);
+  if (!std::isfinite(tol) || !(tol > 0.f)) return fail("warp invert: tol=%g must be finite and > 0", (double)tol);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (enter_stream(h, s)) return -1;
+  if (P == 0) return 0;
+  if (set_window(h, warp_alpha, s)) return -1;
+  const int chunk = std::min(P, h->max_rays);
+  nfb::train::InvertState st{};
+  if (train_prepare_rows(h, chunk) || invert_state(h, &st)) return -1;
+  const bool float_time = c.warp_metadata_encoder == NFB_WARP_ENC_TIME;
+  for (int p0 = 0; p0 < P; p0 += chunk) {
+    const int n = std::min(chunk, P - p0);
+    const TapeLayout t = tape_layout(p, n);
+    const unsigned* ids = warp_id ? warp_id + p0 : nullptr;
+    const float* start = (init ? init : targets) + (size_t)p0 * 3;
+    NFB_CUDA(cudaMemcpyAsync(st.cand, start, (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    nfb::train::InvertStepArgs a{};
+    a.st = st; a.warped = h->d_tape + t.warped; a.target = targets + (size_t)p0 * 3; a.tol = tol; a.n = n;
+    a.points_out = points_out + (size_t)p0 * 3; a.residual_out = residual_out + p0;
+    a.jacobian_out = jacobian_out ? jacobian_out + (size_t)p0 * 9 : nullptr;
+    a.status_out = status_out ? status_out + p0 : nullptr;
+    // a fixed number of iterations, no readback: frozen points ride along unchanged
+    for (int it = 0; it < max_iters; ++it) {
+      if (warp_points_forward(h, n, st.cand, nullptr, ids, float_time, false, s) ||
+          warp_jacobian_on_tape(h, p, t, h->d_tape, nullptr, n, nullptr, nullptr, false, st.jac, s))
+        return -1;
+      a.first = it == 0; a.last = it == max_iters - 1;
+      nfb::train::warp_invert_step_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(a);
+      if (launch_check(h, "warp_invert_step_kernel")) return -1;
+    }
   }
   return 0;
 }

@@ -1,6 +1,7 @@
 """A trained model's surface as a triangle mesh: the density on a 3D grid through the render
 kernels, marching cubes in CUDA (include/nerfies_b200.h, nfb_marching_cubes*), vertex colours and
-a binary PLY writer.  No reference analogue: the reference renders images only.
+a binary PLY writer; the inverse of the warp field (nfb_warp_invert), which carries the template mesh
+into a frame with its topology.  No reference analogue: the reference renders images only.
 
 Grids are (nz, ny, nx) float32 on the device, x fastest; a box ((x0, y0, z0), (x1, y1, z1)) holds the
 grid's first and last points on each axis, so value [k, j, i] lies at box[0] + (i, j, k) * spacing with
@@ -43,22 +44,25 @@ def _axis_points(lo, spacing, n, dev):
 def _metadata_ids(model, metadata, n):
   """(warp_id, app_id, cam_id) device tensors of n rays from scalar metadata, as models.apply reads them."""
   md = metadata or {}
-  dev = model.device
+  return (_warp_ids(model, md, n), _ids(model, md, 'appearance', model.use_appearance_metadata, n),
+          _ids(model, md, 'camera', model.use_camera_metadata, n))
 
-  def ids(key, used):
-    if not used:
-      return None
-    if key not in md:
-      raise KeyError(f"metadata['{key}'] is required by this model")
-    return torch.full((n,), int(md[key]), dtype=torch.int32, device=dev)
 
+def _ids(model, md, key, used, n):
+  if not used:
+    return None
+  if key not in md:
+    raise KeyError(f"metadata['{key}'] is required by this model")
+  return torch.full((n,), int(md[key]), dtype=torch.int32, device=model.device)
+
+
+def _warp_ids(model, md, n):
+  """The warp metadata of n rays or points: float timestamps with the 'time' encoder, ids otherwise."""
   if model.use_warp and model.warp_metadata_encoder_type == 'time':
     if 'time' not in md:
       raise KeyError("metadata['time'] is required by this model")
-    warp_id = torch.full((n,), float(md['time']), dtype=torch.float32, device=dev)
-  else:
-    warp_id = ids('warp', model.use_warp)
-  return warp_id, ids('appearance', model.use_appearance_metadata), ids('camera', model.use_camera_metadata)
+    return torch.full((n,), float(md['time']), dtype=torch.float32, device=model.device)
+  return _ids(model, md, 'warp', model.use_warp, n)
 
 
 def _prepare(model, params, warp_extra, use_warp, level):
@@ -152,6 +156,59 @@ def vertex_colors(model, params, vertices, normals, warp_extra=None, metadata=No
           _ptr(app_id), _ptr(cam_id), alpha, flags, None, None, _ptr(samples), None, _stream()))
       colors[first:first + B] = samples[:B, 0, :3]
   return colors
+
+
+def invert_warp(model, params, targets, warp_extra=None, metadata=None, init=None, max_iters=16, tol=1e-5,
+                return_jacobian=False):
+  """The points x of the frame the metadata names whose warp W(x) is `targets` (P, 3) template points
+  (nfb_warp_invert: damped Newton on the warp field and its Jacobian, from `init` or the targets).
+  Returns {'points' (P, 3), 'residual' (P,) |W(points) - targets|, 'status' (P,) int32
+  (_lib.INVERT_STATUS)[, 'jacobian' (P, 3, 3) J at points]}, all on the model's device.  Only points
+  whose status is converged are within `tol` of a preimage; the others hold the best iterate found."""
+  if not model.use_warp:
+    raise ValueError('invert_warp: the model has no warp field')
+  dev = model.device
+  targets = torch.as_tensor(targets).to(device=dev, dtype=torch.float32).contiguous()
+  if targets.dim() != 2 or targets.shape[-1] != 3:
+    raise ValueError(f'invert_warp: targets must be (P, 3), got {tuple(targets.shape)}')
+  P = targets.shape[0]
+  if init is not None:
+    init = torch.as_tensor(init).to(device=dev, dtype=torch.float32).contiguous()
+    if init.shape != targets.shape:
+      raise ValueError(f'invert_warp: init must be {tuple(targets.shape)}, got {tuple(init.shape)}')
+  hd, alpha, _, _ = _prepare(model, params, warp_extra, True, 'coarse')
+  warp_id = _warp_ids(model, metadata or {}, P)
+  out = {'points': torch.empty(P, 3, device=dev), 'residual': torch.empty(P, device=dev),
+         'status': torch.empty(P, dtype=torch.int32, device=dev)}
+  jac = torch.empty(P, 3, 3, device=dev) if return_jacobian else None
+  if P == 0:
+    return dict(out, jacobian=jac) if return_jacobian else out
+  with torch.cuda.device(dev):
+    _lib.check(hd.lib.nfb_warp_invert(hd.h, P, _ptr(targets), _ptr(init), _ptr(warp_id), alpha, int(max_iters),
+                                      float(tol), _ptr(out['points']), _ptr(out['residual']), _ptr(jac),
+                                      _ptr(out['status']), _stream()))
+  if return_jacobian:
+    out['jacobian'] = jac
+  return out
+
+
+def track_surface(model, params, vertices, normals, warp_extra, metadata, init=None, tol=1e-5, max_iters=16):
+  """A template mesh's vertices (V, 3) and outward normals carried into the frame the metadata names:
+  the vertices are invert_warp's points, the normals normalize(J^T n), the gradient direction of
+  sigma_template(W(x)) (zero where n is).  Where det J <= 0 the warp folds locally and the faces'
+  winding flips there; such vertices are counted ('folded'), not repaired.
+  Returns {'vertices', 'normals', 'residual', 'status', 'folded' (int)}."""
+  if vertices.dim() != 2 or vertices.shape[-1] != 3 or normals.shape != vertices.shape:
+    raise ValueError(f'vertices and normals must both be (V, 3), got {tuple(vertices.shape)} and '
+                     f'{tuple(normals.shape)}')
+  inv = invert_warp(model, params, vertices, warp_extra, metadata, init=init, max_iters=max_iters, tol=tol,
+                    return_jacobian=True)
+  J = inv['jacobian']
+  n = normals.to(device=J.device, dtype=torch.float32)
+  moved = torch.nn.functional.normalize((J.transpose(1, 2) @ n.unsqueeze(-1)).squeeze(-1), dim=-1)
+  folded = int((torch.linalg.det(J.double()) <= 0).sum()) if len(J) else 0
+  return {'vertices': inv['points'], 'normals': moved, 'residual': inv['residual'], 'status': inv['status'],
+          'folded': folded}
 
 
 def marching_cubes(grid, level, bbox, return_axes=False):
