@@ -662,6 +662,38 @@ int nfb_selftest_train_gemm(int train_precision, int mode, long long rows, int n
                             const float* bias, float* y, const float* dy, float* dx, float* din, float* dw,
                             long long k_split, long long* k_split_used, void* stream);
 
+/* Self-tests of the training step's seed and regulariser kernels: each launches the production kernel with the
+ * production launch configuration and argument struct on caller buffers.  Device pointers; no handle; allocates
+ * nothing; asynchronous on `stream`.  Bad arguments fail (nfb_last_error).  No reference analogue.
+ *
+ * nfb_selftest_composite_vjp: raw_to_samples_kernel, then composite_vjp_kernel (the adjoint of
+ *   volumetric_rendering) for R rays of S <= 1024 samples.  rgb_raw (R*S, ld_rgb >= 3), alpha_raw (R*S, ld_a >= 1),
+ *   z (R,S), directions (R,3); d_out (R,6: rgb, depth, med_depth (ignored), acc) and d_weights (R,S) are the
+ *   cotangents, each nullable; sigma_act an activation of nfb_config.  Writes samples_out (R*S, 4: sigmoid(rgb),
+ *   sigma; 16-byte aligned) and d_rgb_raw, d_alpha_raw in the layouts of rgb_raw and alpha_raw (=, columns 0-2 and 0).
+ * nfb_selftest_elastic: jac_elastic_kernel at R points.  warp_type 1 (translation: J = I + Th^T) or 2 (SE(3); heads
+ *   [w v (pivot) (translation)], nh = 6 + 3 pivot + 3 trans).  head (rows, ld) and pts (rows, 3) are indexed by
+ *   sel[r] (nullable: r), thead ((3R), ld) by r: row 3r + j holds d head / d x_j.  loss_type NFB_ELASTIC_*;
+ *   row_w (rows) nullable; grad_scale multiplies the gradients.  Outputs, each nullable (at least one): jac_out
+ *   (R,9) = J, stats += [sum w loss, sum residual, sum det, sum div, sum |curl|], d_thead (=, same layout as thead),
+ *   d_head (+=, rows of head; needed with d_thead when warp_type is 2).
+ * nfb_selftest_depth_index: depth_index_kernel, sel[r] = r S + the median-depth sample of weights (R,S) (0 when the
+ *   cumulative weight never reaches 0.5).
+ * nfb_selftest_warp_mag_loss: warp_mag_loss_kernel, the robust loss (alpha, scale > 0) of |warped - pts|^2 at rows
+ *   sel[r] (nullable: r) of pts, warped (rows,3): stats += [sum loss, sum |warped - pts|], dwarped (nullable)
+ *   += grad_scale d loss / d warped. */
+int nfb_selftest_composite_vjp(int R, int S, const float* rgb_raw, int ld_rgb, const float* alpha_raw, int ld_a,
+                               const float* z, const float* directions, const float* d_out, const float* d_weights,
+                               int white_bg, int sample_at_infinity, int sigma_act, float* samples_out,
+                               float* d_rgb_raw, float* d_alpha_raw, void* stream);
+int nfb_selftest_elastic(long long R, int warp_type, int pivot, int trans, int loss_type, const float* head,
+                         const float* thead, int ld, const float* pts, const int* sel, const float* row_w,
+                         float grad_scale, float* jac_out, float* d_head, float* d_thead, float* stats,
+                         void* stream);
+int nfb_selftest_depth_index(int R, int S, const float* weights, int* sel, void* stream);
+int nfb_selftest_warp_mag_loss(long long R, const float* pts, const float* warped, const int* sel, float alpha,
+                               float scale, float grad_scale, float* dwarped, float* stats, void* stream);
+
 /* Number of CUDA kernels this handle has launched so far (bench accounting). */
 long long nfb_kernel_launches(const nfb_handle* h);
 /* Thread-local description of the last error returned on this thread. */

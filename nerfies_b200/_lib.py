@@ -26,7 +26,8 @@ SYMBOLS = [
     'nfb_frame_pyramid', 'nfb_blur_scores_workspace_size', 'nfb_blur_scores', 'nfb_camera_project',
     'nfb_near_far_workspace_size', 'nfb_near_far', 'nfb_marching_cubes_workspace_size',
     'nfb_marching_cubes_count', 'nfb_marching_cubes', 'nfb_marching_cubes_table', 'nfb_warp_invert',
-    'nfb_point_visibility', 'nfb_flow_colorize',
+    'nfb_point_visibility', 'nfb_flow_colorize', 'nfb_selftest_composite_vjp', 'nfb_selftest_elastic',
+    'nfb_selftest_depth_index', 'nfb_selftest_warp_mag_loss',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -263,6 +264,14 @@ def load():
   lib.nfb_selftest_sgemm.restype = ci
   lib.nfb_selftest_train_gemm.argtypes = [ci] + lib.nfb_selftest_sgemm.argtypes
   lib.nfb_selftest_train_gemm.restype = ci
+  lib.nfb_selftest_composite_vjp.argtypes = [ci, ci, vp, ci, vp, ci] + [vp] * 4 + [ci, ci, ci, vp, vp, vp, vp]
+  lib.nfb_selftest_composite_vjp.restype = ci
+  lib.nfb_selftest_elastic.argtypes = [ll, ci, ci, ci, ci, vp, vp, ci, vp, vp, vp, cf, vp, vp, vp, vp, vp]
+  lib.nfb_selftest_elastic.restype = ci
+  lib.nfb_selftest_depth_index.argtypes = [ci, ci, vp, vp, vp]
+  lib.nfb_selftest_depth_index.restype = ci
+  lib.nfb_selftest_warp_mag_loss.argtypes = [ll, vp, vp, vp, cf, cf, cf, vp, vp, vp]
+  lib.nfb_selftest_warp_mag_loss.restype = ci
   lib.nfb_set_train_precision.argtypes = [vp, ci]
   lib.nfb_set_train_precision.restype = ci
   lib.nfb_debug_provoke_timeout.argtypes = [vp, ci]

@@ -1047,3 +1047,96 @@ int nfb_selftest_train_gemm(int train_precision, int mode, long long rows, int n
 }
 
 }  // extern "C"
+
+namespace {
+// The handle-less self-tests below have no launch counter to bump.
+int selftest_launched(const char* what) {
+  const cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("%s launch failed: %s", what, cudaGetErrorString(e));
+}
+}  // namespace
+
+extern "C" {
+
+// raw_to_samples_kernel then composite_vjp_kernel, launched as level_forward and level_backward launch them.
+int nfb_selftest_composite_vjp(int R, int S, const float* rgb_raw, int ld_rgb, const float* alpha_raw, int ld_a,
+                               const float* z, const float* directions, const float* d_out, const float* d_weights,
+                               int white_bg, int sample_at_infinity, int sigma_act, float* samples_out,
+                               float* d_rgb_raw, float* d_alpha_raw, void* stream) {
+  using namespace nfb::train;
+  if (R < 0) return fail("selftest_composite_vjp: R=%d must be >= 0", R);
+  if (S < 1 || S > nfb::kMaxSamples) return fail("selftest_composite_vjp: S=%d outside [1, %d]", S, nfb::kMaxSamples);
+  if (ld_rgb < 3 || ld_a < 1) return fail("selftest_composite_vjp: a leading dimension is below its width");
+  if (sigma_act < nfb::kNone || sigma_act > nfb::kSoftplus)
+    return fail("selftest_composite_vjp: bad activation %d", sigma_act);
+  if (!rgb_raw || !alpha_raw || !z || !directions || !samples_out || !d_rgb_raw || !d_alpha_raw)
+    return fail("selftest_composite_vjp: null input or output");
+  if (reinterpret_cast<uintptr_t>(samples_out) % 16) return fail("selftest_composite_vjp: samples_out is not 16-byte aligned");
+  if (R == 0) return 0;
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long rows = (long long)R * S;
+  float4* samples = reinterpret_cast<float4*>(samples_out);
+  raw_to_samples_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, s>>>(rgb_raw, ld_rgb, alpha_raw, ld_a, sigma_act,
+                                                                      samples, rows);
+  if (selftest_launched("raw_to_samples_kernel")) return -1;
+  CompositeVjpArgs c{};
+  c.samples = samples; c.z = z; c.directions = directions;
+  c.d_out = d_out; c.d_weights = d_weights;
+  c.rgb_raw = rgb_raw; c.ld_rgb = ld_rgb; c.alpha_raw = alpha_raw; c.ld_a = ld_a;
+  c.d_rgb_raw = d_rgb_raw; c.d_alpha_raw = d_alpha_raw;
+  c.num_rays = R; c.S = S;
+  c.white_bg = white_bg != 0; c.sample_at_infinity = sample_at_infinity != 0; c.sigma_act = sigma_act;
+  const int nblk = (R + nfb::kRaysPerBlock - 1) / nfb::kRaysPerBlock;
+  composite_vjp_kernel<<<nblk, 32 * nfb::kRaysPerBlock, composite_vjp_smem(S), s>>>(c);
+  return selftest_launched("composite_vjp_kernel");
+}
+
+// jac_elastic_kernel with JacArgs filled as warp_jacobian_on_tape fills them.
+int nfb_selftest_elastic(long long R, int warp_type, int pivot, int trans, int loss_type, const float* head,
+                         const float* thead, int ld, const float* pts, const int* sel, const float* row_w,
+                         float grad_scale, float* jac_out, float* d_head, float* d_thead, float* stats,
+                         void* stream) {
+  using namespace nfb::train;
+  if (R < 0) return fail("selftest_elastic: R=%lld must be >= 0", R);
+  if (warp_type != 1 && warp_type != 2) return fail("selftest_elastic: warp_type %d is not 1 or 2", warp_type);
+  if ((pivot != 0 && pivot != 1) || (trans != 0 && trans != 1) || (warp_type == 1 && (pivot || trans)))
+    return fail("selftest_elastic: pivot / translation heads belong to warp_type 2");
+  if (loss_type < kLogSvals || loss_type > kLogDet) return fail("selftest_elastic: unknown loss type %d", loss_type);
+  const int nh = warp_type == 2 ? 6 + 3 * pivot + 3 * trans : 3;
+  if (ld < nh) return fail("selftest_elastic: ld=%d is below the %d head outputs", ld, nh);
+  if (!head || !thead || !pts) return fail("selftest_elastic: null head / thead / pts");
+  if (!jac_out && !stats && !d_thead) return fail("selftest_elastic: no output");
+  if (d_thead && warp_type == 2 && !d_head) return fail("selftest_elastic: warp_type 2 needs d_head with d_thead");
+  if (R == 0) return 0;
+  JacArgs j{};
+  j.head = head; j.ld = ld; j.thead = thead; j.pts = pts;
+  j.sel = sel; j.row_w = row_w; j.jac_out = jac_out; j.R = R;
+  j.warp_type = warp_type; j.pivot = pivot; j.trans = trans;
+  j.with_loss = 1; j.loss_type = loss_type; j.stats = stats;
+  j.d_head = d_head; j.d_thead = d_thead; j.grad_scale = grad_scale;
+  jac_elastic_kernel<<<(unsigned)((R + 63) / 64), 64, 0, (cudaStream_t)stream>>>(j);
+  return selftest_launched("jac_elastic_kernel");
+}
+
+int nfb_selftest_depth_index(int R, int S, const float* weights, int* sel, void* stream) {
+  if (R < 0) return fail("selftest_depth_index: R=%d must be >= 0", R);
+  if (S < 1 || S > nfb::kMaxSamples) return fail("selftest_depth_index: S=%d outside [1, %d]", S, nfb::kMaxSamples);
+  if (!weights || !sel) return fail("selftest_depth_index: null weights / sel");
+  if (R == 0) return 0;
+  nfb::train::depth_index_kernel<<<(unsigned)((R + 7) / 8), 256, 0, (cudaStream_t)stream>>>(weights, R, S, sel);
+  return selftest_launched("depth_index_kernel");
+}
+
+int nfb_selftest_warp_mag_loss(long long R, const float* pts, const float* warped, const int* sel, float alpha,
+                               float scale, float grad_scale, float* dwarped, float* stats, void* stream) {
+  if (R < 0) return fail("selftest_warp_mag_loss: R=%lld must be >= 0", R);
+  if (std::isnan(alpha)) return fail("selftest_warp_mag_loss: alpha is NaN");
+  if (!(scale > 0.f) || !std::isfinite(scale)) return fail("selftest_warp_mag_loss: scale=%g must be finite and > 0", (double)scale);
+  if (!pts || !warped || !stats) return fail("selftest_warp_mag_loss: null pts / warped / stats");
+  if (R == 0) return 0;
+  nfb::train::WarpMagArgs wm{pts, warped, sel, dwarped, stats, alpha, scale, grad_scale, R};
+  nfb::train::warp_mag_loss_kernel<<<(unsigned)((R + 127) / 128), 128, 0, (cudaStream_t)stream>>>(wm);
+  return selftest_launched("warp_mag_loss_kernel");
+}
+
+}  // extern "C"

@@ -292,6 +292,17 @@ def se3_field_warp(params: Dict[str, Any], spec: OracleSpec, points: Tensor,
                      spec.warp_skips, 'relu')
   w = dense(params['branches_w']['logit'], trunk_output)
   v = dense(params['branches_v']['logit'], trunk_output)
+  pivot = (dense(params['branches_p']['logit'], trunk_output)
+           if spec.warp_use_pivot else None)
+  translation = (dense(params['branches_t']['logit'], trunk_output)
+                 if spec.warp_use_translation else None)
+  return se3_tail(w, v, points, pivot, translation)
+
+
+def se3_tail(w: Tensor, v: Tensor, points: Tensor, pivot: Optional[Tensor] = None,
+             translation: Optional[Tensor] = None) -> Tensor:
+  """SE3Field.warp after its branch MLPs (warping.py:330-353): the screw axis
+  (w, v) scaled by theta = |w|, the optional pivot and translation heads."""
   theta = torch.linalg.norm(w, dim=-1)
   w = w / theta[..., None]
   v = v / theta[..., None]
@@ -299,15 +310,14 @@ def se3_field_warp(params: Dict[str, Any], spec: OracleSpec, points: Tensor,
   # from_homogenous(transform @ to_homogenous(x)) (rigid_body.py:92-97); the
   # homogeneous coordinate is exactly 1.
   warped = points
-  if spec.warp_use_pivot:                               # warping.py:339-342
-    pivot = dense(params['branches_p']['logit'], trunk_output)
+  if pivot is not None:                                 # warping.py:339-342
     warped = warped + pivot
   warped = (R @ warped[..., None])[..., 0] + p
   warped = warped / torch.ones_like(warped[..., :1])
-  if spec.warp_use_pivot:                               # warping.py:347-348
+  if pivot is not None:                                 # warping.py:347-348
     warped = warped - pivot
-  if spec.warp_use_translation:                         # warping.py:350-352
-    warped = warped + dense(params['branches_t']['logit'], trunk_output)
+  if translation is not None:                           # warping.py:350-352
+    warped = warped + translation
   return warped
 
 

@@ -87,3 +87,56 @@ def test_camera_entry_points_fail_loudly_without_a_device():
   assert b'no CUDA device' in lib.nfb_last_error()
   assert lib.nfb_camera_rays(ctypes.byref(cam), 10, 16, None, ctypes.c_void_p(16), None, None) != 0
   assert b'exceeds' in lib.nfb_last_error()
+
+
+def test_selftest_entries_refuse_bad_arguments():
+  """The training kernels' self-test entries refuse bad arguments before touching a device (every call here
+  is refused, so the fake pointers are never read)."""
+  lib = _lib.load()
+  p = ctypes.c_void_p(256)
+
+  def refused(status, what):
+    assert status != 0
+    assert what in lib.nfb_last_error().decode(), lib.nfb_last_error()
+
+  def vjp(R=4, S=8, ld_rgb=3, ld_a=1, act=6, rgb=p, d_rgb=p, samples=p):
+    return lib.nfb_selftest_composite_vjp(R, S, rgb, ld_rgb, p, ld_a, p, p, None, None, 0, 1, act, samples, d_rgb, p,
+                                          None)
+  refused(vjp(S=1025), 'S=1025 outside [1, 1024]')
+  refused(vjp(S=0), 'S=0 outside')
+  refused(vjp(R=-1), 'R=-1 must be >= 0')
+  refused(vjp(ld_rgb=2), 'leading dimension is below its width')
+  refused(vjp(ld_a=0), 'leading dimension is below its width')
+  refused(vjp(act=7), 'bad activation 7')
+  refused(vjp(act=-1), 'bad activation -1')
+  refused(vjp(rgb=None), 'null input or output')
+  refused(vjp(d_rgb=None), 'null input or output')
+  refused(vjp(samples=ctypes.c_void_p(264)), 'not 16-byte aligned')
+
+  def elastic(R=4, warp_type=2, pivot=0, trans=0, loss_type=0, ld=6, head=p, jac=p, d_head=p, d_thead=p, stats=p):
+    return lib.nfb_selftest_elastic(R, warp_type, pivot, trans, loss_type, head, p, ld, p, None, None, 1.0, jac,
+                                    d_head, d_thead, stats, None)
+  refused(elastic(R=-2), 'R=-2 must be >= 0')
+  refused(elastic(warp_type=0), 'warp_type 0 is not 1 or 2')
+  refused(elastic(warp_type=1, pivot=1), 'belong to warp_type 2')
+  refused(elastic(trans=2), 'belong to warp_type 2')
+  refused(elastic(loss_type=6), 'unknown loss type 6')
+  refused(elastic(loss_type=-1), 'unknown loss type -1')
+  refused(elastic(pivot=1, trans=1, ld=11), 'ld=11 is below the 12 head outputs')
+  refused(elastic(warp_type=1, ld=2), 'ld=2 is below the 3 head outputs')
+  refused(elastic(head=None), 'null head / thead / pts')
+  refused(elastic(jac=None, d_thead=None, stats=None), 'no output')
+  refused(elastic(d_head=None), 'needs d_head with d_thead')
+
+  refused(lib.nfb_selftest_depth_index(4, 1025, p, p, None), 'S=1025 outside [1, 1024]')
+  refused(lib.nfb_selftest_depth_index(-1, 8, p, p, None), 'R=-1 must be >= 0')
+  refused(lib.nfb_selftest_depth_index(4, 8, p, None, None), 'null weights / sel')
+
+  def mag(R=4, alpha=-2.0, scale=0.03, pts=p, stats=p):
+    return lib.nfb_selftest_warp_mag_loss(R, pts, p, None, alpha, scale, 1.0, None, stats, None)
+  refused(mag(R=-1), 'R=-1 must be >= 0')
+  refused(mag(alpha=float('nan')), 'alpha is NaN')
+  refused(mag(scale=0.0), 'must be finite and > 0')
+  refused(mag(scale=float('inf')), 'must be finite and > 0')
+  refused(mag(stats=None), 'null pts / warped / stats')
+  refused(mag(pts=None), 'null pts / warped / stats')
