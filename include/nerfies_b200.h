@@ -272,12 +272,40 @@ int nfb_render_vjp(nfb_handle* h, int num_rays, const float* origins, const floa
                    const float* d_warped_fine, float* d_warp_code, float* d_app_code, float* d_cam_code,
                    int chunk_rays, float* const* grads, const long long* numels, int count, void* stream);
 
+/* Vector-Jacobian product of one nfb_render_forward call with respect to its rays (and, with
+ * NFB_FLAG_METADATA_ENCODED, its codes); the parameters are constants.  The adjoint iNeRF-style camera
+ * registration needs: a pose moves the rays.
+ *   h ... d_warped_fine: as nfb_render_vjp (same meaning, same refusals).  The sample points are
+ *     x = o + z d with z a constant; alpha_i = 1 - exp(-sigma_i dz_i |d|) also depends on |d|;
+ *   d_origins (B,3), d_directions (B,3), d_viewdirs (B,3): nullable, overwritten (=).  Without viewdirs the
+ *     kernels encode the directions as view directions, and that share goes into d_directions; d_viewdirs
+ *     then must be null.  A model without use_viewdirs writes zeros to d_viewdirs;
+ *   d_warp_code, d_app_code, d_cam_code: as nfb_render_vjp (+=, NFB_FLAG_METADATA_ENCODED only);
+ *   at least one of the six outputs must be non-null.
+ * Per chunk of chunk_rays rays and level: the taped forward at the given z, then its backward through every
+ * layer's dX only (no weight or bias gradient is formed), in the handle's training precision.  B = 0 returns
+ * 0.  Uses the parameters of the last nfb_set_params and the time_alpha of the last nfb_set_time_alpha. */
+int nfb_render_ray_vjp(nfb_handle* h, int num_rays, const float* origins, const float* directions,
+                       const float* viewdirs, const unsigned* warp_id, const unsigned* appearance_id,
+                       const unsigned* camera_id, float warp_alpha, unsigned flags, const float* z_coarse,
+                       const float* z_fine, const float* d_out_coarse, const float* d_out_fine,
+                       const float* d_weights_coarse, const float* d_weights_fine, const float* d_warped_coarse,
+                       const float* d_warped_fine, float* d_origins, float* d_directions, float* d_viewdirs,
+                       float* d_warp_code, float* d_app_code, float* d_cam_code, int chunk_rays, void* stream);
+
 /* The same for nfb_warp_forward (warp_field.apply on free points): d_warped (P,3) -> the warp field's parameter
  * gradients (+= into grads, laid out as nfb_train_value_and_grad's) and, with NFB_FLAG_METADATA_ENCODED,
  * d_code (P, num_warp_features), nullable (+=).  Training precision, chunks of max_rays points. */
 int nfb_warp_vjp(nfb_handle* h, int num_points, const float* points, const unsigned* warp_id, float warp_alpha,
                  unsigned flags, const float* d_warped, float* d_code, float* const* grads,
                  const long long* numels, int count, void* stream);
+
+/* The warp field's metadata code of n rays or points, code_out (n, num_warp_features): what
+ * NFB_FLAG_METADATA_ENCODED expects in warp_id.  warp_id holds GLO ids ('glo', 'blend') or, with
+ * NFB_WARP_ENC_TIME, const float* timestamps; the code is the GLO row, the TimeEncoder's output at the time
+ * ('time', at the time_alpha of the last nfb_set_time_alpha) or their blend ('blend').  Lets a caller fit the
+ * other codes encoded while the warp code stays that of a fixed time. */
+int nfb_warp_code(nfb_handle* h, int n, const unsigned* warp_id, float* code_out, void* stream);
 
 /* Jacobian of the warp field at free points: jacobian_out (P,3,3), J[i][j] = d warped_i / d point_j
  * (jax.jacfwd(self.warp, argnums=0), warping.py:196-198, 385-387); warped_out (P,3) nullable.

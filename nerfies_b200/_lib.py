@@ -27,7 +27,8 @@ SYMBOLS = [
     'nfb_near_far_workspace_size', 'nfb_near_far', 'nfb_marching_cubes_workspace_size',
     'nfb_marching_cubes_count', 'nfb_marching_cubes', 'nfb_marching_cubes_table', 'nfb_warp_invert',
     'nfb_point_visibility', 'nfb_flow_colorize', 'nfb_selftest_composite_vjp', 'nfb_selftest_elastic',
-    'nfb_selftest_depth_index', 'nfb_selftest_warp_mag_loss',
+    'nfb_selftest_depth_index', 'nfb_selftest_warp_mag_loss', 'nfb_render_ray_vjp',
+    'nfb_warp_code',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -192,6 +193,10 @@ def load():
   lib.nfb_render_vjp.argtypes = [vp, ci] + [vp] * 6 + [cf, cu] + [vp] * 11 + [ci, ctypes.POINTER(vp),
                                                                               ctypes.POINTER(ctypes.c_longlong), ci, vp]
   lib.nfb_render_vjp.restype = ci
+  lib.nfb_render_ray_vjp.argtypes = [vp, ci] + [vp] * 6 + [cf, cu] + [vp] * 14 + [ci, vp]
+  lib.nfb_render_ray_vjp.restype = ci
+  lib.nfb_warp_code.argtypes = [vp, ci, vp, vp, vp]
+  lib.nfb_warp_code.restype = ci
   lib.nfb_warp_vjp.argtypes = [vp, ci, vp, vp, cf, cu, vp, vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_longlong),
                                ci, vp]
   lib.nfb_warp_vjp.restype = ci

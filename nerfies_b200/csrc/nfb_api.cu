@@ -320,9 +320,10 @@ int launch_check(nfb_handle* h, const char* what) {
 
 // `time_encoder` false leaves the TimeEncoder's share of the warp block to the caller (the training tier runs
 // it on a tape of its own: time_forward, train_api.cuh).
+// With `warp_out` (B, G) the warp block alone is written there (nfb_warp_code; viewdirs may be null).
 int run_cond(nfb_handle* h, int B, const float* viewdirs, const unsigned* warp_id,
              const unsigned* app_id, const unsigned* cam_id, cudaStream_t s, bool encoded = false,
-             bool time_encoder = true) {
+             bool time_encoder = true, float* warp_out = nullptr) {
   const nfb_config& c = h->cfg;
   nfb::CondArgs a{};
   a.viewdirs = viewdirs; a.warp_id = warp_id; a.app_id = app_id; a.cam_id = cam_id;
@@ -330,7 +331,12 @@ int run_cond(nfb_handle* h, int B, const float* viewdirs, const unsigned* warp_i
   a.n_warp = c.num_warp_embeddings; a.n_app = c.num_appearance_embeddings; a.n_cam = c.num_camera_embeddings;
   a.layout = h->cond_layout; a.cond = h->d_cond; a.num_rays = B;
   a.encoded = encoded;
-  const nfb::CondLayout& L = h->cond_layout;
+  if (warp_out) {
+    nfb::CondLayout w{};
+    w.G = h->cond_layout.G; w.A = h->cond_layout.A; w.C = h->cond_layout.C; w.stride = w.G;
+    a.layout = w; a.cond = warp_out;
+  }
+  const nfb::CondLayout& L = a.layout;
   if (L.G + L.tc + L.ac + L.rc() == 0) return 0;
   const long long total = (long long)B * L.stride;
   const int enc = c.warp_field_type != NFB_WARP_NONE ? c.warp_metadata_encoder : NFB_WARP_ENC_GLO;
@@ -347,7 +353,7 @@ int run_cond(nfb_handle* h, int B, const float* viewdirs, const unsigned* warp_i
     const float alpha = enc == NFB_WARP_ENC_TIME ? h->time_alpha : (float)t.F;   // modules.py:318-319
     easing_window(alpha, t.F, t.window);
     t.blend = enc == NFB_WARP_ENC_BLEND; t.time_alpha = h->time_alpha;
-    t.cond = h->d_cond; t.stride = L.stride; t.G = L.G; t.num_rays = B;
+    t.cond = a.cond; t.stride = L.stride; t.G = L.G; t.num_rays = B;
     nfb::time_embed_kernel<<<(B + nfb::kTimeRays - 1) / nfb::kTimeRays, nfb::kTimeThreads, 0, s>>>(t);
     return launch_check(h, "time_embed_kernel");
   }
@@ -1280,7 +1286,7 @@ void nfb_destroy(nfb_handle* h) {
   for (float* p : bufs) if (p) cudaFree(p);
   if (h->d_src) cudaFree(h->d_src);
   float* tbufs[] = {h->d_tape, h->d_gpacked, h->d_gwarp, h->d_gapp, h->d_gcam, h->d_dcond, h->d_tr_out, h->d_tr_w, h->d_loss,
-                    h->d_ttape, reinterpret_cast<float*>(h->d_sel), h->d_time_tape};
+                    h->d_ttape, reinterpret_cast<float*>(h->d_sel), h->d_time_tape, h->d_ray_pts};
   for (float* p : tbufs) if (p) cudaFree(p);
   if (h->d_ids) cudaFree(h->d_ids);
   if (h->d_invert) cudaFree(h->d_invert);
@@ -1500,6 +1506,16 @@ int nfb_warp_forward(nfb_handle* h, int P, const float* points, const unsigned* 
   if (run_cond(h, P, points, warp_id, nullptr, nullptr, s, (flags & NFB_FLAG_METADATA_ENCODED) != 0)) return -1;
   // Free points: rows = points, z = 0 (x = p + 0 * p = p exactly for finite p).
   return run_warp(h, 0, P, 1, points, points, nullptr, warped, s);
+}
+
+int nfb_warp_code(nfb_handle* h, int n, const unsigned* warp_id, float* code_out, void* stream) {
+  if (check_call(h, n)) return -1;
+  if (h->cfg.warp_field_type == NFB_WARP_NONE) return fail("warp code: the model has no warp field");
+  if (n == 0) return 0;
+  if (!warp_id || !code_out) return fail("warp code: warp_id / code_out is null");
+  cudaStream_t s = (cudaStream_t)stream;
+  if (enter_stream(h, s)) return -1;
+  return run_cond(h, n, nullptr, warp_id, nullptr, nullptr, s, false, true, code_out);
 }
 
 int nfb_point_visibility(nfb_handle* h, int P, const float* points, const unsigned* warp_id,

@@ -448,6 +448,8 @@ struct CompositeVjpArgs {
   const float* rgb_raw; int ld_rgb; const float* alpha_raw; int ld_a;
   float* d_rgb_raw; float* d_alpha_raw;     // same layouts: = (not +=)
   int num_rays, S, white_bg, sample_at_infinity, sigma_act;
+  // (R) or null: = dL/d|d| of each ray, through dist_i = dz_i |d| in alpha_i = 1 - exp(-sigma_i dist_i)
+  float* d_dnorm;
 };
 // Shared memory: three floats per sample of each of kRaysPerBlock rays.
 constexpr size_t composite_vjp_smem(int S) { return (size_t)kRaysPerBlock * 3 * S * sizeof(float); }
@@ -518,6 +520,7 @@ __global__ void __launch_bounds__(32 * kRaysPerBlock) composite_vjp_kernel(const
   }
   float acc = __shfl_down_sync(0xffffffffu, incl_suf, 1);
   if (lane == 31) acc = 0.f;
+  float sd = 0.f;                      // the lane's sum of dsigma_i sigma_i (d_dnorm)
   for (int i = e - 1; i >= b; --i) {
     const size_t m = base + i;
     const float4 c = a.samples[m];
@@ -536,6 +539,121 @@ __global__ void __launch_bounds__(32 * kRaysPerBlock) composite_vjp_kernel(const
     a.d_rgb_raw[m * a.ld_rgb + 0] = g[0] * w * c.x * (1.f - c.x);
     a.d_rgb_raw[m * a.ld_rgb + 1] = g[1] * w * c.y * (1.f - c.y);
     a.d_rgb_raw[m * a.ld_rgb + 2] = g[2] * w * c.z * (1.f - c.z);
+    // dL/d|d| = sum_i dL/d dist_i dz_i = sum_i dsigma_i sigma_i / |d|.  The last sample (dz 1e10 or 1e-19)
+    // counts like the others: where sigma is finite its exp(-sigma dist) makes it 0 (or leaves its true
+    // value), as the reference's autograd does.
+    if (a.d_dnorm) sd = fmaf(dsigma, c.w, sd);
+  }
+  if (a.d_dnorm) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) sd += __shfl_xor_sync(0xffffffffu, sd, o);
+    if (lane == 0) a.d_dnorm[ray] = sd / dnorm;
+  }
+}
+
+// ---------------------------------------------------------------------------
+// Ray adjoints (nfb_render_ray_vjp): the sample points x_{r,s} = o_r + z_{r,s} d_r with z a constant.
+// ---------------------------------------------------------------------------
+// The warp tail's direct term in the point gradient: dpts += (d warped / d x)^T dwarped at the head outputs
+// of the tape, by forward mode on x (three tangents; the head is a constant here, its own adjoint is
+// warp_tail_bwd_kernel's).  The identity for the TranslationField.
+struct WarpTailDxArgs {
+  const float* head; int ld; const float* pts; const float* dwarped;   // (rows,3)
+  float* dpts;                // (rows,3): +=
+  int warp_type, pivot, trans;
+  long long rows;
+};
+__global__ void warp_tail_dx_kernel(const WarpTailDxArgs a) {
+  const long long m = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= a.rows) return;
+  const float g[3] = {a.dwarped[m * 3], a.dwarped[m * 3 + 1], a.dwarped[m * 3 + 2]};
+  float* dx = a.dpts + m * 3;
+  if (a.warp_type != 2) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) dx[c] += g[c];
+    return;
+  }
+  using S = Fwd<3, float>;
+  const int nh = 6 + (a.pivot ? 3 : 0) + (a.trans ? 3 : 0);
+  S in[12], xs[3], y[3];
+  for (int q = 0; q < 12; ++q) in[q] = Num<S>::c(q < nh ? a.head[m * a.ld + q] : 0.f);
+  for (int c = 0; c < 3; ++c) { xs[c] = Num<S>::c(a.pts[m * 3 + c]); xs[c].d[c] = 1.f; }
+  se3_tail(in, xs, a.pivot != 0, a.trans != 0, y);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) dx[c] += g[0] * y[0].d[c] + g[1] * y[1].d[c] + g[2] * y[2].d[c];
+}
+
+// Per ray of S samples (one warp per ray, shuffle sums), += over the levels:
+//   d_origins    += sum_s g_s
+//   d_directions += sum_s z_s g_s + (dL/d|d|) d / |d|
+// with g the level's point gradient (rows,3) and dL/d|d| from composite_vjp_kernel (nullable).
+struct RayReduceArgs {
+  const float* dpts; const float* z; const float* directions; const float* d_dnorm;
+  float* d_origins; float* d_directions;   // (R,3), nullable
+  int num_rays, S;
+};
+__global__ void __launch_bounds__(32 * kRaysPerBlock) ray_reduce_kernel(const RayReduceArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int ray = blockIdx.x * kRaysPerBlock + (threadIdx.x >> 5);
+  if (ray >= a.num_rays) return;
+  float so[3] = {0.f, 0.f, 0.f}, sd[3] = {0.f, 0.f, 0.f};
+  const size_t base = (size_t)ray * a.S;
+  for (int i = lane; i < a.S; i += 32) {
+    const float z = a.z[base + i];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float g = a.dpts[(base + i) * 3 + c];
+      so[c] += g;
+      sd[c] = fmaf(z, g, sd[c]);
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      so[c] += __shfl_xor_sync(0xffffffffu, so[c], o);
+      sd[c] += __shfl_xor_sync(0xffffffffu, sd[c], o);
+    }
+  if (lane != 0) return;
+  if (a.d_origins)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) a.d_origins[ray * 3 + c] += so[c];
+  if (a.d_directions) {
+    const float* d = a.directions + ray * 3;
+    float k = 0.f;
+    if (a.d_dnorm) k = a.d_dnorm[ray] / sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) a.d_directions[ray * 3 + c] += fmaf(k, d[c], sd[c]);
+  }
+}
+
+// The adjoint of the viewdir block of the rgb condition (ray_cond_kernel: identity, then sin(2^f v_c [+pi/2])
+// with no window), one thread per ray: out (B,3) = (accumulate ? += : =) dL/d viewdirs.
+struct ViewdirVjpArgs {
+  const float* dcond; int stride, off, F;  // the block is dcond[:, off .. off + 3 + 6F)
+  const float* viewdirs; float* out;
+  int accumulate, num_rays;
+};
+__global__ void viewdir_vjp_kernel(const ViewdirVjpArgs a) {
+  const int ray = blockIdx.x * blockDim.x + threadIdx.x;
+  if (ray >= a.num_rays) return;
+  const float* g = a.dcond + (size_t)ray * a.stride + a.off;
+  float v[3], dv[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) { v[c] = a.viewdirs[ray * 3 + c]; dv[c] = g[c]; }
+  for (int f = 0; f < a.F; ++f) {
+    const float s = exp2f((float)f);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float ang = v[c] * s;
+      dv[c] = fmaf(g[3 + f * 6 + c] * s, cosf(ang), dv[c]);
+      dv[c] = fmaf(g[3 + f * 6 + 3 + c] * s, cosf(ang + kHalfPiF), dv[c]);
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    if (a.accumulate) a.out[ray * 3 + c] += dv[c];
+    else a.out[ray * 3 + c] = dv[c];
   }
 }
 

@@ -111,9 +111,10 @@ int net_forward(nfb_handle* h, const Net& net, const float* in, int ld_in, const
   return 0;
 }
 
+// with_dw = false: dX only (the ray VJP, which differentiates no parameter).
 int net_backward(nfb_handle* h, const Net& net, const float* in, float* d_in, int ld_in,
                  const long long* out_off, const long long* d_out_off, float* arena, long long rows,
-                 cudaStream_t s) {
+                 cudaStream_t s, bool with_dw = true) {
   int producer[nfb::kMaxSteps];
   net_producers(net, producer);
   for (int i = net.n_steps - 1; i >= 0; --i) {
@@ -124,10 +125,11 @@ int net_backward(nfb_handle* h, const Net& net, const float* in, float* d_in, in
     const int ldx = producer[i] >= 0 ? net.steps[producer[i]].npad : ld_in;
     nfb::train::ConcatA a{x, ldx, st.k_x, in + st.in_off, ld_in};
     // dW += [X | IN]^T dZ   (reduction over the rows, split)
-    if (launch_gemm<false, true>(h, K, st.n, rows, nfb::train::ConcatAT{a}, nfb::train::DZB{dz},
+    if (with_dw &&
+        launch_gemm<false, true>(h, K, st.n, rows, nfb::train::ConcatAT{a}, nfb::train::DZB{dz},
                                  nfb::train::AtomicAdd{h->d_gpacked + st.w_off, st.npad}, dw_split_for(h, K, st.n, rows), s, "sgemm (dW)")) return -1;
     // db += colsum(dZ)
-    {
+    if (with_dw) {
       dim3 grid((unsigned)((st.n + 31) / 32), (unsigned)std::min<long long>((rows + 255) / 256, 128));
       nfb::train::colsum_kernel<<<grid, 256, 0, s>>>(dz, rows, st.n, h->d_gpacked + st.b_off);
       if (launch_check(h, "colsum_kernel")) return -1;
@@ -288,9 +290,10 @@ int warp_forward(nfb_handle* h, const nfb::FieldProgram& p, const TapeLayout& t,
 }
 
 // Adjoint of warp_forward: tape.dwarped -> the warp MLP's parameter gradients and, += per ray of S rows,
-// the warp GLO block of `dcond`.
+// the warp GLO block of `dcond`.  With `dpts` (rows,3), = the gradient of the points: the encoding's
+// adjoint plus the tail's direct term; with_dw = false skips the parameter gradients.
 int warp_backward(nfb_handle* h, const nfb::FieldProgram& p, const TapeLayout& t, int S, float* dcond,
-                  cudaStream_t s) {
+                  cudaStream_t s, float* dpts = nullptr, bool with_dw = true) {
   using namespace nfb::train;
   float* A = h->d_tape;
   const unsigned blocks = (unsigned)((t.rows + 127) / 128);
@@ -299,13 +302,18 @@ int warp_backward(nfb_handle* h, const nfb::FieldProgram& p, const TapeLayout& t
                     p.warp_type, p.warp_pivot, p.warp_trans, t.rows};
   warp_tail_bwd_kernel<<<blocks, 128, 0, s>>>(w);
   if (launch_check(h, "warp_tail_bwd_kernel")) return -1;
-  if (net_backward(h, p.warp, A + t.in_w, A + t.d_in_w, t.ld_w, t.out_w, t.d_out_w, A, t.rows, s)) return -1;
+  if (net_backward(h, p.warp, A + t.in_w, A + t.d_in_w, t.ld_w, t.out_w, t.d_out_w, A, t.rows, s, with_dw)) return -1;
   EncodeBwdArgs e{};
   e.pts = A + t.pts; e.window = h->d_window; e.din = A + t.d_in_w; e.F = p.Fw; e.ld = t.ld_w; e.S = S;
-  e.cond_stride = h->cond_layout.stride; e.cond_off = 0; e.n_cond = p.G; e.dpts = nullptr; e.dcond = dcond;
+  e.cond_stride = h->cond_layout.stride; e.cond_off = 0; e.n_cond = p.G; e.dpts = dpts; e.dcond = dcond;
   e.rows = t.rows;
   encode_bwd_kernel<<<blocks, 128, 0, s>>>(e);
-  return launch_check(h, "encode_bwd_kernel");
+  if (launch_check(h, "encode_bwd_kernel")) return -1;
+  if (!dpts) return 0;
+  WarpTailDxArgs x{A + t.out_w[hs], p.warp.steps[hs].npad, A + t.pts, A + t.dwarped, dpts, p.warp_type, p.warp_pivot,
+                   p.warp_trans, t.rows};
+  warp_tail_dx_kernel<<<blocks, 128, 0, s>>>(x);
+  return launch_check(h, "warp_tail_dx_kernel");
 }
 
 // ---- TimeEncoder tape ('time' / 'blend' warp metadata encoders): max_rays rows, one per ray or free point ----
@@ -430,12 +438,14 @@ int level_forward(nfb_handle* h, int level, int R, int S, const float* z, const 
 // composite_vjp_kernel seeded by the cotangents d_out (R,6) and d_weights (R,S) of the level's outputs, the
 // regularisers of `reg` (on the level's `weights`), the NeRF MLP and its encoding, then the warp field, whose
 // warped points also receive d_warped (R,S,3).  d_out, d_weights, d_warped and reg are nullable; `dcond` is the R
-// rays' condition-vector gradient accumulator.
+// rays' condition-vector gradient accumulator.  The ray VJP passes `dpts` (rows,3) and `d_dnorm` (R), which
+// receive (=) the gradients of the sample points and of |d|, and with_dw = false (no parameter gradients).
 static_assert(nfb::train::composite_vjp_smem(nfb::kMaxSamples) <= 48 * 1024,
               "composite_vjp_kernel's shared memory exceeds the default 48 KiB at kMaxSamples");
 int level_backward(nfb_handle* h, int level, int R, int S, const float* z, const float* directions, float* dcond,
                    bool use_warp, int alpha_step, int rgb_step, const float* d_out, const float* d_weights,
-                   const float* d_warped, const float* weights, const RegCfg* reg, cudaStream_t s) {
+                   const float* d_warped, const float* weights, const RegCfg* reg, cudaStream_t s,
+                   float* dpts = nullptr, float* d_dnorm = nullptr, bool with_dw = true) {
   using namespace nfb::train;
   const nfb::FieldProgram& p = h->prog[level];
   const long long rows = (long long)R * S;
@@ -453,7 +463,7 @@ int level_backward(nfb_handle* h, int level, int R, int S, const float* z, const
     c.d_rgb_raw = A + t.d_out_n[rgb_step]; c.d_alpha_raw = A + t.d_out_n[alpha_step];
     c.num_rays = R; c.S = S;
     c.white_bg = h->cfg.use_white_background; c.sample_at_infinity = h->cfg.use_sample_at_infinity;
-    c.sigma_act = p.sigma_act;
+    c.sigma_act = p.sigma_act; c.d_dnorm = d_dnorm;
     const int nblk = (R + nfb::kRaysPerBlock - 1) / nfb::kRaysPerBlock;
     composite_vjp_kernel<<<nblk, 32 * nfb::kRaysPerBlock, composite_vjp_smem(S), s>>>(c);
     if (launch_check(h, "composite_vjp_kernel")) return -1;
@@ -471,12 +481,12 @@ int level_backward(nfb_handle* h, int level, int R, int S, const float* z, const
                               reg, true, nullptr, s))
       return -1;
   }
-  if (net_backward(h, p.nerf, A + t.in_n, A + t.d_in_n, t.ld_n, t.out_n, t.d_out_n, A, rows, s)) return -1;
+  if (net_backward(h, p.nerf, A + t.in_n, A + t.d_in_n, t.ld_n, t.out_n, t.d_out_n, A, rows, s, with_dw)) return -1;
   {
     EncodeBwdArgs e{};
     e.pts = A + t.warped; e.window = nullptr; e.din = A + t.d_in_n; e.F = p.Fp; e.ld = t.ld_n; e.S = S;
     e.cond_stride = h->cond_layout.stride; e.cond_off = p.G; e.n_cond = p.tc + p.ac + p.rc;
-    e.dpts = warp ? A + t.dwarped : nullptr; e.dcond = dcond; e.rows = rows;
+    e.dpts = warp ? A + t.dwarped : dpts; e.dcond = dcond; e.rows = rows;
     encode_bwd_kernel<<<blocks, 128, 0, s>>>(e);
     if (launch_check(h, "encode_bwd_kernel")) return -1;
   }
@@ -494,7 +504,7 @@ int level_backward(nfb_handle* h, int level, int R, int S, const float* z, const
     add_into_kernel<<<(unsigned)((rows * 3 + 255) / 256), 256, 0, s>>>(A + t.dwarped, d_warped, rows * 3);
     if (launch_check(h, "add_into_kernel")) return -1;
   }
-  return warp_backward(h, p, t, S, dcond, s);
+  return warp_backward(h, p, t, S, dcond, s, dpts, with_dw);
 }
 
 // The gradient accumulators of the packed parameters and of the three embedding tables, zeroed.
@@ -531,17 +541,18 @@ int unpack_grads(nfb_handle* h, float* const* grads, int count, cudaStream_t s) 
   return 0;
 }
 
-// The adjoint of run_cond(encoded = true) for `n` rays: dcond -> the dense code gradients (+=), or row 0 of a
-// table for a code the call did not pass.
+// The adjoint of run_cond(encoded = true) for `n` rays: dcond -> the dense code gradients (+=), or (with
+// `tables`) row 0 of a table for a code the call did not pass.
 int cond_vjp_encoded(nfb_handle* h, int n, const float* dcond, bool has_warp, bool has_app, bool has_cam,
-                     float* d_warp, float* d_app, float* d_cam, cudaStream_t s) {
+                     float* d_warp, float* d_app, float* d_cam, cudaStream_t s, bool tables = true) {
   nfb::train::CondVjpEncodedArgs a{};
   a.dcond = dcond; a.num_rays = n;
   a.has_warp = has_warp; a.has_app = has_app; a.has_cam = has_cam;
   a.d_warp = d_warp; a.d_app = d_app; a.d_cam = d_cam;
   // a 'time' encoder has no table: ray_cond_kernel's row-0 fallback reads memory no parameter owns
-  a.d_warp_table = has_time_encoder(h) && h->cfg.warp_metadata_encoder == NFB_WARP_ENC_TIME ? nullptr : h->d_gwarp;
-  a.d_app_table = h->d_gapp; a.d_cam_table = h->d_gcam;
+  a.d_warp_table = !tables || (has_time_encoder(h) && h->cfg.warp_metadata_encoder == NFB_WARP_ENC_TIME) ? nullptr
+                                                                                                          : h->d_gwarp;
+  a.d_app_table = tables ? h->d_gapp : nullptr; a.d_cam_table = tables ? h->d_gcam : nullptr;
   a.layout = h->cond_layout;
   const long long total = (long long)n * a.layout.stride;
   nfb::train::cond_vjp_encoded_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(a);
@@ -860,6 +871,106 @@ int nfb_render_vjp(nfb_handle* h, int B, const float* origins, const float* dire
     return -1;
   }
   return unpack_grads(h, grads, count, s);
+}
+
+int nfb_render_ray_vjp(nfb_handle* h, int B, const float* origins, const float* directions, const float* viewdirs,
+                       const unsigned* warp_id, const unsigned* app_id, const unsigned* cam_id, float warp_alpha,
+                       unsigned flags, const float* z_coarse, const float* z_fine, const float* d_out_coarse,
+                       const float* d_out_fine, const float* d_weights_coarse, const float* d_weights_fine,
+                       const float* d_warped_coarse, const float* d_warped_fine, float* d_origins,
+                       float* d_directions, float* d_viewdirs, float* d_warp_code, float* d_app_code,
+                       float* d_cam_code, int chunk_rays, void* stream) {
+  if (check_call(h, B)) return -1;
+  const nfb_config& c = h->cfg;
+  const bool encoded = (flags & NFB_FLAG_METADATA_ENCODED) != 0;
+  if (!encoded && (d_warp_code || d_app_code || d_cam_code))
+    return fail("ray VJP: code gradients need NFB_FLAG_METADATA_ENCODED");
+  if (!d_origins && !d_directions && !d_viewdirs && !d_warp_code && !d_app_code && !d_cam_code)
+    return fail("ray VJP: every output is null");
+  const bool use_warp = !(flags & NFB_FLAG_NO_WARP);
+  const bool warp = use_warp && c.warp_field_type != NFB_WARP_NONE;
+  const bool coarse = d_out_coarse || d_weights_coarse || d_warped_coarse;
+  const bool fine = d_out_fine || d_weights_fine || d_warped_fine;
+  if (fine && (c.num_fine_samples == 0 || (flags & NFB_FLAG_COARSE_ONLY)))
+    return fail("ray VJP: fine-level cotangents, but the call renders no fine level");
+  if (!warp && (d_warped_coarse || d_warped_fine))
+    return fail("ray VJP: warped-point cotangents, but the call does not warp");
+  cudaStream_t s = (cudaStream_t)stream;
+  if (enter_stream(h, s)) return -1;
+  if (B == 0) return 0;
+  if (!origins || !directions) return fail("ray VJP: origins / directions are null");
+  if (d_viewdirs && !viewdirs) return fail("ray VJP: d_viewdirs without viewdirs (the directions are encoded)");
+  if ((coarse && !z_coarse) || (fine && !z_fine)) return fail("ray VJP: the z values of a level with cotangents are null");
+  if (chunk_rays < 1) chunk_rays = 256;
+  chunk_rays = std::min(chunk_rays, B);
+  const int nc = c.num_coarse_samples;
+  if (train_prepare(h, chunk_rays)) return -1;
+  const bool want_pts = d_origins || d_directions;
+  // the point gradient of a chunk's level: handle scratch of its own, so the tape keeps the training layout
+  if (want_pts && grow(&h->d_ray_pts, &h->ray_pts_cap, (long long)chunk_rays * (nc + c.num_fine_samples) * 3,
+                       "ray VJP point gradient"))
+    return -1;
+  if (set_window(h, warp_alpha, s)) return -1;
+  // the ray outputs are =: zeroed here, then summed over the levels (and the view directions' share)
+  if (d_origins) NFB_CUDA(cudaMemsetAsync(d_origins, 0, (size_t)B * 3 * sizeof(float), s));
+  if (d_directions) NFB_CUDA(cudaMemsetAsync(d_directions, 0, (size_t)B * 3 * sizeof(float), s));
+  const float* vd = viewdirs ? viewdirs : directions;
+  const bool time_enc = warp && !encoded && has_time_encoder(h);
+  if (time_enc ? train_cond(h, B, vd, warp_id, c.warp_metadata_encoder == NFB_WARP_ENC_TIME, app_id, cam_id, s)
+               : run_cond(h, B, vd, warp_id, app_id, cam_id, s, encoded, false))
+    return -1;
+  NFB_CUDA(cudaMemsetAsync(h->d_dcond, 0, (size_t)B * h->cond_layout.stride * sizeof(float), s));
+  const int nfine = nc + c.num_fine_samples;
+  float* d_dnorm = h->d_tr_out;                       // (R) per level: dL/d|d| of the chunk's rays
+  auto at = [](const float* p, size_t off) { return p ? p + off : nullptr; };
+  for (int r0 = 0; r0 < B; r0 += chunk_rays) {
+    const int R = std::min(chunk_rays, B - r0);
+    const float* cond = h->d_cond + (size_t)r0 * h->cond_layout.stride;
+    float* dcond = h->d_dcond + (size_t)r0 * h->cond_layout.stride;
+    const float* o = origins + (size_t)r0 * 3;
+    const float* d = directions + (size_t)r0 * 3;
+    // the taped forward of one level at z, its backward without parameter gradients, then the point gradient
+    // summed per ray
+    auto level = [&](int lv, int S, const float* z, const float* d_out, const float* d_weights, const float* d_warped) {
+      int alpha_step = -1, rgb_step = -1;
+      // the forward's outputs are not needed: they go to the (R,6) rows past d_dnorm's
+      if (level_forward(h, lv, R, S, z, o, d, cond, use_warp, h->d_tr_out + 6 * (size_t)R, nullptr, s, &alpha_step,
+                        &rgb_step))
+        return -1;
+      float* dpts = want_pts ? h->d_ray_pts : nullptr;
+      if (level_backward(h, lv, R, S, z, d, dcond, use_warp, alpha_step, rgb_step, d_out, d_weights, d_warped,
+                         nullptr, nullptr, s, dpts, d_directions ? d_dnorm : nullptr, false))
+        return -1;
+      if (!want_pts) return 0;
+      nfb::train::RayReduceArgs a{dpts, z, d, d_directions ? d_dnorm : nullptr,
+                                  d_origins ? d_origins + (size_t)r0 * 3 : nullptr,
+                                  d_directions ? d_directions + (size_t)r0 * 3 : nullptr, R, S};
+      nfb::train::ray_reduce_kernel<<<(R + nfb::kRaysPerBlock - 1) / nfb::kRaysPerBlock, 32 * nfb::kRaysPerBlock, 0,
+                                      s>>>(a);
+      return launch_check(h, "ray_reduce_kernel");
+    };
+    if (coarse && level(0, nc, z_coarse + (size_t)r0 * nc, at(d_out_coarse, (size_t)r0 * 6),
+                        at(d_weights_coarse, (size_t)r0 * nc), at(d_warped_coarse, (size_t)r0 * nc * 3)))
+      return -1;
+    if (fine && level(1, nfine, z_fine + (size_t)r0 * nfine, at(d_out_fine, (size_t)r0 * 6),
+                      at(d_weights_fine, (size_t)r0 * nfine), at(d_warped_fine, (size_t)r0 * nfine * 3)))
+      return -1;
+  }
+  // the rgb condition's view-direction block: to d_viewdirs, or into d_directions when the directions were
+  // encoded in their place
+  const nfb::CondLayout& L = h->cond_layout;
+  float* vd_out = viewdirs ? d_viewdirs : d_directions;
+  if (L.dv > 0 && vd_out) {
+    nfb::train::ViewdirVjpArgs v{h->d_dcond, L.stride, L.G + L.tc + L.ac, c.num_nerf_viewdir_freqs, vd, vd_out,
+                                 viewdirs ? 0 : 1, B};
+    nfb::train::viewdir_vjp_kernel<<<(unsigned)((B + 127) / 128), 128, 0, s>>>(v);
+    if (launch_check(h, "viewdir_vjp_kernel")) return -1;
+  } else if (d_viewdirs) {
+    NFB_CUDA(cudaMemsetAsync(d_viewdirs, 0, (size_t)B * 3 * sizeof(float), s));
+  }
+  if (encoded && (d_warp_code || d_app_code || d_cam_code))
+    return cond_vjp_encoded(h, B, h->d_dcond, warp_id, app_id, cam_id, d_warp_code, d_app_code, d_cam_code, s, false);
+  return 0;
 }
 
 int nfb_warp_vjp(nfb_handle* h, int P, const float* points, const unsigned* warp_id, float warp_alpha,

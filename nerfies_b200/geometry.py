@@ -453,3 +453,226 @@ def _host(t, dtype, what):
     raise ValueError(f'{what} must be (N, 3), got {a.shape}')
   return a
 
+
+
+# ---------------------------------------------------------------------------
+# Camera registration (iNeRF-style): fit a camera pose, and the photo's codes, to a photo by gradient descent
+# on the photometric loss through NerfModel.render_rays (nfb_render_ray_vjp).
+# ---------------------------------------------------------------------------
+OPTIMIZE = ('pose', 'appearance', 'camera', 'warp')
+DEFAULT_LRS = {'rotation': 2e-3, 'position': 2e-3, 'appearance': 1e-2, 'camera': 1e-2, 'warp': 1e-2}
+
+
+def _skew(w):
+  z = torch.zeros((), dtype=w.dtype, device=w.device)
+  return torch.stack([torch.stack([z, -w[2], w[1]]), torch.stack([w[2], z, -w[0]]),
+                      torch.stack([-w[1], w[0], z])])
+
+
+def rotvec_to_matrix(w):
+  """exp([w]x) of a (3,) rotation vector (Rodrigues, differentiable, in w's dtype):
+  I + sin(t)/t K + 2 sin^2(t/2)/t^2 K^2 with t = |w|, K = [w]x; below t^2 = 1e-4 both factors are their
+  Taylor series to t^4 (the remainder is below fp32 rounding), so w = 0 has a gradient."""
+  t2 = (w * w).sum()
+  small = t2 < 1e-4
+  t = torch.sqrt(torch.where(small, torch.ones_like(t2), t2))
+  a = torch.where(small, 1 - t2 / 6 + t2 * t2 / 120, torch.sin(t) / t)
+  h = torch.sin(t / 2)
+  b = torch.where(small, 0.5 - t2 / 24 + t2 * t2 / 720, 2 * h * h / (t * t))
+  K = _skew(w)
+  return torch.eye(3, dtype=w.dtype, device=w.device) + a * K + b * (K @ K)
+
+
+def pose_rays(local, orientation, position, omega, offset):
+  """Rays of camera-frame unit directions `local` (N,3) under the pose (omega, offset) applied to a camera
+  with world-to-camera rotation `orientation` (R0) and centre `position` (p0): a rotation by omega about
+  the camera centre in the world frame and a move of the centre by offset.
+    directions = exp(omega) R0^T local,  origins = p0 + offset."""
+  R = rotvec_to_matrix(omega)
+  directions = (local @ orientation) @ R.T
+  origins = (position + offset).expand_as(directions)
+  return origins, directions
+
+
+def posed_camera(camera, omega, offset):
+  """The Camera of pose_rays: orientation R0 exp(omega)^T, position p0 + offset (float64, stored float32)."""
+  R = rotvec_to_matrix(torch.as_tensor(omega, dtype=torch.float64).detach().cpu()).numpy()
+  out = camera.copy()
+  out.orientation = (camera.orientation.astype(np.float64) @ R.T).astype(np.float32)
+  out.position = (camera.position.astype(np.float64) +
+                  np.asarray(torch.as_tensor(offset).detach().cpu(), np.float64)).astype(np.float32)
+  return out
+
+
+def photometric_loss(out, target):
+  """training.py's rgb loss: the mean squared error of each level's rgb, summed over the levels."""
+  return sum(((lv['rgb'] - target)**2).mean() for lv in out.values())
+
+
+def registration_codes(model, params, metadata, warp_extra=None):
+  """The codes a registration starts from, as (1, width) float32 tensors on the model's device: the
+  embedding rows `metadata` names ({'appearance': id, 'camera': id, 'warp': id}) and, with a 'time' /
+  'blend' warp encoder, the warp code of metadata['time'] / metadata['warp'] at warp_extra's time_alpha
+  (nfb_warp_code: the TimeEncoder's output, or its blend with the GLO row).  An id outside its table
+  raises ValueError."""
+  metadata = metadata or {}
+  codes = {}
+
+  def row(key, table):
+    node = params
+    for part in table + ('embed', 'embedding'):
+      node = node[part]
+    i = int(metadata[key])
+    if not 0 <= i < node.shape[0]:
+      raise ValueError(f"metadata['{key}'] = {i}: outside the {node.shape[0]} rows of its embedding table")
+    return node[i:i + 1].detach().to(device=model.device, dtype=torch.float32).clone()
+
+  enc = model.warp_metadata_encoder_type
+  for key, used in (('warp', model.use_warp), ('appearance', model.use_appearance_metadata),
+                    ('camera', model.use_camera_metadata)):
+    need = 'time' if key == 'warp' and used and enc == 'time' else key
+    if used and need not in metadata:
+      raise KeyError(f"metadata['{need}'] is required by this model")
+  if model.use_warp:
+    if enc == 'glo':
+      codes['warp'] = row('warp', ('warp_field', 'metadata_encoder'))
+    else:
+      if enc == 'blend':
+        row('warp', ('warp_field', 'glo_encoder'))                  # the id's range
+        wid = torch.tensor([int(metadata['warp'])], dtype=torch.int32, device=model.device)
+      else:
+        wid = torch.tensor([float(metadata['time'])], dtype=torch.float32, device=model.device)
+      hd = model.handle()
+      hd.set_params(params)
+      model._set_time_alpha(hd, (warp_extra or {}).get('time_alpha'))
+      code = torch.empty(1, model.num_warp_features, device=model.device)
+      with torch.cuda.device(model.device):
+        _lib.check(hd.lib.nfb_warp_code(hd.h, 1, _ptr(wid), _ptr(code), _stream()))
+      codes['warp'] = code
+  if model.use_appearance_metadata:
+    codes['appearance'] = row('appearance', ('appearance_encoder',))
+  if model.use_camera_metadata:
+    codes['camera'] = row('camera', ('camera_encoder',))
+  return codes
+
+
+def check_registration(model, optimize, steps, batch_rays):
+  """Refuses what cannot be registered: raises ValueError.  Returns the optimised groups as a tuple."""
+  optimize = tuple(optimize)
+  for k in optimize:
+    if k not in OPTIMIZE:
+      raise ValueError(f'unknown optimize entry {k!r}: expected some of {OPTIMIZE}')
+  if not optimize:
+    raise ValueError('optimize is empty: nothing to fit')
+  if 'appearance' in optimize and not model.use_appearance_metadata:
+    raise ValueError("optimize 'appearance': the model has no appearance metadata")
+  if 'camera' in optimize and not model.use_camera_metadata:
+    raise ValueError("optimize 'camera': the model has no camera metadata")
+  time_enc = model.use_warp and model.warp_metadata_encoder_type != 'glo'
+  if 'warp' in optimize and (not model.use_warp or time_enc):
+    raise ValueError("optimize 'warp': the model has no warp field" if not model.use_warp else
+                     f"optimize 'warp': the '{model.warp_metadata_encoder_type}' encoder's code is a function of "
+                     'time, not a free code')
+  if int(steps) < 1:
+    raise ValueError(f'steps={steps}: must be >= 1')
+  if int(batch_rays) < 1:
+    raise ValueError(f'batch_rays={batch_rays}: must be >= 1')
+  return optimize
+
+
+def register_camera(model, params, camera, image, warp_extra=None, codes=None, optimize=('pose', 'appearance'),
+                    steps=200, batch_rays=1024, lrs=None, seed=0, log_every=1, lr_decay=1.0):
+  """Fits `camera`'s pose (and the photo's codes) to `image` (H, W, 3) float in [0, 1], the model held fixed.
+
+  The pose is a rotation vector omega about the camera centre (world frame) and a centre offset v
+  (pose_rays), both starting at 0; the codes start from the embedding rows `codes` names
+  ({'appearance': id, 'camera': id, 'warp': id, or 'time': t with a 'time' warp encoder;
+  registration_codes), and with a 'time' / 'blend' warp encoder the warp code stays that of the fixed time.  Each
+  step draws `batch_rays` pixels uniformly from a device generator seeded with `seed`, renders them with
+  deterministic sampling (as eval.py) through NerfModel.render_rays and takes one Adam step on
+  photometric_loss, with the learning rate of each group in `lrs` ('rotation', 'position',
+  'appearance', 'camera', 'warp'; DEFAULT_LRS otherwise).  With lr_decay < 1 each rate decays
+  exponentially from its value at the first step to lr_decay times it at the last.  The camera-frame directions come from
+  Camera's own ray kernel on an identity-pose copy, so distortion is the kernel's.
+
+  Returns (camera, codes, history): the registered Camera, the fitted codes {'appearance': (1, A), ...}
+  and one dict per logged step (step, loss, psnr of the batch's fine (else coarse) level, rotation_deg
+  |omega| in degrees, translation |v|), before that step's update."""
+  from nerfies_b200 import camera as camera_lib
+  optimize = check_registration(model, optimize, steps, batch_rays)
+  lrs = dict(DEFAULT_LRS, **(lrs or {}))
+  dev = model.device
+  h, w = camera.image_shape
+  image = torch.as_tensor(image).to(device=dev, dtype=torch.float32)
+  if tuple(image.shape) != (h, w, 3):
+    raise ValueError(f'image shape {tuple(image.shape)} does not match the camera\'s {h} x {w} x 3')
+  ident = camera.copy()
+  ident.orientation = np.eye(3, dtype=np.float32)
+  ident.position = np.zeros(3, np.float32)
+  local = camera_lib.camera_to_rays(ident, dev)['directions'].reshape(-1, 3)
+  target = image.reshape(-1, 3)
+  R0 = torch.as_tensor(camera.orientation, device=dev)
+  p0 = torch.as_tensor(camera.position, device=dev)
+  encoded = any(k in optimize for k in ('appearance', 'camera', 'warp'))
+  md = dict(codes or {})
+  if encoded:
+    start = registration_codes(model, params, md, warp_extra)
+  else:
+    start = {}
+  fit = {k: v.clone().requires_grad_(k in optimize) for k, v in start.items()}
+  omega = torch.zeros(3, device=dev, requires_grad='pose' in optimize)
+  offset = torch.zeros(3, device=dev, requires_grad='pose' in optimize)
+  groups = []
+  if 'pose' in optimize:
+    groups += [{'params': [omega], 'lr': lrs['rotation']}, {'params': [offset], 'lr': lrs['position']}]
+  groups += [{'params': [fit[k]], 'lr': lrs[k]} for k in fit if k in optimize]
+  opt = torch.optim.Adam(groups)
+  base_lrs = [g['lr'] for g in groups]
+  gen = torch.Generator(device=dev)
+  gen.manual_seed(int(seed))
+  history = []
+  n = h * w
+  for step in range(int(steps)):
+    idx = torch.randint(0, n, (int(batch_rays),), device=dev, generator=gen)
+    origins, directions = pose_rays(local[idx], R0, p0, omega, offset)
+    if encoded:
+      metadata = {k: v.expand(len(idx), -1) for k, v in fit.items()}
+    else:
+      metadata = {k: torch.full((len(idx), 1), v, device=dev,
+                                dtype=torch.float32 if k == 'time' else torch.int32) for k, v in md.items()}
+    opt.zero_grad()
+    out = model.render_rays({'params': params}, {'origins': origins, 'directions': directions, 'metadata': metadata},
+                            warp_extra=warp_extra, metadata_encoded=encoded)
+    loss = photometric_loss(out, target[idx])
+    loss.backward()
+    if step % max(1, int(log_every)) == 0 or step == int(steps) - 1:
+      last = out['fine'] if 'fine' in out else out['coarse']
+      mse = float(((last['rgb'].detach() - target[idx])**2).mean())
+      history.append({'step': step, 'loss': float(loss), 'psnr': float(-10.0 * np.log10(max(mse, 1e-30))),
+                      'rotation_deg': float(torch.linalg.norm(omega.detach())) * 180.0 / np.pi,
+                      'translation': float(torch.linalg.norm(offset.detach()))})
+    opt.step()
+    for g, lr in zip(opt.param_groups, base_lrs):
+      g['lr'] = lr * float(lr_decay)**((step + 1) / max(1, int(steps) - 1))
+  out_codes = {k: v.detach() for k, v in fit.items()}
+  return posed_camera(camera, omega, offset), out_codes, history
+
+
+def render_camera(model, params, camera, warp_extra, codes, chunk=None):
+  """The (H, W, 3) rgb of `camera`'s frame (the fine level, else the coarse one) with the per-frame codes
+  `codes` ({'warp': (1, G), 'appearance': (1, A), 'camera': (1, C)}, registration_codes) passed encoded,
+  deterministic sampling, in chunks of `chunk` rays (default: the model's batch size)."""
+  from nerfies_b200 import camera as camera_lib
+  rays = camera_lib.camera_to_rays(camera, model.device)
+  h, w = camera.image_shape
+  o, d = rays['origins'].reshape(-1, 3), rays['directions'].reshape(-1, 3)
+  chunk = int(chunk or model.batch_size)
+  out = []
+  with torch.no_grad():
+    for i in range(0, o.shape[0], chunk):
+      n = min(chunk, o.shape[0] - i)
+      md = {k: v.expand(n, -1) for k, v in codes.items()}
+      lv = model.apply({'params': params}, {'origins': o[i:i + n], 'directions': d[i:i + n], 'metadata': md},
+                       warp_extra=warp_extra, metadata_encoded=True)
+      out.append((lv['fine'] if 'fine' in lv else lv['coarse'])['rgb'])
+  return torch.cat(out).reshape(h, w, 3)

@@ -282,6 +282,72 @@ class _WarpVjp(torch.autograd.Function):
     return (None, None, *st.input_grads(ctx, hd, flat, code_grads))
 
 
+def _flat_leaves(tree, prefix=''):
+  """(name, leaf) pairs of a parameter pytree."""
+  if isinstance(tree, Mapping):
+    for k, v in tree.items():
+      yield from _flat_leaves(v, f'{prefix}{k}/')
+  else:
+    yield prefix[:-1], tree
+
+
+class _RayVjp(torch.autograd.Function):
+  """NerfModel.render_rays as an autograd.Function: the forward is nfb_render_forward keeping its z values;
+  the backward is nfb_render_ray_vjp at those z.  Inputs: origins, directions, viewdirs and the three codes
+  (None where absent); outputs: out_c, w_c, out_f, w_f (None without a fine level)."""
+
+  @staticmethod
+  def forward(ctx, st, origins, directions, viewdirs, warp_code, app_code, cam_code):
+    ctx.set_materialize_grads(False)
+    m = st.model
+    hd = st.fwd_handle
+    lib, h, dev, B = hd.lib, hd.h, m.device, st.B
+    nc, nf = m.num_coarse_samples, m.num_fine_samples
+    ids = st.ids
+    with torch.cuda.device(dev):
+      out_c = torch.empty(B, 6, device=dev)
+      w_c = torch.empty(B, nc, device=dev)
+      out_f = torch.empty(B, 6, device=dev) if nf > 0 else None
+      w_f = torch.empty(B, nc + nf, device=dev) if nf > 0 else None
+      z_f = torch.empty(B, nc + nf, device=dev) if nf > 0 else None
+      z_c = torch.empty(B, nc, device=dev)
+      _lib.check(lib.nfb_render_forward(
+          h, B, _ptr(origins), _ptr(directions), _ptr(viewdirs), *[_ptr(t) for t in ids], st.alpha,
+          _ptr(st.t_rand), _ptr(st.u_rand), st.flags, _ptr(out_c), _ptr(out_f), _ptr(w_c), _ptr(w_f), _ptr(z_f),
+          _stream()))
+      _lib.check(lib.nfb_coarse_z_vals(h, B, _ptr(st.t_rand), _ptr(z_c), _stream()))
+    st.z_c, st.z_f, st.fwd_handle = z_c, z_f, None
+    ctx.st = st
+    ctx.save_for_backward(origins, directions, viewdirs)
+    return out_c, w_c, out_f, w_f
+
+  @staticmethod
+  @torch.autograd.function.once_differentiable
+  def backward(ctx, d_out_c, d_w_c, d_out_f, d_w_f):
+    st = ctx.st
+    m = st.model
+    o, d, v = ctx.saved_tensors
+    need = ctx.needs_input_grad
+    if all(t is None for t in (d_out_c, d_w_c, d_out_f, d_w_f)) or not any(need[1:]):
+      return (None,) * 7
+    hd = st.handle()
+    dev = m.device
+    d_o = torch.empty(st.B, 3, device=dev) if need[1] else None
+    d_d = torch.empty(st.B, 3, device=dev) if need[2] else None
+    d_v = torch.empty(st.B, 3, device=dev) if need[3] else None
+    widths = (m.num_warp_features, m.num_appearance_features, m.num_camera_features)
+    code_grads = [torch.zeros(st.B, widths[k], device=dev) if need[4 + k] else None for k in range(3)]
+    cot = [_contig(t) for t in (d_out_c, d_out_f, d_w_c, d_w_f)]
+    if not any(t is not None for t in [d_o, d_d, d_v] + code_grads):
+      return (None,) * 7
+    with torch.cuda.device(dev):
+      _lib.check(hd.lib.nfb_render_ray_vjp(
+          hd.h, st.B, _ptr(o), _ptr(d), _ptr(v), *[_ptr(t) for t in st.ids], st.alpha, st.flags,
+          _ptr(st.z_c), _ptr(st.z_f), *[_ptr(t) for t in cot], None, None, _ptr(d_o), _ptr(d_d), _ptr(d_v),
+          *[_ptr(t) for t in code_grads], int(m.vjp_chunk_rays), _stream()))
+    return (None, d_o, d_d, d_v, *code_grads)
+
+
 class NerfModel:
   """Mirror of nerfies.models.NerfModel (models.py:31-375), forward only."""
 
@@ -578,39 +644,8 @@ class NerfModel:
     B = origins.shape[0]
     viewdirs = (_prep_f32(rays_dict['viewdirs'], dev)
                 if 'viewdirs' in rays_dict else None)
-    md = rays_dict.get('metadata', {})
     use_warp = self.use_warp and use_warp
-    if metadata_encoded:
-      # models.py:198-213,251 / warping.py:186-187: the metadata leaves are the
-      # per-ray embeddings themselves, (B, num_*_features) float32.
-      def enc(key, width, used):
-        if not used:
-          return None
-        v = md.get(key)
-        if v is None:
-          return None
-        v = _prep_f32(v, dev)
-        if v.shape != (B, width):
-          raise ValueError(f"metadata_encoded=True: metadata['{key}'] must be ({B}, {width}), "
-                           f'got {tuple(v.shape)}')
-        return v
-      warp_id = enc('warp', self.num_warp_features, self.use_warp)
-      app_id = enc('appearance', self.num_appearance_features, self.use_appearance_metadata)
-      cam_id = enc('camera', self.num_camera_features, self.use_camera_metadata)
-    else:
-      if self.use_warp and self.warp_metadata_encoder_type == 'time':
-        # models.py:252-254: the warp field reads metadata['time'] (B,1) float32
-        t = md.get('time')
-        warp_id = None if t is None else _prep_f32(t, dev).reshape(-1)
-      else:
-        warp_id = _prep_ids(md.get('warp'), dev) if self.use_warp else None
-      app_id = (_prep_ids(md.get('appearance'), dev)
-                if self.use_appearance_metadata else None)
-      cam_id = (_prep_ids(md.get('camera'), dev)
-                if self.use_camera_metadata else None)
-    if self.use_warp and use_warp and warp_id is None:
-      key = 'time' if self.warp_metadata_encoder_type == 'time' else 'warp'
-      raise KeyError(f"rays_dict['metadata']['{key}'] is required")
+    warp_id, app_id, cam_id = self._call_metadata(rays_dict, B, metadata_encoded, use_warp)
     return_weights = self.use_weights or return_weights
     if t_rand is None and u_rand is None:
       t_rand, u_rand = self._draws(rngs, B)
@@ -735,6 +770,92 @@ class NerfModel:
     return out
 
   __call__ = apply
+
+  def _call_metadata(self, rays_dict, B, metadata_encoded, use_warp):
+    """(warp_id, app_id, cam_id) device tensors of a call's rays_dict['metadata'] (None where unused)."""
+    md = rays_dict.get('metadata', {})
+    dev = self.device
+    if metadata_encoded:
+      # models.py:198-213,251 / warping.py:186-187: the metadata leaves are the
+      # per-ray embeddings themselves, (B, num_*_features) float32.
+      def enc(key, width, used):
+        if not used:
+          return None
+        v = md.get(key)
+        if v is None:
+          return None
+        v = _prep_f32(v, dev)
+        if v.shape != (B, width):
+          raise ValueError(f"metadata_encoded=True: metadata['{key}'] must be ({B}, {width}), "
+                           f'got {tuple(v.shape)}')
+        return v
+      warp_id = enc('warp', self.num_warp_features, self.use_warp)
+      app_id = enc('appearance', self.num_appearance_features, self.use_appearance_metadata)
+      cam_id = enc('camera', self.num_camera_features, self.use_camera_metadata)
+    else:
+      if self.use_warp and self.warp_metadata_encoder_type == 'time':
+        # models.py:252-254: the warp field reads metadata['time'] (B,1) float32
+        t = md.get('time')
+        warp_id = None if t is None else _prep_f32(t, dev).reshape(-1)
+      else:
+        warp_id = _prep_ids(md.get('warp'), dev) if self.use_warp else None
+      app_id = (_prep_ids(md.get('appearance'), dev)
+                if self.use_appearance_metadata else None)
+      cam_id = (_prep_ids(md.get('camera'), dev)
+                if self.use_camera_metadata else None)
+    if self.use_warp and use_warp and warp_id is None:
+      key = 'time' if self.warp_metadata_encoder_type == 'time' else 'warp'
+      raise KeyError(f"rays_dict['metadata']['{key}'] is required")
+    return warp_id, app_id, cam_id
+
+  def render_rays(self, variables, rays_dict, warp_extra=None, metadata_encoded=False, t_rand=None,
+                  u_rand=None, use_warp=True):
+    """model.apply's level dicts (rgb, depth, med_depth, acc, weights, and the z_vals used), differentiable with respect to the
+    RAYS: origins, directions and viewdirs and, with metadata_encoded=True, the metadata codes.  The
+    parameters are constants; a parameter leaf that requires grad raises ValueError (its gradient would
+    be dropped - model.apply differentiates the parameters).
+
+    The forward is model.apply's fast path (nfb_render_forward, deterministic samples unless `t_rand` /
+    `u_rand` are given); `loss.backward()` runs nfb_render_ray_vjp at the z values it used, which are
+    constants, as in the reference (z_fine is stop_gradient'ed).  med_depth has no gradient.  Chunks of
+    `vjp_chunk_rays`, the model's train_precision."""
+    params = variables['params']
+    for name, t in _flat_leaves(params):
+      if torch.is_tensor(t) and t.requires_grad:
+        raise ValueError(f'render_rays: parameter {name!r} requires grad; render_rays holds the parameters '
+                         'constant (model.apply differentiates them)')
+    warp_extra = warp_extra or {'alpha': 0.0, 'time_alpha': 0.0}
+    alpha = float(warp_extra.get('alpha', 0.0))
+    dev = self.device
+    origins = _prep_f32(rays_dict['origins'], dev)
+    directions = _prep_f32(rays_dict['directions'], dev)
+    if origins.dim() != 2 or origins.shape[-1] != 3 or directions.shape != origins.shape:
+      raise ValueError('origins and directions must be (B, 3)')
+    B = origins.shape[0]
+    viewdirs = _prep_f32(rays_dict['viewdirs'], dev) if 'viewdirs' in rays_dict else None
+    if viewdirs is not None and viewdirs.shape != origins.shape:
+      raise ValueError('viewdirs must be (B, 3)')
+    use_warp = self.use_warp and use_warp
+    warp_id, app_id, cam_id = self._call_metadata(rays_dict, B, metadata_encoded, use_warp)
+    if not metadata_encoded:
+      warp_id, app_id, cam_id = (None if t is None else t.detach() for t in (warp_id, app_id, cam_id))
+    t_rand = None if t_rand is None else _prep_f32(t_rand, dev).detach()
+    u_rand = None if u_rand is None else _prep_f32(u_rand, dev).detach()
+    hd = self.handle(B)
+    hd.set_params(params)
+    self._set_time_alpha(hd, warp_extra.get('time_alpha'))
+    flags = (0 if use_warp else _lib.FLAG_NO_WARP) | (_lib.FLAG_METADATA_ENCODED if metadata_encoded else 0)
+    codes = (warp_id, app_id, cam_id) if metadata_encoded else (None, None, None)
+    st = _VjpState(self, hd, None, B=B, alpha=alpha, time_alpha=warp_extra.get('time_alpha'), flags=flags,
+                   t_rand=t_rand, u_rand=u_rand, fwd_handle=hd,
+                   ids=tuple(None if t is None else t.detach() for t in (warp_id, app_id, cam_id)))
+    out_c, w_c, out_f, w_f = _RayVjp.apply(st, origins, directions, viewdirs, *codes)
+    ret = {}
+    for lv, o, w, z in (('coarse', out_c, w_c, st.z_c), ('fine', out_f, w_f, st.z_f)):
+      if o is not None:
+        ret[lv] = {'rgb': o[:, 0:3], 'depth': o[:, 3], 'med_depth': o[:, 4], 'acc': o[:, 5], 'weights': w,
+                   'z_vals': z}
+    return ret
 
   def _set_time_alpha(self, hd, time_alpha):
     """warp_extra['time_alpha'] for the 'time' / 'blend' encoders (None -> the
