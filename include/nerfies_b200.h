@@ -245,6 +245,26 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
                                  int chunk_rays, const nfb_train_reg* reg, float* const* grads,
                                  const long long* numels, int count, float* loss_out, void* stream);
 
+/* nfb_train_value_and_grad_reg plus the gradients of the same loss with respect to the batch's rays, for
+ * refining the training cameras' poses (nfb_pose_grad):
+ *   d_origins (B,3), d_directions (B,3): device, nullable, overwritten (=).  With both null the call is
+ *     nfb_train_value_and_grad_reg, launch for launch.
+ * The ray gradient is that of the total loss the call differentiates with the sample points x = o + z d, z a
+ * constant (as nfb_render_ray_vjp), with one exception: the elastic loss's Jacobian is evaluated at points
+ * held constant (stop_gradient), since its derivative in the points needs the warp's second derivative.  So
+ * both photometric losses and the warp regulariser (through its warped term and its direct term in the
+ * points) contribute; the elastic and background losses contribute nothing.  Without viewdirs the directions
+ * are encoded as view directions, and that share is in d_directions; with viewdirs it is not.  The
+ * parameter gradients and loss_out are those of nfb_train_value_and_grad_reg (up to the order of its float
+ * atomics). */
+int nfb_train_value_and_grad_rays(nfb_handle* h, int B, const float* origins, const float* directions,
+                                  const float* viewdirs, const unsigned* warp_id, const unsigned* app_id,
+                                  const unsigned* cam_id, float warp_alpha, const float* t_rand,
+                                  const float* u_rand, unsigned flags, const float* rgb_target,
+                                  int chunk_rays, const nfb_train_reg* reg, float* const* grads,
+                                  const long long* numels, int count, float* loss_out, float* d_origins,
+                                  float* d_directions, void* stream);
+
 /* Vector-Jacobian product of one nfb_render_forward call with respect to the parameters: what jax.vjp of
  * NerfModel.__call__ gives for any loss on its outputs (training.py:228-264 is one such loss).
  *   origins ... flags: the forward call's arguments (NFB_FLAG_NO_WARP, NFB_FLAG_COARSE_ONLY and
@@ -408,6 +428,33 @@ typedef struct nfb_ray_table {
 int nfb_gather_rays(const nfb_ray_table* table, long long first, long long count,
                     float* origins, float* directions, float* pixels, float* rgb,
                     int* appearance, int* camera, int* warp, float* time, void* stream);
+
+/* ---- training camera poses ---------------------------------------------------
+ * Image k of a ray table has a pose p_k = (omega_k, v_k), six floats, zero for the capture's camera:
+ *   directions d = exp(omega_k) d0 (a rotation about the camera centre in the world frame),
+ *   origins    o = o0 + v_k (a move of the centre),
+ * with d0, o0 the rays of nfb_gather_rays and exp the Rodrigues formula (Taylor series below |omega|^2 =
+ * 1e-4).
+ *
+ * nfb_gather_rays of origins and directions with image k's camera moved by pose k ((num_images,6) device,
+ * nullable: a null or zero pose returns nfb_gather_rays' rays bit for bit), and image (count) int32
+ * (nullable), the table image of each ray. */
+int nfb_gather_rays_posed(const nfb_ray_table* table, long long first, long long count, const float* pose,
+                          float* origins, float* directions, int* image, void* stream);
+
+/* Bytes of device workspace nfb_pose_grad needs (< 0: invalid arguments). */
+long long nfb_pose_grad_workspace_size(int num_images, long long count);
+
+/* grad (num_images,6) += the pose gradient of count rays of images image (count) (nfb_gather_rays_posed):
+ *   dL/dv_k     = sum over image k's rays of d_origins,
+ *   dL/domega_k = J_l(omega_k)^T sum over image k's rays of (directions x d_directions),
+ * J_l being SO(3)'s left Jacobian (same series threshold as the pose).  directions are the posed ones; pose
+ * (nullable: zero); d_origins or d_directions may be null (zero), not both.  A segmented reduction in fp64
+ * with no atomics: two calls on the same inputs give the same bits.  An image with no ray gets 0; a ray
+ * whose image is outside [0, num_images) is ignored.  Needs no handle. */
+int nfb_pose_grad(int num_images, const float* pose, const int* image, const float* directions,
+                  const float* d_origins, const float* d_directions, long long count, float* grad, void* workspace,
+                  long long workspace_bytes, void* stream);
 
 /* ---- per-frame image metrics of eval.py:process_batch ------------------------
  * Images are (num_images, height, width, channels) float32, channels interleaved (what

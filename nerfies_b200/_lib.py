@@ -28,7 +28,8 @@ SYMBOLS = [
     'nfb_marching_cubes_count', 'nfb_marching_cubes', 'nfb_marching_cubes_table', 'nfb_warp_invert',
     'nfb_point_visibility', 'nfb_flow_colorize', 'nfb_selftest_composite_vjp', 'nfb_selftest_elastic',
     'nfb_selftest_depth_index', 'nfb_selftest_warp_mag_loss', 'nfb_render_ray_vjp',
-    'nfb_warp_code',
+    'nfb_warp_code', 'nfb_train_value_and_grad_rays', 'nfb_gather_rays_posed', 'nfb_pose_grad_workspace_size',
+    'nfb_pose_grad',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -190,6 +191,8 @@ def load():
   lib.nfb_train_value_and_grad_reg.argtypes = [vp, ci] + [vp] * 6 + [cf, vp, vp, cu, vp, ci, vp, ctypes.POINTER(vp),
                                                ctypes.POINTER(ctypes.c_longlong), ci, vp, vp]
   lib.nfb_train_value_and_grad_reg.restype = ci
+  lib.nfb_train_value_and_grad_rays.argtypes = lib.nfb_train_value_and_grad_reg.argtypes[:-1] + [vp, vp, vp]
+  lib.nfb_train_value_and_grad_rays.restype = ci
   lib.nfb_render_vjp.argtypes = [vp, ci] + [vp] * 6 + [cf, cu] + [vp] * 11 + [ci, ctypes.POINTER(vp),
                                                                               ctypes.POINTER(ctypes.c_longlong), ci, vp]
   lib.nfb_render_vjp.restype = ci
@@ -231,6 +234,12 @@ def load():
   lib.nfb_pixels_to_rays.restype = ci
   lib.nfb_gather_rays.argtypes = [ctypes.POINTER(NfbRayTable), ll, ll] + [vp] * 9
   lib.nfb_gather_rays.restype = ci
+  lib.nfb_gather_rays_posed.argtypes = [ctypes.POINTER(NfbRayTable), ll, ll, vp, vp, vp, vp, vp]
+  lib.nfb_gather_rays_posed.restype = ci
+  lib.nfb_pose_grad_workspace_size.argtypes = [ci, ll]
+  lib.nfb_pose_grad_workspace_size.restype = ll
+  lib.nfb_pose_grad.argtypes = [ci, vp, vp, vp, vp, vp, ll, vp, vp, ll, vp]
+  lib.nfb_pose_grad.restype = ci
   lib.nfb_image_metrics_workspace_size.argtypes = [ci, ci, ci, ci]
   lib.nfb_image_metrics_workspace_size.restype = ll
   lib.nfb_image_metrics.argtypes = [ci, ci, ci, ci, vp, vp, vp, vp, vp, ll, vp, vp, vp, vp]

@@ -168,7 +168,19 @@ def restore_checkpoint(ckpt_dir, target=None, step=None, prefix='checkpoint_', d
   state.step = int(np.asarray(opt.get('state', {}).get('step', 0)).reshape(-1)[0])
   # Adam's moments, {'model': {...: {'grad_ema', 'grad_sq_ema'}}}: what a resumed run needs
   state.param_states = _to_torch(opt.get('state', {}).get('param_states') or {}, device)
+  # refined training cameras (training.CameraPoses.state_dict), host arrays; None without
+  state.camera_poses = state_dict.get('camera_poses')
   return state
+
+
+def checkpoint_camera_poses(ckpt_dir, prefix='checkpoint_'):
+  """The saved camera poses of the newest checkpoint in `ckpt_dir` (None without one or without poses).
+  Host only: lets a driver refuse a checkpoint before any GPU work."""
+  path = latest_checkpoint(ckpt_dir, prefix)
+  if path is None:
+    return None
+  with open(path, 'rb') as fp:
+    return msgpack_restore(fp.read()).get('camera_poses')
 
 
 def _check_same_structure(want, got, where):
@@ -197,6 +209,9 @@ def save_checkpoint(ckpt_dir, state, step, prefix='checkpoint_', keep=2):
       'warp_alpha': np.asarray(state.warp_alpha, np.float32),
       'time_alpha': np.asarray(state.time_alpha, np.float32),
   }
+  poses = getattr(state, 'camera_poses', None)
+  if poses is not None:
+    tree['camera_poses'] = poses.state_dict() if hasattr(poses, 'state_dict') else poses
   path = os.path.join(ckpt_dir, f'{prefix}{step}')
   tmp = path + '.tmp'
   with open(tmp, 'wb') as fp:

@@ -132,6 +132,13 @@ class TrainConfig:
   warp_reg_loss_alpha: float = -2.0
   warp_reg_loss_scale: float = 0.001
   shuffle_buffer_size: int = 5000000
+  # Refine the training cameras' poses jointly with the model (training.CameraPoses): a rotation about each
+  # camera centre and a move of the centre per train item, starting at zero.
+  refine_camera_poses: bool = False
+  # One Adam learning rate for the rotation (radians) and the translation (scene units), which are comparable
+  # in a normalised scene.  The default is a guess that nobody has tuned.
+  camera_pose_lr_schedule: ScheduleDef = dataclasses.field(default_factory=lambda: {
+      'type': 'exponential', 'initial_value': 1e-3, 'final_value': 1e-5, 'num_steps': 1000000})
   save_every: int = 10000
   log_every: int = 500
   histogram_every: int = 5000

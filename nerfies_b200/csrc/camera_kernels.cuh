@@ -194,7 +194,43 @@ struct GatherArgs {
   float* rgb;          // (count,3)
   int *appearance, *camera, *warp;   // (count)
   float* time;         // (count)
+  const float* pose;   // (num_images,6) [omega | v] or null: image k's camera moved by pose k (pose_moved_ray)
+  int* image;          // (count) the table image of each ray
 };
+
+// exp([w]x) of a rotation vector, as geometry.rotvec_to_matrix: I + a K + b K^2 with a = sin(t)/t and
+// b = 2 sin^2(t/2)/t^2, their Taylor series to t^4 below t^2 = 1e-4.  Row-major.
+__host__ __device__ __forceinline__ void rotvec_matrix(const float w[3], float R[9]) {
+  const float t2 = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
+  float a, b;
+  if (t2 < 1e-4f) {
+    a = 1.f - t2 / 6.f + t2 * t2 / 120.f;
+    b = 0.5f - t2 / 24.f + t2 * t2 / 720.f;
+  } else {
+    const float t = sqrtf(t2), h = sinf(0.5f * t);
+    a = sinf(t) / t;
+    b = 2.f * h * h / t2;
+  }
+  const float K[9] = {0.f, -w[2], w[1], w[2], 0.f, -w[0], -w[1], w[0], 0.f};
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) {
+      const float kk = K[3 * i] * K[j] + K[3 * i + 1] * K[3 + j] + K[3 * i + 2] * K[6 + j];
+      R[3 * i + j] = (i == j ? 1.f : 0.f) + a * K[3 * i + j] + b * kk;
+    }
+}
+
+// A ray of a camera moved by the pose p = (omega, v) (geometry.pose_rays): d <- exp(omega) d, o <- o + v.
+// A zero pose gives exp(0) = I exactly, so the ray is returned bit for bit.
+__device__ __forceinline__ void pose_moved_ray(const float* p, float* o, float* d) {
+  float R[9];
+  rotvec_matrix(p, R);
+  const float x = d[0], y = d[1], z = d[2];
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    d[j] = R[3 * j] * x + R[3 * j + 1] * y + R[3 * j + 2] * z;
+    o[j] = o[j] + p[3 + j];
+  }
+}
 
 __global__ void __launch_bounds__(256) gather_rays_kernel(const GatherArgs a) {
   const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
@@ -211,17 +247,18 @@ __global__ void __launch_bounds__(256) gather_rays_kernel(const GatherArgs a) {
     if (__ldg(t.pixel_offsets + mid) <= r) lo = mid; else hi = mid;
   }
   const nfb_camera& c = t.cameras[lo];
+  if (a.image) a.image[i] = lo;
   if (a.origins || a.directions || a.pixels) {
     float px, py;
     camera_pixel_center(c, r - __ldg(t.pixel_offsets + lo), px, py);
-    if (a.directions) {
-      float d[3];
-      camera_pixel_direction(c, camera_has_distortion(c), px, py, d);
+    float o[3] = {c.position[0], c.position[1], c.position[2]}, d[3] = {0.f, 0.f, 0.f};   // datasets/core.py:176
+    if (a.directions) camera_pixel_direction(c, camera_has_distortion(c), px, py, d);
+    if (a.pose) pose_moved_ray(a.pose + 6 * lo, o, d);
+    if (a.directions)
       for (int j = 0; j < 3; ++j) a.directions[3 * i + j] = d[j];
-    }
     if (a.pixels) { a.pixels[2 * i] = px; a.pixels[2 * i + 1] = py; }
     if (a.origins)
-      for (int j = 0; j < 3; ++j) a.origins[3 * i + j] = c.position[j];   // datasets/core.py:176
+      for (int j = 0; j < 3; ++j) a.origins[3 * i + j] = o[j];
   }
   if (a.rgb)   // datasets/nerfies.py:62: float32(u8) / 255.0, an IEEE division
     for (int j = 0; j < 3; ++j) a.rgb[3 * i + j] = (float)__ldg(t.rgb + 3 * r + j) / 255.f;

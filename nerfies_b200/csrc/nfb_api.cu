@@ -16,6 +16,7 @@
 #include "field_simt.cuh"
 #include "ray_kernels.cuh"
 #include "camera_kernels.cuh"
+#include "pose_kernels.cuh"
 #include "metrics_kernels.cuh"
 #include "image_kernels.cuh"
 #include "viz_kernels.cuh"
@@ -651,6 +652,33 @@ void launch_metrics(const MetricsPlan& p, int N, const float* image, const float
   finalize_kernel<<<N, kThreads, 0, s>>>(fa);
 }
 
+// nfb_gather_rays, and with `pose` / `image` nfb_gather_rays_posed: one kernel, one pixel-to-ray path.
+int gather_rays(const nfb_ray_table* table, long long first, long long count, float* origins, float* directions,
+                float* pixels, float* rgb, int* appearance, int* camera, int* warp, float* time, const float* pose,
+                int* image, void* stream) {
+  if (!table) return fail("null ray table");
+  const nfb_ray_table& t = *table;
+  if (t.num_images < 1) return fail("ray table has %d images", t.num_images);
+  if (t.num_rays < 1) return fail("ray table has %lld rays", t.num_rays);
+  if (count < 0 || first < 0) return fail("negative ray range (first %lld, count %lld)", first, count);
+  if (!t.cameras || !t.pixel_offsets) return fail("ray table needs cameras and pixel_offsets");
+  if (rgb && !t.rgb) return fail("rgb requested but the ray table has none");
+  if ((appearance && !t.appearance) || (camera && !t.camera) || (warp && !t.warp) || (time && !t.time))
+    return fail("metadata requested but the ray table has none of that kind");
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
+    return fail("no CUDA device: nerfies_b200 has no CPU path");
+  if (count == 0) return 0;
+  nfb::GatherArgs a{};
+  a.t = t; a.first = first; a.count = count;
+  a.origins = origins; a.directions = directions; a.pixels = pixels; a.rgb = rgb;
+  a.appearance = appearance; a.camera = camera; a.warp = warp; a.time = time;
+  a.pose = pose; a.image = image;
+  nfb::gather_rays_kernel<<<(unsigned)((count + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("gather_rays_kernel launch failed: %s", cudaGetErrorString(e));
+  return 0;
+}
 }  // namespace
 
 extern "C" {
@@ -689,28 +717,46 @@ static int launch_camera(const nfb_camera* cam, const float* pixels_in, long lon
 int nfb_gather_rays(const nfb_ray_table* table, long long first, long long count, float* origins,
                     float* directions, float* pixels, float* rgb, int* appearance, int* camera, int* warp,
                     float* time, void* stream) {
-  if (!table) return fail("null ray table");
-  const nfb_ray_table& t = *table;
-  if (t.num_images < 1) return fail("ray table has %d images", t.num_images);
-  if (t.num_rays < 1) return fail("ray table has %lld rays", t.num_rays);
-  if (count < 0 || first < 0) return fail("negative ray range (first %lld, count %lld)", first, count);
-  if (!t.cameras || !t.pixel_offsets) return fail("ray table needs cameras and pixel_offsets");
-  if (rgb && !t.rgb) return fail("rgb requested but the ray table has none");
-  if ((appearance && !t.appearance) || (camera && !t.camera) || (warp && !t.warp) || (time && !t.time))
-    return fail("metadata requested but the ray table has none of that kind");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-    return fail("no CUDA device: nerfies_b200 has no CPU path");
+  return gather_rays(table, first, count, origins, directions, pixels, rgb, appearance, camera, warp, time, nullptr,
+                     nullptr, stream);
+}
+
+int nfb_gather_rays_posed(const nfb_ray_table* table, long long first, long long count, const float* pose,
+                          float* origins, float* directions, int* image, void* stream) {
+  return gather_rays(table, first, count, origins, directions, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                     pose, image, stream);
+}
+
+long long nfb_pose_grad_workspace_size(int num_images, long long count) {
+  if (num_images < 1 || count < 0) return -1;
+  return std::max<long long>(1, (count + nfb::kPoseRays - 1) / nfb::kPoseRays) * num_images * 6 * (long long)sizeof(double);
+}
+
+int nfb_pose_grad(int num_images, const float* pose, const int* image, const float* directions,
+                  const float* d_origins, const float* d_directions, long long count, float* grad, void* workspace,
+                  long long workspace_bytes, void* stream) {
+  if (num_images < 1) return fail("pose grad: num_images=%d must be >= 1", num_images);
+  if (count < 0) return fail("pose grad: count=%lld must be >= 0", count);
+  if (!grad) return fail("pose grad: null grad");
+  if (count > 0 && (!image || !directions)) return fail("pose grad: null image / directions");
+  if (!d_origins && !d_directions) return fail("pose grad: d_origins and d_directions are both null");
+  const long long need = nfb_pose_grad_workspace_size(num_images, count);
+  if (!workspace || workspace_bytes < need)
+    return fail("pose grad: the workspace holds %lld bytes, %lld needed", workspace_bytes, need);
   if (count == 0) return 0;
-  nfb::GatherArgs a{};
-  a.t = t; a.first = first; a.count = count;
-  a.origins = origins; a.directions = directions; a.pixels = pixels; a.rgb = rgb;
-  a.appearance = appearance; a.camera = camera; a.warp = warp; a.time = time;
-  nfb::gather_rays_kernel<<<(unsigned)((count + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a);
+  const int blocks = (int)((count + nfb::kPoseRays - 1) / nfb::kPoseRays);
+  nfb::PoseGradArgs a{num_images, count, pose, image, directions, d_origins, d_directions,
+                      static_cast<double*>(workspace), grad};
+  cudaStream_t s = (cudaStream_t)stream;
+  nfb::pose_partials_kernel<<<blocks, nfb::kPoseRays, 0, s>>>(a);
   cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail("gather_rays_kernel launch failed: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail("pose_partials_kernel launch failed: %s", cudaGetErrorString(e));
+  nfb::pose_finish_kernel<<<(num_images + 127) / 128, 128, 0, s>>>(a, blocks);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("pose_finish_kernel launch failed: %s", cudaGetErrorString(e));
   return 0;
 }
+
 
 int nfb_camera_rays(const nfb_camera* cam, long long first_pixel, long long count, float* origins,
                     float* directions, float* pixels, void* stream) {

@@ -474,13 +474,17 @@ int level_backward(nfb_handle* h, int level, int R, int S, const float* z, const
     depth_index_kernel<<<(unsigned)((R + 7) / 8), 256, 0, s>>>(weights, R, S, h->d_sel);
     if (launch_check(h, "depth_index_kernel")) return -1;
   }
-  if (reg && reg->elastic && level == 0 && warp) {
-    // training.py:176-193 (the coarse level only: training.py:242-244)
+  // training.py:176-193 (the coarse level only: training.py:242-244).  The elastic loss holds the sample points
+  // constant, so with `dpts` the primal-head gradient of an SE(3) field's elastic loss (which the warp MLP's
+  // backward would carry to the points) is taken through a warp backward of its own after the main one.
+  const bool elastic = reg && reg->elastic && level == 0 && warp;
+  const bool elastic_late = elastic && dpts && p.warp_type == 2;
+  auto run_elastic = [&]() {
     const bool median = reg->reduce == 0;
-    if (warp_jacobian_on_tape(h, p, t, A, median ? h->d_sel : nullptr, median ? R : rows, median ? nullptr : weights,
-                              reg, true, nullptr, s))
-      return -1;
-  }
+    return warp_jacobian_on_tape(h, p, t, A, median ? h->d_sel : nullptr, median ? R : rows,
+                                 median ? nullptr : weights, reg, true, nullptr, s);
+  };
+  if (elastic && !elastic_late && run_elastic()) return -1;
   if (net_backward(h, p.nerf, A + t.in_n, A + t.d_in_n, t.ld_n, t.out_n, t.d_out_n, A, rows, s, with_dw)) return -1;
   {
     EncodeBwdArgs e{};
@@ -504,7 +508,18 @@ int level_backward(nfb_handle* h, int level, int R, int S, const float* z, const
     add_into_kernel<<<(unsigned)((rows * 3 + 255) / 256), 256, 0, s>>>(A + t.dwarped, d_warped, rows * 3);
     if (launch_check(h, "add_into_kernel")) return -1;
   }
-  return warp_backward(h, p, t, S, dcond, s, dpts, with_dw);
+  if (warp_backward(h, p, t, S, dcond, s, dpts, with_dw)) return -1;
+  if (dpts && reg && reg->warp_reg) {
+    // the warp-reg loss's direct term in the points, -(its share of dwarped), after warp_backward has set dpts
+    WarpMagArgs wm{A + t.pts, A + t.warped, h->d_sel, nullptr, nullptr, reg->warp_reg_alpha, reg->warp_reg_scale,
+                   reg->warp_reg_weight / (float)reg->batch_rays, R, dpts};
+    warp_mag_loss_kernel<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(wm);
+    if (launch_check(h, "warp_mag_loss_kernel")) return -1;
+  }
+  if (!elastic_late) return 0;
+  NFB_CUDA(cudaMemsetAsync(A + t.grad_begin, 0, (size_t)(t.grad_end - t.grad_begin) * sizeof(float), s));
+  if (run_elastic()) return -1;
+  return warp_backward(h, p, t, S, dcond, s, nullptr, with_dw);
 }
 
 // The gradient accumulators of the packed parameters and of the three embedding tables, zeroed.
@@ -703,6 +718,18 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
                                  const float* u_rand, unsigned flags, const float* rgb_target,
                                  int chunk_rays, const nfb_train_reg* reg, float* const* grads,
                                  const long long* numels, int count, float* loss_out, void* stream) {
+  return nfb_train_value_and_grad_rays(h, B, origins, directions, viewdirs, warp_id, app_id, cam_id, warp_alpha,
+                                       t_rand, u_rand, flags, rgb_target, chunk_rays, reg, grads, numels, count,
+                                       loss_out, nullptr, nullptr, stream);
+}
+
+int nfb_train_value_and_grad_rays(nfb_handle* h, int B, const float* origins, const float* directions,
+                                  const float* viewdirs, const unsigned* warp_id, const unsigned* app_id,
+                                  const unsigned* cam_id, float warp_alpha, const float* t_rand,
+                                  const float* u_rand, unsigned flags, const float* rgb_target,
+                                  int chunk_rays, const nfb_train_reg* reg, float* const* grads,
+                                  const long long* numels, int count, float* loss_out, float* d_origins,
+                                  float* d_directions, void* stream) {
   if (check_call(h, B)) return -1;
   if (!rgb_target || !grads || !numels || !loss_out) return fail("null argument");
   if (count != (int)h->specs.size()) return fail("expected %d gradient tensors, got %d", (int)h->specs.size(), count);
@@ -718,6 +745,12 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
   const int nc = c.num_coarse_samples, nfine = nc + c.num_fine_samples;
   const bool use_warp = !(flags & NFB_FLAG_NO_WARP);
   const bool fine = c.num_fine_samples > 0;
+  // the ray gradients: a level's point gradient (rows,3), then dL/d|d| (R), in nfb_render_ray_vjp's buffer
+  const bool want_rays = d_origins || d_directions;
+  const size_t pts_floats = (size_t)chunk_rays * nfine * 3;
+  if (want_rays && grow(&h->d_ray_pts, &h->ray_pts_cap, (long long)pts_floats + chunk_rays, "ray gradient")) return -1;
+  if (d_origins) NFB_CUDA(cudaMemsetAsync(d_origins, 0, (size_t)B * 3 * sizeof(float), s));
+  if (d_directions) NFB_CUDA(cudaMemsetAsync(d_directions, 0, (size_t)B * 3 * sizeof(float), s));
   if (set_window(h, warp_alpha, s)) return -1;
   if (zero_grads(h, s)) return -1;
   NFB_CUDA(cudaMemsetAsync(h->d_loss, 0, nfb::train::kLossSlots * sizeof(float), s));
@@ -759,8 +792,17 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
       nfb::train::photometric_loss_kernel<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(out, tg, scale, R, d_out,
                                                                                      h->d_loss + loss_slot);
       if (launch_check(h, "photometric_loss_kernel")) return -1;
-      return level_backward(h, lv, R, S, z, d, dcond, use_warp, alpha_step, rgb_step, d_out, nullptr, nullptr, w,
-                            rcfg, s);
+      float* dpts = want_rays ? h->d_ray_pts : nullptr;
+      float* dnorm = d_directions ? h->d_ray_pts + pts_floats : nullptr;
+      if (level_backward(h, lv, R, S, z, d, dcond, use_warp, alpha_step, rgb_step, d_out, nullptr, nullptr, w,
+                         rcfg, s, dpts, dnorm))
+        return -1;
+      if (!want_rays) return 0;
+      nfb::train::RayReduceArgs a{dpts, z, d, dnorm, d_origins ? d_origins + (size_t)r0 * 3 : nullptr,
+                                  d_directions ? d_directions + (size_t)r0 * 3 : nullptr, R, S};
+      nfb::train::ray_reduce_kernel<<<(R + nfb::kRaysPerBlock - 1) / nfb::kRaysPerBlock, 32 * nfb::kRaysPerBlock, 0,
+                                      s>>>(a);
+      return launch_check(h, "ray_reduce_kernel");
     };
     float* zc = h->d_zc + (size_t)r0 * nc;
     if (level(0, nc, zc, h->d_tr_out, nfb::train::kSlotRgbCoarse)) return -1;
@@ -770,6 +812,14 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
           level(1, nfine, zf, h->d_tr_out + 6 * (size_t)R, nfb::train::kSlotRgbFine))
         return -1;
     }
+  }
+  // the directions are encoded as view directions when the batch has none: that share goes to d_directions
+  const nfb::CondLayout& L = h->cond_layout;
+  if (d_directions && !viewdirs && L.dv > 0) {
+    nfb::train::ViewdirVjpArgs v{h->d_dcond, L.stride, L.G + L.tc + L.ac, c.num_nerf_viewdir_freqs, directions,
+                                 d_directions, 1, B};
+    nfb::train::viewdir_vjp_kernel<<<(unsigned)((B + 127) / 128), 128, 0, s>>>(v);
+    if (launch_check(h, "viewdir_vjp_kernel")) return -1;
   }
   if (run_cond_bwd(h, B, h->d_dcond, warp_id, app_id, cam_id, s) || time_backward(h, B, h->d_dcond, s)) return -1;
   // background loss (training.py:118-135, 246-257): warp_field.apply on free points

@@ -334,10 +334,11 @@ __global__ void __launch_bounds__(64) jac_elastic_kernel(const JacArgs a) {
 // ---------------------------------------------------------------------------
 struct WarpMagArgs {
   const float* pts; const float* warped; const int* sel;
-  float* dwarped;                // (rows,3): += at the selected rows
-  float* stats;                  // += [loss, sqrt(residual)] sums
+  float* dwarped;                // (rows,3): += at the selected rows, or null
+  float* stats;                  // += [loss, sqrt(residual)] sums, or null
   float alpha, scale, grad_scale;
   long long R;
+  float* dpts;                   // (rows,3): -= at the selected rows (the loss's direct term in x), or null
 };
 __global__ void warp_mag_loss_kernel(const WarpMagArgs a) {
   const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -347,10 +348,14 @@ __global__ void warp_mag_loss_kernel(const WarpMagArgs a) {
   for (int c = 0; c < 3; ++c) { d[c] = a.warped[row * 3 + c] - a.pts[row * 3 + c]; sq += d[c] * d[c]; }
   float loss, dl;
   general_loss(sq, a.alpha, a.scale, loss, dl);
-  atomicAdd(a.stats + 0, loss);
-  atomicAdd(a.stats + 1, sqrtf(sq));
+  if (a.stats) {
+    atomicAdd(a.stats + 0, loss);
+    atomicAdd(a.stats + 1, sqrtf(sq));
+  }
   if (a.dwarped)
     for (int c = 0; c < 3; ++c) a.dwarped[row * 3 + c] += a.grad_scale * dl * 2.f * d[c];
+  if (a.dpts)
+    for (int c = 0; c < 3; ++c) a.dpts[row * 3 + c] -= a.grad_scale * dl * 2.f * d[c];
 }
 
 __global__ void add_noise_kernel(const float* __restrict__ p, const float* __restrict__ noise, float* __restrict__ o,

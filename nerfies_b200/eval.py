@@ -182,6 +182,20 @@ def delete_old_renders(render_dir, max_renders):
     shutil.rmtree(path)
 
 
+def refined_items(items, saved_poses):
+  """(id, camera, metadata, rgb) items with each camera moved by its saved pose (training.CameraPoses'
+  state_dict; geometry.posed_camera).  Items without a saved pose keep their camera."""
+  from nerfies_b200 import geometry
+  out = []
+  for item_id, cam, md, rgb in items:
+    pose = saved_poses['items'].get(str(item_id))
+    if pose is not None:
+      p = np.asarray(pose['pose'], np.float64).reshape(6)
+      cam = geometry.posed_camera(cam, p[:3], p[3:])
+    out.append((item_id, cam, md, rgb))
+  return out
+
+
 def evaluate(exp_config, model_config, train_config, eval_config, base_folder, data_dir=None,
              precision='fp16x3', poll_seconds=10.0, datasource=None, construct_fn=models.construct_nerf,
              frame_fn=render_and_score, log=print, save_viz=False):
@@ -227,6 +241,12 @@ def evaluate(exp_config, model_config, train_config, eval_config, base_folder, d
       state = checkpoints.restore_checkpoint(str(dirs['checkpoints']), init_state, step=step, device=device)
       save_dir = dirs['renders'] if eval_config.save_output and rank == 0 else None
       todo = list(sets)
+      saved_poses = getattr(state, 'camera_poses', None)
+      if saved_poses is not None:
+        # train items from the cameras refined in training; val items keep the capture's (register_camera
+        # aligns a held-out view)
+        todo = [(tag, refined_items(items, saved_poses) if tag == 'train' else items) for tag, items in todo]
+        log(f'Step {step}: rendering train items from the refined camera poses of the checkpoint')
       if test_cameras:
         md = choose_test_metadata(datasource, step)
         todo.append(('test', [(f'{k:03d}', cam, md, None) for k, cam in enumerate(test_cameras)]))

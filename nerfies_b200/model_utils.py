@@ -16,6 +16,9 @@ class TrainState:
   optimizer: Optimizer
   warp_alpha: float = 0.0
   time_alpha: float = 0.0
+  # training.CameraPoses while refining the training cameras; a restored checkpoint's saved poses
+  # ({'step', 'items': {item_id: {'pose', 'grad_ema', 'grad_sq_ema'}}}); or None
+  camera_poses: Any = None
 
   @property
   def warp_extra(self):

@@ -21,6 +21,7 @@ Where this differs from the reference, on purpose:
     ids and noise from the key it is given and returns it unchanged; the reference splits its key
     every step (training.py:163).  The driver passes a new key per step instead.
 """
+import json
 import sys
 import time
 
@@ -42,14 +43,44 @@ def step_key(random_seed, rank, step):
 
 
 def flatten_stats(stats):
-  """train_step's stats under the tags of train.py:71-78: '<key>/<branch>' and 'loss/background'."""
+  """train_step's stats under the tags of train.py:71-78: '<key>/<branch>' and 'loss/background';
+  with refined cameras also 'camera_poses/rotation_deg' and 'camera_poses/translation' (means over them)."""
   out = {}
   for branch in ('coarse', 'fine'):
     for key, value in stats.get(branch, {}).items():
       out[f'{key}/{branch}'] = value
   if 'background_loss' in stats:
     out['loss/background'] = stats['background_loss']
+  for key, value in stats.get('camera_poses', {}).items():
+    out[f'camera_poses/{key}'] = value
   return out
+
+
+def check_camera_poses(train_config, saved, train_ids=None):
+  """Refuses, with ValueError, a checkpoint whose saved camera poses (checkpoints.checkpoint_camera_poses)
+  do not fit the run: poses with refine_camera_poses off (training on would silently revert the cameras),
+  or poses of other items than `train_ids`."""
+  if saved is None:
+    return
+  if not train_config.refine_camera_poses:
+    raise ValueError('the checkpoint holds refined camera poses but TrainConfig.refine_camera_poses is off: '
+                     'training on would silently revert the cameras to the capture\'s')
+  if train_ids is not None:
+    training.CameraPoses(train_ids, 'cpu').check(saved)
+
+
+def write_cameras(datasource, poses, directory):
+  """`<directory>/<item>.json` of each refined train camera at the capture's original scale."""
+  from nerfies_b200 import camera as camera_lib
+  from nerfies_b200 import geometry
+  from nerfies_b200 import register_camera
+  directory.mkdir(parents=True, exist_ok=True)
+  pose = poses.pose.detach().cpu().double()
+  for k, item in enumerate(poses.item_ids):
+    cam = geometry.posed_camera(datasource.load_camera(item), pose[k, :3], pose[k, 3:])
+    template = camera_lib.Camera.from_json(datasource.camera_dir / f'{item}{datasource.camera_ext}')
+    (directory / f'{item}.json').write_text(
+        json.dumps(register_camera.original_scale_camera(datasource, cam, template).to_json(), indent=2))
 
 
 def train(exp_config, model_config, train_config, base_folder, data_dir=None, precision='fp32',
@@ -77,8 +108,11 @@ def _train(exp_config, model_config, train_config, base_folder, data_dir, precis
   if train_config.batch_size % world != 0:
     raise ValueError('Batch size must be divisible by the number of devices.')
 
+  saved_poses = checkpoints.checkpoint_camera_poses(str(dirs['checkpoints']))
+  check_camera_poses(train_config, saved_poses)
   if datasource is None:
     datasource = driver_utils.make_datasource(exp_config, model_config, data_dir)
+  check_camera_poses(train_config, saved_poses, datasource.train_ids)
   learning_rate_sched = schedules.from_config(train_config.lr_schedule)          # train.py:199-203
   warp_alpha_sched = schedules.from_config(train_config.warp_alpha_schedule)
   time_alpha_sched = schedules.from_config(train_config.time_alpha_schedule)
@@ -97,11 +131,21 @@ def _train(exp_config, model_config, train_config, base_folder, data_dir, precis
     state.optimizer.load(restored)
     model.invalidate_params()
   init_step = state.optimizer.step + 1
+  pose_kw = {}
+  if train_config.refine_camera_poses:
+    pose_lr_sched = schedules.from_config(train_config.camera_pose_lr_schedule)
+    poses = training.CameraPoses(datasource.train_ids, model.device)
+    if restored is not state and restored.camera_poses is None:
+      log('The checkpoint holds no camera poses: refining them from the capture\'s cameras (zero poses)')
+    elif restored is not state:
+      poses.load(restored.camera_poses)
+    state.camera_poses = poses
+    pose_kw = {'poses': poses.pose}
 
   first_batch = init_step - 1
   train_iter = datasource.create_iterator(                                       # train.py:175-183
       datasource.train_ids, flatten=True, shuffle=True, batch_size=train_config.batch_size,
-      shuffle_buffer_size=train_config.shuffle_buffer_size, first_batch=first_batch)
+      shuffle_buffer_size=train_config.shuffle_buffer_size, first_batch=first_batch, **pose_kw)
   points_iter = None
   if train_config.use_background_loss:                                           # train.py:185-197
     points = datasource.load_points(shuffle=True)
@@ -120,6 +164,8 @@ def _train(exp_config, model_config, train_config, base_folder, data_dir, precis
   def save(step):
     if rank == 0:
       checkpoints.save_checkpoint(str(dirs['checkpoints']), state, step, keep=2)   # training.py:46-53
+      if state.camera_poses is not None:
+        write_cameras(datasource, state.camera_poses, dirs['exp'] / 'cameras' / f'{step:08d}')
 
   log(f'Starting training at step {init_step} of {train_config.max_steps} on {world} GPU(s)')
   mark = torch.cuda.Event(enable_timing=True)
@@ -131,6 +177,8 @@ def _train(exp_config, model_config, train_config, base_folder, data_dir, precis
       batch['background_points'] = next(points_iter)
     scalar_params.learning_rate = learning_rate_sched(step)
     scalar_params.elastic_loss_weight = elastic_loss_weight_sched(step)
+    if pose_kw:
+      scalar_params.camera_pose_learning_rate = pose_lr_sched(step)
     state.warp_alpha = warp_alpha_sched(step)
     state.time_alpha = time_alpha_sched(step)
     state, stats, _ = training.train_step(

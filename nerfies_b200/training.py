@@ -23,6 +23,7 @@ import dataclasses
 import math
 from typing import Any, Dict
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -41,6 +42,7 @@ class ScalarParams:
   warp_reg_loss_scale: float = 0.001
   background_loss_weight: float = 0.0
   background_noise_std: float = 0.001
+  camera_pose_learning_rate: float = 0.0    # Adam's rate for TrainState.camera_poses (TrainConfig.refine_camera_poses)
 
 
 class AdamOptimizer(model_utils.Optimizer):
@@ -130,6 +132,70 @@ def create_train_state(model, params, warp_alpha=0.0, time_alpha=0.0):
   return model_utils.TrainState(opt, warp_alpha=warp_alpha, time_alpha=time_alpha)
 
 
+class CameraPoses:
+  """The training cameras' poses, refined with the model: pose k = (omega_k, v_k) of item_ids[k] (the ray
+  table's image order) moves that camera's rays as nfb_gather_rays_posed does (geometry.pose_rays),
+  directions exp(omega_k) R0_k^T local and origins p0_k + v_k.  `pose` (N,6) is a device vector with its own
+  Adam moments and step count; it starts at zero."""
+
+  def __init__(self, item_ids, device, beta1=0.9, beta2=0.999, eps=1e-8):
+    self.item_ids = [str(i) for i in item_ids]
+    n = len(self.item_ids)
+    self.pose = torch.zeros(n, 6, device=device, dtype=torch.float32)
+    self.m = torch.zeros_like(self.pose)
+    self.v = torch.zeros_like(self.pose)
+    self.step = 0
+    self.beta1, self.beta2, self.eps = beta1, beta2, eps
+    self._workspace = None
+
+  def state_dict(self):
+    """{'step', 'items': {item_id: {'pose' (6,), 'grad_ema', 'grad_sq_ema'}}} on the host (checkpoints)."""
+    pose, m, v = (t.detach().cpu().numpy() for t in (self.pose, self.m, self.v))
+    return {'step': np.asarray(self.step, np.int32),
+            'items': {k: {'pose': pose[i], 'grad_ema': m[i], 'grad_sq_ema': v[i]}
+                      for i, k in enumerate(self.item_ids)}}
+
+  def check(self, saved):
+    """Raises ValueError when `saved` (state_dict's layout) holds poses of other items than item_ids."""
+    got = set((saved or {}).get('items', {}))
+    if got != set(self.item_ids):
+      raise ValueError(f'the checkpoint holds camera poses of items {sorted(got)}, but the train items are '
+                       f'{sorted(self.item_ids)}')
+
+  def load(self, saved):
+    """Copies a saved state_dict (the same items, any order) into the device buffers."""
+    self.check(saved)
+    items = saved['items']
+    for key, t in (('pose', self.pose), ('grad_ema', self.m), ('grad_sq_ema', self.v)):
+      t.copy_(torch.stack([torch.as_tensor(items[k][key]).reshape(6) for k in self.item_ids]))
+    self.step = int(np.asarray(saved.get('step', 0)).reshape(-1)[0])
+
+  def grad(self, image, directions, d_origins, d_directions, out):
+    """out (N,6) += the pose gradient of a batch's ray gradients (nfb_pose_grad)."""
+    lib = _lib.load()
+    n, count = self.pose.shape[0], int(image.numel())
+    need = int(lib.nfb_pose_grad_workspace_size(n, count))
+    if self._workspace is None or self._workspace.numel() < need:
+      self._workspace = torch.empty(need, dtype=torch.uint8, device=self.pose.device)
+    with torch.cuda.device(self.pose.device):
+      _lib.check(lib.nfb_pose_grad(n, _ptr(self.pose), _ptr(image), _ptr(directions), _ptr(d_origins),
+                                   _ptr(d_directions), count, _ptr(out), _ptr(self._workspace),
+                                   self._workspace.numel(), _stream()))
+
+  def apply_gradient(self, grad, learning_rate):
+    """One Adam step of the poses (nfb_adam_step), in place."""
+    self.step += 1
+    lib = _lib.load()
+    with torch.cuda.device(self.pose.device):
+      _lib.check(lib.nfb_adam_step(_ptr(self.pose), _ptr(grad), _ptr(self.m), _ptr(self.v), self.pose.numel(),
+                                   float(learning_rate), self.beta1, self.beta2, self.eps, self.step, _stream()))
+
+  def stats(self):
+    """Device scalars: the mean |omega| in degrees and the mean |v| over the images."""
+    return {'rotation_deg': torch.rad2deg(self.pose[:, :3].norm(dim=1)).mean(),
+            'translation': self.pose[:, 3:].norm(dim=1).mean()}
+
+
 def make_reg(model, scalar_params=None, use_elastic_loss=False, elastic_reduce_method='median',
              elastic_loss_type='log_svals', use_background_loss=False, use_warp_reg_loss=False,
              background_points=None, background_warp_ids=None, background_noise=None):
@@ -165,10 +231,12 @@ def make_reg(model, scalar_params=None, use_elastic_loss=False, elastic_reduce_m
 
 
 def value_and_grad(model, params, batch, warp_extra, rngs=None, chunk_rays=256, t_rand=None,
-                   u_rand=None, grads=None, reg=None):
+                   u_rand=None, grads=None, reg=None, ray_grads=None):
   """(loss dict, flat gradient) of the training loss (training.py:171-259, 263-264): the
   photometric terms and, with `reg` (make_reg), the regularisers.
-  `grads` (flat, zeroed by the caller) may be passed to accumulate into."""
+  `grads` (flat, zeroed by the caller) may be passed to accumulate into.  `ray_grads`, a pair of
+  (B,3) float32 device tensors (either may be None), receives the loss's gradient with respect to the
+  origins and directions (nfb_train_value_and_grad_rays: the elastic loss holds its points constant)."""
   dev = model.device
   origins = _prep_f32(batch['origins'], dev)
   directions = _prep_f32(batch['directions'], dev)
@@ -200,12 +268,16 @@ def value_and_grad(model, params, batch, warp_extra, rngs=None, chunk_rays=256, 
     off += k
   loss = torch.zeros(16, device=dev)
   reg_struct, keep = reg if isinstance(reg, tuple) else (reg, None)
+  d_origins, d_directions = ray_grads or (None, None)
+  for t in (d_origins, d_directions):
+    if t is not None and (t.dtype != torch.float32 or t.device != torch.device(dev) or not t.is_contiguous() or t.numel() != B * 3):
+      raise ValueError(f'ray_grads: expected contiguous float32 ({B}, 3) tensors on {dev}')
   with torch.cuda.device(dev):
-    _lib.check(hd.lib.nfb_train_value_and_grad_reg(
+    _lib.check(hd.lib.nfb_train_value_and_grad_rays(
         hd.h, B, _ptr(origins), _ptr(directions), _ptr(viewdirs), _ptr(warp_id), _ptr(app_id),
         _ptr(cam_id), float((warp_extra or {}).get('alpha', 0.0)), _ptr(t_rand), _ptr(u_rand), 0,
         _ptr(target), int(chunk_rays), ctypes.byref(reg_struct) if reg_struct is not None else None,
-        ptrs, (ctypes.c_longlong * n)(*numels), n, _ptr(loss), _stream()))
+        ptrs, (ctypes.c_longlong * n)(*numels), n, _ptr(loss), _ptr(d_origins), _ptr(d_directions), _stream()))
   del keep
   out = {'coarse': loss[0], 'fine': loss[1]}
   if reg_struct is not None:
@@ -261,8 +333,22 @@ def train_step(model, rng_key, state, batch, scalar_params, use_elastic_loss=Fal
     ev[0].record()
   params = opt.target['model']
   model.invalidate_params()     # the Adam kernel rewrote the flat vector under the views
+  poses = state.camera_poses
+  grads = ray_grads = None
+  if poses is not None:
+    if 'image' not in batch:
+      raise ValueError("refining camera poses needs batches with 'image' (create_iterator(..., poses=...))")
+    # the pose gradient rides at the tail of the flat gradient vector: still one all-reduce per step
+    n_params = opt.flat.numel()
+    grads = torch.zeros(n_params + poses.pose.numel(), device=model.device, dtype=torch.float32)
+    B = batch['origins'].shape[0]
+    ray_grads = tuple(torch.empty(B, 3, device=model.device, dtype=torch.float32) for _ in range(2))
   losses, grads = value_and_grad(model, params, batch, state.warp_extra,
-                                 rngs={'coarse': rng_key, 'fine': rng_key}, chunk_rays=chunk_rays, reg=reg)
+                                 rngs={'coarse': rng_key, 'fine': rng_key}, chunk_rays=chunk_rays, reg=reg,
+                                 grads=grads, ray_grads=ray_grads)
+  if poses is not None:
+    poses.grad(_prep_ids(batch['image'], model.device), _prep_f32(batch['directions'], model.device), *ray_grads,
+               out=grads[n_params:])
   if ev:
     ev[1].record()
   # stats of _compute_loss_and_stats (training.py:171-226)
@@ -290,6 +376,9 @@ def train_step(model, rng_key, state, batch, scalar_params, use_elastic_loss=Fal
   if ev:
     ev[2].record()
   opt.apply_gradient(grads, learning_rate=scalar_params.learning_rate)
+  if poses is not None:
+    poses.apply_gradient(grads[n_params:], scalar_params.camera_pose_learning_rate)
+    stats['camera_poses'] = poses.stats()
   if ev:
     ev[3].record()
     ev[3].synchronize()
