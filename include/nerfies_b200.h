@@ -737,6 +737,42 @@ int nfb_selftest_train_gemm(int train_precision, int mode, long long rows, int n
                             const float* bias, float* y, const float* dy, float* dx, float* din, float* dw,
                             long long k_split, long long* k_split_used, void* stream);
 
+/* Self-test of the training tier's layer walker (net_forward / net_backward) on one network of the handle, in its
+ * training precision (nfb_set_train_precision), with the handle's parameters (nfb_set_params first).
+ *   net NFB_NET_WARP: the warp field's trunk and heads (level 0).  NFB_NET_NERF: the NeRF MLP of `level` (0 coarse,
+ *   1 fine: trunk, bottleneck, alpha head, rgb branch).  NFB_NET_TIME: the TimeEncoder's MLP (level 0).
+ * nfb_selftest_net_steps: *n_steps receives the network's Dense layers in execution order (at most 16) and steps
+ *   NFB_NET_STEP_FIELDS ints per layer: [n, npad, k_x, k_in, in_off, act, producer].  The layer computes
+ *   act([X | IN[:, in_off:in_off + k_in]] W + b) of n outputs, X the first k_x columns of the output of layer
+ *   `producer` (-1: none, k_x = 0); act an activation of nfb_config.  Host pointers.
+ * nfb_selftest_net: the forward and the backward of the network on `rows` rows of `in` (rows, ld_in).  `tape` holds
+ *   every layer's output Y_s (rows, npad_s), layer after layer, and then every layer's adjoint dY_s in the same
+ *   layout.  The caller seeds the adjoints with the cotangent (zero where there is none); the backward adds each
+ *   consumer's dX into its producer's adjoint, so on return they hold the whole dY.  d_in (rows, ld_in; nullable)
+ *   += dIN.  with_dw = 1 also forms the parameter gradients and adds them into `grads` (count tensors of `numels`
+ *   elements, in nfb_param_info order, as nfb_train_value_and_grad; the other networks' and the tables' are 0),
+ *   the dW reductions split into slices of k_split rows (0: the training step's split).  Device pointers;
+ *   asynchronous on `stream`.  Bad arguments fail (nfb_last_error).  No reference analogue. */
+enum { NFB_NET_WARP = 0, NFB_NET_NERF = 1, NFB_NET_TIME = 2, NFB_NET_STEP_FIELDS = 7 };
+int nfb_selftest_net_steps(const nfb_handle* h, int level, int net, int* n_steps, int* steps);
+int nfb_selftest_net(nfb_handle* h, int level, int net, long long rows, const float* in, int ld_in, float* tape,
+                     float* d_in, int with_dw, long long k_split, float* const* grads, const long long* numels,
+                     int count, void* stream);
+
+/* Self-test of the condition vectors' adjoints on the handle's layout ([warp | trunk | alpha | rgb], the rgb block
+ * [viewdirs | appearance | camera]), from dcond (B, stride) of B rays.  encoded = 0: cond_bwd_kernel, the
+ * scatter-add into the embedding tables' gradients at the ids (nullable: row 0; clamped to the table), the warp
+ * block scaled by 1 ('glo'), 1 - time_alpha ('blend') or 0 ('time'); d_time (B, G; nullable) = the TimeEncoder
+ * output's gradient (time_cond_bwd_kernel).  encoded = 1: cond_vjp_encoded_kernel, d_warp (B,G), d_app (B,A),
+ * d_cam (B,C) += the blocks of the codes has_codes names (bits 1, 2, 4; a null pointer drops that code), and the
+ * codes it does not name to row 0 of their tables.  The tables' gradients are added into `grads` (count tensors
+ * of `numels` elements in nfb_param_info order; the others are 0).  Device pointers; asynchronous on `stream`.
+ * Bad arguments fail (nfb_last_error).  No reference analogue. */
+int nfb_selftest_cond_vjp(nfb_handle* h, int B, const float* dcond, const unsigned* warp_id, const unsigned* app_id,
+                          const unsigned* cam_id, int encoded, int has_codes, float* d_warp, float* d_app,
+                          float* d_cam, float* d_time, float* const* grads, const long long* numels, int count,
+                          void* stream);
+
 /* Self-tests of the training step's seed and regulariser kernels: each launches the production kernel with the
  * production launch configuration and argument struct on caller buffers.  Device pointers; no handle; allocates
  * nothing; asynchronous on `stream`.  Bad arguments fail (nfb_last_error).  No reference analogue.
@@ -768,6 +804,28 @@ int nfb_selftest_elastic(long long R, int warp_type, int pivot, int trans, int l
 int nfb_selftest_depth_index(int R, int S, const float* weights, int* sel, void* stream);
 int nfb_selftest_warp_mag_loss(long long R, const float* pts, const float* warped, const int* sel, float alpha,
                                float scale, float grad_scale, float* dwarped, float* stats, void* stream);
+
+/* Self-tests of the adjoints between the MLPs and the rays, with the same conventions:
+ * nfb_selftest_encode_bwd: encode_bwd_kernel, the adjoint of the encoding [x | sin(2^f x) | sin(2^f x + pi/2) |
+ *   cond] (rows of S samples per ray): din (rows, ld >= 3 + 6F + n_cond), pts (rows,3), window (F; nullable);
+ *   dpts (rows,3; nullable) = dL/dx, dcond (rays, cond_stride; nullable) += the cond columns at cond_off (atomic
+ *   over a ray's samples; zero entries skipped).
+ * nfb_selftest_warp_tail_bwd: warp_tail_bwd_kernel, dhead (rows, ld; nullable) += (d warped / d head)^T dwarped, and
+ *   warp_tail_dx_kernel, dpts (rows,3; nullable) += (d warped / d x)^T dwarped, for the translation (warp_type 1)
+ *   or SE(3) tail (2; heads [w v (pivot) (translation)]) at head (rows, ld) and pts (rows,3).
+ * nfb_selftest_ray_reduce: ray_reduce_kernel for R rays of S <= 1024 samples: d_origins (R,3) += sum_s dpts,
+ *   d_directions (R,3) += sum_s z dpts + d_dnorm d / |d| (d_dnorm (R) nullable); either output nullable.
+ * nfb_selftest_viewdir_vjp: viewdir_vjp_kernel, out (R,3) (= or, with accumulate, +=) the adjoint of the view
+ *   direction encoding (F frequencies) whose gradient is dcond[:, off .. off + 3 + 6F) (R, stride). */
+int nfb_selftest_encode_bwd(long long rows, int S, const float* pts, const float* window, const float* din, int F,
+                            int ld, int cond_stride, int cond_off, int n_cond, float* dpts, float* dcond,
+                            void* stream);
+int nfb_selftest_warp_tail_bwd(long long rows, int warp_type, int pivot, int trans, const float* head, int ld,
+                               const float* pts, const float* dwarped, float* dhead, float* dpts, void* stream);
+int nfb_selftest_ray_reduce(int R, int S, const float* dpts, const float* z, const float* directions,
+                            const float* d_dnorm, float* d_origins, float* d_directions, void* stream);
+int nfb_selftest_viewdir_vjp(int R, const float* dcond, int stride, int off, int F, const float* viewdirs,
+                             float* out, int accumulate, void* stream);
 
 /* Number of CUDA kernels this handle has launched so far (bench accounting). */
 long long nfb_kernel_launches(const nfb_handle* h);

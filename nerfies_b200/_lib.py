@@ -29,7 +29,8 @@ SYMBOLS = [
     'nfb_point_visibility', 'nfb_flow_colorize', 'nfb_selftest_composite_vjp', 'nfb_selftest_elastic',
     'nfb_selftest_depth_index', 'nfb_selftest_warp_mag_loss', 'nfb_render_ray_vjp',
     'nfb_warp_code', 'nfb_train_value_and_grad_rays', 'nfb_gather_rays_posed', 'nfb_pose_grad_workspace_size',
-    'nfb_pose_grad',
+    'nfb_pose_grad', 'nfb_selftest_net_steps', 'nfb_selftest_net', 'nfb_selftest_cond_vjp',
+    'nfb_selftest_encode_bwd', 'nfb_selftest_warp_tail_bwd', 'nfb_selftest_ray_reduce', 'nfb_selftest_viewdir_vjp',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -286,6 +287,22 @@ def load():
   lib.nfb_selftest_depth_index.restype = ci
   lib.nfb_selftest_warp_mag_loss.argtypes = [ll, vp, vp, vp, cf, cf, cf, vp, vp, vp]
   lib.nfb_selftest_warp_mag_loss.restype = ci
+  lib.nfb_selftest_net_steps.argtypes = [vp, ci, ci, ctypes.POINTER(ci), ctypes.POINTER(ci)]
+  lib.nfb_selftest_net_steps.restype = ci
+  lib.nfb_selftest_net.argtypes = [vp, ci, ci, ll, vp, ci, vp, vp, ci, ll, ctypes.POINTER(vp),
+                                   ctypes.POINTER(ll), ci, vp]
+  lib.nfb_selftest_net.restype = ci
+  lib.nfb_selftest_cond_vjp.argtypes = [vp, ci] + [vp] * 4 + [ci, ci] + [vp] * 4 + [ctypes.POINTER(vp),
+                                                                                    ctypes.POINTER(ll), ci, vp]
+  lib.nfb_selftest_cond_vjp.restype = ci
+  lib.nfb_selftest_encode_bwd.argtypes = [ll, ci, vp, vp, vp, ci, ci, ci, ci, ci, vp, vp, vp]
+  lib.nfb_selftest_encode_bwd.restype = ci
+  lib.nfb_selftest_warp_tail_bwd.argtypes = [ll, ci, ci, ci, vp, ci, vp, vp, vp, vp, vp]
+  lib.nfb_selftest_warp_tail_bwd.restype = ci
+  lib.nfb_selftest_ray_reduce.argtypes = [ci, ci] + [vp] * 7
+  lib.nfb_selftest_ray_reduce.restype = ci
+  lib.nfb_selftest_viewdir_vjp.argtypes = [ci, vp, ci, ci, ci, vp, vp, ci, vp]
+  lib.nfb_selftest_viewdir_vjp.restype = ci
   lib.nfb_set_train_precision.argtypes = [vp, ci]
   lib.nfb_set_train_precision.restype = ci
   lib.nfb_debug_provoke_timeout.argtypes = [vp, ci]

@@ -111,10 +111,11 @@ int net_forward(nfb_handle* h, const Net& net, const float* in, int ld_in, const
   return 0;
 }
 
-// with_dw = false: dX only (the ray VJP, which differentiates no parameter).
+// with_dw = false: dX only (the ray VJP, which differentiates no parameter).  k_split > 0 sets the rows per
+// slice of every dW reduction (nfb_selftest_net); 0 is dw_split_for's choice.
 int net_backward(nfb_handle* h, const Net& net, const float* in, float* d_in, int ld_in,
                  const long long* out_off, const long long* d_out_off, float* arena, long long rows,
-                 cudaStream_t s, bool with_dw = true) {
+                 cudaStream_t s, bool with_dw = true, long long k_split = 0) {
   int producer[nfb::kMaxSteps];
   net_producers(net, producer);
   for (int i = net.n_steps - 1; i >= 0; --i) {
@@ -127,7 +128,8 @@ int net_backward(nfb_handle* h, const Net& net, const float* in, float* d_in, in
     // dW += [X | IN]^T dZ   (reduction over the rows, split)
     if (with_dw &&
         launch_gemm<false, true>(h, K, st.n, rows, nfb::train::ConcatAT{a}, nfb::train::DZB{dz},
-                                 nfb::train::AtomicAdd{h->d_gpacked + st.w_off, st.npad}, dw_split_for(h, K, st.n, rows), s, "sgemm (dW)")) return -1;
+                                 nfb::train::AtomicAdd{h->d_gpacked + st.w_off, st.npad},
+                                 k_split > 0 ? k_split : dw_split_for(h, K, st.n, rows), s, "sgemm (dW)")) return -1;
     // db += colsum(dZ)
     if (with_dw) {
       dim3 grid((unsigned)((st.n + 31) / 32), (unsigned)std::min<long long>((rows + 255) / 256, 128));
@@ -365,21 +367,27 @@ int time_forward(nfb_handle* h, int n, const float* time_f, const unsigned* time
   return launch_check(h, "time_cond_kernel");
 }
 
+// The adjoint of time_cond_kernel for `n` rows: dy (n, ld) = d cond[:, 0:G] / d Y (time_alpha, a constant of
+// the step, scales it under 'blend').
+int time_cond_bwd(nfb_handle* h, int n, const float* dcond, float* dy, int ld, cudaStream_t s) {
+  const int G = h->cond_layout.G;
+  const float scale = h->cfg.warp_metadata_encoder == NFB_WARP_ENC_BLEND ? h->time_alpha : 1.f;
+  nfb::train::time_cond_bwd_kernel<<<(unsigned)(((long long)n * G + 255) / 256), 256, 0, s>>>(
+      dcond, h->cond_layout.stride, G, scale, dy, ld, n);
+  return launch_check(h, "time_cond_bwd_kernel");
+}
+
 // Adjoint of time_forward: the condition-vector gradient of the same `n` rows -> the TimeEncoder's parameter
-// gradients (d_gpacked).  time_alpha is a constant of the step.
+// gradients (d_gpacked).
 int time_backward(nfb_handle* h, int n, const float* dcond, cudaStream_t s) {
-  using namespace nfb::train;
   if (!has_time_encoder(h)) return 0;
   const nfb_config& c = h->cfg;
   const Net& net = h->time_net;
   const TimeTapeLayout t = time_tape_layout(net, c.time_encoder_num_freqs, n);
   float* T = h->d_time_tape;
   NFB_CUDA(cudaMemsetAsync(T + t.grad_begin, 0, (size_t)(t.total - t.grad_begin) * sizeof(float), s));
-  const int last = net.n_steps - 1, G = h->cond_layout.G;
-  const float scale = c.warp_metadata_encoder == NFB_WARP_ENC_BLEND ? h->time_alpha : 1.f;
-  time_cond_bwd_kernel<<<(unsigned)(((long long)n * G + 255) / 256), 256, 0, s>>>(
-      dcond, h->cond_layout.stride, G, scale, T + t.d_out[last], net.steps[last].npad, n);
-  if (launch_check(h, "time_cond_bwd_kernel")) return -1;
+  const int last = net.n_steps - 1;
+  if (time_cond_bwd(h, n, dcond, T + t.d_out[last], net.steps[last].npad, s)) return -1;
   return net_backward(h, net, T + t.in, nullptr, t.ld, t.out, t.d_out, T, n, s);
 }
 
@@ -1210,6 +1218,93 @@ int nfb_selftest_train_gemm(int train_precision, int mode, long long rows, int n
 }  // extern "C"
 
 namespace {
+// The network nfb_selftest_net(_steps) names: the warp field's, a level's NeRF MLP or the TimeEncoder's.
+int selftest_net_of(const nfb_handle* h, int level, int net, const Net** out, const char* what) {
+  if (!h) return fail("%s: null handle", what);
+  if (net == NFB_NET_NERF) {
+    if (level != 0 && level != 1) return fail("%s: level %d is not 0 or 1", what, level);
+    if (level == 1 && h->cfg.num_fine_samples <= 0) return fail("%s: level 1 needs fine samples", what);
+    *out = &h->prog[level].nerf;
+    return 0;
+  }
+  if (net != NFB_NET_WARP && net != NFB_NET_TIME) return fail("%s: net %d is not a network of the handle", what, net);
+  if (level != 0) return fail("%s: level %d: the warp field and the TimeEncoder belong to level 0", what, level);
+  if (net == NFB_NET_WARP && h->prog[0].warp_type == 0) return fail("%s: the model has no warp field", what);
+  if (net == NFB_NET_TIME && !has_time_encoder(h)) return fail("%s: the model has no TimeEncoder", what);
+  *out = net == NFB_NET_WARP ? &h->prog[0].warp : &h->time_net;
+  return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int nfb_selftest_net_steps(const nfb_handle* h, int level, int net, int* n_steps, int* steps) {
+  const Net* nt = nullptr;
+  if (selftest_net_of(h, level, net, &nt, "selftest_net_steps")) return -1;
+  if (!n_steps || !steps) return fail("selftest_net_steps: null n_steps / steps");
+  int producer[nfb::kMaxSteps];
+  net_producers(*nt, producer);
+  *n_steps = nt->n_steps;
+  for (int i = 0; i < nt->n_steps; ++i) {
+    const Step& st = nt->steps[i];
+    const int f[NFB_NET_STEP_FIELDS] = {st.n, st.npad, st.k_x, st.k_in, st.in_off, st.act, producer[i]};
+    for (int j = 0; j < NFB_NET_STEP_FIELDS; ++j) steps[i * NFB_NET_STEP_FIELDS + j] = f[j];
+  }
+  return 0;
+}
+
+// net_forward, then net_backward, on one network of the handle and caller rows.
+int nfb_selftest_net(nfb_handle* h, int level, int net, long long rows, const float* in, int ld_in, float* tape,
+                     float* d_in, int with_dw, long long k_split, float* const* grads, const long long* numels,
+                     int count, void* stream) {
+  const Net* nt = nullptr;
+  if (selftest_net_of(h, level, net, &nt, "selftest_net")) return -1;
+  if (check_call(h, 0)) return -1;
+  if (rows < 1) return fail("selftest_net: rows=%lld must be >= 1", rows);
+  if (!in || !tape) return fail("selftest_net: null in / tape");
+  int width = 0;
+  for (int i = 0; i < nt->n_steps; ++i) width = std::max(width, nt->steps[i].in_off + nt->steps[i].k_in);
+  if (ld_in < width) return fail("selftest_net: ld_in=%d is below the network's %d input columns", ld_in, width);
+  if (with_dw != 0 && with_dw != 1) return fail("selftest_net: with_dw=%d is not 0 or 1", with_dw);
+  if (k_split < 0 || (k_split > 0 && !with_dw)) return fail("selftest_net: k_split=%lld needs with_dw and >= 0", k_split);
+  if (with_dw && check_grads(h, grads, numels, count)) return -1;
+  long long out_off[nfb::kMaxSteps], d_out_off[nfb::kMaxSteps], off = 0;
+  for (int i = 0; i < nt->n_steps; ++i) { out_off[i] = off; off += rows * nt->steps[i].npad; }
+  for (int i = 0; i < nt->n_steps; ++i) { d_out_off[i] = off; off += rows * nt->steps[i].npad; }
+  cudaStream_t s = (cudaStream_t)stream;
+  if (with_dw && (train_prepare(h, 1) || zero_grads(h, s))) return -1;
+  if (net_forward(h, *nt, in, ld_in, out_off, tape, rows, s)) return -1;
+  if (net_backward(h, *nt, in, d_in, ld_in, out_off, d_out_off, tape, rows, s, with_dw != 0, k_split)) return -1;
+  return with_dw ? unpack_grads(h, grads, count, s) : 0;
+}
+
+// The condition vectors' adjoints as the training step and the VJPs run them.
+int nfb_selftest_cond_vjp(nfb_handle* h, int B, const float* dcond, const unsigned* warp_id, const unsigned* app_id,
+                          const unsigned* cam_id, int encoded, int has_codes, float* d_warp, float* d_app,
+                          float* d_cam, float* d_time, float* const* grads, const long long* numels, int count,
+                          void* stream) {
+  if (check_call(h, 0)) return -1;
+  if (B < 0) return fail("selftest_cond_vjp: B=%d must be >= 0", B);
+  if (!dcond) return fail("selftest_cond_vjp: null dcond");
+  if (encoded != 0 && encoded != 1) return fail("selftest_cond_vjp: encoded=%d is not 0 or 1", encoded);
+  if (has_codes < 0 || has_codes > 7 || (!encoded && has_codes))
+    return fail("selftest_cond_vjp: has_codes=%d: bits 1 warp, 2 appearance, 4 camera, with encoded only", has_codes);
+  if (d_time && (encoded || !has_time_encoder(h))) return fail("selftest_cond_vjp: d_time needs a TimeEncoder, not encoded");
+  if (check_grads(h, grads, numels, count)) return -1;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (train_prepare(h, 1) || zero_grads(h, s)) return -1;
+  if (B > 0) {
+    if (encoded ? cond_vjp_encoded(h, B, dcond, has_codes & 1, has_codes & 2, has_codes & 4, d_warp, d_app, d_cam, s)
+                : run_cond_bwd(h, B, dcond, warp_id, app_id, cam_id, s))
+      return -1;
+    if (d_time && time_cond_bwd(h, B, dcond, d_time, h->cond_layout.G, s)) return -1;
+  }
+  return unpack_grads(h, grads, count, s);
+}
+
+}  // extern "C"
+
+namespace {
 // The handle-less self-tests below have no launch counter to bump.
 int selftest_launched(const char* what) {
   const cudaError_t e = cudaGetLastError();
@@ -1298,6 +1393,77 @@ int nfb_selftest_warp_mag_loss(long long R, const float* pts, const float* warpe
   nfb::train::WarpMagArgs wm{pts, warped, sel, dwarped, stats, alpha, scale, grad_scale, R};
   nfb::train::warp_mag_loss_kernel<<<(unsigned)((R + 127) / 128), 128, 0, (cudaStream_t)stream>>>(wm);
   return selftest_launched("warp_mag_loss_kernel");
+}
+
+// encode_bwd_kernel with EncodeBwdArgs filled as level_backward / warp_backward fill them.
+int nfb_selftest_encode_bwd(long long rows, int S, const float* pts, const float* window, const float* din, int F,
+                            int ld, int cond_stride, int cond_off, int n_cond, float* dpts, float* dcond,
+                            void* stream) {
+  if (rows < 0) return fail("selftest_encode_bwd: rows=%lld must be >= 0", rows);
+  if (S < 1) return fail("selftest_encode_bwd: S=%d must be >= 1", S);
+  if (F < 0 || n_cond < 0 || cond_off < 0) return fail("selftest_encode_bwd: negative F / n_cond / cond_off");
+  if (ld < 3 + 6 * F + n_cond) return fail("selftest_encode_bwd: ld=%d is below 3 + 6 F + n_cond", ld);
+  if (dcond && cond_stride < cond_off + n_cond) return fail("selftest_encode_bwd: cond_stride is below cond_off + n_cond");
+  if (!din || (dpts && !pts) || (!dpts && !dcond)) return fail("selftest_encode_bwd: null din / pts, or no output");
+  if (rows == 0) return 0;
+  nfb::train::EncodeBwdArgs e{};
+  e.pts = pts; e.window = window; e.din = din; e.F = F; e.ld = ld; e.S = S;
+  e.cond_stride = cond_stride; e.cond_off = cond_off; e.n_cond = n_cond; e.dpts = dpts; e.dcond = dcond; e.rows = rows;
+  nfb::train::encode_bwd_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, (cudaStream_t)stream>>>(e);
+  return selftest_launched("encode_bwd_kernel");
+}
+
+// warp_tail_bwd_kernel (dhead) and warp_tail_dx_kernel (dpts) as warp_backward launches them.
+int nfb_selftest_warp_tail_bwd(long long rows, int warp_type, int pivot, int trans, const float* head, int ld,
+                               const float* pts, const float* dwarped, float* dhead, float* dpts, void* stream) {
+  using namespace nfb::train;
+  if (rows < 0) return fail("selftest_warp_tail_bwd: rows=%lld must be >= 0", rows);
+  if (warp_type != 1 && warp_type != 2) return fail("selftest_warp_tail_bwd: warp_type %d is not 1 or 2", warp_type);
+  if ((pivot != 0 && pivot != 1) || (trans != 0 && trans != 1) || (warp_type == 1 && (pivot || trans)))
+    return fail("selftest_warp_tail_bwd: pivot / translation heads belong to warp_type 2");
+  const int nh = warp_type == 2 ? 6 + 3 * pivot + 3 * trans : 3;
+  if (ld < nh) return fail("selftest_warp_tail_bwd: ld=%d is below the %d head outputs", ld, nh);
+  if (!head || !pts || !dwarped || (!dhead && !dpts)) return fail("selftest_warp_tail_bwd: null input, or no output");
+  if (rows == 0) return 0;
+  const unsigned blocks = (unsigned)((rows + 127) / 128);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (dhead) {
+    WarpTailBwdArgs w{head, ld, pts, dwarped, dhead, warp_type, pivot, trans, rows};
+    warp_tail_bwd_kernel<<<blocks, 128, 0, s>>>(w);
+    if (selftest_launched("warp_tail_bwd_kernel")) return -1;
+  }
+  if (dpts) {
+    WarpTailDxArgs x{head, ld, pts, dwarped, dpts, warp_type, pivot, trans, rows};
+    warp_tail_dx_kernel<<<blocks, 128, 0, s>>>(x);
+    if (selftest_launched("warp_tail_dx_kernel")) return -1;
+  }
+  return 0;
+}
+
+// ray_reduce_kernel as the ray VJPs launch it.
+int nfb_selftest_ray_reduce(int R, int S, const float* dpts, const float* z, const float* directions,
+                            const float* d_dnorm, float* d_origins, float* d_directions, void* stream) {
+  if (R < 0) return fail("selftest_ray_reduce: R=%d must be >= 0", R);
+  if (S < 1 || S > nfb::kMaxSamples) return fail("selftest_ray_reduce: S=%d outside [1, %d]", S, nfb::kMaxSamples);
+  if (!dpts || !z || !directions || (!d_origins && !d_directions)) return fail("selftest_ray_reduce: null input, or no output");
+  if (R == 0) return 0;
+  nfb::train::RayReduceArgs a{dpts, z, directions, d_dnorm, d_origins, d_directions, R, S};
+  nfb::train::ray_reduce_kernel<<<(R + nfb::kRaysPerBlock - 1) / nfb::kRaysPerBlock, 32 * nfb::kRaysPerBlock, 0,
+                                  (cudaStream_t)stream>>>(a);
+  return selftest_launched("ray_reduce_kernel");
+}
+
+// viewdir_vjp_kernel as the ray VJPs launch it.
+int nfb_selftest_viewdir_vjp(int R, const float* dcond, int stride, int off, int F, const float* viewdirs,
+                             float* out, int accumulate, void* stream) {
+  if (R < 0) return fail("selftest_viewdir_vjp: R=%d must be >= 0", R);
+  if (F < 0 || off < 0 || stride < off + 3 + 6 * F) return fail("selftest_viewdir_vjp: stride is below off + 3 + 6 F");
+  if (accumulate != 0 && accumulate != 1) return fail("selftest_viewdir_vjp: accumulate=%d is not 0 or 1", accumulate);
+  if (!dcond || !viewdirs || !out) return fail("selftest_viewdir_vjp: null dcond / viewdirs / out");
+  if (R == 0) return 0;
+  nfb::train::ViewdirVjpArgs v{dcond, stride, off, F, viewdirs, out, accumulate, R};
+  nfb::train::viewdir_vjp_kernel<<<(unsigned)((R + 127) / 128), 128, 0, (cudaStream_t)stream>>>(v);
+  return selftest_launched("viewdir_vjp_kernel");
 }
 
 }  // extern "C"

@@ -140,3 +140,44 @@ def test_selftest_entries_refuse_bad_arguments():
   refused(mag(scale=float('inf')), 'must be finite and > 0')
   refused(mag(stats=None), 'null pts / warped / stats')
   refused(mag(pts=None), 'null pts / warped / stats')
+
+  # the layer walker's entries take a handle; the rest of their refusals are in test_train_net_gpu.py
+  n = ctypes.c_int()
+  steps = (ctypes.c_int * 112)()
+  refused(lib.nfb_selftest_net_steps(None, 0, 1, ctypes.byref(n), steps), 'selftest_net_steps: null handle')
+  refused(lib.nfb_selftest_net(None, 0, 1, 4, p, 64, p, None, 0, 0, None, None, 0, None), 'selftest_net: null handle')
+  refused(lib.nfb_selftest_cond_vjp(None, 4, p, None, None, None, 0, 0, None, None, None, None, None, None, 0, None),
+          'null handle')
+
+  def enc(rows=4, S=2, F=2, ld=20, stride=8, off=0, n_cond=4, din=p, dpts=p, dcond=p):
+    return lib.nfb_selftest_encode_bwd(rows, S, p, None, din, F, ld, stride, off, n_cond, dpts, dcond, None)
+  refused(enc(rows=-1), 'rows=-1 must be >= 0')
+  refused(enc(S=0), 'S=0 must be >= 1')
+  refused(enc(F=-1), 'negative F')
+  refused(enc(ld=18), 'ld=18 is below 3 + 6 F + n_cond')
+  refused(enc(stride=3), 'cond_stride is below')
+  refused(enc(din=None), 'null din')
+  refused(enc(dpts=None, dcond=None), 'no output')
+
+  def tail(rows=4, warp_type=2, pivot=0, trans=0, ld=6, head=p, dhead=p, dpts=p):
+    return lib.nfb_selftest_warp_tail_bwd(rows, warp_type, pivot, trans, head, ld, p, p, dhead, dpts, None)
+  refused(tail(rows=-1), 'rows=-1 must be >= 0')
+  refused(tail(warp_type=0), 'warp_type 0 is not 1 or 2')
+  refused(tail(warp_type=1, trans=1), 'belong to warp_type 2')
+  refused(tail(pivot=1, trans=1, ld=11), 'ld=11 is below the 12 head outputs')
+  refused(tail(head=None), 'null input, or no output')
+  refused(tail(dhead=None, dpts=None), 'null input, or no output')
+
+  def reduce(R=4, S=8, dpts=p, d_o=p, d_d=p):
+    return lib.nfb_selftest_ray_reduce(R, S, dpts, p, p, None, d_o, d_d, None)
+  refused(reduce(R=-1), 'R=-1 must be >= 0')
+  refused(reduce(S=1025), 'S=1025 outside [1, 1024]')
+  refused(reduce(dpts=None), 'null input, or no output')
+  refused(reduce(d_o=None, d_d=None), 'null input, or no output')
+
+  def viewdir(R=4, stride=27, off=0, F=4, acc=0, out=p):
+    return lib.nfb_selftest_viewdir_vjp(R, p, stride, off, F, p, out, acc, None)
+  refused(viewdir(R=-1), 'R=-1 must be >= 0')
+  refused(viewdir(stride=28, off=2), 'stride is below off + 3 + 6 F')
+  refused(viewdir(acc=2), 'accumulate=2 is not 0 or 1')
+  refused(viewdir(out=None), 'null dcond / viewdirs / out')

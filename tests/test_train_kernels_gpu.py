@@ -1,5 +1,7 @@
-"""The training step's seed and regulariser kernels on their own, through their self-test entry points
-(nfb_selftest_composite_vjp, nfb_selftest_elastic, nfb_selftest_depth_index, nfb_selftest_warp_mag_loss),
+"""The training step's seed and regulariser kernels, and the adjoints between its MLPs and the rays and tables, on
+their own, through their self-test entry points (nfb_selftest_composite_vjp, nfb_selftest_elastic,
+nfb_selftest_depth_index, nfb_selftest_warp_mag_loss, nfb_selftest_encode_bwd, nfb_selftest_warp_tail_bwd,
+nfb_selftest_ray_reduce, nfb_selftest_viewdir_vjp, nfb_selftest_cond_vjp),
 against torch.autograd of the oracle's own functions in float64, element by element.
 
 Each entry launches the production kernel with the production launch configuration and argument struct, so
@@ -41,11 +43,17 @@ Median index: exact on dyadic weights (every summation order gives the same sums
 disagreement only where the fp64 cumulative weight at either index lies within S u of 0.5.
 Robust loss: the derivative to 32 u relative; the loss to max(16 u |ref|, 3 x the fp32 oracle's distance
 from fp64) (the formula itself cancels at tiny residuals).
+The adjoints between the MLPs and the rays / tables (nfb_selftest_encode_bwd, _warp_tail_bwd, _ray_reduce,
+_viewdir_vjp, _cond_vjp): sums of n fp32 terms within gamma_{n + k} of their absolute sum, k the roundings each
+term carries (a product, cosf's 2 ulp, the += onto a prefill); the encodings' adjoints against the fp64 derivative
+at the fp32 angle the reference itself forms (2^f x exact, 2^f x + fl32(pi/2) rounded); the SE(3) tail's first
+derivatives as its second derivatives above.  Each test states its bound.
 Each case prints its worst error as a fraction of its bound.
 """
 import ctypes
 import math
 
+import numpy as np
 import pytest
 import torch
 
@@ -818,3 +826,358 @@ def test_warp_mag_loss(alpha, use_sel):
   _report(f'alpha={alpha:g} sel={use_sel} dwarped', r_dw)
   _report(f'alpha={alpha:g} sel={use_sel} loss sum', r_loss)
   _report(f'alpha={alpha:g} sel={use_sel} residual sum', r_res)
+
+
+# ---------------------------------------------------------------------------
+# 5. The adjoints between the MLPs and the rays / tables
+# ---------------------------------------------------------------------------
+def _posenc_ref(x, F, window, g, ld_off=0):
+  """fp64 adjoint of the encoding [x | w_f sin(2^f x) | w_f sin(fl32(2^f x + fl32(pi/2)))] of x (rows,3) under the
+  cotangent g (rows, >= 3 + 6F) (columns ld_off..): (the gradient, the sum of its terms' absolute values).  The
+  shifted angle is rounded to fp32 as the reference's fp32 encoding rounds it (O.HALF_PI_F32); 2^f x is exact."""
+  x = x.double()
+  dx = g[:, ld_off:ld_off + 3].double().clone()
+  mag = dx.abs()
+  for f in range(F):
+    s = 2.0**f
+    w = 1.0 if window is None else float(window[f])
+    ang = x * s
+    ang2 = (x.float() * s + torch.tensor(O.HALF_PI_F32)).double()
+    for gc, a in ((g[:, ld_off + 3 + 6 * f:ld_off + 6 + 6 * f], ang), (g[:, ld_off + 6 + 6 * f:ld_off + 9 + 6 * f], ang2)):
+      t = gc.double() * w * s * torch.cos(a)
+      dx += t
+      mag += t.abs()
+  return dx, mag
+
+
+@pytest.mark.parametrize('windowed', [False, True])
+@pytest.mark.parametrize('F,S', [(1, 1), (4, 33), (8, 128), (10, 512)])
+def test_encode_bwd(F, S, windowed):
+  """dpts and the per-ray dcond atomics of encode_bwd_kernel: F up to 10 (angles up to 2^9 |x|), a window with
+  zero and fractional entries, cond columns with zero entries (skipped) and a prefilled dcond (+=).
+  dpts: (2F + 10) u times the sum of its terms' absolute values (2F + 1 fused additions; cosf's 2 ulp and the
+  products' roundings per term).  dcond: gamma_{S+1} times the sum of the absolute values of the S entries and
+  the prefill."""
+  R, n_cond, off, stride = 5, 13, 4, 21
+  rows = R * S
+  ld = 3 + 6 * F + n_cond + 2
+  g = torch.Generator().manual_seed(F * 100 + S)
+  pts = 2.0 * torch.randn(rows, 3, generator=g)
+  din = torch.randn(rows, ld, generator=g)
+  din[:, 3 + 6 * F:][torch.rand(rows, ld - 3 - 6 * F, generator=g) < 0.3] = 0.0
+  din[:, -2:] = float('nan')                                # beyond the block: never read
+  window = torch.from_numpy(O.cosine_easing_window(F, 0.55 * F + 0.3)) if windowed else None
+  if windowed and F > 1:
+    assert (window == 0).any() and ((window > 0) & (window < 1)).any()
+  dcond0 = torch.randn(R, stride, generator=g)
+  dpts = torch.full((rows, 3), float('nan'), device=DEV)
+  dcond = dcond0.to(DEV)
+  L = _lib()
+  dev = lambda t: None if t is None else t.contiguous().to(DEV)
+  pd, wd, dind = dev(pts), dev(window), dev(din)          # held until the kernel has run
+  L.check(L.load().nfb_selftest_encode_bwd(rows, S, _ptr(pd), _ptr(wd), _ptr(dind), F, ld, stride, off, n_cond,
+                                           _ptr(dpts), _ptr(dcond), None))
+  torch.cuda.synchronize()
+  ref, mag = _posenc_ref(pts, F, window, din)
+  _report(f'encode_bwd F={F} S={S} window={windowed} dpts', _ratio(dpts.cpu(), ref, (2 * F + 10) * U * mag))
+  blk = din[:, 3 + 6 * F:3 + 6 * F + n_cond].double().reshape(R, S, n_cond)
+  ref_c = dcond0.double().clone()
+  ref_c[:, off:off + n_cond] += blk.sum(1)
+  tol_c = torch.zeros_like(ref_c)
+  tol_c[:, off:off + n_cond] = 1.01 * (S + 1) * U * (blk.abs().sum(1) + dcond0[:, off:off + n_cond].double().abs())
+  got_c = dcond.cpu()
+  assert torch.equal(got_c[:, :off], dcond0[:, :off]) and torch.equal(got_c[:, off + n_cond:], dcond0[:, off + n_cond:])
+  _report(f'encode_bwd F={F} S={S} dcond', _ratio(got_c, ref_c, tol_c))
+
+
+def _tail_ref(head, x, warp_type, pivot, trans, dw, dtype):
+  """(d head, d x) of <dw, O.se3_tail(...)> (or x + t) and the contractions sum_i |dw_i| |dy_i / d.|."""
+  h = head.to(dtype).clone().requires_grad_(True)
+  xx = x.to(dtype).clone().requires_grad_(True)
+  if warp_type == 1:
+    y = xx + h[:, :3]
+  else:
+    k = 6 + 3 * pivot
+    y = O.se3_tail(h[:, :3], h[:, 3:6], xx, h[:, 6:9] if pivot else None, h[:, k:k + 3] if trans else None)
+  jh = torch.stack([torch.autograd.grad(y[:, i].sum(), h, retain_graph=True)[0] for i in range(3)], 1)
+  jx = torch.stack([torch.autograd.grad(y[:, i].sum(), xx, retain_graph=True)[0] for i in range(3)], 1)
+  d = dw.to(dtype)
+  return ((d[:, :, None] * jh).sum(1).double(), (d[:, :, None] * jx).sum(1).double(),
+          (d.abs()[:, :, None] * jh.abs()).sum(1).double(), (d.abs()[:, :, None] * jx.abs()).sum(1).double())
+
+
+@pytest.mark.parametrize('theta', [1e-3, 0.3, 3.0])
+@pytest.mark.parametrize('layout', ['translation'] + list(LAYOUTS))
+def test_warp_tail_adjoints(layout, theta):
+  """warp_tail_bwd_kernel (dhead +=) and warp_tail_dx_kernel (dpts +=) at every head layout, into prefilled
+  outputs.  Bound: 3 x the band (the fp32 oracle's distance from fp64 and fp64 under one-rounding moves of
+  head and x), plus (2^-16 + 8 u / theta^2) x the contraction sum_i |dw_i| |dy_i / d.| (the nested fp32
+  forward mode, and theta - sin(theta), 1 - cos(theta) kept to u theta absolute, as for the second order above;
+  at theta = 1e-3 this term is about half of the w and v entries, which are then barely pinned), plus one
+  rounding of the sum with the prefill.  The translation field's adjoints are the identity, to one rounding."""
+  if layout == 'translation' and theta != 0.3:
+    pytest.skip('the translation has no angle')
+  warp_type, (pivot, trans) = (1, (0, 0)) if layout == 'translation' else (2, LAYOUTS[layout])
+  nh = 3 if warp_type == 1 else 6 + 3 * pivot + 3 * trans
+  rows, ld = 300, 16
+  head_s, _, x = _se3_inputs(rows, max(nh, 6), theta, seed=nh + int(theta * 10) + 7)
+  g = torch.Generator().manual_seed(5)
+  head = torch.full((rows, ld), float('nan'))
+  head[:, :nh] = head_s[:, :nh] if warp_type == 2 else 0.2 * torch.randn(rows, 3, generator=g)
+  dw = torch.randn(rows, 3, generator=g)
+  dh0, dx0 = torch.randn(rows, ld, generator=g), torch.randn(rows, 3, generator=g)
+  dh, dx = dh0.to(DEV), dx0.to(DEV)
+  L = _lib()
+  hd_, xd, dwd = head.to(DEV), x.to(DEV), dw.to(DEV)
+  L.check(L.load().nfb_selftest_warp_tail_bwd(rows, warp_type, pivot, trans, _ptr(hd_), ld, _ptr(xd), _ptr(dwd),
+                                              _ptr(dh), _ptr(dx), None))
+  torch.cuda.synchronize()
+  dh, dx = dh.cpu(), dx.cpu()
+  assert torch.equal(dh[:, nh:], dh0[:, nh:]), 'dhead changed beyond the head outputs'
+  hs = head[:, :nh]
+  rh, rx, ah, ax = _tail_ref(hs, x, warp_type, pivot, trans, dw, torch.float64)
+  h32, x32, _, _ = _tail_ref(hs, x, warp_type, pivot, trans, dw, torch.float32)
+  bh, bx = (h32 - rh).abs(), (x32 - rx).abs()
+  for s in (1, 2):
+    gm = torch.Generator().manual_seed(200 + s)
+    mv = lambda t: t.double() * (1 + U * (2 * torch.rand(t.shape, generator=gm, dtype=torch.float64) - 1))
+    mh, mx, _, _ = _tail_ref(mv(hs), mv(x), warp_type, pivot, trans, dw, torch.float64)
+    bh, bx = torch.maximum(bh, (mh - rh).abs()), torch.maximum(bx, (mx - rx).abs())
+  k = 0.0 if warp_type == 1 else 2.0**-16 + 8 * U / theta**2
+  got_h, got_x = dh[:, :nh].double(), dx.double()
+  ref_h, ref_x = dh0[:, :nh].double() + rh, dx0.double() + rx
+  _report(f'warp tail {layout} theta={theta:g} dhead',
+          _ratio(got_h, ref_h, 3 * bh + k * ah + U * ref_h.abs() + 2.0**-149))
+  _report(f'warp tail {layout} theta={theta:g} dpts',
+          _ratio(got_x, ref_x, 3 * bx + k * ax + U * ref_x.abs() + 2.0**-149))
+
+
+@pytest.mark.parametrize('dnorm', [False, True])
+@pytest.mark.parametrize('S', [1, 31, 32, 33, 512])
+def test_ray_reduce(S, dnorm):
+  """d_origins += sum_s g_s and d_directions += sum_s z_s g_s + d_dnorm d / |d| over R = 7 rays (a last block of
+  kRaysPerBlock = 4 left short), twice into the same outputs (a coarse level of S samples, a fine one of
+  S + 5), onto a prefill.  Bound: gamma_{S+S'+2} times the absolute sums and the prefill, plus 6 u |d_dnorm d / |d||
+  per level (the norm's square root and the division)."""
+  R = 7
+  g = torch.Generator().manual_seed(S)
+  dirs = torch.randn(R, 3, generator=g)
+  o0, d0 = torch.randn(R, 3, generator=g), torch.randn(R, 3, generator=g)
+  do, dd = o0.to(DEV), d0.to(DEV)
+  ref_o, ref_d = o0.double().clone(), d0.double().clone()
+  mag_o, mag_d = o0.double().abs(), d0.double().abs()
+  L = _lib()
+  n_terms = 0
+  for lv, s_lv in enumerate((S, S + 5)):
+    z = torch.sort(0.02 + 0.81 * torch.rand(R, s_lv, generator=g), -1).values
+    gp = torch.randn(R, s_lv, 3, generator=g)
+    gp[:, ::4] = 0.0
+    dn = torch.randn(R, generator=g) if dnorm else None
+    dev = lambda t: None if t is None else t.contiguous().to(DEV)
+    gpd, zd, dirsd, dnd = dev(gp), dev(z), dev(dirs), dev(dn)
+    L.check(L.load().nfb_selftest_ray_reduce(R, s_lv, _ptr(gpd), _ptr(zd), _ptr(dirsd), _ptr(dnd), _ptr(do), _ptr(dd),
+                                             None))
+    torch.cuda.synchronize()
+    ref_o += gp.double().sum(1)
+    mag_o += gp.double().abs().sum(1)
+    zg = z.double()[..., None] * gp.double()
+    ref_d += zg.sum(1)
+    mag_d += zg.abs().sum(1)
+    if dnorm:
+      k = dn.double()[:, None] * dirs.double() / dirs.double().norm(dim=-1, keepdim=True)
+      ref_d += k
+      mag_d += 7 * k.abs()
+    n_terms += s_lv + 1
+  torch.cuda.synchronize()
+  gam = 1.01 * (n_terms + 2) * U
+  _report(f'ray_reduce S={S} d_dnorm={dnorm} d_origins', _ratio(do.cpu(), ref_o, gam * mag_o))
+  _report(f'ray_reduce S={S} d_dnorm={dnorm} d_directions', _ratio(dd.cpu(), ref_d, gam * mag_d))
+
+
+@pytest.mark.parametrize('accumulate', [0, 1])
+def test_viewdir_vjp(accumulate):
+  """The view-direction block's adjoint (F = 4, no window) at a block offset inside a wider dcond, = or +=
+  a prefill.  Bound: as encode_bwd's dpts, plus one rounding of the prefill's sum."""
+  R, F, off, stride = 133, 4, 11, 11 + 27 + 9
+  g = torch.Generator().manual_seed(accumulate)
+  vd = torch.randn(R, 3, generator=g)
+  vd = vd / vd.norm(dim=-1, keepdim=True)
+  dcond = torch.randn(R, stride, generator=g)
+  out0 = torch.randn(R, 3, generator=g)
+  out = out0.to(DEV)
+  L = _lib()
+  dcd, vdd = dcond.to(DEV), vd.to(DEV)
+  L.check(L.load().nfb_selftest_viewdir_vjp(R, _ptr(dcd), stride, off, F, _ptr(vdd), _ptr(out), accumulate, None))
+  torch.cuda.synchronize()
+  ref, mag = _posenc_ref(vd, F, None, dcond, ld_off=off)
+  if accumulate:
+    ref, mag = ref + out0.double(), mag + out0.double().abs()
+  _report(f'viewdir_vjp accumulate={accumulate}', _ratio(out.cpu(), ref, (2 * F + 11) * U * mag))
+
+
+# ---- the condition vectors' adjoints (nfb_selftest_cond_vjp, on a handle's layout) ----
+_COND_BASE = dict(num_coarse_samples=8, num_fine_samples=0, near=0.02, far=0.83, nerf_trunk_depth=2,
+                  nerf_trunk_width=32, nerf_rgb_branch_width=16, num_nerf_point_freqs=2, use_warp=True,
+                  warp_trunk_depth=2, warp_trunk_width=32, warp_skips=(), num_warp_embeddings=6,
+                  use_appearance_metadata=True, num_appearance_embeddings=5, use_camera_metadata=True,
+                  num_camera_embeddings=3, num_camera_features=4, use_trunk_condition=True,
+                  use_alpha_condition=True)
+COND_MODELS = {
+    'glo': dict(warp_field_type='se3'),
+    'blend': dict(warp_field_type='translation', warp_metadata_encoder_type='blend', metadata_encoder_num_freqs=2),
+    'time': dict(warp_field_type='se3', warp_metadata_encoder_type='time', metadata_encoder_num_freqs=2),
+}
+
+
+def _cond_handle(kind):
+  from tests.golden_util import model_from_spec, spec_to_dict, tree_to_device
+  spec = O.OracleSpec(**{**_COND_BASE, **COND_MODELS[kind]})
+  model = model_from_spec(spec_to_dict(spec), device=DEV)
+  hd = model.handle()
+  hd.set_params(tree_to_device(O.init_params(spec, 1), DEV))
+  G, A, C = spec.num_warp_features, spec.num_appearance_features, spec.num_camera_features
+  dv = 3 + 6 * spec.num_nerf_viewdir_freqs
+  # [warp | trunk (A) | alpha (A) | rgb: viewdirs, appearance (A), camera]
+  blocks = [('warp', 0, G), ('app', G, A), ('app', G + A, A), ('app', G + 2 * A + dv, A), ('cam', G + 3 * A + dv, C)]
+  return spec, hd, blocks, G + 3 * A + dv + C
+
+
+def _cond_call(hd, B, dcond, ids, encoded, has, dense, d_time):
+  L = _lib()
+  specs = hd.param_specs
+  grads = [torch.zeros(r * c, device=DEV) for _, r, c in specs]
+  gp = (ctypes.c_void_p * len(grads))(*[t.data_ptr() for t in grads])
+  ne = (ctypes.c_longlong * len(grads))(*[t.numel() for t in grads])
+  dev = lambda t: None if t is None else t.contiguous().to(DEV)
+  dcd = dev(dcond)
+  idd = [dev(ids.get(k)) for k in ('warp', 'app', 'cam')]      # held until the kernel has run
+  L.check(L.load().nfb_selftest_cond_vjp(hd.h, B, _ptr(dcd), *[_ptr(t) for t in idd], encoded, has,
+                                         *[_ptr(dense.get(k)) for k in ('warp', 'app', 'cam')], _ptr(d_time), gp, ne,
+                                         len(grads), None))
+  torch.cuda.synchronize()
+  return {name: t.view(r, c).cpu() for t, (name, r, c) in zip(grads, specs)}
+
+
+TABLES = {'warp': ('warp_field/metadata_encoder/embed/embedding', 'warp_field/glo_encoder/embed/embedding'),
+          'app': ('appearance_encoder/embed/embedding',), 'cam': ('camera_encoder/embed/embedding',)}
+
+
+def _table(grads, key):
+  return next((grads[n] for n in TABLES[key] if n in grads), None)
+
+
+@pytest.mark.parametrize('ids', ['spread', 'one_id', 'clamped'])
+@pytest.mark.parametrize('case', ['glo', 'blend_0', 'blend_0.35', 'blend_1', 'time'])
+def test_cond_bwd(case, ids):
+  """cond_bwd_kernel's scatter-add into the tables: the appearance code's three blocks summed, the warp block
+  scaled by 1 ('glo'), 1 - time_alpha ('blend') or not scattered ('time', no table), every ray on one id
+  (atomic contention), ids at and past n - 1 (clamped to the last row); and time_cond_bwd_kernel's scale (1,
+  or time_alpha under 'blend').  Bound: gamma_{n+1} times the absolute sum of the n entries a row receives
+  (atomic additions in any order, each entry scaled by one rounding)."""
+  kind, alpha = (case.split('_') + ['0'])[:2]
+  spec, hd, blocks, stride = _cond_handle(kind)
+  L = _lib()
+  L.check(L.load().nfb_set_time_alpha(hd.h, float(alpha)))
+  B = 300
+  g = torch.Generator().manual_seed(len(case) + len(ids))
+  dcond = torch.randn(B, stride, generator=g)
+  dcond[torch.rand(B, stride, generator=g) < 0.2] = 0.0
+  n = {'warp': spec.num_warp_embeddings, 'app': spec.num_appearance_embeddings, 'cam': spec.num_camera_embeddings}
+  if ids == 'spread':
+    idv = {k: torch.randint(0, v, (B,), generator=g) for k, v in n.items()}
+  elif ids == 'one_id':
+    idv = {k: torch.full((B,), v // 2, dtype=torch.long) for k, v in n.items()}
+  else:
+    idv = {k: torch.tensor([v - 1, v, v + 3, 2**31 + 5])[torch.randint(0, 4, (B,), generator=g)] for k, v in n.items()}
+  ids32 = {k: torch.from_numpy(v.numpy().astype(np.uint32).view(np.int32)) for k, v in idv.items()}   # uint32 bits
+  G = spec.num_warp_features
+  d_time = torch.full((B, G), float('nan'), device=DEV) if kind != 'glo' else None
+  grads = _cond_call(hd, B, dcond, ids32, 0, 0, {}, d_time)
+  a32 = np.float32(alpha)                                   # time_alpha is an fp32 of the handle
+  scale = {'glo': 1.0, 'blend': float(np.float32(1) - a32), 'time': 0.0}[kind]
+  for key in ('warp', 'app', 'cam'):
+    got = _table(grads, key)
+    if got is None:
+      assert key == 'warp' and kind == 'time'
+      continue
+    rows = idv[key].clamp(max=n[key] - 1)
+    ref = torch.zeros(n[key], got.shape[1], dtype=torch.float64)
+    mag = torch.zeros_like(ref)
+    cnt = torch.zeros(n[key], 1, dtype=torch.float64)
+    for name, off, w in blocks:
+      if name != key:
+        continue
+      v = dcond[:, off:off + w].double() * (scale if key == 'warp' else 1.0)
+      ref.index_add_(0, rows, v)
+      mag.index_add_(0, rows, v.abs())
+      cnt.index_add_(0, rows, torch.ones(B, 1, dtype=torch.float64))
+    per = 3 if key == 'app' else 1
+    _report(f'cond_bwd {case} ids={ids} {key}', _ratio(got, ref, 1.01 * (per * cnt + 2) * U * mag))
+  if d_time is not None:
+    ts = float(a32) if kind == 'blend' else 1.0
+    ref = ts * dcond[:, :G].double()
+    _report(f'time_cond_bwd {case}', _ratio(d_time.cpu(), ref, U * ref.abs()))
+
+
+@pytest.mark.parametrize('dense', [False, True])
+@pytest.mark.parametrize('has', range(8))
+def test_cond_vjp_encoded(has, dense):
+  """cond_vjp_encoded_kernel: each code the call passed (has: bits 1 warp, 2 appearance, 4 camera) gets its
+  blocks' gradient in its dense output (+= a prefill; dropped with a null pointer), the appearance code the sum
+  of its three blocks; a code it did not pass sends its blocks' sum over every ray to row 0 of its table.
+  Bound: gamma_{n+2} times the absolute sum of the n entries (and the prefill)."""
+  spec, hd, blocks, stride = _cond_handle('glo')
+  B = 77
+  g = torch.Generator().manual_seed(has)
+  dcond = torch.randn(B, stride, generator=g)
+  dcond[torch.rand(B, stride, generator=g) < 0.2] = 0.0
+  widths = {'warp': spec.num_warp_features, 'app': spec.num_appearance_features, 'cam': spec.num_camera_features}
+  bits = {'warp': 1, 'app': 2, 'cam': 4}
+  pre = {k: torch.randn(B, w, generator=g) for k, w in widths.items()}
+  out = {k: pre[k].to(DEV) for k in widths if dense}
+  grads = _cond_call(hd, B, dcond, {}, 1, has, out, None)
+  for key, w in widths.items():
+    ref = torch.zeros(B, w, dtype=torch.float64)
+    mag = torch.zeros_like(ref)
+    for name, off, bw in blocks:
+      if name == key:
+        ref += dcond[:, off:off + bw].double()
+        mag += dcond[:, off:off + bw].double().abs()
+    table = _table(grads, key)
+    if has & bits[key]:
+      assert float(table.abs().sum()) == 0, f'{key}: a passed code sent a gradient to its table'
+      if dense:
+        r = ref + pre[key].double()
+        _report(f'cond_vjp_encoded has={has} {key} dense', _ratio(out[key].cpu(), r, 4 * U * (mag + pre[key].double().abs())))
+    else:
+      if dense:
+        assert torch.equal(out[key].cpu(), pre[key]), f'{key}: a code the call did not pass got a dense gradient'
+      r0 = ref.sum(0)
+      _report(f'cond_vjp_encoded has={has} {key} row 0', _ratio(table[0], r0, 1.01 * (3 * B + 2) * U * mag.sum(0)))
+      assert float(table[1:].abs().sum()) == 0
+
+
+def test_cond_vjp_rejects_bad_arguments():
+  spec, hd, _, stride = _cond_handle('glo')
+  L = _lib()
+  lib = L.load()
+  d = torch.zeros(4 * stride, device=DEV)
+  n = len(hd.param_specs)
+  grads = [torch.zeros(r * c, device=DEV) for _, r, c in hd.param_specs]
+  gp = (ctypes.c_void_p * n)(*[t.data_ptr() for t in grads])
+  ne = (ctypes.c_longlong * n)(*[t.numel() for t in grads])
+
+  def call(B=4, dcond=_ptr(d), encoded=0, has=0, d_time=None, count=n):
+    return lib.nfb_selftest_cond_vjp(hd.h, B, dcond, None, None, None, encoded, has, None, None, None, d_time, gp, ne,
+                                     count, None)
+
+  def refused(status, what):
+    assert status != 0
+    assert what in lib.nfb_last_error().decode(), lib.nfb_last_error()
+  refused(call(B=-1), 'B=-1 must be >= 0')
+  refused(call(dcond=None), 'null dcond')
+  refused(call(encoded=2), 'encoded=2 is not 0 or 1')
+  refused(call(has=1), 'with encoded only')
+  refused(call(encoded=1, has=8), 'has_codes=8')
+  refused(call(d_time=_ptr(d)), 'd_time needs a TimeEncoder')
+  refused(call(count=n - 1), f'expected {n} gradient tensors')
