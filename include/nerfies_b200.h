@@ -456,6 +456,49 @@ int nfb_pose_grad(int num_images, const float* pose, const int* image, const flo
                   const float* d_origins, const float* d_directions, long long count, float* grad, void* workspace,
                   long long workspace_bytes, void* stream);
 
+/* ---- training camera intrinsics ----------------------------------------------
+ * An intrinsics delta is eight floats q = (s, dcx, dcy, dk1, dk2, dk3, dp1, dp2), zero for the capture's camera.
+ * Applied to a camera with focal length f0, principal point c0, radial k0 and tangential p0 distortion:
+ *   focal length f = f0 exp(s) (the y focal f * pixel_aspect_ratio follows; skew and aspect stay),
+ *   principal point c = c0 + f0 dc (in focal-length units: a rate independent of the image scale),
+ *   radial k = k0 + dk, tangential p = p0 + dp.
+ * q = 0 gives the capture's rays bit for bit; undistortion runs when a refined coefficient is non-zero.  Images
+ * share deltas through a group map: group (num_images) int32 device, image k -> delta intrinsics[group[k]]. */
+enum { NFB_INTRINSICS_FOCAL = 1, NFB_INTRINSICS_PRINCIPAL_POINT = 2, NFB_INTRINSICS_RADIAL = 4,
+       NFB_INTRINSICS_TANGENTIAL = 8 };
+
+/* nfb_gather_rays_posed with each image's camera also refined by its group's delta: intrinsics
+ * (num_groups,8) device, nullable (a null or zero delta gives nfb_gather_rays_posed's rays bit for bit); group
+ * (num_images) device, needed with intrinsics (an image whose group is outside [0, num_groups) keeps its
+ * camera); pixels (count,2) the pixel positions, as nfb_gather_rays.  pose, origins, directions, pixels and
+ * image are nullable. */
+int nfb_gather_rays_refined(const nfb_ray_table* table, long long first, long long count, const float* pose,
+                            const float* intrinsics, const int* group, int num_groups, float* origins,
+                            float* directions, float* pixels, int* image, void* stream);
+
+/* nfb_pixels_to_rays of the camera refined by the delta intrinsics (8 floats, device; nullable: the camera's
+ * own rays, bit for bit). */
+int nfb_pixels_to_rays_refined(const nfb_camera* cam, const float* intrinsics, const float* pixels, long long n,
+                               float* directions, void* stream);
+
+/* Bytes of device workspace nfb_intrinsics_grad needs (< 0: invalid arguments). */
+long long nfb_intrinsics_grad_workspace_size(int num_groups, long long count);
+
+/* grad (num_groups,8) += the intrinsics gradient of count rays (nfb_gather_rays_refined) of images image
+ * (count): dL/dq of each ray's group delta through pixel -> ray, summed over the group's rays.
+ *   cameras (num_images) device: the ray table's cameras; pose (num_images,6) nullable; intrinsics
+ *   (num_groups,8) nullable (zero); group (num_images); pixels (count,2), directions (count,3) the posed world
+ *   directions, d_directions (count,3) their gradients; parts: NFB_INTRINSICS_* bits, the entries given a
+ *   gradient (the others get nothing added).
+ * The undistortion is differentiated at its fixed point (implicit function theorem, with the Newton step's
+ * Jacobian), in fp64.  A segmented reduction in fp64 with no atomics: two calls on the same inputs give the
+ * same bits.  A group with no ray gets 0; a ray whose image is outside [0, num_images), or whose group is
+ * outside [0, num_groups), is ignored.  Needs no handle. */
+int nfb_intrinsics_grad(const nfb_camera* cameras, int num_images, const float* pose, const float* intrinsics,
+                        const int* group, int num_groups, unsigned parts, const int* image, const float* pixels,
+                        const float* directions, const float* d_directions, long long count, float* grad,
+                        void* workspace, long long workspace_bytes, void* stream);
+
 /* ---- per-frame image metrics of eval.py:process_batch ------------------------
  * Images are (num_images, height, width, channels) float32, channels interleaved (what
  * render_frame returns for 'rgb'), channels in 1..4, height and width >= 161 (MS-SSIM's five

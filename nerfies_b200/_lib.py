@@ -31,6 +31,8 @@ SYMBOLS = [
     'nfb_warp_code', 'nfb_train_value_and_grad_rays', 'nfb_gather_rays_posed', 'nfb_pose_grad_workspace_size',
     'nfb_pose_grad', 'nfb_selftest_net_steps', 'nfb_selftest_net', 'nfb_selftest_cond_vjp',
     'nfb_selftest_encode_bwd', 'nfb_selftest_warp_tail_bwd', 'nfb_selftest_ray_reduce', 'nfb_selftest_viewdir_vjp',
+    'nfb_gather_rays_refined', 'nfb_pixels_to_rays_refined', 'nfb_intrinsics_grad_workspace_size',
+    'nfb_intrinsics_grad',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -55,6 +57,9 @@ TRAIN_PRECISIONS = {'fp32': 0, 'tf32x3': 1}
 FLAG_COARSE_ONLY = 1
 FLAG_NO_WARP = 2
 FLAG_METADATA_ENCODED = 4
+# the parts of an intrinsics delta (NFB_INTRINSICS_*): its entries (s, dcx, dcy, dk1, dk2, dk3, dp1, dp2) by part
+INTRINSICS_PARTS = {'focal': 1, 'principal_point': 2, 'radial': 4, 'tangential': 8}
+INTRINSICS_ENTRIES = {'focal': (0,), 'principal_point': (1, 2), 'radial': (3, 4, 5), 'tangential': (6, 7)}
 # nfb_warp_invert's per-point status (NFB_INVERT_*)
 INVERT_STATUS = {'converged': 0, 'max_iters': 1, 'singular': 2, 'stalled': 3, 'nonfinite': 4}
 # nfb_point_visibility's per-point status (NFB_TRACK_*), and 'no_surface', which only the Python layer
@@ -241,6 +246,14 @@ def load():
   lib.nfb_pose_grad_workspace_size.restype = ll
   lib.nfb_pose_grad.argtypes = [ci, vp, vp, vp, vp, vp, ll, vp, vp, ll, vp]
   lib.nfb_pose_grad.restype = ci
+  lib.nfb_gather_rays_refined.argtypes = [ctypes.POINTER(NfbRayTable), ll, ll, vp, vp, vp, ci, vp, vp, vp, vp, vp]
+  lib.nfb_gather_rays_refined.restype = ci
+  lib.nfb_pixels_to_rays_refined.argtypes = [ctypes.POINTER(NfbCamera), vp, vp, ll, vp, vp]
+  lib.nfb_pixels_to_rays_refined.restype = ci
+  lib.nfb_intrinsics_grad_workspace_size.argtypes = [ci, ll]
+  lib.nfb_intrinsics_grad_workspace_size.restype = ll
+  lib.nfb_intrinsics_grad.argtypes = [vp, ci, vp, vp, vp, ci, cu, vp, vp, vp, vp, ll, vp, vp, ll, vp]
+  lib.nfb_intrinsics_grad.restype = ci
   lib.nfb_image_metrics_workspace_size.argtypes = [ci, ci, ci, ci]
   lib.nfb_image_metrics_workspace_size.restype = ll
   lib.nfb_image_metrics.argtypes = [ci, ci, ci, ci, vp, vp, vp, vp, vp, ll, vp, vp, vp, vp]

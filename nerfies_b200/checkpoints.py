@@ -170,17 +170,18 @@ def restore_checkpoint(ckpt_dir, target=None, step=None, prefix='checkpoint_', d
   state.param_states = _to_torch(opt.get('state', {}).get('param_states') or {}, device)
   # refined training cameras (training.CameraPoses.state_dict), host arrays; None without
   state.camera_poses = state_dict.get('camera_poses')
+  state.camera_intrinsics = state_dict.get('camera_intrinsics')
   return state
 
 
-def checkpoint_camera_poses(ckpt_dir, prefix='checkpoint_'):
-  """The saved camera poses of the newest checkpoint in `ckpt_dir` (None without one or without poses).
-  Host only: lets a driver refuse a checkpoint before any GPU work."""
+def checkpoint_camera_poses(ckpt_dir, prefix='checkpoint_', key='camera_poses'):
+  """The saved camera poses (key='camera_intrinsics': intrinsics) of the newest checkpoint in `ckpt_dir`
+  (None without one or without them).  Host only: lets a driver refuse a checkpoint before any GPU work."""
   path = latest_checkpoint(ckpt_dir, prefix)
   if path is None:
     return None
   with open(path, 'rb') as fp:
-    return msgpack_restore(fp.read()).get('camera_poses')
+    return msgpack_restore(fp.read()).get(key)
 
 
 def _check_same_structure(want, got, where):
@@ -212,6 +213,9 @@ def save_checkpoint(ckpt_dir, state, step, prefix='checkpoint_', keep=2):
   poses = getattr(state, 'camera_poses', None)
   if poses is not None:
     tree['camera_poses'] = poses.state_dict() if hasattr(poses, 'state_dict') else poses
+  intrinsics = getattr(state, 'camera_intrinsics', None)
+  if intrinsics is not None:
+    tree['camera_intrinsics'] = intrinsics.state_dict() if hasattr(intrinsics, 'state_dict') else intrinsics
   path = os.path.join(ckpt_dir, f'{prefix}{step}')
   tmp = path + '.tmp'
   with open(tmp, 'wb') as fp:

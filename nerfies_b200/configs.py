@@ -139,6 +139,16 @@ class TrainConfig:
   # in a normalised scene.  The default is a guess that nobody has tuned.
   camera_pose_lr_schedule: ScheduleDef = dataclasses.field(default_factory=lambda: {
       'type': 'exponential', 'initial_value': 1e-3, 'final_value': 1e-5, 'num_steps': 1000000})
+  # Refine the training cameras' intrinsics jointly with the model (training.CameraIntrinsics): the parts named
+  # here, some of 'focal', 'principal_point', 'radial' and 'tangential', of one delta per group of train items
+  # whose capture intrinsics are all equal, starting at zero.  Works with or without refine_camera_poses, but
+  # a group's principal-point shift is nearly a rotation of each of its cameras about its centre: with both
+  # on, 'principal_point' and the poses are close to degenerate.
+  refine_camera_intrinsics: Tuple[str, ...] = ()
+  # One Adam learning rate for the focal log-scale, the principal point (in focal lengths) and the distortion
+  # coefficients.  The default is a guess that nobody has tuned.
+  camera_intrinsics_lr_schedule: ScheduleDef = dataclasses.field(default_factory=lambda: {
+      'type': 'exponential', 'initial_value': 1e-4, 'final_value': 1e-6, 'num_steps': 1000000})
   save_every: int = 10000
   log_every: int = 500
   histogram_every: int = 5000

@@ -7,7 +7,8 @@
 // HBM-bound elementwise work: 0 or 8 B read and 24-32 B written per pixel; one
 // thread per pixel, fully coalesced stores of consecutive pixels.  fp32, written
 // operation for operation as the reference's float32 numpy (the build uses
-// -fmad=false and IEEE division / sqrt).
+// -fmad=false and IEEE division / sqrt).  refined_camera applies an intrinsics delta (nfb_gather_rays_refined,
+// nfb_pixels_to_rays_refined); intrinsics_kernels.cuh holds its adjoint.
 #pragma once
 #include "../../include/nerfies_b200.h"
 
@@ -21,33 +22,44 @@ struct CameraArgs {
   float* directions;        // (n,3)
   float* pixels_out;        // (n,2) nullable
   int has_distortion;
+  const float* intrinsics;  // (8) device or null: cam refined by this delta (refined_camera)
 };
 
-__device__ __forceinline__ void undistort_point(float xd, float yd, float k1, float k2, float k3,
-                                                float p1, float p2, float& xo, float& yo) {
-  float x = xd, y = yd;
-  const float eps = 1e-9f;
-  const float two_p1 = 2.f * p1, two_p2 = 2.f * p2, six_p1 = 6.f * p1, six_p2 = 6.f * p2;
-  const float two_k2 = 2.f * k2, three_k3 = 3.f * k3;
+// The Newton system of camera.py:42-68 at (x, y): the residual F = D(x, y) - (xd, yd) of the distortion D and
+// its 2x2 Jacobian J = dD/d(x, y) = [fx_x, fx_y, fy_x, fy_y].  T = float is the ray kernels' arithmetic
+// operation for operation; T = double serves the intrinsics adjoint (intrinsics_kernels.cuh).
+template <typename T>
+__device__ __forceinline__ void distortion_newton_terms(T x, T y, T xd, T yd, T k1, T k2, T k3, T p1, T p2,
+                                                        T& fx, T& fy, T J[4]) {
+  const T two_p1 = (T)2 * p1, two_p2 = (T)2 * p2, six_p1 = (T)6 * p1, six_p2 = (T)6 * p2;
+  const T two_k2 = (T)2 * k2, three_k3 = (T)3 * k3;
+  const T r = x * x + y * y;                              // camera.py:42
+  const T d = (T)1 + r * (k1 + r * (k2 + k3 * r));        // camera.py:43
+  fx = d * x + two_p1 * x * y + p2 * (r + (T)2 * x * x) - xd;   // camera.py:55
+  fy = d * y + two_p2 * x * y + p1 * (r + (T)2 * y * y) - yd;   // camera.py:56
+  const T d_r = k1 + r * (two_k2 + three_k3 * r);         // camera.py:59
+  const T d_x = (T)2 * x * d_r;
+  const T d_y = (T)2 * y * d_r;
+  J[0] = d + d_x * x + two_p1 * y + six_p2 * x;           // camera.py:64
+  J[1] = d_y * x + two_p1 * x + two_p2 * y;
+  J[2] = d_x * y + two_p2 * y + two_p1 * x;               // camera.py:68
+  J[3] = d + d_y * y + two_p2 * x + six_p1 * y;
+}
+
+template <typename T>
+__device__ __forceinline__ void undistort_point(T xd, T yd, T k1, T k2, T k3, T p1, T p2, T& xo, T& yo) {
+  T x = xd, y = yd;
+  const T eps = (T)1e-9f;
 #pragma unroll 1
   for (int it = 0; it < 10; ++it) {                       // camera.py:90 (no early exit)
-    const float r = x * x + y * y;                        // camera.py:42
-    const float d = 1.f + r * (k1 + r * (k2 + k3 * r));   // camera.py:43
-    const float fx = d * x + two_p1 * x * y + p2 * (r + 2.f * x * x) - xd;   // camera.py:55
-    const float fy = d * y + two_p2 * x * y + p1 * (r + 2.f * y * y) - yd;   // camera.py:56
-    const float d_r = k1 + r * (two_k2 + three_k3 * r);   // camera.py:59
-    const float d_x = 2.f * x * d_r;
-    const float d_y = 2.f * y * d_r;
-    const float fx_x = d + d_x * x + two_p1 * y + six_p2 * x;   // camera.py:64
-    const float fx_y = d_y * x + two_p1 * x + two_p2 * y;
-    const float fy_x = d_x * y + two_p2 * y + two_p1 * x;       // camera.py:68
-    const float fy_y = d + d_y * y + two_p2 * x + six_p1 * y;
-    const float den = fy_x * fx_y - fx_x * fy_y;                // camera.py:93-95
-    const float xn = fx * fy_y - fy * fx_y;
-    const float yn = fy * fx_x - fx * fy_x;
-    const bool ok = fabsf(den) > eps;
-    x = x + (ok ? xn / den : 0.f);
-    y = y + (ok ? yn / den : 0.f);
+    T fx, fy, J[4];
+    distortion_newton_terms<T>(x, y, xd, yd, k1, k2, k3, p1, p2, fx, fy, J);
+    const T den = J[2] * J[1] - J[0] * J[3];              // camera.py:93-95
+    const T xn = fx * J[3] - fy * J[1];
+    const T yn = fy * J[0] - fx * J[2];
+    const bool ok = fabs(den) > eps;
+    x = x + (ok ? xn / den : (T)0);
+    y = y + (ok ? yn / den : (T)0);
   }
   xo = x; yo = y;
 }
@@ -72,7 +84,7 @@ __device__ __forceinline__ void camera_pixel_direction(const nfb_camera& c, int 
   float y = (py - c.principal_point[1]) / sy;              // camera.py:227
   float x = (px - c.principal_point[0] - y * c.skew) / c.focal_length;   // camera.py:228-229
   if (has_distortion)
-    undistort_point(x, y, c.radial_distortion[0], c.radial_distortion[1], c.radial_distortion[2],
+    undistort_point<float>(x, y, c.radial_distortion[0], c.radial_distortion[1], c.radial_distortion[2],
                     c.tangential_distortion[0], c.tangential_distortion[1], x, y);
   // camera.py:241-242: dirs / ||dirs||, dirs = (x, y, 1)
   const float n = sqrtf(x * x + y * y + 1.f);
@@ -86,6 +98,30 @@ __device__ __forceinline__ void camera_pixel_direction(const nfb_camera& c, int 
 #pragma unroll
   for (int j = 0; j < 3; ++j) d[j] = d[j] / n2;
   out_d[0] = d[0]; out_d[1] = d[1]; out_d[2] = d[2];
+}
+
+// Image k's camera refined by its intrinsics delta q = (s, dcx, dcy, dk1, dk2, dk3, dp1, dp2)
+// (nfb_gather_rays_refined): focal f0 exp(s), principal point c0 + f0 dc, radial k0 + dk, tangential p0 + dp;
+// skew, pixel aspect ratio, pose and image size stay.  q = 0 gives c0's ray bit for bit: exp(0) = 1 and
+// x + 0 = x, and camera_has_distortion reads the refined coefficients.
+__host__ __device__ __forceinline__ nfb_camera refined_camera(const nfb_camera& c0, const float* q) {
+  nfb_camera c = c0;
+  c.focal_length = c0.focal_length * expf(q[0]);
+  for (int j = 0; j < 2; ++j) c.principal_point[j] = c0.principal_point[j] + c0.focal_length * q[1 + j];
+  for (int j = 0; j < 3; ++j) c.radial_distortion[j] = c0.radial_distortion[j] + q[3 + j];
+  for (int j = 0; j < 2; ++j) c.tangential_distortion[j] = c0.tangential_distortion[j] + q[6 + j];
+  return c;
+}
+
+// camera_pixel_direction of c0 refined by q (refined_camera); q null: c0's own.
+__device__ __forceinline__ void refined_pixel_direction(const nfb_camera& c0, const float* q, float px, float py,
+                                                        float* out_d) {
+  if (!q) {
+    camera_pixel_direction(c0, camera_has_distortion(c0), px, py, out_d);
+    return;
+  }
+  const nfb_camera c = refined_camera(c0, q);
+  camera_pixel_direction(c, camera_has_distortion(c), px, py, out_d);
 }
 
 // Camera.project (camera.py:279-315) of the world point (X, Y, Z) in arithmetic T, written operation
@@ -139,7 +175,10 @@ __device__ __forceinline__ void camera_ray_of_pixel(const CameraArgs& a, long lo
   } else {
     camera_pixel_center(a.cam, a.first + i, px, py);
   }
-  camera_pixel_direction(a.cam, a.has_distortion, px, py, out_d);
+  if (a.intrinsics)
+    refined_pixel_direction(a.cam, a.intrinsics, px, py, out_d);
+  else
+    camera_pixel_direction(a.cam, a.has_distortion, px, py, out_d);
   out_p[0] = px; out_p[1] = py;
 }
 
@@ -196,6 +235,9 @@ struct GatherArgs {
   float* time;         // (count)
   const float* pose;   // (num_images,6) [omega | v] or null: image k's camera moved by pose k (pose_moved_ray)
   int* image;          // (count) the table image of each ray
+  const float* intrinsics;   // (num_groups,8) or null: image k's camera refined by intrinsics[group[k]]
+  const int* group;          // (num_images) each image's intrinsics group; one outside [0, num_groups): none
+  int num_groups;
 };
 
 // exp([w]x) of a rotation vector, as geometry.rotvec_to_matrix: I + a K + b K^2 with a = sin(t)/t and
@@ -252,7 +294,10 @@ __global__ void __launch_bounds__(256) gather_rays_kernel(const GatherArgs a) {
     float px, py;
     camera_pixel_center(c, r - __ldg(t.pixel_offsets + lo), px, py);
     float o[3] = {c.position[0], c.position[1], c.position[2]}, d[3] = {0.f, 0.f, 0.f};   // datasets/core.py:176
-    if (a.directions) camera_pixel_direction(c, camera_has_distortion(c), px, py, d);
+    if (a.directions) {
+      const int gk = a.intrinsics ? __ldg(a.group + lo) : -1;
+      refined_pixel_direction(c, gk >= 0 && gk < a.num_groups ? a.intrinsics + 8 * gk : nullptr, px, py, d);
+    }
     if (a.pose) pose_moved_ray(a.pose + 6 * lo, o, d);
     if (a.directions)
       for (int j = 0; j < 3; ++j) a.directions[3 * i + j] = d[j];

@@ -17,6 +17,7 @@
 #include "ray_kernels.cuh"
 #include "camera_kernels.cuh"
 #include "pose_kernels.cuh"
+#include "intrinsics_kernels.cuh"
 #include "metrics_kernels.cuh"
 #include "image_kernels.cuh"
 #include "viz_kernels.cuh"
@@ -652,10 +653,11 @@ void launch_metrics(const MetricsPlan& p, int N, const float* image, const float
   finalize_kernel<<<N, kThreads, 0, s>>>(fa);
 }
 
-// nfb_gather_rays, and with `pose` / `image` nfb_gather_rays_posed: one kernel, one pixel-to-ray path.
+// nfb_gather_rays, and with `pose` / `image` nfb_gather_rays_posed, and with `intrinsics`
+// nfb_gather_rays_refined: one kernel, one pixel-to-ray path.
 int gather_rays(const nfb_ray_table* table, long long first, long long count, float* origins, float* directions,
                 float* pixels, float* rgb, int* appearance, int* camera, int* warp, float* time, const float* pose,
-                int* image, void* stream) {
+                int* image, const float* intrinsics, const int* group, int num_groups, void* stream) {
   if (!table) return fail("null ray table");
   const nfb_ray_table& t = *table;
   if (t.num_images < 1) return fail("ray table has %d images", t.num_images);
@@ -665,6 +667,8 @@ int gather_rays(const nfb_ray_table* table, long long first, long long count, fl
   if (rgb && !t.rgb) return fail("rgb requested but the ray table has none");
   if ((appearance && !t.appearance) || (camera && !t.camera) || (warp && !t.warp) || (time && !t.time))
     return fail("metadata requested but the ray table has none of that kind");
+  if (intrinsics && (!group || num_groups < 1))
+    return fail("intrinsics need a group map and num_groups >= 1 (got %d)", num_groups);
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     return fail("no CUDA device: nerfies_b200 has no CPU path");
@@ -674,6 +678,7 @@ int gather_rays(const nfb_ray_table* table, long long first, long long count, fl
   a.origins = origins; a.directions = directions; a.pixels = pixels; a.rgb = rgb;
   a.appearance = appearance; a.camera = camera; a.warp = warp; a.time = time;
   a.pose = pose; a.image = image;
+  a.intrinsics = intrinsics; a.group = group; a.num_groups = num_groups;
   nfb::gather_rays_kernel<<<(unsigned)((count + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail("gather_rays_kernel launch failed: %s", cudaGetErrorString(e));
@@ -688,7 +693,8 @@ const char* nfb_version(void) { return "nerfies_b200 0.1 sm_90a"; }
 long long nfb_kernel_launches(const nfb_handle* h) { return h ? h->launches : 0; }
 
 static int launch_camera(const nfb_camera* cam, const float* pixels_in, long long first, long long count,
-                         float* origins, float* directions, float* pixels_out, void* stream) {
+                         float* origins, float* directions, float* pixels_out, const float* intrinsics,
+                         void* stream) {
   if (!cam) return fail("null argument");
   if (count < 0 || first < 0) return fail("negative pixel range");
   if (cam->image_size[0] < 1 || cam->image_size[1] < 1) return fail("image_size must be positive");
@@ -708,6 +714,7 @@ static int launch_camera(const nfb_camera* cam, const float* pixels_in, long lon
   a.cam = *cam; a.pixels_in = pixels_in; a.first = first; a.count = count;
   a.origins = origins; a.directions = directions; a.pixels_out = pixels_out;
   a.has_distortion = nfb::camera_has_distortion(*cam);
+  a.intrinsics = intrinsics;
   nfb::camera_rays_kernel<<<(unsigned)((count + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail("camera_rays_kernel launch failed: %s", cudaGetErrorString(e));
@@ -718,13 +725,20 @@ int nfb_gather_rays(const nfb_ray_table* table, long long first, long long count
                     float* directions, float* pixels, float* rgb, int* appearance, int* camera, int* warp,
                     float* time, void* stream) {
   return gather_rays(table, first, count, origins, directions, pixels, rgb, appearance, camera, warp, time, nullptr,
-                     nullptr, stream);
+                     nullptr, nullptr, nullptr, 0, stream);
 }
 
 int nfb_gather_rays_posed(const nfb_ray_table* table, long long first, long long count, const float* pose,
                           float* origins, float* directions, int* image, void* stream) {
   return gather_rays(table, first, count, origins, directions, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-                     pose, image, stream);
+                     pose, image, nullptr, nullptr, 0, stream);
+}
+
+int nfb_gather_rays_refined(const nfb_ray_table* table, long long first, long long count, const float* pose,
+                            const float* intrinsics, const int* group, int num_groups, float* origins,
+                            float* directions, float* pixels, int* image, void* stream) {
+  return gather_rays(table, first, count, origins, directions, pixels, nullptr, nullptr, nullptr, nullptr, nullptr,
+                     pose, image, intrinsics, group, num_groups, stream);
 }
 
 long long nfb_pose_grad_workspace_size(int num_images, long long count) {
@@ -760,13 +774,53 @@ int nfb_pose_grad(int num_images, const float* pose, const int* image, const flo
 
 int nfb_camera_rays(const nfb_camera* cam, long long first_pixel, long long count, float* origins,
                     float* directions, float* pixels, void* stream) {
-  return launch_camera(cam, nullptr, first_pixel, count, origins, directions, pixels, stream);
+  return launch_camera(cam, nullptr, first_pixel, count, origins, directions, pixels, nullptr, stream);
 }
 
 int nfb_pixels_to_rays(const nfb_camera* cam, const float* pixels, long long n, float* directions,
                        void* stream) {
   if (!pixels && n > 0) return fail("null argument");
-  return launch_camera(cam, pixels, 0, n, nullptr, directions, nullptr, stream);
+  return launch_camera(cam, pixels, 0, n, nullptr, directions, nullptr, nullptr, stream);
+}
+
+int nfb_pixels_to_rays_refined(const nfb_camera* cam, const float* intrinsics, const float* pixels, long long n,
+                               float* directions, void* stream) {
+  if (!pixels && n > 0) return fail("null argument");
+  return launch_camera(cam, pixels, 0, n, nullptr, directions, nullptr, intrinsics, stream);
+}
+
+long long nfb_intrinsics_grad_workspace_size(int num_groups, long long count) {
+  if (num_groups < 1 || count < 0) return -1;
+  return std::max<long long>(1, (count + nfb::kIntrinsicsRays - 1) / nfb::kIntrinsicsRays) * num_groups * 8 *
+         (long long)sizeof(double);
+}
+
+int nfb_intrinsics_grad(const nfb_camera* cameras, int num_images, const float* pose, const float* intrinsics,
+                        const int* group, int num_groups, unsigned parts, const int* image, const float* pixels,
+                        const float* directions, const float* d_directions, long long count, float* grad,
+                        void* workspace, long long workspace_bytes, void* stream) {
+  if (num_images < 1) return fail("intrinsics grad: num_images=%d must be >= 1", num_images);
+  if (num_groups < 1) return fail("intrinsics grad: num_groups=%d must be >= 1", num_groups);
+  if (count < 0) return fail("intrinsics grad: count=%lld must be >= 0", count);
+  if (parts & ~15u) return fail("intrinsics grad: unknown parts bits 0x%x", parts);
+  if (!grad || !cameras || !group) return fail("intrinsics grad: null grad / cameras / group");
+  if (count > 0 && (!image || !pixels || !directions || !d_directions))
+    return fail("intrinsics grad: null image / pixels / directions / d_directions");
+  const long long need = nfb_intrinsics_grad_workspace_size(num_groups, count);
+  if (!workspace || workspace_bytes < need)
+    return fail("intrinsics grad: the workspace holds %lld bytes, %lld needed", workspace_bytes, need);
+  if (count == 0 || parts == 0) return 0;
+  const int blocks = (int)((count + nfb::kIntrinsicsRays - 1) / nfb::kIntrinsicsRays);
+  nfb::IntrinsicsGradArgs a{cameras, num_images, pose, intrinsics, group, num_groups, parts, image, pixels,
+                            directions, d_directions, count, static_cast<double*>(workspace), grad};
+  cudaStream_t s = (cudaStream_t)stream;
+  nfb::intrinsics_partials_kernel<<<blocks, nfb::kIntrinsicsRays, 0, s>>>(a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("intrinsics_partials_kernel launch failed: %s", cudaGetErrorString(e));
+  nfb::intrinsics_finish_kernel<<<(num_groups + 127) / 128, 128, 0, s>>>(a, blocks);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("intrinsics_finish_kernel launch failed: %s", cudaGetErrorString(e));
+  return 0;
 }
 
 long long nfb_image_metrics_workspace_size(int num_images, int height, int width, int channels) {

@@ -148,10 +148,13 @@ class DeviceRayTable:
     ts = [self.rgb, self.cameras, self.pixel_offsets, self.order, *self.metadata.values()]
     return sum(t.numel() * t.element_size() for t in ts if t is not None)
 
-  def gather(self, first, count, order=True, poses=None):
+  def gather(self, first, count, order=True, poses=None, intrinsics=None):
     """Rays [first, first + count) of the (repeated) order; `order=False`: identity order.  With `poses`
     ((num_images, 6) float32 on the device), origins and directions come from the cameras moved by the
-    poses (nfb_gather_rays_posed) and the batch carries 'image' (count,) int32, each ray's table image."""
+    poses, and with `intrinsics` (a pair: (G, 8) float32 deltas and the (num_images,) int32 image -> group
+    map, both on the device; training.CameraIntrinsics' delta and group) from the cameras refined by their
+    group's delta (nfb_gather_rays_refined); either way the batch carries 'image' (count,) int32, each ray's
+    table image."""
     dev = self.device
     f32 = dict(dtype=torch.float32, device=dev)
     out = {'origins': torch.empty(count, 3, **f32), 'directions': torch.empty(count, 3, **f32),
@@ -168,6 +171,18 @@ class DeviceRayTable:
       if (not torch.is_tensor(poses) or poses.dtype != torch.float32 or poses.device != dev or
           tuple(poses.shape) != (len(self.shapes), 6) or not poses.is_contiguous()):
         raise ValueError(f'poses must be a contiguous float32 ({len(self.shapes)}, 6) tensor on {dev}')
+    delta = group = None
+    if intrinsics is not None:
+      delta, group = intrinsics
+      n = len(self.shapes)
+      if (not torch.is_tensor(delta) or delta.dtype != torch.float32 or delta.device != dev or delta.dim() != 2 or
+          delta.shape[1] != 8 or delta.shape[0] < 1 or not delta.is_contiguous()):
+        raise ValueError(f'intrinsics deltas must be a contiguous float32 (G, 8) tensor on {dev}')
+      if (not torch.is_tensor(group) or group.dtype != torch.int32 or group.device != dev or
+          tuple(group.shape) != (n,) or not group.is_contiguous()):
+        raise ValueError(f'the intrinsics group map must be a contiguous int32 ({n},) tensor on {dev}')
+      posed = True
+    if posed:
       out['image'] = torch.empty(count, dtype=torch.int32, device=dev)
     stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
     with torch.cuda.device(dev):
@@ -177,9 +192,10 @@ class DeviceRayTable:
           None if posed else ptr(out['directions']), ptr(out['pixels']), ptr(out['rgb']),
           *[ptr(md.get(k)) for k in _METADATA_KEYS], stream))
       if posed:
-        _lib.check(lib.nfb_gather_rays_posed(ctypes.byref(t), int(first), int(count), ptr(poses),
-                                             ptr(out['origins']), ptr(out['directions']), ptr(out['image']),
-                                             stream))
+        _lib.check(lib.nfb_gather_rays_refined(ctypes.byref(t), int(first), int(count), ptr(poses), ptr(delta),
+                                               ptr(group), 0 if delta is None else delta.shape[0],
+                                               ptr(out['origins']), ptr(out['directions']), None, ptr(out['image']),
+                                               stream))
     return out
 
   def item(self, k):
@@ -375,7 +391,7 @@ class NerfiesDataSource:
 
   def create_iterator(self, item_ids, batch_size, repeat=True, flatten=False, shuffle=False,
                       prefetch_size=0, shuffle_buffer_size=1000000, devices=None, rank=None,
-                      world_size=None, first_batch=0, poses=None):
+                      world_size=None, first_batch=0, poses=None, intrinsics=None):
     """The batches of core.py:352-372 with preload (see the module docstring).  With
     `batch_size=0`, whole items as (h, w, ·) tensors; otherwise dicts of rank `rank`'s
     batch_size / world_size rays ('metadata' values (b, 1)).  `prefetch_size`,
@@ -385,7 +401,9 @@ class NerfiesDataSource:
     run continues where the interrupted one stopped instead of replaying the order's head.
     `poses` (flattened rays only; a (len(item_ids), 6) float32 device tensor, training.CameraPoses.pose)
     moves each item's camera (DeviceRayTable.gather) and adds 'image' to the batches.  The tensor is read
-    when a batch is made: with no prefetch, step t's rays see the poses after step t-1's update."""
+    when a batch is made: with no prefetch, step t's rays see the poses after step t-1's update.
+    `intrinsics` (flattened rays only; training.CameraIntrinsics' (delta, group)) refines each item's camera
+    the same way (DeviceRayTable.gather)."""
     del prefetch_size, shuffle_buffer_size, devices
     if not self.preload:
       raise NotImplementedError('preload=False is the lazy tf.data path with shuffle buffers; it has no '
@@ -401,12 +419,12 @@ class NerfiesDataSource:
     table = _upload(host, self.device, order if shuffle else None)
     if first_batch and not (flatten and batch_size > 0):
       raise NotImplementedError('first_batch is for batches of flattened rays')
-    if poses is not None and not (flatten and batch_size > 0):
-      raise NotImplementedError('poses are for batches of flattened rays')
+    if (poses is not None or intrinsics is not None) and not (flatten and batch_size > 0):
+      raise NotImplementedError('poses and intrinsics are for batches of flattened rays')
     if batch_size <= 0:
       return _item_iterator(table, repeat)
     if flatten:
-      return _ray_iterator(table, batch_size, repeat, rank, world_size, first_batch, poses)
+      return _ray_iterator(table, batch_size, repeat, rank, world_size, first_batch, poses, intrinsics)
     return _item_batch_iterator(table, batch_size, repeat, rank, world_size)
 
   def create_cameras_dataset(self, cameras, flatten=False, shuffle=False):
@@ -442,10 +460,10 @@ def _item_iterator(table, repeat):
       return
 
 
-def _ray_iterator(table, batch_size, repeat, rank, world_size, first_batch=0, poses=None):
+def _ray_iterator(table, batch_size, repeat, rank, world_size, first_batch=0, poses=None, intrinsics=None):
   for start, size in _batch_starts(table.num_rays, batch_size, repeat, first_batch):
     offset, count = _rank_slice(size, rank, world_size)
-    yield table.gather(start + offset, count, poses=poses)
+    yield table.gather(start + offset, count, poses=poses, intrinsics=intrinsics)
 
 
 def _item_batch_iterator(table, batch_size, repeat, rank, world_size):

@@ -182,16 +182,21 @@ def delete_old_renders(render_dir, max_renders):
     shutil.rmtree(path)
 
 
-def refined_items(items, saved_poses):
+def refined_items(items, saved_poses, saved_intrinsics=None):
   """(id, camera, metadata, rgb) items with each camera moved by its saved pose (training.CameraPoses'
-  state_dict; geometry.posed_camera).  Items without a saved pose keep their camera."""
+  state_dict; geometry.posed_camera) and refined by its group's saved intrinsics delta (training.
+  CameraIntrinsics' state_dict; geometry.refined_camera).  Items without a saved pose or delta keep that part
+  of their camera; either may be None."""
   from nerfies_b200 import geometry
+  deltas = {str(i): g['delta'] for g in (saved_intrinsics or {}).get('groups', {}).values() for i in g['items']}
   out = []
   for item_id, cam, md, rgb in items:
-    pose = saved_poses['items'].get(str(item_id))
+    pose = (saved_poses or {}).get('items', {}).get(str(item_id))
     if pose is not None:
       p = np.asarray(pose['pose'], np.float64).reshape(6)
       cam = geometry.posed_camera(cam, p[:3], p[3:])
+    if str(item_id) in deltas:
+      cam = geometry.refined_camera(cam, deltas[str(item_id)])
     out.append((item_id, cam, md, rgb))
   return out
 
@@ -242,11 +247,16 @@ def evaluate(exp_config, model_config, train_config, eval_config, base_folder, d
       save_dir = dirs['renders'] if eval_config.save_output and rank == 0 else None
       todo = list(sets)
       saved_poses = getattr(state, 'camera_poses', None)
-      if saved_poses is not None:
+      saved_intrinsics = getattr(state, 'camera_intrinsics', None)
+      if saved_poses is not None or saved_intrinsics is not None:
         # train items from the cameras refined in training; val items keep the capture's (register_camera
         # aligns a held-out view)
-        todo = [(tag, refined_items(items, saved_poses) if tag == 'train' else items) for tag, items in todo]
-        log(f'Step {step}: rendering train items from the refined camera poses of the checkpoint')
+        todo = [(tag, refined_items(items, saved_poses, saved_intrinsics) if tag == 'train' else items)
+                for tag, items in todo]
+        if saved_poses is not None:
+          log(f'Step {step}: rendering train items from the refined camera poses of the checkpoint')
+        if saved_intrinsics is not None:
+          log(f'Step {step}: rendering train items from the refined camera intrinsics of the checkpoint')
       if test_cameras:
         md = choose_test_metadata(datasource, step)
         todo.append(('test', [(f'{k:03d}', cam, md, None) for k, cam in enumerate(test_cameras)]))

@@ -460,7 +460,13 @@ def _host(t, dtype, what):
 # on the photometric loss through NerfModel.render_rays (nfb_render_ray_vjp).
 # ---------------------------------------------------------------------------
 OPTIMIZE = ('pose', 'appearance', 'camera', 'warp')
-DEFAULT_LRS = {'rotation': 2e-3, 'position': 2e-3, 'appearance': 1e-2, 'camera': 1e-2, 'warp': 1e-2}
+# the camera intrinsics parts a registration can also fit (register_camera's `intrinsics`, kept apart from
+# `optimize`): 'focal', 'principal_point', 'radial', 'tangential'
+INTRINSICS_PARTS = tuple(_lib.INTRINSICS_PARTS)
+# the intrinsics parts' rates are for the entries of the delta (refined_camera): the focal log-scale, the
+# principal point in focal lengths and the distortion coefficients
+DEFAULT_LRS = {'rotation': 2e-3, 'position': 2e-3, 'appearance': 1e-2, 'camera': 1e-2, 'warp': 1e-2,
+               'focal': 1e-3, 'principal_point': 1e-4, 'radial': 1e-3, 'tangential': 1e-4}
 
 
 def _skew(w):
@@ -502,6 +508,65 @@ def posed_camera(camera, omega, offset):
   out.position = (camera.position.astype(np.float64) +
                   np.asarray(torch.as_tensor(offset).detach().cpu(), np.float64)).astype(np.float32)
   return out
+
+
+def refined_camera(camera, delta):
+  """The Camera of an intrinsics delta q = (s, dcx, dcy, dk1, dk2, dk3, dp1, dp2) (nfb_gather_rays_refined):
+  focal f0 exp(s), principal point c0 + f0 dc, radial k0 + dk, tangential p0 + dp (float64, stored float32).
+  The delta does not depend on the image scale: a camera scaled by Camera.scale and then refined is the
+  refined camera scaled."""
+  q = np.asarray(torch.as_tensor(delta).detach().cpu(), np.float64).reshape(8)
+  f0 = float(camera.focal_length)
+  out = camera.copy()
+  out.focal_length = np.array(f0 * np.exp(q[0]), np.float32)
+  out.principal_point = (camera.principal_point.astype(np.float64) + f0 * q[1:3]).astype(np.float32)
+  out.radial_distortion = (camera.radial_distortion.astype(np.float64) + q[3:6]).astype(np.float32)
+  out.tangential_distortion = (camera.tangential_distortion.astype(np.float64) + q[6:8]).astype(np.float32)
+  return out
+
+
+class _RefinedDirections(torch.autograd.Function):
+  """Camera-frame directions of pixel positions under an intrinsics delta: forward nfb_pixels_to_rays_refined
+  of the identity-pose camera, backward nfb_intrinsics_grad with one image and one group."""
+
+  @staticmethod
+  def forward(ctx, delta, pixels, camera, parts):
+    lib = _lib.load()
+    dev = pixels.device
+    delta = delta.detach().to(torch.float32).contiguous()
+    out = torch.empty(pixels.shape[0], 3, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+      _lib.check(lib.nfb_pixels_to_rays_refined(ctypes.byref(camera._struct()), _ptr(delta), _ptr(pixels),
+                                                pixels.shape[0], _ptr(out), _stream()))
+    ctx.save_for_backward(delta, pixels, out)
+    ctx.camera, ctx.parts = camera, parts
+    return out
+
+  @staticmethod
+  def backward(ctx, grad_out):
+    delta, pixels, out = ctx.saved_tensors
+    lib = _lib.load()
+    dev, n = pixels.device, pixels.shape[0]
+    cams = torch.frombuffer(bytearray(bytes(ctx.camera._struct())), dtype=torch.uint8).to(dev)
+    zeros = torch.zeros(n, dtype=torch.int32, device=dev)
+    grad = torch.zeros(8, dtype=torch.float32, device=dev)
+    ws = torch.empty(int(lib.nfb_intrinsics_grad_workspace_size(1, n)), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+      _lib.check(lib.nfb_intrinsics_grad(_ptr(cams), 1, None, _ptr(delta), _ptr(zeros), 1, ctx.parts, _ptr(zeros),
+                                         _ptr(pixels), _ptr(out), _ptr(grad_out.to(torch.float32).contiguous()), n,
+                                         _ptr(grad), _ptr(ws), ws.numel(), _stream()))
+    return grad, None, None, None
+
+
+def refined_directions(camera, delta, pixels, parts):
+  """Unit directions (N,3) in `camera`'s frame of float32 pixel positions (N,2) on the device, with the camera
+  refined by the (8,) delta (refined_camera); differentiable in `delta` for the entries of `parts` (names of
+  _lib.INTRINSICS_PARTS) and no others."""
+  ident = camera.copy()
+  ident.orientation = np.eye(3, dtype=np.float32)
+  ident.position = np.zeros(3, np.float32)
+  bits = sum(_lib.INTRINSICS_PARTS[p] for p in parts)
+  return _RefinedDirections.apply(delta, pixels.reshape(-1, 2).to(torch.float32).contiguous(), ident, bits)
 
 
 def photometric_loss(out, target):
@@ -556,13 +621,19 @@ def registration_codes(model, params, metadata, warp_extra=None):
   return codes
 
 
-def check_registration(model, optimize, steps, batch_rays):
-  """Refuses what cannot be registered: raises ValueError.  Returns the optimised groups as a tuple."""
+def check_registration(model, optimize, steps, batch_rays, intrinsics=()):
+  """Refuses what cannot be registered: raises ValueError.  Returns the optimised groups as a tuple.
+  `intrinsics` names the camera intrinsics parts to fit (INTRINSICS_PARTS); they are not `optimize` entries."""
   optimize = tuple(optimize)
   for k in optimize:
     if k not in OPTIMIZE:
-      raise ValueError(f'unknown optimize entry {k!r}: expected some of {OPTIMIZE}')
-  if not optimize:
+      hint = (f'; the camera intrinsics {INTRINSICS_PARTS} are fitted through intrinsics= (--intrinsics)'
+              if k in INTRINSICS_PARTS else '')
+      raise ValueError(f'unknown optimize entry {k!r}: expected some of {OPTIMIZE}{hint}')
+  for k in intrinsics:
+    if k not in INTRINSICS_PARTS:
+      raise ValueError(f'unknown intrinsics part {k!r}: expected some of {INTRINSICS_PARTS}')
+  if not optimize and not tuple(intrinsics):
     raise ValueError('optimize is empty: nothing to fit')
   if 'appearance' in optimize and not model.use_appearance_metadata:
     raise ValueError("optimize 'appearance': the model has no appearance metadata")
@@ -581,7 +652,7 @@ def check_registration(model, optimize, steps, batch_rays):
 
 
 def register_camera(model, params, camera, image, warp_extra=None, codes=None, optimize=('pose', 'appearance'),
-                    steps=200, batch_rays=1024, lrs=None, seed=0, log_every=1, lr_decay=1.0):
+                    steps=200, batch_rays=1024, lrs=None, seed=0, log_every=1, lr_decay=1.0, intrinsics=()):
   """Fits `camera`'s pose (and the photo's codes) to `image` (H, W, 3) float in [0, 1], the model held fixed.
 
   The pose is a rotation vector omega about the camera centre (world frame) and a centre offset v
@@ -591,15 +662,22 @@ def register_camera(model, params, camera, image, warp_extra=None, codes=None, o
   step draws `batch_rays` pixels uniformly from a device generator seeded with `seed`, renders them with
   deterministic sampling (as eval.py) through NerfModel.render_rays and takes one Adam step on
   photometric_loss, with the learning rate of each group in `lrs` ('rotation', 'position',
-  'appearance', 'camera', 'warp'; DEFAULT_LRS otherwise).  With lr_decay < 1 each rate decays
+  'appearance', 'camera', 'warp', 'focal', 'principal_point', 'radial', 'tangential'; DEFAULT_LRS otherwise).
+  With lr_decay < 1 each rate decays
   exponentially from its value at the first step to lr_decay times it at the last.  The camera-frame directions come from
-  Camera's own ray kernel on an identity-pose copy, so distortion is the kernel's.
+  Camera's own ray kernel on an identity-pose copy, so distortion is the kernel's.  The parts `intrinsics`
+  names (some of 'focal', 'principal_point', 'radial', 'tangential') fit an intrinsics delta (refined_camera)
+  starting at 0:
+  the batch's directions then come from refined_directions each step; 'radial' and 'tangential' also fit a
+  camera without distortion.
 
   Returns (camera, codes, history): the registered Camera, the fitted codes {'appearance': (1, A), ...}
+  (with an intrinsics part also 'intrinsics', the (1, 8) delta, which the returned camera already applies)
   and one dict per logged step (step, loss, psnr of the batch's fine (else coarse) level, rotation_deg
-  |omega| in degrees, translation |v|), before that step's update."""
+  |omega| in degrees, translation |v|, focal_change_pct 100 (exp(s) - 1), principal_point_px |f0 dc| at the
+  camera's scale), before that step's update."""
   from nerfies_b200 import camera as camera_lib
-  optimize = check_registration(model, optimize, steps, batch_rays)
+  optimize = check_registration(model, optimize, steps, batch_rays, intrinsics)
   lrs = dict(DEFAULT_LRS, **(lrs or {}))
   dev = model.device
   h, w = camera.image_shape
@@ -609,7 +687,14 @@ def register_camera(model, params, camera, image, warp_extra=None, codes=None, o
   ident = camera.copy()
   ident.orientation = np.eye(3, dtype=np.float32)
   ident.position = np.zeros(3, np.float32)
-  local = camera_lib.camera_to_rays(ident, dev)['directions'].reshape(-1, 3)
+  ident_rays = camera_lib.camera_to_rays(ident, dev)
+  local = ident_rays['directions'].reshape(-1, 3)
+  pixels = ident_rays['pixels'].reshape(-1, 2)
+  intr_parts = tuple(intrinsics)
+  # the delta's entries by part, each fitted (at its own rate) or held at 0
+  pieces = {k: torch.zeros(len(_lib.INTRINSICS_ENTRIES[k]), device=dev, requires_grad=k in intr_parts)
+            for k in INTRINSICS_PARTS}
+  delta = lambda: torch.cat([pieces[k] for k in INTRINSICS_PARTS])
   target = image.reshape(-1, 3)
   R0 = torch.as_tensor(camera.orientation, device=dev)
   p0 = torch.as_tensor(camera.position, device=dev)
@@ -626,6 +711,7 @@ def register_camera(model, params, camera, image, warp_extra=None, codes=None, o
   if 'pose' in optimize:
     groups += [{'params': [omega], 'lr': lrs['rotation']}, {'params': [offset], 'lr': lrs['position']}]
   groups += [{'params': [fit[k]], 'lr': lrs[k]} for k in fit if k in optimize]
+  groups += [{'params': [pieces[k]], 'lr': lrs[k]} for k in intr_parts]
   opt = torch.optim.Adam(groups)
   base_lrs = [g['lr'] for g in groups]
   gen = torch.Generator(device=dev)
@@ -634,7 +720,8 @@ def register_camera(model, params, camera, image, warp_extra=None, codes=None, o
   n = h * w
   for step in range(int(steps)):
     idx = torch.randint(0, n, (int(batch_rays),), device=dev, generator=gen)
-    origins, directions = pose_rays(local[idx], R0, p0, omega, offset)
+    loc = refined_directions(camera, delta(), pixels[idx], intr_parts) if intr_parts else local[idx]
+    origins, directions = pose_rays(loc, R0, p0, omega, offset)
     if encoded:
       metadata = {k: v.expand(len(idx), -1) for k, v in fit.items()}
     else:
@@ -650,12 +737,19 @@ def register_camera(model, params, camera, image, warp_extra=None, codes=None, o
       mse = float(((last['rgb'].detach() - target[idx])**2).mean())
       history.append({'step': step, 'loss': float(loss), 'psnr': float(-10.0 * np.log10(max(mse, 1e-30))),
                       'rotation_deg': float(torch.linalg.norm(omega.detach())) * 180.0 / np.pi,
-                      'translation': float(torch.linalg.norm(offset.detach()))})
+                      'translation': float(torch.linalg.norm(offset.detach())),
+                      'focal_change_pct': 100.0 * float(torch.expm1(pieces['focal'].detach()[0])),
+                      'principal_point_px': float(camera.focal_length) * float(torch.linalg.norm(
+                          pieces['principal_point'].detach()))})
     opt.step()
     for g, lr in zip(opt.param_groups, base_lrs):
       g['lr'] = lr * float(lr_decay)**((step + 1) / max(1, int(steps) - 1))
   out_codes = {k: v.detach() for k, v in fit.items()}
-  return posed_camera(camera, omega, offset), out_codes, history
+  registered = posed_camera(camera, omega, offset)
+  if intr_parts:
+    out_codes['intrinsics'] = delta().detach().reshape(1, 8)
+    registered = refined_camera(registered, out_codes['intrinsics'])
+  return registered, out_codes, history
 
 
 def render_camera(model, params, camera, warp_extra, codes, chunk=None):

@@ -19,6 +19,9 @@ class TrainState:
   # training.CameraPoses while refining the training cameras; a restored checkpoint's saved poses
   # ({'step', 'items': {item_id: {'pose', 'grad_ema', 'grad_sq_ema'}}}); or None
   camera_poses: Any = None
+  # training.CameraIntrinsics while refining the training cameras' intrinsics; a restored checkpoint's saved
+  # deltas ({'step', 'groups': {group: {'items', 'delta', 'grad_ema', 'grad_sq_ema'}}}); or None
+  camera_intrinsics: Any = None
 
   @property
   def warp_extra(self):

@@ -44,7 +44,8 @@ def step_key(random_seed, rank, step):
 
 def flatten_stats(stats):
   """train_step's stats under the tags of train.py:71-78: '<key>/<branch>' and 'loss/background';
-  with refined cameras also 'camera_poses/rotation_deg' and 'camera_poses/translation' (means over them)."""
+  with refined cameras also 'camera_poses/rotation_deg' and 'camera_poses/translation' (means over them), and
+  'camera_intrinsics/focal_change_pct' and 'camera_intrinsics/principal_point_px' (means over the groups)."""
   out = {}
   for branch in ('coarse', 'fine'):
     for key, value in stats.get(branch, {}).items():
@@ -53,6 +54,8 @@ def flatten_stats(stats):
     out['loss/background'] = stats['background_loss']
   for key, value in stats.get('camera_poses', {}).items():
     out[f'camera_poses/{key}'] = value
+  for key, value in stats.get('camera_intrinsics', {}).items():
+    out[f'camera_intrinsics/{key}'] = value
   return out
 
 
@@ -69,18 +72,46 @@ def check_camera_poses(train_config, saved, train_ids=None):
     training.CameraPoses(train_ids, 'cpu').check(saved)
 
 
-def write_cameras(datasource, poses, directory):
-  """`<directory>/<item>.json` of each refined train camera at the capture's original scale."""
+def check_camera_intrinsics(train_config, saved, train_cameras=None):
+  """Refuses, with ValueError, refine_camera_intrinsics naming an unknown part, or a checkpoint whose saved
+  intrinsics (checkpoints.checkpoint_camera_poses(..., key='camera_intrinsics')) do not fit the run: intrinsics
+  with the refinement off, or groups of other items than those of `train_cameras` ({item_id: Camera}, the
+  train items' capture cameras).  Host only."""
+  training.check_intrinsics_parts(train_config.refine_camera_intrinsics)
+  if saved is None:
+    return
+  if not train_config.refine_camera_intrinsics:
+    raise ValueError('the checkpoint holds refined camera intrinsics but TrainConfig.refine_camera_intrinsics is '
+                     'empty: training on would silently revert the cameras to the capture\'s')
+  if train_cameras is not None:
+    ids = list(train_cameras)
+    _, members = training.intrinsics_groups([train_cameras[i] for i in ids])
+    want = {frozenset(str(ids[k]) for k in m) for m in members}
+    got = {frozenset(str(i) for i in g['items']) for g in saved.get('groups', {}).values()}
+    if got != want:
+      raise ValueError(f'the checkpoint holds camera intrinsics of the item groups {sorted(sorted(g) for g in got)}, '
+                       f'but the train items group as {sorted(sorted(g) for g in want)}')
+
+
+def write_cameras(datasource, item_ids, poses, intrinsics, directory):
+  """`<directory>/<item>.json` of each refined train camera at the capture's original scale: moved by its
+  pose (training.CameraPoses or None) and refined by its group's intrinsics delta (training.CameraIntrinsics or
+  None), which does not depend on the image scale."""
   from nerfies_b200 import camera as camera_lib
   from nerfies_b200 import geometry
   from nerfies_b200 import register_camera
   directory.mkdir(parents=True, exist_ok=True)
-  pose = poses.pose.detach().cpu().double()
-  for k, item in enumerate(poses.item_ids):
-    cam = geometry.posed_camera(datasource.load_camera(item), pose[k, :3], pose[k, 3:])
+  pose = None if poses is None else poses.pose.detach().cpu().double()
+  delta = None if intrinsics is None else intrinsics.item_delta()
+  for k, item in enumerate(item_ids):
+    cam = datasource.load_camera(item)
+    if pose is not None:
+      cam = geometry.posed_camera(cam, pose[k, :3], pose[k, 3:])
     template = camera_lib.Camera.from_json(datasource.camera_dir / f'{item}{datasource.camera_ext}')
-    (directory / f'{item}.json').write_text(
-        json.dumps(register_camera.original_scale_camera(datasource, cam, template).to_json(), indent=2))
+    out = register_camera.original_scale_camera(datasource, cam, template)
+    if delta is not None:
+      out = geometry.refined_camera(out, delta[str(item)])
+    (directory / f'{item}.json').write_text(json.dumps(out.to_json(), indent=2))
 
 
 def train(exp_config, model_config, train_config, base_folder, data_dir=None, precision='fp32',
@@ -110,9 +141,15 @@ def _train(exp_config, model_config, train_config, base_folder, data_dir, precis
 
   saved_poses = checkpoints.checkpoint_camera_poses(str(dirs['checkpoints']))
   check_camera_poses(train_config, saved_poses)
+  saved_intrinsics = checkpoints.checkpoint_camera_poses(str(dirs['checkpoints']), key='camera_intrinsics')
+  check_camera_intrinsics(train_config, saved_intrinsics)
   if datasource is None:
     datasource = driver_utils.make_datasource(exp_config, model_config, data_dir)
   check_camera_poses(train_config, saved_poses, datasource.train_ids)
+  train_cameras = None
+  if train_config.refine_camera_intrinsics:
+    train_cameras = {i: datasource.load_camera(i) for i in datasource.train_ids}
+    check_camera_intrinsics(train_config, saved_intrinsics, train_cameras)
   learning_rate_sched = schedules.from_config(train_config.lr_schedule)          # train.py:199-203
   warp_alpha_sched = schedules.from_config(train_config.warp_alpha_schedule)
   time_alpha_sched = schedules.from_config(train_config.time_alpha_schedule)
@@ -141,6 +178,16 @@ def _train(exp_config, model_config, train_config, base_folder, data_dir, precis
       poses.load(restored.camera_poses)
     state.camera_poses = poses
     pose_kw = {'poses': poses.pose}
+  if train_config.refine_camera_intrinsics:
+    intrinsics_lr_sched = schedules.from_config(train_config.camera_intrinsics_lr_schedule)
+    intrinsics = training.CameraIntrinsics(datasource.train_ids, list(train_cameras.values()),
+                                           train_config.refine_camera_intrinsics, model.device)
+    if restored is not state and restored.camera_intrinsics is None:
+      log('The checkpoint holds no camera intrinsics: refining them from the capture\'s cameras (zero deltas)')
+    elif restored is not state:
+      intrinsics.load(restored.camera_intrinsics)
+    state.camera_intrinsics = intrinsics
+    pose_kw['intrinsics'] = (intrinsics.delta, intrinsics.group)
 
   first_batch = init_step - 1
   train_iter = datasource.create_iterator(                                       # train.py:175-183
@@ -164,8 +211,9 @@ def _train(exp_config, model_config, train_config, base_folder, data_dir, precis
   def save(step):
     if rank == 0:
       checkpoints.save_checkpoint(str(dirs['checkpoints']), state, step, keep=2)   # training.py:46-53
-      if state.camera_poses is not None:
-        write_cameras(datasource, state.camera_poses, dirs['exp'] / 'cameras' / f'{step:08d}')
+      if state.camera_poses is not None or state.camera_intrinsics is not None:
+        write_cameras(datasource, datasource.train_ids, state.camera_poses, state.camera_intrinsics,
+                      dirs['exp'] / 'cameras' / f'{step:08d}')
 
   log(f'Starting training at step {init_step} of {train_config.max_steps} on {world} GPU(s)')
   mark = torch.cuda.Event(enable_timing=True)
@@ -177,8 +225,10 @@ def _train(exp_config, model_config, train_config, base_folder, data_dir, precis
       batch['background_points'] = next(points_iter)
     scalar_params.learning_rate = learning_rate_sched(step)
     scalar_params.elastic_loss_weight = elastic_loss_weight_sched(step)
-    if pose_kw:
+    if state.camera_poses is not None:
       scalar_params.camera_pose_learning_rate = pose_lr_sched(step)
+    if state.camera_intrinsics is not None:
+      scalar_params.camera_intrinsics_learning_rate = intrinsics_lr_sched(step)
     state.warp_alpha = warp_alpha_sched(step)
     state.time_alpha = time_alpha_sched(step)
     state, stats, _ = training.train_step(

@@ -43,6 +43,7 @@ class ScalarParams:
   background_loss_weight: float = 0.0
   background_noise_std: float = 0.001
   camera_pose_learning_rate: float = 0.0    # Adam's rate for TrainState.camera_poses (TrainConfig.refine_camera_poses)
+  camera_intrinsics_learning_rate: float = 0.0   # Adam's rate for TrainState.camera_intrinsics
 
 
 class AdamOptimizer(model_utils.Optimizer):
@@ -196,6 +197,120 @@ class CameraPoses:
             'translation': self.pose[:, 3:].norm(dim=1).mean()}
 
 
+def check_intrinsics_parts(parts):
+  """The intrinsics parts to fit as a tuple; raises ValueError on a part outside _lib.INTRINSICS_PARTS."""
+  parts = tuple(parts)
+  for p in parts:
+    if p not in _lib.INTRINSICS_PARTS:
+      raise ValueError(f'unknown camera intrinsics part {p!r}: expected some of {tuple(_lib.INTRINSICS_PARTS)}')
+  return parts
+
+
+def intrinsics_groups(cameras):
+  """Images whose capture intrinsics are all equal (focal length, principal point, skew, pixel aspect ratio,
+  radial and tangential distortion and image size) share one intrinsics delta.  Returns (group, the image ->
+  group map as (N,) int32 numpy, groups numbered in order of their first image; members, one list of image
+  indices per group)."""
+  keys, group, members = {}, [], []
+  for k, c in enumerate(cameras):
+    key = tuple(np.concatenate([np.asarray(getattr(c, f), np.float64).reshape(-1) for f in (
+        'focal_length', 'principal_point', 'skew', 'pixel_aspect_ratio', 'radial_distortion',
+        'tangential_distortion', 'image_size')]).tolist())
+    if key not in keys:
+      keys[key] = len(members)
+      members.append([])
+    group.append(keys[key])
+    members[keys[key]].append(k)
+  return np.asarray(group, np.int32), members
+
+
+class CameraIntrinsics:
+  """The training cameras' intrinsics, refined with the model: one delta q = (s, dcx, dcy, dk1, dk2, dk3, dp1,
+  dp2) per group of items with equal capture intrinsics (intrinsics_groups), applied as nfb_gather_rays_refined
+  does (geometry.refined_camera).  `delta` (G,8) is a device vector with its own Adam moments and step count;
+  it starts at zero.  Only the entries of `parts` get a gradient, so under Adam the others stay exactly 0.
+  `cameras` are the items' capture cameras at the experiment's scale, in the ray table's image order."""
+
+  def __init__(self, item_ids, cameras, parts, device, beta1=0.9, beta2=0.999, eps=1e-8):
+    self.item_ids = [str(i) for i in item_ids]
+    self.parts = check_intrinsics_parts(parts)
+    group, members = intrinsics_groups(cameras)
+    self.group_items = [[self.item_ids[k] for k in m] for m in members]
+    self.focal = np.asarray([float(cameras[m[0]].focal_length) for m in members], np.float64)   # f0 per group
+    self.group = torch.as_tensor(group).to(device)
+    self.delta = torch.zeros(len(members), 8, device=device, dtype=torch.float32)
+    self.m = torch.zeros_like(self.delta)
+    self.v = torch.zeros_like(self.delta)
+    self.step = 0
+    self.beta1, self.beta2, self.eps = beta1, beta2, eps
+    self.part_bits = sum(_lib.INTRINSICS_PARTS[p] for p in self.parts)
+    structs = (_lib.NfbCamera * len(cameras))(*[c._struct() for c in cameras])
+    self.cameras = torch.frombuffer(bytearray(bytes(structs)), dtype=torch.uint8).to(device)
+    self._workspace = None
+
+  def item_delta(self):
+    """{item_id: its group's delta (8,) float64 numpy} on the host."""
+    delta = self.delta.detach().cpu().double().numpy()
+    return {i: delta[g] for g, items in enumerate(self.group_items) for i in items}
+
+  def state_dict(self):
+    """{'step', 'groups': {g: {'items', 'delta' (8,), 'grad_ema', 'grad_sq_ema'}}} on the host (checkpoints)."""
+    delta, m, v = (t.detach().cpu().numpy() for t in (self.delta, self.m, self.v))
+    return {'step': np.asarray(self.step, np.int32),
+            'groups': {str(g): {'items': list(items), 'delta': delta[g], 'grad_ema': m[g], 'grad_sq_ema': v[g]}
+                       for g, items in enumerate(self.group_items)}}
+
+  @staticmethod
+  def _saved_groups(saved):
+    return {frozenset(str(i) for i in g['items']): g for g in (saved or {}).get('groups', {}).values()}
+
+  def check(self, saved):
+    """Raises ValueError when `saved` (state_dict's layout) holds other groups of items than these."""
+    got = set(self._saved_groups(saved))
+    want = {frozenset(items) for items in self.group_items}
+    if got != want:
+      raise ValueError(f'the checkpoint holds camera intrinsics of the item groups '
+                       f'{sorted(sorted(g) for g in got)}, but the train items group as '
+                       f'{sorted(sorted(g) for g in want)}')
+
+  def load(self, saved):
+    """Copies a saved state_dict (the same groups, any order) into the device buffers."""
+    self.check(saved)
+    groups = self._saved_groups(saved)
+    for key, t in (('delta', self.delta), ('grad_ema', self.m), ('grad_sq_ema', self.v)):
+      t.copy_(torch.stack([torch.as_tensor(groups[frozenset(items)][key]).reshape(8) for items in self.group_items]))
+    self.step = int(np.asarray(saved.get('step', 0)).reshape(-1)[0])
+
+  def grad(self, image, pixels, directions, d_directions, pose, out):
+    """out (G,8) += the intrinsics gradient of a batch's direction gradients (nfb_intrinsics_grad); `pose` is
+    the (N,6) camera poses the batch was drawn with, or None."""
+    lib = _lib.load()
+    g, count = self.delta.shape[0], int(image.numel())
+    need = int(lib.nfb_intrinsics_grad_workspace_size(g, count))
+    if self._workspace is None or self._workspace.numel() < need:
+      self._workspace = torch.empty(need, dtype=torch.uint8, device=self.delta.device)
+    with torch.cuda.device(self.delta.device):
+      _lib.check(lib.nfb_intrinsics_grad(
+          _ptr(self.cameras), self.group.numel(), _ptr(pose), _ptr(self.delta), _ptr(self.group), g,
+          self.part_bits, _ptr(image), _ptr(pixels), _ptr(directions), _ptr(d_directions), count, _ptr(out),
+          _ptr(self._workspace), self._workspace.numel(), _stream()))
+
+  def apply_gradient(self, grad, learning_rate):
+    """One Adam step of the deltas (nfb_adam_step), in place."""
+    self.step += 1
+    lib = _lib.load()
+    with torch.cuda.device(self.delta.device):
+      _lib.check(lib.nfb_adam_step(_ptr(self.delta), _ptr(grad), _ptr(self.m), _ptr(self.v), self.delta.numel(),
+                                   float(learning_rate), self.beta1, self.beta2, self.eps, self.step, _stream()))
+
+  def stats(self):
+    """Device scalars: the mean |s| as a focal-length change in percent and the mean |f0 dc| in pixels over
+    the groups."""
+    f0 = torch.as_tensor(self.focal, dtype=torch.float32, device=self.delta.device)
+    return {'focal_change_pct': 100.0 * self.delta[:, 0].abs().mean(),
+            'principal_point_px': (f0 * self.delta[:, 1:3].norm(dim=1)).mean()}
+
+
 def make_reg(model, scalar_params=None, use_elastic_loss=False, elastic_reduce_method='median',
              elastic_loss_type='log_svals', use_background_loss=False, use_warp_reg_loss=False,
              background_points=None, background_warp_ids=None, background_noise=None):
@@ -333,22 +448,31 @@ def train_step(model, rng_key, state, batch, scalar_params, use_elastic_loss=Fal
     ev[0].record()
   params = opt.target['model']
   model.invalidate_params()     # the Adam kernel rewrote the flat vector under the views
-  poses = state.camera_poses
+  poses, intrinsics = state.camera_poses, state.camera_intrinsics
   grads = ray_grads = None
-  if poses is not None:
-    if 'image' not in batch:
-      raise ValueError("refining camera poses needs batches with 'image' (create_iterator(..., poses=...))")
-    # the pose gradient rides at the tail of the flat gradient vector: still one all-reduce per step
+  if poses is not None or intrinsics is not None:
+    if 'image' not in batch or (intrinsics is not None and 'pixels' not in batch):
+      raise ValueError("refining the cameras needs batches with 'image' and 'pixels' "
+                       '(create_iterator(..., poses=..., intrinsics=...))')
+    # the camera gradients ride at the tail of the flat gradient vector, poses then intrinsics: still one
+    # all-reduce per step
     n_params = opt.flat.numel()
-    grads = torch.zeros(n_params + poses.pose.numel(), device=model.device, dtype=torch.float32)
+    n_poses = 0 if poses is None else poses.pose.numel()
+    n_intrinsics = 0 if intrinsics is None else intrinsics.delta.numel()
+    grads = torch.zeros(n_params + n_poses + n_intrinsics, device=model.device, dtype=torch.float32)
     B = batch['origins'].shape[0]
-    ray_grads = tuple(torch.empty(B, 3, device=model.device, dtype=torch.float32) for _ in range(2))
+    ray_grads = tuple(torch.empty(B, 3, device=model.device, dtype=torch.float32) if need else None
+                      for need in (poses is not None, True))
   losses, grads = value_and_grad(model, params, batch, state.warp_extra,
                                  rngs={'coarse': rng_key, 'fine': rng_key}, chunk_rays=chunk_rays, reg=reg,
                                  grads=grads, ray_grads=ray_grads)
+  if ray_grads is not None:
+    image, directions = _prep_ids(batch['image'], model.device), _prep_f32(batch['directions'], model.device)
   if poses is not None:
-    poses.grad(_prep_ids(batch['image'], model.device), _prep_f32(batch['directions'], model.device), *ray_grads,
-               out=grads[n_params:])
+    poses.grad(image, directions, *ray_grads, out=grads[n_params:n_params + n_poses])
+  if intrinsics is not None:
+    intrinsics.grad(image, _prep_f32(batch['pixels'], model.device), directions, ray_grads[1],
+                    None if poses is None else poses.pose, out=grads[n_params + n_poses:])
   if ev:
     ev[1].record()
   # stats of _compute_loss_and_stats (training.py:171-226)
@@ -377,8 +501,11 @@ def train_step(model, rng_key, state, batch, scalar_params, use_elastic_loss=Fal
     ev[2].record()
   opt.apply_gradient(grads, learning_rate=scalar_params.learning_rate)
   if poses is not None:
-    poses.apply_gradient(grads[n_params:], scalar_params.camera_pose_learning_rate)
+    poses.apply_gradient(grads[n_params:n_params + n_poses], scalar_params.camera_pose_learning_rate)
     stats['camera_poses'] = poses.stats()
+  if intrinsics is not None:
+    intrinsics.apply_gradient(grads[n_params + n_poses:], scalar_params.camera_intrinsics_learning_rate)
+    stats['camera_intrinsics'] = intrinsics.stats()
   if ev:
     ev[3].record()
     ev[3].synchronize()
