@@ -334,6 +334,21 @@ int nfb_warp_code(nfb_handle* h, int n, const unsigned* warp_id, float* code_out
 int nfb_warp_jacobian(nfb_handle* h, int P, const float* points, const unsigned* warp_id, float warp_alpha,
                       float* warped_out, float* jacobian_out, void* stream);
 
+/* The density of a level's NeRF MLP and its gradient at free points x of the frame warp_id names:
+ *   sigma = sigma_act(raw(y)), y = W(x), and grad_x sigma = J_W(x)^T grad_y sigma (P,3), by forward mode
+ *   through the warp field and the NeRF trunk (three tangent rows per point) in the handle's training
+ *   precision (fp32 or tf32x3), whatever nfb_config.precision is.  The derivative of a relu at 0 is 0.
+ *   level 0 or 1 (1 needs a fine level); warp_id (P): GLO ids or, with NFB_WARP_ENC_TIME, const float*
+ *   timestamps, as nfb_warp_jacobian; appearance_id (P) nullable (row 0): feeds the trunk and alpha
+ *   conditions (the camera code and the view directions do not reach sigma).
+ *   flags: NFB_FLAG_NO_WARP = the canonical field (J = I); NFB_FLAG_METADATA_ENCODED and every other flag are
+ *   refused, as is a warp MLP with an activation other than relu when warping.
+ *   sigma_out (P) nullable, grad_out (P,3), warped_out (P,3) nullable (y: the point itself without a warp).
+ * Chunks of max_rays points; no parameter gradients, no autograd. */
+int nfb_density_grad(nfb_handle* h, int level, int P, const float* points, const unsigned* warp_id,
+                     const unsigned* appearance_id, float warp_alpha, unsigned flags, float* sigma_out,
+                     float* grad_out, float* warped_out, void* stream);
+
 /* Per-point outcome of nfb_warp_invert. */
 enum { NFB_INVERT_CONVERGED = 0,   /* |W(x) - target| <= tol                                         */
        NFB_INVERT_MAX_ITERS = 1,   /* still improving when the iterations ran out                     */

@@ -32,7 +32,7 @@ SYMBOLS = [
     'nfb_pose_grad', 'nfb_selftest_net_steps', 'nfb_selftest_net', 'nfb_selftest_cond_vjp',
     'nfb_selftest_encode_bwd', 'nfb_selftest_warp_tail_bwd', 'nfb_selftest_ray_reduce', 'nfb_selftest_viewdir_vjp',
     'nfb_gather_rays_refined', 'nfb_pixels_to_rays_refined', 'nfb_intrinsics_grad_workspace_size',
-    'nfb_intrinsics_grad',
+    'nfb_intrinsics_grad', 'nfb_density_grad',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -211,6 +211,8 @@ def load():
   lib.nfb_warp_vjp.restype = ci
   lib.nfb_warp_jacobian.argtypes = [vp, ci, vp, vp, cf, vp, vp, vp]
   lib.nfb_warp_jacobian.restype = ci
+  lib.nfb_density_grad.argtypes = [vp, ci, ci, vp, vp, vp, cf, cu, vp, vp, vp, vp]
+  lib.nfb_density_grad.restype = ci
   lib.nfb_warp_invert.argtypes = [vp, ci, vp, vp, vp, cf, ci, cf, vp, vp, vp, vp, vp]
   lib.nfb_warp_invert.restype = ci
   lib.nfb_point_visibility.argtypes = [vp, ci, vp, vp, vp, vp, cf, cu, ctypes.POINTER(NfbCamera), cf, vp, vp, vp, vp,

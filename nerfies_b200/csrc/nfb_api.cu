@@ -1386,7 +1386,7 @@ void nfb_destroy(nfb_handle* h) {
   for (float* p : bufs) if (p) cudaFree(p);
   if (h->d_src) cudaFree(h->d_src);
   float* tbufs[] = {h->d_tape, h->d_gpacked, h->d_gwarp, h->d_gapp, h->d_gcam, h->d_dcond, h->d_tr_out, h->d_tr_w, h->d_loss,
-                    h->d_ttape, reinterpret_cast<float*>(h->d_sel), h->d_time_tape, h->d_ray_pts};
+                    h->d_ttape, reinterpret_cast<float*>(h->d_sel), h->d_time_tape, h->d_ray_pts, h->d_ntape};
   for (float* p : tbufs) if (p) cudaFree(p);
   if (h->d_ids) cudaFree(h->d_ids);
   if (h->d_invert) cudaFree(h->d_invert);

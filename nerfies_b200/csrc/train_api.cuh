@@ -716,6 +716,47 @@ int train_background(nfb_handle* h, int P, const float* points, const unsigned* 
   return 0;
 }
 
+// ---- nfb_density_grad: forward mode through a level's NeRF MLP up to the raw density ----
+// The steps the alpha head depends on, in program order: the trunk, the bottleneck only when the alpha head
+// reads it (an alpha condition; models.py:206-207 builds the bottleneck for an rgb condition too, and then the
+// alpha head reads the trunk), and the alpha head, which is the last step of `sub`.  out_primal[i] is the tape
+// offset of sub step i's primal output (its index in the full program differs once a step is dropped).
+int alpha_subnet(const nfb::FieldProgram& p, const TapeLayout& t, Net* sub, long long* out_primal) {
+  int alpha_step = -1;
+  for (int i = 0; i < p.nerf.n_steps; ++i)
+    if (p.nerf.steps[i].dst == p.alpha_slot) alpha_step = i;
+  if (alpha_step < 0) return fail("density gradient: no alpha head in the program");
+  int producer[nfb::kMaxSteps];
+  net_producers(p.nerf, producer);
+  bool need[nfb::kMaxSteps] = {};
+  for (int i = alpha_step; i >= 0; i = producer[i]) need[i] = true;
+  *sub = Net{};
+  for (int i = 0; i <= alpha_step; ++i)
+    if (need[i]) {
+      out_primal[sub->n_steps] = t.out_n[i];
+      sub->steps[sub->n_steps++] = p.nerf.steps[i];
+    }
+  return 0;
+}
+
+// The NeRF tangent tape of `rows` points: the warp Jacobian (rows,9), the zero z of the one-sample level
+// forward (rows), then three tangent rows per point: the encoded input and the output of each step of `sub`.
+struct NTapeLayout {
+  long long trows = 0, jac = 0, z = 0, in_t = 0, total = 0;
+  long long out_t[nfb::kMaxSteps];
+};
+NTapeLayout ntape_layout(const nfb::FieldProgram& p, const Net& sub, long long rows) {
+  NTapeLayout t;
+  t.trows = rows * 3;
+  long long off = 0;
+  auto take = [&](long long n) { long long o = off; off += (n + 63) / 64 * 64; return o; };
+  t.jac = take(rows * 9); t.z = take(rows);
+  t.in_t = take(t.trows * pad32(p.Dp + p.tc + p.ac + p.rc));
+  for (int s = 0; s < sub.n_steps; ++s) t.out_t[s] = take(t.trows * sub.steps[s].npad);
+  t.total = off;
+  return t;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1096,6 +1137,71 @@ int nfb_warp_jacobian(nfb_handle* h, int P, const float* points, const unsigned*
                                cudaMemcpyDeviceToDevice, s));
     if (warp_jacobian_on_tape(h, p, t, h->d_tape, nullptr, n, nullptr, nullptr, false, jacobian_out + (size_t)p0 * 9, s))
       return -1;
+  }
+  return 0;
+}
+
+// grad sigma(W(x)) = J_W(x)^T grad_y sigma(y): per chunk the primal tape of a one-sample level forward (origin =
+// the point, z = 0), the warp Jacobian on it, the NeRF encoding's tangent rows pushed through the steps the
+// raw density depends on, and density_grad_kernel.
+int nfb_density_grad(nfb_handle* h, int level, int P, const float* points, const unsigned* warp_id,
+                     const unsigned* appearance_id, float warp_alpha, unsigned flags, float* sigma_out,
+                     float* grad_out, float* warped_out, void* stream) {
+  using namespace nfb::train;
+  if (!h || !points) return fail("density gradient: null handle / points");
+  if (!grad_out) return fail("density gradient: grad_out is null");
+  if (P < 0) return fail("density gradient: P=%d must be >= 0", P);
+  if (check_call(h, std::min(P, h->max_rays))) return -1;
+  const nfb_config& c = h->cfg;
+  if (level != 0 && level != 1) return fail("density gradient: level %d is not 0 or 1", level);
+  if (level == 1 && c.num_fine_samples <= 0) return fail("density gradient: level 1, but the model is coarse-only");
+  if (flags & NFB_FLAG_METADATA_ENCODED) return fail("density gradient: NFB_FLAG_METADATA_ENCODED is not supported");
+  if (flags & ~NFB_FLAG_NO_WARP) return fail("density gradient: flags 0x%x: only NFB_FLAG_NO_WARP is accepted", flags);
+  const nfb::FieldProgram& p = h->prog[level];
+  const bool warp = !(flags & NFB_FLAG_NO_WARP) && p.warp_type != 0;
+  if (warp && check_relu_warp(p, "density gradient")) return -1;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (enter_stream(h, s)) return -1;
+  if (P == 0) return 0;
+  if (set_window(h, warp_alpha, s)) return -1;
+  const int chunk = std::min(P, h->max_rays);
+  if (train_prepare_rows(h, chunk)) return -1;
+  Net sub;
+  long long out_primal[nfb::kMaxSteps];
+  if (alpha_subnet(p, tape_layout(p, chunk), &sub, out_primal) ||
+      grow(&h->d_ntape, &h->ntape_floats, ntape_layout(p, sub, chunk).total, "density-gradient tangent tape"))
+    return -1;
+  const bool float_time = has_time_encoder(h) && c.warp_metadata_encoder == NFB_WARP_ENC_TIME;
+  for (int p0 = 0; p0 < P; p0 += chunk) {
+    const int n = std::min(chunk, P - p0);
+    const float* x = points + (size_t)p0 * 3;
+    const TapeLayout t = tape_layout(p, n);
+    if (alpha_subnet(p, t, &sub, out_primal)) return -1;
+    const NTapeLayout nt = ntape_layout(p, sub, n);
+    float* A = h->d_tape;
+    float* T = h->d_ntape;
+    // the condition vectors of the points (the view-direction columns do not reach sigma); without a warp the
+    // warp block is not read
+    const unsigned* app = appearance_id ? appearance_id + p0 : nullptr;
+    if (warp ? train_cond(h, n, x, warp_id ? warp_id + p0 : nullptr, float_time, app, nullptr, s)
+             : run_cond(h, n, x, nullptr, app, nullptr, s, false, false))
+      return -1;
+    NFB_CUDA(cudaMemsetAsync(T + nt.z, 0, (size_t)n * sizeof(float), s));
+    int alpha_step = -1, rgb_step = -1;
+    // one sample per point at z = 0; the points double as the (unused) directions
+    if (level_forward(h, level, n, 1, T + nt.z, x, x, h->d_cond, warp, h->d_tr_out, nullptr, s, &alpha_step, &rgb_step))
+      return -1;
+    if (warp && warp_jacobian_on_tape(h, p, t, A, nullptr, n, nullptr, nullptr, false, T + nt.jac, s)) return -1;
+    EncodeTangentArgs e{A + t.warped, nullptr, nullptr, T + nt.in_t, p.Fp, t.ld_n, n, warp ? T + nt.jac : nullptr};
+    encode_tangent_kernel<<<(unsigned)((nt.trows + 127) / 128), 128, 0, s>>>(e);
+    if (launch_check(h, "encode_tangent_kernel")) return -1;
+    if (tnet_forward(h, sub, T + nt.in_t, t.ld_n, nt.out_t, out_primal, A, T, nullptr, nt.trows, s)) return -1;
+    const int last = sub.n_steps - 1;
+    DensityGradArgs d{A + t.out_n[alpha_step], p.nerf.steps[alpha_step].npad, T + nt.out_t[last], A + t.warped,
+                      sigma_out ? sigma_out + p0 : nullptr, grad_out + (size_t)p0 * 3,
+                      warped_out ? warped_out + (size_t)p0 * 3 : nullptr, p.sigma_act, n};
+    density_grad_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(d);
+    if (launch_check(h, "density_grad_kernel")) return -1;
   }
   return 0;
 }

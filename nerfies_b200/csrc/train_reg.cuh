@@ -172,13 +172,16 @@ __global__ void depth_index_kernel(const float* __restrict__ weights, int num_ra
 }
 
 // ---------------------------------------------------------------------------
-// Tangent of the encoded warp input: row r*3 + j = d enc(x) / d x_j of selected row r
+// Tangent of an encoded input: row r*3 + j = d enc(x) / d x_j of selected row r
 // (annealed_sinusoidal_encode, modules.py:231-294: [x, w_f sin(2^f x), w_f sin(2^f x + pi/2)]);
-// the metadata columns do not depend on the point.
+// the metadata / condition columns do not depend on the point.  With `jac` the encoded point is
+// itself a function of the input point u (the warped point y = W(u) of nfb_density_grad): row r*3 + j
+// is then d enc(y) / d u_j = sum_c d enc / d y_c J_cj, J = jac[r] row-major (no sel).
 // ---------------------------------------------------------------------------
 struct EncodeTangentArgs {
   const float* pts; const int* sel; const float* window; float* tin;
   int F, ld; long long R;
+  const float* jac;                // (R,9) input tangents, or null: the unit vectors e_j
 };
 __global__ void encode_tangent_kernel(const EncodeTangentArgs a) {
   const long long m = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -186,9 +189,25 @@ __global__ void encode_tangent_kernel(const EncodeTangentArgs a) {
   const long long r = m / 3;
   const int j = (int)(m - r * 3);
   const long long row = a.sel ? a.sel[r] : r;
-  const float xj = a.pts[row * 3 + j];
   float* o = a.tin + m * a.ld;
   for (int q = 0; q < a.ld; ++q) o[q] = 0.f;
+  if (a.jac) {
+    float x[3], t[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) { x[c] = a.pts[row * 3 + c]; t[c] = a.jac[r * 9 + c * 3 + j]; o[c] = t[c]; }
+    for (int f = 0; f < a.F; ++f) {
+      const float w = a.window ? a.window[f] : 1.f;
+      const float s = exp2f((float)f);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const float ang = x[c] * s;
+        o[3 + f * 6 + c] = w * s * cosf(ang) * t[c];
+        o[3 + f * 6 + 3 + c] = w * s * cosf(ang + kHalfPiF) * t[c];
+      }
+    }
+    return;
+  }
+  const float xj = a.pts[row * 3 + j];
   o[j] = 1.f;
   for (int f = 0; f < a.F; ++f) {
     const float w = a.window ? a.window[f] : 1.f;
@@ -218,6 +237,38 @@ struct DZTB {
   DZT z;
   __device__ float operator()(long long m, int n) const { return z(m, n); }
 };
+
+// ---------------------------------------------------------------------------
+// The density and its gradient at free points (nfb_density_grad): sigma = act(raw) and
+// d sigma / d x_j = act'(raw) * (tangent row r*3 + j of the raw density), the derivative taken as
+// composite_vjp_kernel takes it (relu: 0 where raw <= 0).
+// ---------------------------------------------------------------------------
+struct DensityGradArgs {
+  const float* raw; int ld;        // primal raw density, column 0 of the alpha head's tape rows
+  const float* traw;               // its tangent rows r*3 + j (same ld)
+  const float* pts;                // (R,3) the encoded (warped) points
+  float* sigma;                    // (R) or null
+  float* grad;                     // (R,3)
+  float* warped;                   // (R,3) or null
+  int sigma_act;
+  long long R;
+};
+__global__ void density_grad_kernel(const DensityGradArgs a) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= a.R) return;
+  const float raw = a.raw[r * a.ld];
+  const float sigma = apply_act(raw, a.sigma_act);
+  float dact;
+  if (a.sigma_act == kSoftplus) dact = 1.f / (1.f + expf(-raw));
+  else if (a.sigma_act == kRelu) dact = raw > 0.f ? 1.f : 0.f;
+  else dact = act_grad_from_output(sigma, a.sigma_act);
+  if (a.sigma) a.sigma[r] = sigma;
+#pragma unroll
+  for (int j = 0; j < 3; ++j) a.grad[r * 3 + j] = dact * a.traw[(r * 3 + j) * a.ld];
+  if (a.warped)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) a.warped[r * 3 + c] = a.pts[r * 3 + c];
+}
 
 // ---------------------------------------------------------------------------
 // Jacobian of the warp at the selected rows, the elastic loss and its adjoint.

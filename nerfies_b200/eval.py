@@ -13,6 +13,9 @@ With `--save_viz`, each frame also writes the colour-mapped images of eval.py:87
 two files), and the images the reference sends to TensorBoard, `disparity_expected_viz_`,
 `disparity_median_viz_`, `acc_viz_` and, for items with a target, `rgb_abs_error_viz_` and
 `rgb_sq_error_viz_<id>.png`.
+With `--save_normals`, each frame also writes `normals_<id>.png`: the surface normals at the median depth of
+the frame's last level (geometry.normal_map, coloured in the camera's frame by
+visualization.normals_to_color; black where a ray meets no surface).
 Frames are quantised on the device (`nfb_image_quantize`), copied to pinned host memory without
 blocking, and PNG-encoded by a worker thread while the next frame renders; every worker is joined
 before `evaluate` returns.
@@ -97,16 +100,28 @@ def viz_images(render, rgb_target, near, far):
   return images
 
 
-def render_and_score(model, params, camera, warp_extra, metadata, rgb_target, viz_range=None):
+def normal_image(model, params, camera, warp_extra, metadata, med_depth):
+  """The normal map of a rendered frame as a uint8 (h, w, 3) device image: geometry.normal_map at the median
+  depth of the frame's last level (the fine level when the model has one), visualization.normals_to_color."""
+  from nerfies_b200 import geometry
+  level = 'fine' if model.num_fine_samples > 0 else 'coarse'
+  normals = geometry.normal_map(model, params, camera, med_depth, warp_extra, metadata, level=level)
+  return visualization.normals_to_color(normals['normals'], normals['valid'], camera)
+
+
+def render_and_score(model, params, camera, warp_extra, metadata, rgb_target, viz_range=None, normals=False):
   """One frame on the GPU: ({file stem: uint8 / uint16 device image}, {metric: 0-d device tensor}).
   The images are what eval.py:99-108 saves, plus `viz_images` when `viz_range` is the scene's
-  (near, far); the metrics eval.py:118-125's, without `ssim` for frames MS-SSIM cannot take."""
+  (near, far) and `normal_image` ('normals') with `normals`; the metrics eval.py:118-125's, without
+  `ssim` for frames MS-SSIM cannot take."""
   render = evaluation.render_frame(model, params, camera, warp_extra, metadata)
   images = {'rgb': evaluation.image_to_uint8(render['rgb']),
             'depth_expected': evaluation.depth_to_uint16(render['depth']),
             'depth_median': evaluation.depth_to_uint16(render['med_depth'])}
   if viz_range is not None:
     images.update(viz_images(render, rgb_target, *viz_range))
+  if normals:
+    images['normals'] = normal_image(model, params, camera, warp_extra, metadata, render['med_depth'])
   metrics = {}
   if rgb_target is not None:
     if min(rgb_target.shape[:2]) >= evaluation.MIN_METRICS_SIZE:
@@ -203,11 +218,16 @@ def refined_items(items, saved_poses, saved_intrinsics=None):
 
 def evaluate(exp_config, model_config, train_config, eval_config, base_folder, data_dir=None,
              precision='fp16x3', poll_seconds=10.0, datasource=None, construct_fn=models.construct_nerf,
-             frame_fn=render_and_score, log=print, save_viz=False):
+             frame_fn=render_and_score, log=print, save_viz=False, save_normals=False):
   """Renders and scores checkpoints until `eval_once` is set or step `max_steps` has been rendered.
   Returns the list of steps handled.  `datasource`, `construct_fn` and `frame_fn` replace the data
   source, the model constructor and the renderer (tests run the loop without a GPU that way).
-  `save_viz` passes `viz_range=(near, far)` to `frame_fn`, which then adds the colour-mapped images."""
+  `save_viz` passes `viz_range=(near, far)` to `frame_fn`, which then adds the colour-mapped images;
+  `save_normals` passes `normals=True`, which adds the normal map; it is refused (ValueError, before any GPU
+  work) when EvalConfig.save_output is off, since nothing would be written."""
+  if save_normals and not eval_config.save_output:
+    raise ValueError('--save_normals writes normals_<id>.png among the saved renders, but EvalConfig.save_output '
+                     'is off')
   rank, world, own_group = driver_utils.init_distributed()
   pool = concurrent.futures.ThreadPoolExecutor(max_workers=2)
   writer = None
@@ -221,6 +241,8 @@ def evaluate(exp_config, model_config, train_config, eval_config, base_folder, d
       datasource = driver_utils.make_datasource(exp_config, model_config, data_dir)
     if save_viz:
       frame_fn = functools.partial(frame_fn, viz_range=(datasource.near, datasource.far))
+    if save_normals:
+      frame_fn = functools.partial(frame_fn, normals=True)
 
     def items_of(ids):                                                           # eval.py:297-300
       return [(i, datasource.load_camera(i), item['metadata'], item['rgb'])
@@ -282,6 +304,8 @@ def main(argv=None, poll_seconds=10.0):
   parser.add_argument('--eval_once', action='store_true', help='sets EvalConfig.eval_once')
   parser.add_argument('--save_viz', action='store_true',
                       help='also write the colour-mapped depth, disparity, accumulation and error images')
+  parser.add_argument('--save_normals', action='store_true',
+                      help='also write normals_<id>.png, the surface normals at the median depth')
   args = parser.parse_args(argv)
   driver_utils.parse_configs(args.gin_configs, args.gin_bindings)
   exp_config = configs.ExperimentConfig()                                        # eval.py:238-241
@@ -293,7 +317,8 @@ def main(argv=None, poll_seconds=10.0):
   if args.eval_once:
     eval_config.eval_once = True
   evaluate(exp_config, model_config, train_config, eval_config, args.base_folder, args.data_dir,
-           precision=args.precision, poll_seconds=poll_seconds, save_viz=args.save_viz)
+           precision=args.precision, poll_seconds=poll_seconds, save_viz=args.save_viz,
+           save_normals=args.save_normals)
   return 0
 
 

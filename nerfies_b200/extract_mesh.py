@@ -3,7 +3,7 @@
   python -m nerfies_b200.extract_mesh --base_folder EXP --data_dir CAPTURE --gin_configs X.gin \\
       [--step N] [--resolution 256] [--threshold SIGMA] [--bbox x0 y0 z0 x1 y1 z1] \\
       [--canonical] [--metadata warp=3 ...] [--level fine|coarse] [--colors] [--world_coords] \\
-      [--track [--frames V ...]]
+      [--track [--frames V ...]] [--analytic_normals]
 
 Restores the checkpoint of `--step` (default: the newest) and its warp_extra as render_video does,
 evaluates the density of `--level`'s NeRF MLP on a grid over the box (geometry.density_grid) and
@@ -22,6 +22,11 @@ extracts the surface {sigma > threshold} by marching cubes (geometry.marching_cu
 - Output: `<exp_dir>/meshes/<step, 8 digits>/<canonical | warp_<id> | time_<t>>.ply`, binary PLY
   with normals (and colours with `--colors`: each vertex's colour seen along -normal).  With
   `--world_coords` the vertices are mapped back to the capture's world frame (x / scale + center).
+- Normals: by default the grid's (marching cubes, from the density grid by finite differences at the
+  grid spacing).  `--analytic_normals` replaces them by -grad sigma / |grad sigma| of the same level at
+  each vertex, in the same space as the mesh (geometry.density_gradient); a vertex whose gradient is zero
+  or not finite keeps its grid normal, and the log line counts them.  `--colors` and `--track` then use
+  these normals.
 - `--track [--frames V ...]`: the template mesh (as `--canonical`, written as `canonical.ply`) carried
   into every frame with one topology: each vertex is the inverse of the frame's warp at the template
   vertex (geometry.track_surface; tolerance TRACK_TOL_VOXELS of the voxel size, TRACK_MAX_ITERS
@@ -138,10 +143,21 @@ def track_frames(datasource, model_config, frames=None):
   return found
 
 
+def analytic_normals(model, params, vertices, normals, warp_extra, metadata, use_warp, level):
+  """(normals, kept): -grad sigma / |grad sigma| at the vertices (geometry.density_gradient), the grid normal
+  where the gradient is zero or not finite; `kept` counts those vertices."""
+  grad = geometry.density_gradient(model, params, vertices, warp_extra, metadata, use_warp=use_warp,
+                                   level=level)['gradient']
+  norm = grad.norm(dim=-1)
+  ok = torch.isfinite(grad).all(-1) & torch.isfinite(norm) & (norm > 0)
+  out = torch.where(ok[:, None], -grad / torch.where(ok, norm, 1.0)[:, None], normals.to(grad.device))
+  return out.contiguous(), int((~ok).sum())
+
+
 def extract_mesh(exp_config, model_config, base_folder, data_dir=None, step=None, resolution=256, threshold=None,
                  bbox=None, canonical=False, metadata=(), level='fine', colors=False, world_coords=False,
                  precision='fp16x3', datasource=None, construct_fn=models.construct_nerf, log=print, track=False,
-                 frames=None):
+                 frames=None, analytic=False):
   """Writes the mesh; returns the PLY's path (with `track`, the path of track.npz)."""
   if level not in geometry.LEVELS:
     raise ValueError(f"--level must be 'coarse' or 'fine', got {level!r}")
@@ -181,6 +197,10 @@ def extract_mesh(exp_config, model_config, base_folder, data_dir=None, step=None
   grid = geometry.density_grid(model, params, box, shape, state.warp_extra, md, use_warp=not canonical, level=level)
   vertices, faces, normals, axes = geometry.marching_cubes(grid, threshold, box, return_axes=True)
   log(f'Marching cubes at sigma {threshold:g}: {len(vertices)} vertices, {len(faces)} faces')
+  if analytic:
+    normals, kept = analytic_normals(model, params, vertices, normals, state.warp_extra, md, not canonical, level)
+    log(f'Analytic normals (-grad sigma): {len(vertices) - kept} vertices, {kept} kept their grid normal '
+        '(zero or non-finite gradient)')
   rgb = None
   if colors:
     rgb = geometry.vertex_colors(model, params, vertices, normals, state.warp_extra, md, use_warp=not canonical,
@@ -253,6 +273,8 @@ def make_parser():
                       help='the template mesh carried into every frame with one topology (meshes/<step>/track/)')
   parser.add_argument('--frames', nargs='+', default=None, metavar='V',
                       help='with --track: warp ids (timestamps with the \'time\' encoder); default: the training frames')
+  parser.add_argument('--analytic_normals', action='store_true',
+                      help='vertex normals from the density gradient at the vertices instead of the grid')
   return parser
 
 
@@ -266,7 +288,7 @@ def main(argv=None):
                       bbox=None if args.bbox is None else np.reshape(args.bbox, (2, 3)), canonical=args.canonical,
                       metadata=args.metadata, level=args.level, colors=args.colors,
                       world_coords=args.world_coords, precision=args.precision, track=args.track,
-                      frames=args.frames)
+                      frames=args.frames, analytic=args.analytic_normals)
   print(f'Wrote {path}')
   return 0
 

@@ -160,6 +160,59 @@ def vertex_colors(model, params, vertices, normals, warp_extra=None, metadata=No
   return colors
 
 
+def density_gradient(model, params, points, warp_extra=None, metadata=None, use_warp=True, level='fine'):
+  """The density sigma of `level`'s NeRF MLP at free points (P, 3) and its gradient with respect to the
+  points (nfb_density_grad): with use_warp, of the frame the metadata names (grad_x sigma(W(x)) =
+  J_W(x)^T grad_y sigma(y), y = W(x)); without, of the canonical template.  Forward mode through the warp
+  field and the NeRF trunk in the model's training precision (fp32 or tf32x3); a relu's derivative at 0
+  is 0.  Metadata as density_grid: 'warp' (or 'time') and 'appearance' where the model reads them; the
+  camera code and view directions do not reach sigma.
+  Returns {'sigma' (P,), 'gradient' (P, 3), 'warped_points' (P, 3) (the points themselves without a
+  warp)}, plain float32 tensors on the model's device: parameters that require grad give them no
+  grad_fn, and nothing is differentiated through them."""
+  hd, alpha, flags, lv = _prepare(model, params, warp_extra, use_warp, level)
+  dev = model.device
+  points = _f32(points, dev, 3, 'density_gradient: points')
+  P = points.shape[0]
+  md = metadata or {}
+  warp_id = _warp_ids(model, md, P) if flags != _lib.FLAG_NO_WARP else None
+  app_id = _ids(model, md, 'appearance', model.use_appearance_metadata, P)
+  out = {'sigma': torch.empty(P, device=dev), 'gradient': torch.empty(P, 3, device=dev),
+         'warped_points': torch.empty(P, 3, device=dev)}
+  if P == 0:
+    return out
+  with torch.cuda.device(dev):
+    _lib.check(hd.lib.nfb_density_grad(hd.h, lv, P, _ptr(points), _ptr(warp_id), _ptr(app_id), alpha, flags,
+                                       _ptr(out['sigma']), _ptr(out['gradient']), _ptr(out['warped_points']),
+                                       _stream()))
+  return out
+
+
+def normal_map(model, params, camera, depth, warp_extra=None, metadata=None, level='fine'):
+  """World-frame surface normals of a frame: at each pixel's point x = o + depth * d (the rays of
+  `camera`), n = -grad sigma / |grad sigma| of `level`'s NeRF MLP in the frame the metadata names
+  (density_gradient).  `depth` (H, W) is render_frame's 'med_depth', whose 0 marks a ray with no
+  surface.  A pixel is valid where depth > 0 and the gradient is finite and nonzero; invalid pixels
+  get 0.  Returns {'normals' (H, W, 3), 'valid' (H, W) bool} on the model's device."""
+  from nerfies_b200 import camera as camera_lib
+  dev = model.device
+  h, w = camera.image_shape
+  depth = torch.as_tensor(depth).to(device=dev, dtype=torch.float32)
+  if tuple(depth.shape) != (h, w):
+    raise ValueError(f'normal_map: depth must be the frame\'s (H, W) = ({h}, {w}), got {tuple(depth.shape)}')
+  rays = camera_lib.camera_to_rays(camera, dev)
+  hit = (depth > 0).reshape(-1)
+  points = (rays['origins'] + depth[..., None] * rays['directions']).reshape(-1, 3)[hit]
+  grad = density_gradient(model, params, points, warp_extra, metadata, use_warp=True, level=level)['gradient']
+  norm = grad.norm(dim=-1)
+  ok = torch.isfinite(grad).all(-1) & torch.isfinite(norm) & (norm > 0)
+  normals = torch.zeros(h * w, 3, device=dev)
+  valid = torch.zeros(h * w, dtype=torch.bool, device=dev)
+  normals[hit] = torch.where(ok[:, None], -grad / torch.where(ok, norm, 1.0)[:, None], 0.0)
+  valid[hit] = ok
+  return {'normals': normals.reshape(h, w, 3), 'valid': valid.reshape(h, w)}
+
+
 def invert_warp(model, params, targets, warp_extra=None, metadata=None, init=None, max_iters=16, tol=1e-5,
                 return_jacobian=False):
   """The points x of the frame the metadata names whose warp W(x) is `targets` (P, 3) template points

@@ -2,7 +2,7 @@
 ("Load cameras", "Render video frames", "Show rendered video") over this package's CUDA path.
 
   python -m nerfies_b200.render_video --base_folder EXP --data_dir CAPTURE --gin_configs configs/x.gin \\
-      [--camera_path camera-paths/orbit-mild] [--fps 30] [--step N] [--metadata appearance=3 ...]
+      [--camera_path camera-paths/orbit-mild] [--fps 30] [--step N] [--metadata appearance=3 ...] [--normals]
 
 Loads every camera of `<data_dir>/<camera_path>` in sorted order, restores the checkpoint of
 `--step` (default: the newest) as `eval.evaluate` does, and renders each camera with
@@ -13,7 +13,9 @@ handed to one worker thread, which writes `frame_<i:05d>.png` and appends the fr
 (OpenCV, mp4v, `--fps`) in order while the next frame renders.  The video's sides are even, as 4:2:0
 video needs: an odd last row or column of the frame is repeated in it (the PNGs are exact).  Output:
 `<exp_dir>/videos/<camera path name>/<step, 8 digits>/`; not under `renders/`, whose oldest entries
-eval deletes.
+eval deletes.  With `--normals`, each frame's normal map at the same median depth (eval.normal_image:
+colours in the camera's frame, black where a ray meets no surface) also goes to `normals_<i:05d>.png` and
+`normals.mp4` in that directory.
 
 Metadata: every input the model reads is 0 ('appearance', 'warp', 'camera' ids) or 0.0 ('time'),
 the notebook's zeros, unless `--metadata key=value` sets it.  The notebook builds no 'camera' id,
@@ -58,29 +60,34 @@ def default_metadata(datasource, overrides=()):
   return metadata
 
 
-def render_video_frame(model, params, camera, warp_extra, metadata, near, far):
-  """One video frame on the device: uint8 (h, 2w, 3), rgb | colour-mapped median depth."""
+def render_video_frame(model, params, camera, warp_extra, metadata, near, far, normals=False):
+  """One video frame on the device: uint8 (h, 2w, 3), rgb | colour-mapped median depth; with `normals`,
+  the pair (frame, the normal map at the same median depth, uint8 (h, w, 3): eval.normal_image)."""
   render = evaluation.render_frame(model, params, camera, warp_extra, metadata)
-  return visualization.video_frame(render['rgb'], render['med_depth'], near, far)
+  frame = visualization.video_frame(render['rgb'], render['med_depth'], near, far)
+  if not normals:
+    return frame
+  return frame, eval_lib.normal_image(model, params, camera, warp_extra, metadata, render['med_depth'])
 
 
 class _VideoSink:
-  """frame_<i>.png files and one mp4, written in the order frames arrive."""
+  """<stem>_<i>.png files and one mp4, written in the order frames arrive."""
 
-  def __init__(self, out_dir, fps):
+  def __init__(self, out_dir, fps, stem='frame', video='video.mp4'):
     self.out_dir, self.fps, self.writer, self.count = out_dir, fps, None, 0
+    self.stem, self.video = stem, video
 
   def write(self, frame):
     import cv2
-    eval_lib.write_png(self.out_dir / f'frame_{self.count:05d}.png', frame)
+    eval_lib.write_png(self.out_dir / f'{self.stem}_{self.count:05d}.png', frame)
     h, w = frame.shape[:2]
     # 4:2:0 video needs even sides: an odd last row / column is repeated (the encoder would drop it)
     bgr = np.pad(frame[:, :, ::-1], ((0, h % 2), (0, w % 2), (0, 0)), mode='edge')
     if self.writer is None:
-      self.writer = cv2.VideoWriter(str(self.out_dir / 'video.mp4'), cv2.VideoWriter_fourcc(*'mp4v'), self.fps,
+      self.writer = cv2.VideoWriter(str(self.out_dir / self.video), cv2.VideoWriter_fourcc(*'mp4v'), self.fps,
                                     (bgr.shape[1], bgr.shape[0]))
       if not self.writer.isOpened():
-        raise IOError(f'could not open {self.out_dir / "video.mp4"} for writing')
+        raise IOError(f'could not open {self.out_dir / self.video} for writing')
     self.writer.write(np.ascontiguousarray(bgr))
     self.count += 1
 
@@ -91,13 +98,14 @@ class _VideoSink:
 
 def render_video(exp_config, model_config, base_folder, data_dir=None, camera_path='camera-paths/orbit-mild',
                  fps=30.0, step=None, metadata=(), precision='fp16x3', datasource=None,
-                 construct_fn=models.construct_nerf, frame_fn=render_video_frame, log=print):
+                 construct_fn=models.construct_nerf, frame_fn=render_video_frame, log=print, normals=False):
   """Renders the camera path; returns the output directory.  `datasource`, `construct_fn` and
   `frame_fn` replace the data source, the model constructor and the frame renderer (tests run the
-  loop without a GPU that way)."""
+  loop without a GPU that way).  With `normals`, frame_fn is called with normals=True and returns
+  (frame, normal map)."""
   rank, world, own_group = driver_utils.init_distributed()
   pool = concurrent.futures.ThreadPoolExecutor(max_workers=1)          # one worker: frames stay in order
-  sink = None
+  sink = normal_sink = None
   try:
     dirs = driver_utils.experiment_dirs(base_folder, exp_config.subname)
     if datasource is None:
@@ -127,21 +135,28 @@ def render_video(exp_config, model_config, base_folder, data_dir=None, camera_pa
     if rank == 0:
       out_dir.mkdir(parents=True, exist_ok=True)
       sink = _VideoSink(out_dir, fps)
+      if normals:
+        normal_sink = _VideoSink(out_dir, fps, 'normals', 'normals.mp4')
     pending = []
     for i, camera in enumerate(cameras):
       log(f'Rendering frame {i + 1}/{len(cameras)}')
       frame = frame_fn(model, state.optimizer.target['model'], camera, state.warp_extra, md, datasource.near,
-                       datasource.far)
+                       datasource.far, **({'normals': True} if normals else {}))
+      frame, normal_frame = frame if normals else (frame, None)
       if sink is not None:
         wait = eval_lib._host_copy(frame)
         pending.append(pool.submit(lambda w=wait: sink.write(w())))
+      if normal_sink is not None:
+        wait = eval_lib._host_copy(normal_frame)
+        pending.append(pool.submit(lambda w=wait: normal_sink.write(w())))
     for future in pending:
       future.result()
     return out_dir
   finally:
     pool.shutdown(wait=True)
-    if sink is not None:
-      sink.close()
+    for s in (sink, normal_sink):
+      if s is not None:
+        s.close()
     if own_group:
       torch.distributed.destroy_process_group()
 
@@ -154,12 +169,15 @@ def main(argv=None):
   parser.add_argument('--step', type=int, default=None, help='checkpoint step (default: the newest)')
   parser.add_argument('--metadata', action='append', default=[], metavar='KEY=VALUE',
                       help="metadata of every frame, e.g. appearance=3 or time=0.5 (default 0)")
+  parser.add_argument('--normals', action='store_true',
+                      help='also write normals_<i>.png and normals.mp4, the surface normals at the median depth')
   args = parser.parse_args(argv)
   driver_utils.parse_configs(args.gin_configs, args.gin_bindings)
   exp_config = configs.ExperimentConfig()
   model_config = configs.ModelConfig(use_stratified_sampling=False)
   out_dir = render_video(exp_config, model_config, args.base_folder, args.data_dir, camera_path=args.camera_path,
-                         fps=args.fps, step=args.step, metadata=args.metadata, precision=args.precision)
+                         fps=args.fps, step=args.step, metadata=args.metadata, precision=args.precision,
+                         normals=args.normals)
   print(f'Wrote {out_dir}')
   return 0
 

@@ -158,6 +158,25 @@ def video_frame(rgb, depth, near, far, cmap='magma'):
   return frame
 
 
+def normals_to_color(normals, valid, camera):
+  """A normal map (geometry.normal_map's world-frame (h, w, 3) normals and (h, w) valid mask) as a
+  torch.uint8 (h, w, 3) image: each normal in the camera's frame (n_c = camera.orientation @ n; x right,
+  y down, z forward) coloured RGB = (n_c * (1, -1, -1) + 1) / 2, so a surface facing the camera is
+  (0.5, 0.5, 1) and one facing up is green; invalid pixels are black.  Quantised by nfb_image_quantize."""
+  normals = _check('normals', normals)
+  if normals.dim() != 3 or normals.shape[-1] != 3:
+    raise ValueError(f'normals must be (h, w, 3), got {tuple(normals.shape)}')
+  if not torch.is_tensor(valid) or valid.device != normals.device or tuple(valid.shape) != tuple(normals.shape[:2]):
+    raise ValueError(f'valid must be an (h, w) = {tuple(normals.shape[:2])} tensor on {normals.device}')
+  from nerfies_b200 import evaluation
+  dev = normals.device
+  rot = torch.as_tensor(np.asarray(camera.orientation, np.float32), device=dev)
+  flip = torch.tensor([1.0, -1.0, -1.0], device=dev)
+  rgb = (normals @ rot.T * flip + 1.0) * 0.5
+  rgb = torch.where(valid.bool()[..., None], rgb, 0.0)
+  return evaluation.image_to_uint8(rgb.contiguous())
+
+
 def flow_to_color(flow, status=None, max_flow=None):
   """Optical flow (h, w, 2) float32 on a CUDA device in the colour coding of Baker et al. (IJCV 2011),
   torch.uint8 (h, w, 3) on the same device (nfb_flow_colorize).  `status` (h, w) (_lib.TRACK_STATUS
