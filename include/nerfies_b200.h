@@ -227,6 +227,12 @@ typedef struct nfb_train_reg {
                                             uint32 ids for every encoder (a TimeEncoder reads float(id)) */
   const float* background_noise;         /* device (P,3) or NULL: noise_std * random.normal(key, points.shape) */
   float background_loss_weight;          /* ScalarParams.background_loss_weight */
+  /* Depth supervision (no reference counterpart): per level, the L1 error of the expected depth
+   * sum_i w_i z_i against depth_target, averaged over the rays of the batch whose target is finite and > 0.
+   * Zero / NULL: off, and the call launches exactly what it launches without these fields. */
+  int use_depth_loss;
+  float depth_loss_weight;               /* ScalarParams.depth_loss_weight */
+  const float* depth_target;             /* device (B): ray distance in scene units; NaN or <= 0: no target */
 } nfb_train_reg;
 
 /* nfb_train_value_and_grad plus the regularisers (reg may be NULL).  loss_out: 16 device floats
@@ -234,10 +240,13 @@ typedef struct nfb_train_reg {
  *   [4] metric/jacobian_det  [5] metric/jacobian_div  [6] metric/jacobian_curl (means over the rows whose
  *   Jacobian the loss uses: the reference averages these three over every coarse sample, training.py:214-222)
  *   [7] loss/warp_reg coarse  [8] residual/warp_reg coarse  [9] loss/warp_reg fine  [10] residual fine
- *   [11] background loss (unweighted mean)  [12] mean |warped - x| of the background points.
+ *   [11] background loss (unweighted mean)  [12] mean |warped - x| of the background points
+ *   [13] depth loss coarse  [14] depth loss fine (unweighted: mean |depth - target| over the valid rays, 0
+ *   when there are none)  [15] the number of valid depth targets in the batch (0 with the depth loss off).
  * The gradient is that of  rgb_coarse + rgb_fine + elastic_loss_weight * [2] + warp_reg_loss_weight *
- * ([7] + [9]) + background_loss_weight * [11]  (training.py:176-212, 228-259).  Replaces
- * jax.value_and_grad(_loss_fn) (training.py:263-264) with every regulariser of train_step. */
+ * ([7] + [9]) + background_loss_weight * [11] + depth_loss_weight * ([13] + [14])  (training.py:176-212,
+ * 228-259, and the depth term).  The subgradient of |e| at e = 0 is 0.  Replaces jax.value_and_grad(_loss_fn)
+ * (training.py:263-264) with every regulariser of train_step. */
 int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, const float* directions,
                                  const float* viewdirs, const unsigned* warp_id, const unsigned* app_id,
                                  const unsigned* cam_id, float warp_alpha, const float* t_rand,
@@ -252,8 +261,9 @@ int nfb_train_value_and_grad_reg(nfb_handle* h, int B, const float* origins, con
  * The ray gradient is that of the total loss the call differentiates with the sample points x = o + z d, z a
  * constant (as nfb_render_ray_vjp), with one exception: the elastic loss's Jacobian is evaluated at points
  * held constant (stop_gradient), since its derivative in the points needs the warp's second derivative.  So
- * both photometric losses and the warp regulariser (through its warped term and its direct term in the
- * points) contribute; the elastic and background losses contribute nothing.  Without viewdirs the directions
+ * both photometric losses, the depth loss (through the weights; the target and z are constants) and the warp
+ * regulariser (through its warped term and its direct term in the points) contribute; the elastic and
+ * background losses contribute nothing.  Without viewdirs the directions
  * are encoded as view directions, and that share is in d_directions; with viewdirs it is not.  The
  * parameter gradients and loss_out are those of nfb_train_value_and_grad_reg (up to the order of its float
  * atomics). */
@@ -431,6 +441,7 @@ typedef struct nfb_ray_table {
   const void* order;                 /* (num_rays) permutation; NULL = identity     */
   int order_is_64;                   /* order is int64 (else int32)                 */
   long long num_rays;
+  const float* depth;                /* (num_rays) ray distance in scene units, NaN = no measurement; nullable */
 } nfb_ray_table;
 
 /* Output i (0 <= i < count) is ray r = order[(first + i) mod num_rays] of the table:
@@ -443,6 +454,12 @@ typedef struct nfb_ray_table {
 int nfb_gather_rays(const nfb_ray_table* table, long long first, long long count,
                     float* origins, float* directions, float* pixels, float* rgb,
                     int* appearance, int* camera, int* warp, float* time, void* stream);
+
+/* depth_out (count) = table->depth[r] of the rays nfb_gather_rays draws for the same (table, first, count):
+ * output i is ray order[(first + i) mod num_rays], so the depth batch lines up ray for ray with the rgb batch.
+ * The table must have depth.  No handle, no allocation, ordered on `stream`. */
+int nfb_gather_depth(const nfb_ray_table* table, long long first, long long count, float* depth_out,
+                     void* stream);
 
 /* ---- training camera poses ---------------------------------------------------
  * Image k of a ray table has a pose p_k = (omega_k, v_k), six floats, zero for the capture's camera:
@@ -625,6 +642,17 @@ int nfb_blur_scores(const unsigned char* frames, int num_frames, int height, int
 /* Camera.project (camera.py:283-315) of float32 points (n, 3) -> pixels (n, 2), in float32
  * arithmetic operation for operation as numpy evaluates it.  `cam` is a host struct. */
 int nfb_camera_project(const nfb_camera* cam, const float* points, long long n, float* pixels, void* stream);
+
+/* One sensor depth map onto one frame: src (src_h, src_w) device float32 z-depth (distance along the optical
+ * axis, sensor units; non-finite or <= 0 = missing), at any resolution -> dst (h, w) device float32, the
+ * distance along each pixel centre's unit ray (camera_pixel_direction of `cam`, distortion included) in scene
+ * units: t = z / (d . a) * factor, a the optical axis, factor = metric_scale * scene scale.  `cam` is the
+ * frame's camera at the output scale (host struct; image_size = (w, h)).  Each output pixel takes the mean of
+ * the valid source pixels whose centres lie in its footprint, or, when there are none, the valid source pixel
+ * containing its centre; NaN when neither exists (a missing pixel is never blended).  One launch, one thread
+ * per output pixel. */
+int nfb_depth_resample(const nfb_camera* cam, const float* src, int src_h, int src_w, float factor, float* dst,
+                       void* stream);
 
 /* Per-point outcome of nfb_point_visibility. */
 enum { NFB_TRACK_VISIBLE = 0,      /* the ray from the camera to the point reaches opacity 1/2 at the point    */

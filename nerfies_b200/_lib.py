@@ -32,7 +32,7 @@ SYMBOLS = [
     'nfb_pose_grad', 'nfb_selftest_net_steps', 'nfb_selftest_net', 'nfb_selftest_cond_vjp',
     'nfb_selftest_encode_bwd', 'nfb_selftest_warp_tail_bwd', 'nfb_selftest_ray_reduce', 'nfb_selftest_viewdir_vjp',
     'nfb_gather_rays_refined', 'nfb_pixels_to_rays_refined', 'nfb_intrinsics_grad_workspace_size',
-    'nfb_intrinsics_grad', 'nfb_density_grad',
+    'nfb_intrinsics_grad', 'nfb_density_grad', 'nfb_gather_depth', 'nfb_depth_resample',
 ]
 
 class TrainReg(ctypes.Structure):
@@ -43,7 +43,9 @@ class TrainReg(ctypes.Structure):
               ('warp_reg_loss_alpha', ctypes.c_float), ('warp_reg_loss_scale', ctypes.c_float),
               ('use_background_loss', ctypes.c_int), ('num_background_points', ctypes.c_int),
               ('background_points', ctypes.c_void_p), ('background_warp_ids', ctypes.c_void_p),
-              ('background_noise', ctypes.c_void_p), ('background_loss_weight', ctypes.c_float)]
+              ('background_noise', ctypes.c_void_p), ('background_loss_weight', ctypes.c_float),
+              ('use_depth_loss', ctypes.c_int), ('depth_loss_weight', ctypes.c_float),
+              ('depth_target', ctypes.c_void_p)]
 
 
 ELASTIC_TYPES = {'log_svals': 0, 'svals': 1, 'jtj': 2, 'div': 3, 'det': 4, 'log_det': 5}
@@ -142,6 +144,7 @@ class NfbRayTable(ctypes.Structure):
       ('order', ctypes.c_void_p),
       ('order_is_64', ctypes.c_int),
       ('num_rays', ctypes.c_longlong),
+      ('depth', ctypes.c_void_p),
   ]
 
 
@@ -242,6 +245,8 @@ def load():
   lib.nfb_pixels_to_rays.restype = ci
   lib.nfb_gather_rays.argtypes = [ctypes.POINTER(NfbRayTable), ll, ll] + [vp] * 9
   lib.nfb_gather_rays.restype = ci
+  lib.nfb_gather_depth.argtypes = [ctypes.POINTER(NfbRayTable), ll, ll, vp, vp]
+  lib.nfb_gather_depth.restype = ci
   lib.nfb_gather_rays_posed.argtypes = [ctypes.POINTER(NfbRayTable), ll, ll, vp, vp, vp, vp, vp]
   lib.nfb_gather_rays_posed.restype = ci
   lib.nfb_pose_grad_workspace_size.argtypes = [ci, ll]
@@ -274,6 +279,8 @@ def load():
   lib.nfb_blur_scores.restype = ci
   lib.nfb_camera_project.argtypes = [ctypes.POINTER(NfbCamera), vp, ll, vp, vp]
   lib.nfb_camera_project.restype = ci
+  lib.nfb_depth_resample.argtypes = [ctypes.POINTER(NfbCamera), vp, ci, ci, cf, vp, vp]
+  lib.nfb_depth_resample.restype = ci
   lib.nfb_near_far_workspace_size.argtypes = [ci]
   lib.nfb_near_far_workspace_size.restype = ll
   lib.nfb_near_far.argtypes = [vp, ci, vp, ll, ctypes.c_double, ctypes.c_double, vp, ll, vp, vp, vp, vp]

@@ -6,8 +6,11 @@ per-pixel and per-point work runs on the GPU (include/nerfies_b200.h, "capture p
   downsample_frames    the image pyramid of one frame            nfb_frame_pyramid
   blur_scores          variance of the Laplacian per frame       nfb_blur_scores
   estimate_near_far    per-camera depth quantiles                nfb_near_far
+  resample_depth       a sensor depth map onto one frame         nfb_depth_resample
+  depth_scale_pairs    points projected into a frame             nfb_camera_project
 The rest is host arithmetic on a handful of values per camera:
-  blur_filter, filter_outlier_points, scene_info, orbit_camera_path, split_and_metadata.
+  blur_filter, filter_outlier_points, scene_info, orbit_camera_path, split_and_metadata,
+  estimate_depth_scale.
 DESIGN.md §5.5d lists what each step reproduces, including where the notebook's code and its
 comments disagree.
 """
@@ -233,3 +236,68 @@ def split_and_metadata(item_ids):
     i = bisect.bisect_left(train_ids, image_id)
     metadata[image_id] = {'warp_id': i, 'appearance_id': i, 'camera_id': 0}
   return dataset, metadata
+
+
+# ---- per-frame depth maps (process_capture depth) ----
+MIN_DEPTH_SCALE_PAIRS = 32   # fewer (point, sensor depth) pairs than this: ask for --depth_scale
+
+
+def resample_depth(sensor, camera, factor, device):
+  """A sensor depth map onto one frame (nfb_depth_resample): `sensor` (src_h, src_w) float z-depth in sensor
+  units (non-finite or <= 0 = missing), `camera` the frame's camera at the output scale, `factor` =
+  metric_scale * scene scale.  Returns float32 (h, w) numpy on the host: the distance along each pixel
+  centre's unit ray in scene units, NaN where nothing was measured."""
+  src = torch.from_numpy(np.ascontiguousarray(sensor, np.float32)).to(device)
+  h, w = camera.image_shape
+  out = torch.empty(h, w, dtype=torch.float32, device=device)
+  lib = _lib.load()
+  with torch.cuda.device(device):
+    _lib.check(lib.nfb_depth_resample(ctypes.byref(camera._struct()), _ptr(src), src.shape[0], src.shape[1],
+                                      float(factor), _ptr(out), _stream(device)))
+  return out.cpu().numpy()
+
+
+def depth_scale_pairs(points, camera, sensor, device):
+  """(camera z of each point, sensor depth at its pixel) for the points (N, 3) in world units that project
+  inside the frame of `camera` (its capture camera, any scale; nfb_camera_project) in front of it and land
+  where the four sensor pixels around them are all valid.  The sensor depth is interpolated bilinearly in
+  inverse depth, which is exact on a plane seen by a pinhole.  Two float64 vectors."""
+  pts = np.asarray(points, np.float32).reshape(-1, 3)
+  if not len(pts):
+    return np.zeros(0), np.zeros(0)
+  pixels = camera.project(torch.from_numpy(pts).to(device)).cpu().double().numpy()
+  z = (pts.astype(np.float64) - camera.position.astype(np.float64)) @ camera.orientation[2].astype(np.float64)
+  w, h = (int(v) for v in camera.image_size)
+  sh, sw = sensor.shape
+  # sensor pixel coordinates, with the pixel centres at integers
+  u = pixels[:, 0] * (sw / w) - 0.5
+  v = pixels[:, 1] * (sh / h) - 0.5
+  ok = (z > 0) & np.isfinite(u) & np.isfinite(v) & (u >= 0) & (v >= 0) & (u <= sw - 1) & (v <= sh - 1)
+  u, v, z = u[ok], v[ok], z[ok]
+  j0 = np.minimum(np.floor(u).astype(np.int64), max(sw - 2, 0))
+  i0 = np.minimum(np.floor(v).astype(np.int64), max(sh - 2, 0))
+  j1, i1 = np.minimum(j0 + 1, sw - 1), np.minimum(i0 + 1, sh - 1)
+  fu, fv = u - j0, v - i0
+  s = np.asarray(sensor, np.float64)
+  corners = [s[i0, j0], s[i0, j1], s[i1, j0], s[i1, j1]]
+  valid = np.all([np.isfinite(c) & (c > 0) for c in corners], axis=0)
+  with np.errstate(divide='ignore', invalid='ignore'):
+    inv = [1.0 / c for c in corners]
+    inv_d = ((1 - fv) * ((1 - fu) * inv[0] + fu * inv[1]) + fv * ((1 - fu) * inv[2] + fu * inv[3]))
+    depth = 1.0 / inv_d
+  valid &= np.isfinite(depth) & (depth > 0)
+  return z[valid], depth[valid]
+
+
+def estimate_depth_scale(pairs, min_pairs=MIN_DEPTH_SCALE_PAIRS):
+  """metric_scale (sensor units -> world units) from the (camera z, sensor depth) pairs of every frame: the
+  median of z / sensor depth.  Returns (scale, number of pairs, interquartile range of the ratios); raises
+  ValueError with fewer than `min_pairs` pairs."""
+  z = np.concatenate([p[0] for p in pairs]) if pairs else np.zeros(0)
+  d = np.concatenate([p[1] for p in pairs]) if pairs else np.zeros(0)
+  if len(z) < min_pairs:
+    raise ValueError(f'only {len(z)} COLMAP points meet a sensor depth (at least {min_pairs} are needed to '
+                     'estimate the metric scale): pass --depth_scale')
+  ratio = z / d
+  q1, med, q3 = np.percentile(ratio, [25, 50, 75])
+  return float(med), len(ratio), float(q3 - q1)

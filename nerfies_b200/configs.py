@@ -149,6 +149,13 @@ class TrainConfig:
   # coefficients.  The default is a guess that nobody has tuned.
   camera_intrinsics_lr_schedule: ScheduleDef = dataclasses.field(default_factory=lambda: {
       'type': 'exponential', 'initial_value': 1e-4, 'final_value': 1e-6, 'num_steps': 1000000})
+  # Supervise the expected depth of both levels with the per-frame depth maps of the capture (L1 over the rays
+  # with a measurement).  Needs ExperimentConfig.datasource_kwargs = {'use_depth': True} and depth/<s>x/ maps
+  # (process_capture depth).
+  use_depth_loss: bool = False
+  # The weight of the depth loss; its scale is that of scene units against the photometric loss's squared
+  # colours.  The default leaves the loss at no effect until a schedule is chosen.
+  depth_loss_weight_schedule: ScheduleDef = ('constant', 0.0)
   save_every: int = 10000
   log_every: int = 500
   histogram_every: int = 5000

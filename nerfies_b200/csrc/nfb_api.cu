@@ -16,6 +16,7 @@
 #include "field_simt.cuh"
 #include "ray_kernels.cuh"
 #include "camera_kernels.cuh"
+#include "depth_kernels.cuh"
 #include "pose_kernels.cuh"
 #include "intrinsics_kernels.cuh"
 #include "metrics_kernels.cuh"
@@ -741,6 +742,25 @@ int nfb_gather_rays_refined(const nfb_ray_table* table, long long first, long lo
                      pose, image, intrinsics, group, num_groups, stream);
 }
 
+int nfb_gather_depth(const nfb_ray_table* table, long long first, long long count, float* depth_out,
+                     void* stream) {
+  if (!table) return fail("null ray table");
+  const nfb_ray_table& t = *table;
+  if (t.num_rays < 1) return fail("ray table has %lld rays", t.num_rays);
+  if (count < 0 || first < 0) return fail("negative ray range (first %lld, count %lld)", first, count);
+  if (!t.depth) return fail("depth requested but the ray table has none");
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
+    return fail("no CUDA device: nerfies_b200 has no CPU path");
+  if (count == 0) return 0;
+  if (!depth_out) return fail("null argument");
+  nfb::gather_depth_kernel<<<(unsigned)((count + 255) / 256), 256, 0, (cudaStream_t)stream>>>(t, first, count,
+                                                                                             depth_out);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("gather_depth_kernel launch failed: %s", cudaGetErrorString(e));
+  return 0;
+}
+
 long long nfb_pose_grad_workspace_size(int num_images, long long count) {
   if (num_images < 1 || count < 0) return -1;
   return std::max<long long>(1, (count + nfb::kPoseRays - 1) / nfb::kPoseRays) * num_images * 6 * (long long)sizeof(double);
@@ -965,6 +985,29 @@ int nfb_camera_project(const nfb_camera* cam, const float* points, long long n, 
   nfb::camera_project_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(*cam, points, n, pixels);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail("camera_project_kernel launch failed: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+int nfb_depth_resample(const nfb_camera* cam, const float* src, int src_h, int src_w, float factor, float* dst,
+                       void* stream) {
+  if (!cam) return fail("null argument");
+  if (src_h < 1 || src_w < 1) return fail("nfb_depth_resample: source size %d x %d must be positive", src_h, src_w);
+  if (cam->image_size[0] < 1 || cam->image_size[1] < 1) return fail("image_size must be positive");
+  if (!(cam->focal_length != 0.f) || !(cam->pixel_aspect_ratio != 0.f))
+    return fail("focal_length and pixel_aspect_ratio must be non-zero");
+  if (!(factor > 0.f) || !std::isfinite(factor)) return fail("nfb_depth_resample: factor %g must be positive", factor);
+  int sms = 0;
+  if (device_sms(&sms)) return -1;
+  if (!src || !dst) return fail("null argument");
+  nfb::DepthResampleArgs a{};
+  a.cam = *cam; a.has_distortion = nfb::camera_has_distortion(*cam);
+  a.src = src; a.src_h = src_h; a.src_w = src_w;
+  a.sx = (double)src_w / cam->image_size[0]; a.sy = (double)src_h / cam->image_size[1];
+  a.factor = factor; a.dst = dst;
+  const long long n = (long long)cam->image_size[0] * cam->image_size[1];
+  nfb::depth_resample_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("depth_resample_kernel launch failed: %s", cudaGetErrorString(e));
   return 0;
 }
 

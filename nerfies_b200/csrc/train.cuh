@@ -436,6 +436,51 @@ __global__ void photometric_loss_kernel(const float* __restrict__ out, const flo
   atomicAdd(loss, l);
 }
 
+// The depth loss (no reference counterpart): L1 between the expected depth sum_i w_i z_i and a per-ray target,
+// averaged over the rays whose target is finite and > 0.
+__device__ __forceinline__ bool depth_target_valid(float t) { return isfinite(t) && t > 0.f; }
+
+// The number of valid targets of the whole local batch into *count, before the tape's chunk loop: one block, a
+// fixed reduction order, no host synchronisation.  Exact in float up to 2^24 rays.
+__global__ void __launch_bounds__(256) depth_count_kernel(const float* __restrict__ target, int num_rays,
+                                                          float* __restrict__ count) {
+  __shared__ int part[8];
+  int n = 0;
+  for (int i = threadIdx.x; i < num_rays; i += 256) n += depth_target_valid(target[i]) ? 1 : 0;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = n;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int total = 0;
+    for (int w = 0; w < 8; ++w) total += part[w];
+    *count = (float)total;
+  }
+}
+
+// One level's share, launched after photometric_loss_kernel: adds |depth - target| / count of each valid ray to
+// *loss (unweighted) and writes weight * sign(depth - target) / count into column 3 of d_out, beside the
+// photometric seed (sign(0) = 0: torch's subgradient of abs).  An invalid ray keeps the 0 photometric_loss_kernel
+// wrote; with no valid ray nothing is added.
+__global__ void __launch_bounds__(128) depth_loss_kernel(const float* __restrict__ out, const float* __restrict__ target,
+                                                         const float* __restrict__ count, float weight, int num_rays,
+                                                         float* __restrict__ d_out, float* __restrict__ loss) {
+  const int ray = blockIdx.x * blockDim.x + threadIdx.x;
+  float l = 0.f;
+  if (ray < num_rays) {
+    const float t = target[ray];
+    if (depth_target_valid(t)) {
+      const float inv = 1.f / *count;       // >= 1: this ray is counted
+      const float e = out[ray * 6 + 3] - t;
+      d_out[ray * 6 + 3] = e > 0.f ? weight * inv : (e < 0.f ? -weight * inv : 0.f);
+      l = fabsf(e) * inv;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
+  if ((threadIdx.x & 31) == 0 && l != 0.f) atomicAdd(loss, l);
+}
+
 // The adjoint of volumetric_rendering (model_utils.py:104-126) for given cotangents of its outputs: the seed of
 // every backward (the caller's cotangents in nfb_render_vjp, photometric_loss_kernel's in training).  Per ray
 //   d/dw_i = g_rgb . c_i - [white_bg] sum(g_rgb) + g_depth z_i + g_acc [i < S-1 or !sample_at_infinity] + g_w_i

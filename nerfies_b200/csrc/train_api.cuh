@@ -824,6 +824,13 @@ int nfb_train_value_and_grad_rays(nfb_handle* h, int B, const float* origins, co
     rc_.batch_rays = B; rc_.stats = h->d_loss;
     rcfg = &rc_;
   }
+  // the depth loss averages over the valid targets of the whole batch: count them before the chunks
+  const float* depth_target = (reg && reg->use_depth_loss) ? reg->depth_target : nullptr;
+  if (reg && reg->use_depth_loss) {
+    if (!depth_target) return fail("the depth loss needs depth_target");
+    nfb::train::depth_count_kernel<<<1, 256, 0, s>>>(depth_target, B, h->d_loss + nfb::train::kSlotDepthCount);
+    if (launch_check(h, "depth_count_kernel")) return -1;
+  }
   for (int r0 = 0; r0 < B; r0 += chunk_rays) {
     const int R = std::min(chunk_rays, B - r0);
     // the chunk's rays (the kernels index them from 0)
@@ -841,6 +848,12 @@ int nfb_train_value_and_grad_rays(nfb_handle* h, int B, const float* origins, co
       nfb::train::photometric_loss_kernel<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(out, tg, scale, R, d_out,
                                                                                      h->d_loss + loss_slot);
       if (launch_check(h, "photometric_loss_kernel")) return -1;
+      if (depth_target) {
+        nfb::train::depth_loss_kernel<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(
+            out, depth_target + r0, h->d_loss + nfb::train::kSlotDepthCount, reg->depth_loss_weight, R, d_out,
+            h->d_loss + (lv == 0 ? nfb::train::kSlotDepthCoarse : nfb::train::kSlotDepthFine));
+        if (launch_check(h, "depth_loss_kernel")) return -1;
+      }
       float* dpts = want_rays ? h->d_ray_pts : nullptr;
       float* dnorm = d_directions ? h->d_ray_pts + pts_floats : nullptr;
       if (level_backward(h, lv, R, S, z, d, dcond, use_warp, alpha_step, rgb_step, d_out, nullptr, nullptr, w,

@@ -422,6 +422,7 @@ enum LossSlot {
   kSlotElasticLoss = 2, kSlotElasticResidual = 3, kSlotJacDet = 4, kSlotJacDiv = 5, kSlotJacCurl = 6,
   kSlotWarpRegCoarse = 7, kSlotWarpRegResidualCoarse = 8, kSlotWarpRegFine = 9, kSlotWarpRegResidualFine = 10,
   kSlotBackground = 11, kSlotBackgroundResidual = 12,
+  kSlotDepthCoarse = 13, kSlotDepthFine = 14, kSlotDepthCount = 15,
   kLossSlots = 16
 };
 

@@ -16,9 +16,15 @@ or int64 past 2^31 rays).  Batch s of rank r of W is the rays [s * B + r * B / W
 repeated order (repeat() before batch(), then prepare_tf_data's per-device split), so a run draws
 the batches the reference draws for the same `random_seed`.
 
+With `use_depth=True`, each item may carry a depth map `depth/<scale>x/<id>.npy` (float32 (h, w), the
+distance along each pixel centre's unit ray in scene units, as the renderer's `depth`; non-finite or
+<= 0 = no measurement, loaded as NaN; `process_capture depth` writes them).  The ray table then holds
+one float per ray (4 B of device memory per ray, NaN for an item without a map), and every ray batch
+carries 'depth' (count, 1), drawn by `nfb_gather_depth` in the order of the rgb batch.
+
 Not covered (NotImplementedError): the lazy tf.data path (`preload=False`, whose shuffle buffers
-have no order to reproduce), `shuffle_pixels`, `get_item(scale_factor != 1)`, depth, and
-`flatten=False` with `shuffle=True`.
+have no order to reproduce), `shuffle_pixels`, `get_item(scale_factor != 1)`, relative depth
+(`use_relative_depth`), and `flatten=False` with `shuffle=True`.
 """
 import concurrent.futures
 import ctypes
@@ -93,7 +99,7 @@ def _batch_starts(total, batch_size, repeat, first_batch=0):
 class RayTable:
   """A capture's items on the host: uint8 rgb, cameras, pixel offsets and metadata."""
 
-  def __init__(self, images, cameras, metadata):
+  def __init__(self, images, cameras, metadata, depths=None):
     self.shapes = [img.shape[:2] for img in images]
     sizes = [h * w for h, w in self.shapes]
     self.offsets = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
@@ -101,6 +107,7 @@ class RayTable:
     self.images = images
     self.cameras = cameras
     self.metadata = metadata            # {key: (num_images,) int32 | float32}
+    self.depths = depths                # None, or per image a float32 (h, w) map or None (no map)
 
 
 class DeviceRayTable:
@@ -122,6 +129,13 @@ class DeviceRayTable:
     self.cameras = torch.frombuffer(bytearray(bytes(structs)), dtype=torch.uint8).to(device)
     self.pixel_offsets = torch.from_numpy(host.offsets).to(device)
     self.metadata = {k: torch.from_numpy(v).to(device) for k, v in host.metadata.items()}
+    self.depth = None
+    if host.depths is not None:
+      # one float per ray: 4 B of device memory per ray, NaN where an item has no map
+      self.depth = torch.full((host.num_rays,), float('nan'), dtype=torch.float32, device=device)
+      for d, o in zip(host.depths, host.offsets):
+        if d is not None:
+          self.depth[o:o + d.size].copy_(torch.from_numpy(np.ascontiguousarray(d, np.float32).reshape(-1)))
     self.order = None if order is None else self._upload_order(order)
     self._struct = None
 
@@ -141,11 +155,12 @@ class DeviceRayTable:
       t.order = None if self.order is None else self.order.data_ptr()
       t.order_is_64 = int(self.order is not None and self.order.dtype == torch.int64)
       t.num_rays = self.num_rays
+      t.depth = None if self.depth is None else self.depth.data_ptr()
       self._struct = t
     return self._struct
 
   def nbytes(self):
-    ts = [self.rgb, self.cameras, self.pixel_offsets, self.order, *self.metadata.values()]
+    ts = [self.rgb, self.cameras, self.pixel_offsets, self.order, self.depth, *self.metadata.values()]
     return sum(t.numel() * t.element_size() for t in ts if t is not None)
 
   def gather(self, first, count, order=True, poses=None, intrinsics=None):
@@ -154,7 +169,7 @@ class DeviceRayTable:
     poses, and with `intrinsics` (a pair: (G, 8) float32 deltas and the (num_images,) int32 image -> group
     map, both on the device; training.CameraIntrinsics' delta and group) from the cameras refined by their
     group's delta (nfb_gather_rays_refined); either way the batch carries 'image' (count,) int32, each ray's
-    table image."""
+    table image.  A table with depth adds 'depth' (count, 1) float32 (nfb_gather_depth, NaN = no target)."""
     dev = self.device
     f32 = dict(dtype=torch.float32, device=dev)
     out = {'origins': torch.empty(count, 3, **f32), 'directions': torch.empty(count, 3, **f32),
@@ -196,6 +211,9 @@ class DeviceRayTable:
                                                ptr(group), 0 if delta is None else delta.shape[0],
                                                ptr(out['origins']), ptr(out['directions']), None, ptr(out['image']),
                                                stream))
+      if self.depth is not None:
+        out['depth'] = torch.empty(count, 1, **f32)
+        _lib.check(lib.nfb_gather_depth(ctypes.byref(t), int(first), int(count), ptr(out['depth']), stream))
     return out
 
   def item(self, k):
@@ -203,9 +221,12 @@ class DeviceRayTable:
     h, w = self.shapes[k]
     out = self.gather(int(self.offsets[k]), h * w, order=False)
     shape = lambda x: x.reshape(h, w, -1)
-    return {'rgb': shape(out['rgb']), 'origins': shape(out['origins']),
+    item = {'rgb': shape(out['rgb']), 'origins': shape(out['origins']),
             'directions': shape(out['directions']), 'pixels': shape(out['pixels']),
             'metadata': {key: shape(v) for key, v in out['metadata'].items()}}
+    if 'depth' in out:
+      item['depth'] = shape(out['depth'])
+    return item
 
 
 def _upload(host, device, order):
@@ -221,8 +242,8 @@ class NerfiesDataSource:
                random_seed=0, train_stride=1, val_stride=1, preload=True, device=None, **_):
     if shuffle_pixels:
       raise NotImplementedError('shuffle_pixels belongs to the lazy tf.data path, which is not implemented')
-    if use_depth or use_relative_depth:
-      raise NotImplementedError('NerfiesDataSource has no depth (the reference defines no load_depth)')
+    if use_relative_depth:
+      raise NotImplementedError('use_relative_depth (relative or monocular depth) is not implemented')
     if camera_type != 'json':
       raise ValueError(f'Unknown camera type {camera_type!r}.')
     self.data_dir = pathlib.Path(data_dir)
@@ -247,7 +268,8 @@ class NerfiesDataSource:
     self.camera_dir = self.data_dir / 'camera'
     self.use_appearance_id, self.use_camera_id = use_appearance_id, use_camera_id
     self.use_warp_id, self.use_time = use_warp_id, use_time
-    self.use_depth = False
+    self.use_depth = bool(use_depth)
+    self.depth_dir = self.data_dir / 'depth' / f'{image_scale}x'
     self.train_stride, self.val_stride = train_stride, val_stride
     self.rng = np.random.RandomState(random_seed)
     self.preload = preload
@@ -341,14 +363,44 @@ class NerfiesDataSource:
     camera.position = position.astype(np.float32)
     return camera
 
+  def get_depth_path(self, item_id):
+    return self.depth_dir / f'{item_id}.npy'
+
+  def load_depth(self, item_id):
+    """The item's depth map as float32 (h, w) numpy, or None when it has no file (core.py:605-607): the
+    distance along each pixel centre's unit ray in scene units, with every non-finite or <= 0 value (no
+    measurement) turned into NaN."""
+    path = self.get_depth_path(item_id)
+    if not path.exists():
+      return None
+    depth = np.load(path)
+    if depth.ndim != 2 or not np.issubdtype(depth.dtype, np.floating):
+      raise ValueError(f'{path}: a depth map is a 2-D float array, not {depth.dtype} {depth.shape}')
+    depth = depth.astype(np.float32)
+    depth[~(np.isfinite(depth) & (depth > 0))] = np.nan
+    return depth
+
+  def _checked_depth(self, item_id, shape):
+    depth = self.load_depth(item_id)
+    if depth is not None and depth.shape != tuple(shape):
+      raise ValueError(f'item {item_id!r}: depth map {self.get_depth_path(item_id)} is {depth.shape} (h, w) but '
+                       f'its image {self.get_rgb_path(item_id)} is {tuple(shape)}')
+    return depth
+
   def get_item(self, item_id, scale_factor=1.0):
-    """{'camera_params', 'rgb' (device float32), 'metadata'} (core.py:567-619)."""
+    """{'camera_params', 'rgb' (device float32), 'metadata'} (core.py:567-619); with use_depth and a map,
+    also 'depth' (h, w, 1) device float32."""
     if scale_factor != 1.0:
       raise NotImplementedError('get_item(scale_factor != 1) needs image_utils.rescale_image, '
                                 'which is not implemented')
     camera = self.load_camera(item_id)
-    return {'camera_params': camera.get_parameters(), 'rgb': self.load_rgb(item_id),
+    item = {'camera_params': camera.get_parameters(), 'rgb': self.load_rgb(item_id),
             'metadata': self._item_metadata(item_id)}
+    if self.use_depth:
+      depth = self._checked_depth(item_id, item['rgb'].shape[:2])
+      if depth is not None:
+        item['depth'] = torch.from_numpy(depth[..., None]).to(self.device)
+    return item
 
   def load_points(self, shuffle=False):
     """Background points (N, 3) float32 on the device, centred and scaled into the scene; with
@@ -387,7 +439,12 @@ class NerfiesDataSource:
     mds = [self._item_metadata(i) for i in item_ids]
     metadata = {k: np.array([md[k] for md in mds], np.float32 if k == 'time' else np.int32)
                 for k in _METADATA_KEYS if k in mds[0]}
-    return RayTable(images, cameras, metadata)
+    depths = None
+    if self.use_depth:
+      depths = _parallel_map(lambda a: self._checked_depth(a[0], a[1].shape[:2]), list(zip(item_ids, images)))
+      if all(d is None for d in depths):
+        depths = None
+    return RayTable(images, cameras, metadata, depths)
 
   def create_iterator(self, item_ids, batch_size, repeat=True, flatten=False, shuffle=False,
                       prefetch_size=0, shuffle_buffer_size=1000000, devices=None, rank=None,

@@ -13,6 +13,14 @@ With `--save_viz`, each frame also writes the colour-mapped images of eval.py:87
 two files), and the images the reference sends to TensorBoard, `disparity_expected_viz_`,
 `disparity_median_viz_`, `acc_viz_` and, for items with a target, `rgb_abs_error_viz_` and
 `rgb_sq_error_viz_<id>.png`.
+Items that carry a depth map (`NerfiesDataSource(use_depth=True)` and `depth/<s>x/<id>.npy`) are also
+scored by `metrics-eval/depth_abs/{tag}`, the mean over the pixels with a measurement of |target -
+median depth| (eval.py:137-140); with `--save_viz` they also write the reference's three depth images
+(eval.py:139-150): `depth_target_viz_<id>.png` (magma over [near, far], inverted, as the rendered depth),
+`depth_median_error_viz_<id>.png` and `depth_expected_error_viz_<id>.png` (magma over [0, 1] of the
+absolute error of the median and expected depth).  A pixel without a measurement (NaN) is drawn black in all
+three, the colour of a NaN cast to uint8 as the reference's colorize does on x86-64.  An item whose map has
+no measurement at all has no depth score and drops out of the tag's mean.
 With `--save_normals`, each frame also writes `normals_<id>.png`: the surface normals at the median depth of
 the frame's last level (geometry.normal_map, coloured in the camera's frame by
 visualization.normals_to_color; black where a ray meets no surface).
@@ -109,11 +117,23 @@ def normal_image(model, params, camera, warp_extra, metadata, med_depth):
   return visualization.normals_to_color(normals['normals'], normals['valid'], camera)
 
 
-def render_and_score(model, params, camera, warp_extra, metadata, rgb_target, viz_range=None, normals=False):
+def depth_viz_images(render, depth_target, near, far):
+  """The depth images of eval.py:139-150 as uint8 device images, by file stem; depth_target (h, w, 1) or
+  (h, w), NaN where there is no measurement (drawn black)."""
+  viz = visualization.colorize_uint8
+  target = depth_target.reshape(render['med_depth'].shape)
+  return {'depth_target_viz': viz(target, near, far, invert=True),
+          'depth_median_error_viz': viz((target - render['med_depth']).abs(), 0.0, 1.0),
+          'depth_expected_error_viz': viz((target - render['depth']).abs(), 0.0, 1.0)}
+
+
+def render_and_score(model, params, camera, warp_extra, metadata, rgb_target, viz_range=None, normals=False,
+                     depth_target=None):
   """One frame on the GPU: ({file stem: uint8 / uint16 device image}, {metric: 0-d device tensor}).
   The images are what eval.py:99-108 saves, plus `viz_images` when `viz_range` is the scene's
   (near, far) and `normal_image` ('normals') with `normals`; the metrics eval.py:118-125's, without
-  `ssim` for frames MS-SSIM cannot take."""
+  `ssim` for frames MS-SSIM cannot take.  With `depth_target` (h, w, 1), also 'depth_abs' (eval.py:137-140)
+  and, with `viz_range`, `depth_viz_images`."""
   render = evaluation.render_frame(model, params, camera, warp_extra, metadata)
   images = {'rgb': evaluation.image_to_uint8(render['rgb']),
             'depth_expected': evaluation.depth_to_uint16(render['depth']),
@@ -122,14 +142,19 @@ def render_and_score(model, params, camera, warp_extra, metadata, rgb_target, vi
     images.update(viz_images(render, rgb_target, *viz_range))
   if normals:
     images['normals'] = normal_image(model, params, camera, warp_extra, metadata, render['med_depth'])
+  if depth_target is not None and viz_range is not None:
+    images.update(depth_viz_images(render, depth_target, *viz_range))
   metrics = {}
   if rgb_target is not None:
     if min(rgb_target.shape[:2]) >= evaluation.MIN_METRICS_SIZE:
-      out = evaluation.compute_metrics(render['rgb'], rgb_target)
-      metrics = {k: out[k] for k in ('mse', 'psnr', 'ssim')}
-    else:   # nfb_image_metrics takes no frame this small; eval.py:120-121 as written, on the device
+      depth = {} if depth_target is None else {'depth_med': render['med_depth'], 'depth_target': depth_target}
+      out = evaluation.compute_metrics(render['rgb'], rgb_target, **depth)
+      metrics = {k: out[k] for k in ('mse', 'psnr', 'ssim', 'depth_abs') if k in out}
+    else:   # nfb_image_metrics takes no frame this small; eval.py:120-121 and 140 as written, on the device
       mse = ((render['rgb'] - rgb_target)**2).mean()
       metrics = {'mse': mse, 'psnr': evaluation.compute_psnr(mse)}
+      if depth_target is not None:
+        metrics['depth_abs'] = (depth_target.reshape(render['med_depth'].shape) - render['med_depth']).abs().nanmean()
   return images, metrics
 
 
@@ -165,15 +190,17 @@ def write_png(path, array):
 
 
 def process_items(tag, items, step, model, params, warp_extra, save_dir, writer, pool, frame_fn, log):
-  """eval.py:155-214 for one tag.  `items`: (item_id, camera, metadata, rgb target or None)."""
+  """eval.py:155-214 for one tag.  `items`: (item_id, camera, metadata, rgb target or None), and for an item
+  with a depth map a fifth element, its (h, w, 1) depth, which `frame_fn` receives as `depth_target`."""
   save_dir = save_dir / f'{step:08d}' / tag if save_dir else None
   if save_dir:
     save_dir.mkdir(parents=True, exist_ok=True)
   meters, pending, noticed = {}, [], False
-  for i, (item_id, camera, metadata, rgb_target) in enumerate(items):
+  for i, (item_id, camera, metadata, rgb_target, *depth) in enumerate(items):
     log(f'[{tag}:{i + 1}/{len(items)}] Processing {item_id}')
     item_id = str(item_id).replace('/', '_')
-    images, metrics = frame_fn(model, params, camera, warp_extra, metadata, rgb_target)
+    extra = {'depth_target': depth[0]} if depth else {}
+    images, metrics = frame_fn(model, params, camera, warp_extra, metadata, rgb_target, **extra)
     if rgb_target is not None and 'ssim' not in metrics and not noticed:
       log(f'\t{tag}: frames below {evaluation.MIN_METRICS_SIZE} pixels on a side have no MS-SSIM; ssim is not logged')
       noticed = True
@@ -186,8 +213,14 @@ def process_items(tag, items, step, model, params, warp_extra, save_dir, writer,
   for future in pending:
     future.result()
   if meters and writer is not None:                                              # eval.py:210-214
-    writer.write(step, {f'metrics-eval/{k}/{tag}': sum(float(v) for v in vs) / len(vs)
-                        for k, vs in meters.items()})
+    means = {}
+    for k, vs in meters.items():
+      vs = [float(v) for v in vs]
+      if k == 'depth_abs':        # an item without a single measurement has no depth score
+        vs = [v for v in vs if not np.isnan(v)]
+      if vs:
+        means[f'metrics-eval/{k}/{tag}'] = sum(vs) / len(vs)
+    writer.write(step, means)
 
 
 def delete_old_renders(render_dir, max_renders):
@@ -205,14 +238,14 @@ def refined_items(items, saved_poses, saved_intrinsics=None):
   from nerfies_b200 import geometry
   deltas = {str(i): g['delta'] for g in (saved_intrinsics or {}).get('groups', {}).values() for i in g['items']}
   out = []
-  for item_id, cam, md, rgb in items:
+  for item_id, cam, md, rgb, *depth in items:
     pose = (saved_poses or {}).get('items', {}).get(str(item_id))
     if pose is not None:
       p = np.asarray(pose['pose'], np.float64).reshape(6)
       cam = geometry.posed_camera(cam, p[:3], p[3:])
     if str(item_id) in deltas:
       cam = geometry.refined_camera(cam, deltas[str(item_id)])
-    out.append((item_id, cam, md, rgb))
+    out.append((item_id, cam, md, rgb, *depth))
   return out
 
 
@@ -245,7 +278,7 @@ def evaluate(exp_config, model_config, train_config, eval_config, base_folder, d
       frame_fn = functools.partial(frame_fn, normals=True)
 
     def items_of(ids):                                                           # eval.py:297-300
-      return [(i, datasource.load_camera(i), item['metadata'], item['rgb'])
+      return [(i, datasource.load_camera(i), item['metadata'], item['rgb'], *([item['depth']] if 'depth' in item else []))
               for i in ids for item in [datasource.get_item(i)]]
     sets = [('val', items_of(strided_subset(datasource.val_ids, eval_config.num_val_eval))),
             ('train', items_of(strided_subset(datasource.train_ids, eval_config.num_train_eval)))]

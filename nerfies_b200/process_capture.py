@@ -9,6 +9,12 @@ because COLMAP runs between them:
            frames the blur filter selects, and writes scene.json, dataset.json, metadata.json,
            camera/<id>.json, camera-paths/orbit-mild/<i>.json and points.npy (the track-filtered
            COLMAP points in world coordinates, which TrainConfig.use_background_loss reads).
+  depth    per-frame sensor depth (--depth_dir: <id>.npy metric z-depth maps at any resolution, e.g.
+           a phone's LiDAR) to depth/<s>x/<id>.npy for every scale under rgb/: float32 maps of the
+           frame's size holding the distance along each pixel centre's unit ray in scene units (the
+           renderer's depth), NaN where nothing was measured.  Sensor units become COLMAP units by
+           --depth_scale, or by the median ratio of the COLMAP points' camera depth to the sensor depth
+           at their pixels.  Run after `scene`.
 
 The flags are the notebook's @param values; its other literals are constants of
 nerfies_b200.capture.  PNGs are decoded on host threads, each frame is uploaded once, and PNGs
@@ -72,7 +78,15 @@ def make_parser():
   sc.add_argument('--orbit_radius', type=float, default=0.75)
   sc.add_argument('--orbit_x_scale', type=float, default=0.75)
   sc.add_argument('--orbit_y_scale', type=float, default=0.75)
-  for s in (im, sc):
+  dp = sub.add_parser('depth', help='write depth/<s>x/ from per-frame sensor depth maps')
+  dp.add_argument('--data_dir', required=True, help='capture directory (after `scene`)')
+  dp.add_argument('--depth_dir', required=True,
+                  help='directory of <id>.npy sensor z-depth maps (distance along the optical axis), any resolution')
+  dp.add_argument('--depth_scale', type=_positive_float, default=None,
+                  help='sensor units -> COLMAP world units (default: estimated from points.npy)')
+  dp.add_argument('--allow_missing', action='store_true',
+                  help='skip the items without a depth map (no file is written for them)')
+  for s in (im, sc, dp):
     s.add_argument('--device', default='cuda', help='CUDA device')
   return p
 
@@ -158,10 +172,88 @@ def run_scene(args):
   return {'removed': removed, 'scores': dict(zip(registered, scores.tolist())), 'near': near, 'far': far}
 
 
+def _png_size(path):
+  """(h, w) of a PNG from its header."""
+  with open(path, 'rb') as f:
+    head = f.read(24)
+  if head[:8] != b'\x89PNG\r\n\x1a\n':
+    raise ValueError(f'{path} is not a PNG')
+  w, h = (int.from_bytes(head[o:o + 4], 'big') for o in (16, 20))
+  return h, w
+
+
+def _load_sensor_depth(path):
+  depth = np.load(path)
+  if depth.ndim != 2 or not np.issubdtype(depth.dtype, np.floating):
+    raise ValueError(f'{path}: a sensor depth map is a 2-D float array, not {depth.dtype} {depth.shape}')
+  return depth
+
+
+def run_depth(args, log=print):
+  """`depth`: checks everything on the host first (ids, map files and shapes, scene.json, scales, each frame's
+  size against its scaled camera, points), so a refusal writes nothing; then one nfb_depth_resample launch per
+  item and scale.  Returns {'metric_scale', 'pairs', 'iqr',
+  'written': [paths], 'missing': [ids]}."""
+  data_dir, raw_dir = pathlib.Path(args.data_dir), pathlib.Path(args.depth_dir)
+  for name in ('scene.json', 'dataset.json'):
+    if not (data_dir / name).exists():
+      raise FileNotFoundError(f'{data_dir / name} is missing: run `process_capture scene` first')
+  scene = json.loads((data_dir / 'scene.json').read_text())
+  ids = [str(i) for i in json.loads((data_dir / 'dataset.json').read_text())['ids']]
+  missing = [i for i in ids if not (raw_dir / f'{i}.npy').exists()]
+  if missing and not args.allow_missing:
+    raise FileNotFoundError(f'{len(missing)} item(s) have no depth map in {raw_dir}: {missing[:10]} '
+                            '(--allow_missing skips them)')
+  ids = [i for i in ids if i not in missing]
+  if not ids:
+    raise FileNotFoundError(f'no item of {data_dir / "dataset.json"} has a depth map in {raw_dir}')
+  sensors = {i: _load_sensor_depth(raw_dir / f'{i}.npy') for i in ids}
+  scales = sorted(int(p.name[:-1]) for p in (data_dir / 'rgb').glob('*x')
+                  if p.is_dir() and p.name[:-1].isdigit()) if (data_dir / 'rgb').is_dir() else []
+  if not scales:
+    raise FileNotFoundError(f'{data_dir / "rgb"} holds no <s>x/ directory')
+  cameras = {i: datasets.camera_lib.Camera.from_json(data_dir / 'camera' / f'{i}.json') for i in ids}
+  frames = []                 # (item, scale, camera at that scale) of every map to write
+  for i in ids:
+    for s in scales:
+      png = data_dir / 'rgb' / f'{s}x' / f'{i}.png'
+      if not png.exists():
+        continue
+      cam = cameras[i].scale(1.0 / s)
+      if cam.image_shape != _png_size(png):
+        raise ValueError(f'{png} is {_png_size(png)} (h, w) but its camera scaled by 1/{s} gives {cam.image_shape}')
+      frames.append((i, s, cam))
+  points = None
+  if args.depth_scale is None:
+    if not (data_dir / 'points.npy').exists():
+      raise FileNotFoundError(f'{data_dir / "points.npy"} is missing: pass --depth_scale')
+    points = np.load(data_dir / 'points.npy')
+  device = torch.device(args.device)
+  pairs, iqr = 0, None
+  if points is None:
+    metric_scale = float(args.depth_scale)
+  else:
+    metric_scale, pairs, iqr = capture.estimate_depth_scale(
+        [capture.depth_scale_pairs(points, cameras[i], sensors[i], device) for i in ids])
+    log(f'metric scale {metric_scale:.6g} from {pairs} point/depth pairs (interquartile range {iqr:.3g})')
+  factor = metric_scale * float(scene['scale'])
+  written = []
+  for i, s, cam in frames:
+    out = data_dir / 'depth' / f'{s}x' / f'{i}.npy'
+    out.parent.mkdir(parents=True, exist_ok=True)
+    np.save(out, capture.resample_depth(sensors[i], cam, factor, device))
+    written.append(out)
+  log(f'wrote {len(written)} depth maps for {len(ids)} items at scales {scales}'
+      + (f'; {len(missing)} items without a map: {missing[:10]}' if missing else ''))
+  return {'metric_scale': metric_scale, 'pairs': pairs, 'iqr': iqr, 'written': written, 'missing': missing}
+
+
 def main(argv=None):
   args = make_parser().parse_args(argv)
   if args.command == 'images':
     run_images(args.frames_dir, args.data_dir, args.image_scales, torch.device(args.device))
+  elif args.command == 'depth':
+    run_depth(args)
   else:
     run_scene(args)
   return 0

@@ -93,6 +93,19 @@ def check_camera_intrinsics(train_config, saved, train_cameras=None):
                        f'but the train items group as {sorted(sorted(g) for g in want)}')
 
 
+def check_depth(train_config, datasource):
+  """Refuses, with ValueError before any training step, use_depth_loss with a data source that loads no depth:
+  one without use_depth, or one whose train items have no depth map."""
+  if not train_config.use_depth_loss:
+    return
+  if not getattr(datasource, 'use_depth', False):
+    raise ValueError("TrainConfig.use_depth_loss needs depth maps, but the data source loads none: set "
+                     "ExperimentConfig.datasource_kwargs = {'use_depth': True}")
+  if not any(datasource.get_depth_path(i).exists() for i in datasource.train_ids):
+    raise ValueError(f'TrainConfig.use_depth_loss is on but no train item has a depth map under '
+                     f'{datasource.depth_dir} (python -m nerfies_b200.process_capture depth)')
+
+
 def write_cameras(datasource, item_ids, poses, intrinsics, directory):
   """`<directory>/<item>.json` of each refined train camera at the capture's original scale: moved by its
   pose (training.CameraPoses or None) and refined by its group's intrinsics delta (training.CameraIntrinsics or
@@ -145,6 +158,7 @@ def _train(exp_config, model_config, train_config, base_folder, data_dir, precis
   check_camera_intrinsics(train_config, saved_intrinsics)
   if datasource is None:
     datasource = driver_utils.make_datasource(exp_config, model_config, data_dir)
+  check_depth(train_config, datasource)
   check_camera_poses(train_config, saved_poses, datasource.train_ids)
   train_cameras = None
   if train_config.refine_camera_intrinsics:
@@ -154,6 +168,7 @@ def _train(exp_config, model_config, train_config, base_folder, data_dir, precis
   warp_alpha_sched = schedules.from_config(train_config.warp_alpha_schedule)
   time_alpha_sched = schedules.from_config(train_config.time_alpha_schedule)
   elastic_loss_weight_sched = schedules.from_config(train_config.elastic_loss_weight_schedule)
+  depth_loss_weight_sched = schedules.from_config(train_config.depth_loss_weight_schedule)
 
   model, params = models.construct_nerf(                                         # train.py:205-217
       step_key(exp_config.random_seed, 0, 0), model_config, batch_size=train_config.batch_size // world,
@@ -206,7 +221,8 @@ def _train(exp_config, model_config, train_config, base_folder, data_dir, precis
       warp_reg_loss_weight=train_config.warp_reg_loss_weight,
       warp_reg_loss_alpha=train_config.warp_reg_loss_alpha,
       warp_reg_loss_scale=train_config.warp_reg_loss_scale,
-      background_loss_weight=train_config.background_loss_weight)
+      background_loss_weight=train_config.background_loss_weight,
+      depth_loss_weight=depth_loss_weight_sched(0))
 
   def save(step):
     if rank == 0:
@@ -225,6 +241,7 @@ def _train(exp_config, model_config, train_config, base_folder, data_dir, precis
       batch['background_points'] = next(points_iter)
     scalar_params.learning_rate = learning_rate_sched(step)
     scalar_params.elastic_loss_weight = elastic_loss_weight_sched(step)
+    scalar_params.depth_loss_weight = depth_loss_weight_sched(step)
     if state.camera_poses is not None:
       scalar_params.camera_pose_learning_rate = pose_lr_sched(step)
     if state.camera_intrinsics is not None:
@@ -237,7 +254,8 @@ def _train(exp_config, model_config, train_config, base_folder, data_dir, precis
         elastic_reduce_method=train_config.elastic_reduce_method,
         elastic_loss_type=train_config.elastic_loss_type,
         use_background_loss=train_config.use_background_loss,
-        use_warp_reg_loss=train_config.use_warp_reg_loss)
+        use_warp_reg_loss=train_config.use_warp_reg_loss,
+        use_depth_loss=train_config.use_depth_loss)
 
     if step % train_config.print_every == 0 and rank == 0:
       log(f'step={step}, warp_alpha={state.warp_alpha:.04f}, time_alpha={state.time_alpha:.04f}, '
@@ -253,6 +271,8 @@ def _train(exp_config, model_config, train_config, base_folder, data_dir, precis
       scalars = {'params/learning_rate': scalar_params.learning_rate,            # train.py:64-68
                  'params/warp_alpha': state.warp_alpha, 'params/time_alpha': state.time_alpha,
                  'params/elastic_loss/weight': scalar_params.elastic_loss_weight}
+      if train_config.use_depth_loss:
+        scalars['params/depth_loss/weight'] = scalar_params.depth_loss_weight
       scalars.update({k: float(v) for k, v in flatten_stats(stats).items()})     # the synchronisation
       now.synchronize()
       scalars['time/steps_per_sec'] = (step - mark_step) * 1000.0 / max(mark.elapsed_time(now), 1e-6)

@@ -44,6 +44,7 @@ class ScalarParams:
   background_noise_std: float = 0.001
   camera_pose_learning_rate: float = 0.0    # Adam's rate for TrainState.camera_poses (TrainConfig.refine_camera_poses)
   camera_intrinsics_learning_rate: float = 0.0   # Adam's rate for TrainState.camera_intrinsics
+  depth_loss_weight: float = 0.0            # the weight of the depth loss (TrainConfig.use_depth_loss)
 
 
 class AdamOptimizer(model_utils.Optimizer):
@@ -313,8 +314,10 @@ class CameraIntrinsics:
 
 def make_reg(model, scalar_params=None, use_elastic_loss=False, elastic_reduce_method='median',
              elastic_loss_type='log_svals', use_background_loss=False, use_warp_reg_loss=False,
-             background_points=None, background_warp_ids=None, background_noise=None):
+             background_points=None, background_warp_ids=None, background_noise=None, use_depth_loss=False,
+             depth_target=None):
   """The regulariser switches of train_step (training.py:138-147) + ScalarParams -> nfb_train_reg.
+  With `use_depth_loss`, `depth_target` (B,) or (B, 1) is the batch's 'depth' (NaN or <= 0: no target).
   Returns (TrainReg, keepalive list of the device tensors it points to)."""
   sp = scalar_params
   reg = _lib.TrainReg()
@@ -342,6 +345,14 @@ def make_reg(model, scalar_params=None, use_elastic_loss=False, elastic_reduce_m
     reg.background_warp_ids = ids.data_ptr()
     reg.background_noise = None if noise is None else noise.data_ptr()
     reg.background_loss_weight = float(sp.background_loss_weight) if sp else 0.0
+  reg.use_depth_loss = int(bool(use_depth_loss))
+  if use_depth_loss:
+    if depth_target is None:
+      raise ValueError("the depth loss needs the batch's 'depth' (NerfiesDataSource(use_depth=True))")
+    target = _prep_f32(depth_target, model.device).reshape(-1).contiguous()
+    keep.append(target)
+    reg.depth_target = target.data_ptr()
+    reg.depth_loss_weight = float(sp.depth_loss_weight) if sp else 0.0
   return reg, keep
 
 
@@ -400,6 +411,8 @@ def value_and_grad(model, params, batch, warp_extra, rngs=None, chunk_rays=256, 
                 'jacobian_div': loss[5], 'jacobian_curl': loss[6], 'warp_reg_coarse': loss[7],
                 'warp_reg_residual_coarse': loss[8], 'warp_reg_fine': loss[9],
                 'warp_reg_residual_fine': loss[10], 'background': loss[11]})
+    if reg_struct.use_depth_loss:
+      out.update({'depth_coarse': loss[13], 'depth_fine': loss[14], 'depth_count': loss[15]})
   return out, grads
 
 
@@ -421,13 +434,16 @@ def grads_to_tree(model, grads):
 def train_step(model, rng_key, state, batch, scalar_params, use_elastic_loss=False,
                elastic_reduce_method='median', elastic_loss_type='log_svals',
                use_background_loss=False, use_warp_reg_loss=False, chunk_rays=256,
-               timings=None):
+               timings=None, use_depth_loss=False):
   """One optimisation step (training.py:138-271).  Returns (new_state, stats, rng_key).
+
+  use_depth_loss adds depth_loss_weight * mean |depth - batch['depth']| per level over the rays with a
+  target (the stats' 'loss/depth', also added into 'loss/total').
 
   timings (optional dict) receives 'value_and_grad_ms', 'all_reduce_ms', 'adam_ms' measured
   with CUDA events on the current stream."""
   reg = None
-  if use_elastic_loss or use_warp_reg_loss or use_background_loss:
+  if use_elastic_loss or use_warp_reg_loss or use_background_loss or use_depth_loss:
     bg = {}
     if use_background_loss:
       # training.py:122-126: ids ~ random.choice(key, model.warp_ids), noise ~ noise_std * N(0, 1)
@@ -440,8 +456,11 @@ def train_step(model, rng_key, state, batch, scalar_params, use_elastic_loss=Fal
       bg['background_noise'] = batch.get(
           'background_noise',
           scalar_params.background_noise_std * torch.randn(pts.shape[0], 3, generator=gen))
+    if use_depth_loss and 'depth' not in batch:
+      raise ValueError("use_depth_loss needs batches with 'depth' (NerfiesDataSource(use_depth=True))")
     reg = make_reg(model, scalar_params, use_elastic_loss, elastic_reduce_method, elastic_loss_type,
-                   use_background_loss, use_warp_reg_loss, **bg)
+                   use_background_loss, use_warp_reg_loss, **bg, use_depth_loss=use_depth_loss,
+                   depth_target=batch.get('depth'))
   opt = state.optimizer
   ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)] if timings is not None else None
   if ev:
@@ -493,6 +512,10 @@ def train_step(model, rng_key, state, batch, scalar_params, use_elastic_loss=Fal
       stats[lv]['loss/total'] = stats[lv]['loss/total'] + scalar_params.warp_reg_loss_weight * losses['warp_reg_' + lv]
   if use_background_loss:
     stats['background_loss'] = losses['background']
+  if use_depth_loss:
+    for lv in [lv for lv in ('coarse', 'fine') if lv in stats]:
+      stats[lv]['loss/depth'] = losses['depth_' + lv]
+      stats[lv]['loss/total'] = stats[lv]['loss/total'] + scalar_params.depth_loss_weight * losses['depth_' + lv]
   if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
     # jax.lax.pmean(grad, 'batch') (training.py:266): one collective over the flat vector
     dist.all_reduce(grads)
